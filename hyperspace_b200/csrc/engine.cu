@@ -957,6 +957,7 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
   uint32_t* perm = out->perm.get();
   uint32_t* perm_alt = out->perm_alt.get();
   Buf<unsigned long long> d_or_and(ctx, 2);
+  bool sort_deferred = false;
   for (int k = nkeys - 1; k >= 0; k--) {
     DevColumn& kc = out->part.cols[k];
     // The first column sorted (the last indexed column) starts from rows in partition order: its first radix pass reads
@@ -1019,6 +1020,32 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
       launch_encode_keys(ctx, kc.data.get(), kc.type, nullptr, nrows, keys, d_or_and.get());
       first_src = nullptr;
     }
+    // A null-free fixed-width first column is sorted completely in shared memory (k_local_sort): straight from the raw
+    // column when every bucket fits one CTA, else after one MSD pass on the 8 bits below the highest varying bit, as long as
+    // the (bucket, digit) sub-buckets fit -- two HBM passes instead of one per varying byte.  Buckets with more than ~0.85 x
+    // 256 x kLocalSortCap rows would rarely pass the sub-bucket check, so they skip the MSD histogram.
+    // HS_LSD_SORT=1: LSD passes (+ tie-run fix-up) only (A/B switch).
+    const bool lsd_only = getenv("HS_LSD_SORT") != nullptr;
+    if (first_src && !kc.has_nulls && !lsd_only && !full_sort_only) {
+      bool local_done = false;
+      if (max_bucket <= (uint64_t)kLocalSortCap) {
+        segmented_sort_local(ctx, out->bucket_offsets.data(), num_buckets, raw, out->keys.get(), out->perm.get());
+        local_done = true;
+      } else if (nbytes > 2 && max_bucket <= (uint64_t)(0.85 * 256 * kLocalSortCap)) {
+        const int shift = std::max(0, 63 - __builtin_clzll(varying) - 7);
+        local_done = segmented_sort_msd_local(ctx, &out->plan, raw, shift, out->keys.get(), out->keys_alt.get(),
+                                              out->perm.get(), out->perm_alt.get());
+      }
+      if (local_done) {
+        keys = out->keys.get();
+        perm = out->perm.get();
+        keys_alt = out->keys_alt.get();
+        perm_alt = out->perm_alt.get();
+        // a single key column is the last thing this function sorts: the caller need not wait for it
+        sort_deferred = defer_settle && nkeys == 1;
+        continue;  // (null-free: no validity pass)
+      }
+    }
     if (nbytes > want_bytes && !full_sort_only) {
       const uint64_t high_mask = ~0ull << (8 * fourth_from_top);
       const uint64_t low_mask = ~high_mask;
@@ -1051,7 +1078,7 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
   out->sorted_keys = keys;
   out->sorted_perm = perm;
   t_sort->stop();
-  if (out->fix_pending) {  // no synchronisation here: the stage timers are read in settle_sort
+  if (out->fix_pending || sort_deferred) {  // no synchronisation here: the stage timers are read in settle_sort
     out->pending_timers.push_back(IndexedRows::DeferredTimer{std::move(t_sort), &hs_stats::ms_sort});
     return;
   }

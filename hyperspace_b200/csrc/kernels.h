@@ -239,6 +239,21 @@ void segmented_sort_pairs(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t
 // *d_flag is set when a run is longer than max_run (the caller then runs the remaining passes instead).
 void launch_fix_runs(hs_ctx* ctx, SortPlan* plan, uint64_t* keys, uint32_t* vals, uint64_t high_mask, uint64_t low_mask,
                      uint32_t max_run, uint32_t* d_flag);
+// Local sort (k_local_sort): one CTA sorts up to kLocalSortCap pairs completely and stably in shared memory.
+constexpr int kLocalSortCap = 12288;
+struct LocalSortItem {
+  uint32_t start, count;  // a range of pairs that is sorted as a whole
+};
+// Every segment (at most kLocalSortCap rows each) sorted completely on the raw key column in one HBM pass; the result
+// (encoded keys, partition-order row positions) is written to (keys, vals).
+void segmented_sort_local(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, const RawKeyColumn& raw, uint64_t* keys,
+                          uint32_t* vals);
+// Complete sort of the raw key column within every segment in two HBM passes: one stable MSD pass on digit
+// (key >> shift) & 255 into (keys_alt, vals_alt), then k_local_sort of every (segment, digit) sub-bucket into (keys, vals).
+// The bits above shift + 7 must be constant over the input.  Returns false, having queued only the MSD histogram, when a
+// sub-bucket holds more than kLocalSortCap rows; the caller then sorts some other way.  Synchronises the stream once.
+bool segmented_sort_msd_local(hs_ctx* ctx, SortPlan* plan, const RawKeyColumn& raw, int shift, uint64_t* keys,
+                              uint64_t* keys_alt, uint32_t* vals, uint32_t* vals_alt);
 // One extra stable pass on an external 8-bit digit: digit = digits[vals[i]]  (null flags for nullable 64-bit keys)
 void segmented_sort_pass_by_table(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t*& keys_alt, uint32_t*& vals,
                                   uint32_t*& vals_alt, const uint8_t* digits);

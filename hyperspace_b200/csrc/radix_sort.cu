@@ -8,6 +8,9 @@
 // (tile, digit) its global destination) -> k_sort_scatter (stable in-tile ranking with __match_any_sync, exchange
 // through shared memory so each digit's items leave the tile as one contiguous run).  Passes whose digit is constant
 // over the whole input (OR == AND on those bits) are skipped.
+//
+// k_local_sort finishes ranges that fit one CTA in shared memory: whole small segments straight from the raw column, or
+// the (segment, digit) sub-buckets of one MSD pass -- two HBM passes for keys whose LSD sort would take three or more.
 #include "device_utils.cuh"
 #include "kernels.h"
 
@@ -85,10 +88,11 @@ __global__ void __launch_bounds__(256) k_seg_chunk_sums(const SortChunk* __restr
   chunk_sums[(size_t)blockIdx.x * 256 + threadIdx.x] = s;
 }
 
-// B: one CTA per segment: prefix over the segment's chunks, then digit bases
+// B: one CTA per segment: prefix over the segment's chunks, then digit bases (also written to digit_base[seg * 256 + digit]
+// when it is given: the first position of every (segment, digit) sub-bucket)
 __global__ void __launch_bounds__(256) k_seg_scan(const uint32_t* __restrict__ seg_chunk_begin,
                                                    const uint64_t* __restrict__ seg_start,
-                                                   uint32_t* __restrict__ chunk_sums) {
+                                                   uint32_t* __restrict__ chunk_sums, uint32_t* __restrict__ digit_base) {
   __shared__ uint32_t warp_sums[40];
   const uint32_t seg = blockIdx.x;
   const uint32_t c0 = seg_chunk_begin[seg], c1 = seg_chunk_begin[seg + 1];
@@ -99,6 +103,7 @@ __global__ void __launch_bounds__(256) k_seg_scan(const uint32_t* __restrict__ s
     tot += v;
   }
   const uint32_t dbase = block_exclusive_scan(tot, warp_sums, nullptr) + (uint32_t)seg_start[seg];
+  if (digit_base) digit_base[(size_t)seg * 256 + threadIdx.x] = dbase;
   for (uint32_t c = c0; c < c1; c++) chunk_sums[(size_t)c * 256 + threadIdx.x] += dbase;
 }
 
@@ -359,23 +364,242 @@ __global__ void __launch_bounds__(256) k_fix_runs(const SortTile* __restrict__ t
   }
 }
 
+// ---- local sort ---------------------------------------------------------------------------------------------------
+// One CTA sorts one work item -- a range of at most kLocalSortCap pairs that the caller knows to be final as a whole: a
+// whole segment, or consecutive whole (segment, MSD digit) sub-buckets of one segment after the MSD scatter -- completely
+// and stably on its key, in shared memory: one HBM read and one HBM write per pair.
+//
+// The keys and row indices stay where they were loaded; the passes move 16-bit slot numbers.  Stable LSD passes on the
+// item's top varying 8-bit digits, enough of them that the item spreads over more prefixes than twice its rows, then the
+// (short, rare) runs of rows that share that prefix are insertion-sorted on the whole key.  When a run is longer than
+// kLocalMaxRun (low-entropy high bits, heavy ties), the item is sorted again from its load order with LSD passes over all of
+// its varying digits: the result is the same stable order either way.
+constexpr int kLocalThreads = 1024;
+constexpr int kLocalWarps = kLocalThreads / 32;
+constexpr int kLocalItems = kLocalSortCap / kLocalThreads;  // 12 slots per thread
+constexpr int kLocalWarpRows = kLocalSortCap / kLocalWarps; // 384 consecutive slots per warp
+constexpr uint32_t kLocalMaxRun = 64;
+static_assert(kLocalSortCap % kLocalThreads == 0 && kLocalSortCap <= 65536, "slot numbers are 16-bit");
+
+struct LocalShared {
+  uint64_t keys[kLocalSortCap];        // in load order
+  uint32_t vals[kLocalSortCap];        // in load order
+  uint16_t slot[kLocalSortCap];        // sorted position -> load-order slot
+  uint16_t cnt[kLocalWarps][256];
+  uint32_t warp_sums[40];
+  unsigned long long or_bits, and_bits;
+  uint32_t long_run;
+};
+
+// One stable pass on digit (key >> shift) & 255 over sm.slot[0, count).  Ranking as in k_sort_scatter; warps whose slots
+// all lie past the end skip it (their counters stay zero), so small items cost little.
+__device__ __forceinline__ void local_pass(LocalShared& sm, uint32_t count, int shift) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1;
+  {
+    uint32_t* z = reinterpret_cast<uint32_t*>(&sm.cnt[0][0]);
+#pragma unroll
+    for (int i = 0; i < kLocalWarps * 256 / 2 / kLocalThreads; i++) z[threadIdx.x + i * kLocalThreads] = 0;
+  }
+  const uint32_t first = warp * kLocalWarpRows + lane;
+  uint32_t slot_bin[kLocalItems], rank[kLocalItems];  // slot << 8 | digit: one register per row
+#pragma unroll
+  for (int j = 0; j < kLocalItems; j++) {
+    const uint32_t pos = first + j * 32;
+    const uint32_t s = pos < count ? sm.slot[pos] : pos;
+    slot_bin[j] = s << 8 | (pos < count ? (uint32_t)(sm.keys[s] >> shift) & 255u : 255u);
+  }
+  __syncthreads();
+  uint16_t* cnt = sm.cnt[warp];
+#pragma unroll
+  for (int j = 0; j < kLocalItems; j++) {
+    rank[j] = 0;
+    if (warp * kLocalWarpRows + j * 32 < count) {  // warp-uniform
+      const uint32_t bin = slot_bin[j] & 255u;
+      const unsigned peers = match_any_full<8>(bin);
+      const uint32_t before = __popc(peers & lt);
+      const uint32_t pre = cnt[bin];
+      __syncwarp();
+      if (before == 0) cnt[bin] = (uint16_t)(pre + __popc(peers));
+      __syncwarp();
+      rank[j] = pre + before;
+    }
+  }
+  __syncthreads();
+  uint32_t total = 0;
+  if (threadIdx.x < 256) {
+#pragma unroll
+    for (int w = 0; w < kLocalWarps; w++) total += sm.cnt[w][threadIdx.x];
+  }
+  const uint32_t start = block_exclusive_scan(total, sm.warp_sums, nullptr);
+  if (threadIdx.x < 256) {
+    uint32_t run = start;
+#pragma unroll
+    for (int w = 0; w < kLocalWarps; w++) {
+      const uint16_t c = sm.cnt[w][threadIdx.x];
+      sm.cnt[w][threadIdx.x] = (uint16_t)run;
+      run += c;
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < kLocalItems; j++)
+    if (warp * kLocalWarpRows + j * 32 < count) sm.slot[cnt[slot_bin[j] & 255u] + rank[j]] = (uint16_t)(slot_bin[j] >> 8);
+  __syncthreads();
+}
+
+template <typename Src>
+__global__ void __launch_bounds__(kLocalThreads, 1) k_local_sort(const LocalSortItem* __restrict__ items, Src src,
+                                                                 uint64_t* __restrict__ out_keys,
+                                                                 uint32_t* __restrict__ out_vals) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  LocalShared& sm = *reinterpret_cast<LocalShared*>(smem_raw);
+  const LocalSortItem it = items[blockIdx.x];
+  const uint32_t count = it.count;
+  if (threadIdx.x == 0) {
+    sm.or_bits = 0;
+    sm.and_bits = ~0ull;
+    sm.long_run = 0;
+  }
+  // load: half of a thread's loads in flight at once (all of them would not fit in 64 registers); OR / AND of the item's
+  // keys on the way
+  uint64_t k_or = 0, k_and = ~0ull;
+  constexpr int kHalf = kLocalItems / 2;
+#pragma unroll 1
+  for (int h = 0; h < 2; h++) {
+    uint64_t k[kHalf];
+    uint32_t v[kHalf];
+#pragma unroll
+    for (int j = 0; j < kHalf; j++) {
+      const uint32_t i = (h * kHalf + j) * kLocalThreads + threadIdx.x;
+      if (i < count) src.load((uint64_t)it.start + i, k[j], v[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < kHalf; j++) {
+      const uint32_t i = (h * kHalf + j) * kLocalThreads + threadIdx.x;
+      if (i < count) {
+        sm.keys[i] = k[j];
+        sm.vals[i] = v[j];
+        sm.slot[i] = (uint16_t)i;
+        k_or |= k[j];
+        k_and &= k[j];
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    k_or |= __shfl_xor_sync(0xffffffffu, k_or, o);
+    k_and &= __shfl_xor_sync(0xffffffffu, k_and, o);
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) {
+    atomicOr(&sm.or_bits, k_or);
+    atomicAnd(&sm.and_bits, k_and);
+  }
+  __syncthreads();
+  const uint64_t varying = sm.or_bits ^ sm.and_bits;
+  if (varying != 0) {
+    const int top = 63 - __clzll((long long)varying);
+    int pbits = 1;  // prefix bits: at least twice as many prefixes as rows
+    while ((1u << pbits) < 2 * count) pbits++;
+    const int ndig = (min(pbits, top + 1) + 7) / 8;
+    const int low = max(0, top + 1 - 8 * ndig);  // lowest digit: bits [low, low + 8); may overlap the next one
+    for (int d = ndig - 1; d >= 0; d--) {
+      const int shift = max(0, top + 1 - 8 * (d + 1));
+      if ((varying >> shift) & 0xff) local_pass(sm, count, shift);
+    }
+    const uint64_t high_mask = ~0ull << low;
+    if (varying & ~high_mask) {
+      // rows that share the prefix are still in load order: stable insertion sort of every such run on the whole key.
+      // Other threads' runs are being reordered meanwhile, but every row of a run has the run's prefix, so the head test
+      // and the walk (which look one row past a run) read the same prefixes whatever the order inside it.
+      for (uint32_t i = threadIdx.x; i < count; i += kLocalThreads) {
+        const uint64_t kh = sm.keys[sm.slot[i]] & high_mask;
+        if (i > 0 && (sm.keys[sm.slot[i - 1]] & high_mask) == kh) continue;               // not the head of a run
+        if (i + 1 >= count || (sm.keys[sm.slot[i + 1]] & high_mask) != kh) continue;      // a run of one
+        uint32_t len = 2;
+        while (i + len < count && len <= kLocalMaxRun && (sm.keys[sm.slot[i + len]] & high_mask) == kh) len++;
+        if (len > kLocalMaxRun) {
+          sm.long_run = 1;
+          continue;
+        }
+        uint16_t* s = sm.slot + i;
+        for (uint32_t a = 1; a < len; a++) {
+          const uint16_t sa = s[a];
+          const uint64_t ka = sm.keys[sa];
+          uint32_t b = a;
+          while (b > 0 && sm.keys[s[b - 1]] > ka) {
+            s[b] = s[b - 1];
+            b--;
+          }
+          s[b] = sa;
+        }
+      }
+      __syncthreads();
+      if (sm.long_run) {
+        for (uint32_t i = threadIdx.x; i < count; i += kLocalThreads) sm.slot[i] = (uint16_t)i;
+        __syncthreads();
+        for (int shift = 0; shift < 64; shift += 8)
+          if ((varying >> shift) & 0xff) local_pass(sm, count, shift);
+      }
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < kLocalItems; j++) {
+    const uint32_t i = j * kLocalThreads + threadIdx.x;
+    if (i < count) {
+      const uint32_t s = sm.slot[i];
+      out_keys[(uint64_t)it.start + i] = sm.keys[s];
+      out_vals[(uint64_t)it.start + i] = sm.vals[s];
+    }
+  }
+}
+
+template <typename Src>
+void launch_local_sort(hs_ctx* ctx, const std::vector<LocalSortItem>& items, Src src, uint64_t* out_keys,
+                       uint32_t* out_vals) {
+  if (items.empty()) return;
+  Buf<LocalSortItem> d_items(ctx, items.size());
+  copy_h2d(ctx, d_items.get(), items.data(), items.size() * sizeof(LocalSortItem));
+  static DeviceOnce attr_once;  // one per Src instantiation
+  bool& attr = attr_once(ctx->device);
+  if (!attr) {
+    HS_CUDA(cudaFuncSetAttribute(k_local_sort<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LocalShared)));
+    attr = true;
+  }
+  KernelScope _ks(ctx, "k_local_sort");
+  k_local_sort<Src><<<(unsigned)items.size(), kLocalThreads, sizeof(LocalShared), ctx->stream>>>(d_items.get(), src,
+                                                                                                 out_keys, out_vals);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+// histogram of one pass and the (segment, digit) bases; digit_base (optional) receives the bases, see k_seg_scan
 template <typename Src, typename Digit>
-void run_pass(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, const uint32_t* seg_chunk_begin,
-              uint32_t* chunk_sums, Src src, uint64_t* out_keys, uint32_t* out_vals, Digit digit) {
+void run_hist(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, const uint32_t* seg_chunk_begin,
+              uint32_t* chunk_sums, Src src, Digit digit, uint32_t* digit_base) {
   {
     KernelScope _ks(ctx, "k_sort_hist");
     k_sort_hist<Src, Digit><<<(unsigned)plan->ntiles, kHistThreads, 0, ctx->stream>>>(plan->tiles.get(), src, digit,
                                                                                  plan->tile_hist.get());
     HS_LAUNCH_CHECK(ctx);
   }
-  KernelScope* _scan = new KernelScope(ctx, "k_seg_scan");
+  KernelScope _ks(ctx, "k_seg_scan");
   k_seg_chunk_sums<<<(unsigned)nchunks, 256, 0, ctx->stream>>>(chunks, plan->tile_hist.get(), chunk_sums);
   HS_LAUNCH_CHECK(ctx);
-  k_seg_scan<<<(unsigned)plan->nseg, 256, 0, ctx->stream>>>(seg_chunk_begin, plan->seg_start.get(), chunk_sums);
+  k_seg_scan<<<(unsigned)plan->nseg, 256, 0, ctx->stream>>>(seg_chunk_begin, plan->seg_start.get(), chunk_sums, digit_base);
   HS_LAUNCH_CHECK(ctx);
-  k_seg_apply<<<(unsigned)nchunks, 1024, 0, ctx->stream>>>(chunks, plan->tile_hist.get(), plan->tile_dst.get(), chunk_sums);
-  HS_LAUNCH_CHECK(ctx);
-  delete _scan;
+}
+
+// the scatter of a pass whose histogram run_hist queued
+template <typename Src, typename Digit>
+void run_scatter(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, uint32_t* chunk_sums, Src src,
+                 uint64_t* out_keys, uint32_t* out_vals, Digit digit) {
+  {
+    KernelScope _ks(ctx, "k_seg_scan");
+    k_seg_apply<<<(unsigned)nchunks, 1024, 0, ctx->stream>>>(chunks, plan->tile_hist.get(), plan->tile_dst.get(), chunk_sums);
+    HS_LAUNCH_CHECK(ctx);
+  }
   static DeviceOnce attr_once;  // one per (Src, Digit) instantiation
   bool& attr = attr_once(ctx->device);
   if (!attr) {
@@ -387,6 +611,13 @@ void run_pass(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchu
   k_sort_scatter<Src, Digit><<<(unsigned)plan->ntiles, kThreads, sizeof(ScatterShared), ctx->stream>>>(
       plan->tiles.get(), src, digit, plan->tile_dst.get(), out_keys, out_vals);
   HS_LAUNCH_CHECK(ctx);
+}
+
+template <typename Src, typename Digit>
+void run_pass(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, const uint32_t* seg_chunk_begin,
+              uint32_t* chunk_sums, Src src, uint64_t* out_keys, uint32_t* out_vals, Digit digit) {
+  run_hist(ctx, plan, chunks, nchunks, seg_chunk_begin, chunk_sums, src, digit, nullptr);
+  run_scatter(ctx, plan, chunks, nchunks, chunk_sums, src, out_keys, out_vals, digit);
 }
 
 struct ChunkPlan {
@@ -492,6 +723,67 @@ void segmented_sort_pairs(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t
     std::swap(vals, vals_alt);
   }
   if (first) fail(HS_EINVAL, "segmented_sort_pairs: raw first-pass source given but no pass ran");
+}
+
+namespace {
+// f(SrcRaw<T>{...}) for the column's type
+template <typename F>
+void with_raw_source(const RawKeyColumn& raw, F&& f) {
+  switch (raw.type) {
+    case HS_TYPE_INT32: f(SrcRaw<HS_TYPE_INT32>{raw.data}); break;
+    case HS_TYPE_INT64: f(SrcRaw<HS_TYPE_INT64>{raw.data}); break;
+    case HS_TYPE_FLOAT: f(SrcRaw<HS_TYPE_FLOAT>{raw.data}); break;
+    case HS_TYPE_DOUBLE: f(SrcRaw<HS_TYPE_DOUBLE>{raw.data}); break;
+    default: fail(HS_EUNSUPPORTED, "sort: key type %d", raw.type);
+  }
+}
+}  // namespace
+
+void segmented_sort_local(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, const RawKeyColumn& raw, uint64_t* keys,
+                          uint32_t* vals) {
+  std::vector<LocalSortItem> items;
+  for (int s = 0; s < nseg; s++) {
+    const uint64_t n = seg_offsets[s + 1] - seg_offsets[s];
+    if (n > (uint64_t)kLocalSortCap) fail(HS_EINVAL, "segmented_sort_local: segment of %llu rows", (unsigned long long)n);
+    if (n) items.push_back(LocalSortItem{(uint32_t)seg_offsets[s], (uint32_t)n});
+  }
+  with_raw_source(raw, [&](auto src) { launch_local_sort(ctx, items, src, keys, vals); });
+}
+
+bool segmented_sort_msd_local(hs_ctx* ctx, SortPlan* plan, const RawKeyColumn& raw, int shift, uint64_t* keys,
+                              uint64_t* keys_alt, uint32_t* vals, uint32_t* vals_alt) {
+  if (plan->ntiles == 0) return false;
+  ChunkPlan cp = build_chunks(ctx, plan->h_seg_tile_begin);
+  const size_t nsub = (size_t)plan->nseg * 256;
+  Buf<uint32_t> d_base(ctx, nsub);
+  const DigitShift digit{shift};
+  with_raw_source(raw, [&](auto src) {
+    run_hist(ctx, plan, cp.chunks.get(), cp.nchunks, cp.seg_chunk_begin.get(), cp.chunk_sums.get(), src, digit, d_base.get());
+  });
+  std::vector<uint32_t> base(nsub + 1);
+  copy_d2h(ctx, base.data(), d_base.get(), nsub * 4);
+  sync_stream(ctx);
+  base[nsub] = (uint32_t)plan->n;
+  // work items: consecutive whole sub-buckets of one segment, up to kLocalSortCap rows
+  std::vector<LocalSortItem> items;
+  for (int s = 0; s < plan->nseg; s++) {
+    LocalSortItem cur{base[(size_t)s * 256], 0};
+    for (size_t d = (size_t)s * 256; d < (size_t)(s + 1) * 256; d++) {
+      const uint32_t sz = base[d + 1] - base[d];
+      if (sz > (uint32_t)kLocalSortCap) return false;
+      if (cur.count + sz > (uint32_t)kLocalSortCap) {
+        items.push_back(cur);
+        cur = LocalSortItem{base[d], 0};
+      }
+      cur.count += sz;
+    }
+    if (cur.count) items.push_back(cur);
+  }
+  with_raw_source(raw, [&](auto src) {
+    run_scatter(ctx, plan, cp.chunks.get(), cp.nchunks, cp.chunk_sums.get(), src, keys_alt, vals_alt, digit);
+  });
+  launch_local_sort(ctx, items, SrcPairs{keys_alt, vals_alt}, keys, vals);
+  return true;
 }
 
 void launch_fix_runs(hs_ctx* ctx, SortPlan* plan, uint64_t* keys, uint32_t* vals, uint64_t high_mask, uint64_t low_mask,
