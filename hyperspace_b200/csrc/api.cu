@@ -630,8 +630,8 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
 
       EncodeRequest req;
       req.table = &rows.part;
-      req.d_perm = rows.sorted_perm;
-      req.d_sorted_keys = rows.sorted_keys;
+      req.d_perm = rows.sorted.perm();
+      req.d_sorted_keys = rows.sorted.keys();
       req.plan = &rows.plan;
       req.seg_offsets = rows.bucket_offsets;
       req.rows_per_page = spec->rows_per_page;
@@ -653,8 +653,8 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
       encode_segments(ctx, req, &enc, &st);  // synchronises the stream before it returns
       if (settle_sort(ctx, &rows, &st)) {    // (rare) the fix-up gave up on a long run of equal key prefixes: the rows were sorted
         req.probe = nullptr;                 // again with full passes, so the pages are gathered again
-        req.d_perm = rows.sorted_perm;
-        req.d_sorted_keys = rows.sorted_keys;
+        req.d_perm = rows.sorted.perm();
+        req.d_sorted_keys = rows.sorted.keys();
         enc = EncodedFiles();
         encode_segments(ctx, req, &enc, &st);
       }
@@ -1067,8 +1067,8 @@ static void prepare_join_side(hs_ctx* ctx, SourceSet* src, const hs_source_file*
     const int kw = rows->part.cols[0].width;
     const int ktype = rows->part.cols[0].type;
     Buf<uint8_t> sk(ctx, (size_t)std::max<int64_t>(1, rows->part.nrows) * kw);
-    launch_gather_plain(ctx, rows->part.cols[0].data.get(), rows->sorted_perm, rows->part.nrows, kw, sk.get());
-    rows->keys_alt.release();
+    launch_gather_plain(ctx, rows->part.cols[0].data.get(), rows->sorted.perm(), rows->part.nrows, kw, sk.get());
+    rows->sorted.keys_buf[rows->sorted.cur ^ 1].release();  // the sort's scratch keys
     t->cols.clear();
     t->cols = std::move(rows->part.cols);
     t->nrows = rows->part.nrows;
@@ -1080,7 +1080,7 @@ static void prepare_join_side(hs_ctx* ctx, SourceSet* src, const hs_source_file*
     kc.data = std::move(sk);
     t->cols.push_back(std::move(kc));
     *d_keys = str_key ? (const int64_t*)t->cols.back().data.get() : widened_key(ctx, t->cols.back(), t->nrows, k64);
-    *d_perm = rows->sorted_perm;
+    *d_perm = rows->sorted.perm();
   }
 }
 
@@ -1270,7 +1270,7 @@ int hs_k_sort_perm(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64
     memset(&st, 0, sizeof st);
     index_rows(ctx, t, nkeys, num_buckets, &rows, &st);
     Buf<uint8_t> orig(ctx, (size_t)std::max<int64_t>(1, nrows) * 4);
-    launch_gather_plain(ctx, rows.part.cols[nkeys].data.get(), rows.sorted_perm, nrows, 4, orig.get());
+    launch_gather_plain(ctx, rows.part.cols[nkeys].data.get(), rows.sorted.perm(), nrows, 4, orig.get());
     std::vector<uint32_t> h(nrows);
     if (nrows) copy_d2h(ctx, h.data(), orig.get(), 4 * nrows);
     sync_stream(ctx);

@@ -11,7 +11,6 @@
 
 #include <algorithm>
 #include <array>
-#include <cmath>
 #include <map>
 #include <random>
 
@@ -936,9 +935,8 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
 }
 
 void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle) {
-  const int64_t nrows = out->part.nrows;
   auto t_sort = std::make_unique<StageTimer>(ctx);
-  // ---- K4: segmented sort on the indexed columns, last column first ---------------------------------------------
+  // ---- K4: segmented sort on the indexed columns (radix_sort.cu) -----------------------------------------------
   if (defer_settle && !out->probe) {
     // rows that arrived through the fused exchange: the probes need the peers' rows (i.e. the closing barrier), and their
     // results must be on the host before the sort is queued if the encoder is to plan while the GPU sorts -- one
@@ -948,137 +946,14 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
   }
   t_sort->start();
   build_sort_plan(ctx, out->bucket_offsets.data(), num_buckets, &out->plan);
-  out->keys.alloc(ctx, std::max<int64_t>(1, nrows));
-  out->keys_alt.alloc(ctx, std::max<int64_t>(1, nrows));
-  out->perm.alloc(ctx, std::max<int64_t>(1, nrows));
-  out->perm_alt.alloc(ctx, std::max<int64_t>(1, nrows));
-  uint64_t* keys = out->keys.get();
-  uint64_t* keys_alt = out->keys_alt.get();
-  uint32_t* perm = out->perm.get();
-  uint32_t* perm_alt = out->perm_alt.get();
-  Buf<unsigned long long> d_or_and(ctx, 2);
-  bool sort_deferred = false;
-  for (int k = nkeys - 1; k >= 0; k--) {
-    DevColumn& kc = out->part.cols[k];
-    // The first column sorted (the last indexed column) starts from rows in partition order: its first radix pass reads
-    // the raw column and encodes on the fly, so neither the identity permutation nor the encoded keys are written out
-    // beforehand; only the OR / AND of the encoded keys is needed to pick the passes.
-    const bool from_raw = k == nkeys - 1 && kc.type >= HS_TYPE_INT32 && kc.type <= HS_TYPE_DOUBLE;
-    if (k == nkeys - 1 && !from_raw) launch_iota_u32(ctx, perm, nrows);
-    if (kc.type == HS_TYPE_STRING) {
-      // A string key is sorted piecewise: stable LSD passes on the length, then on its 8-byte pieces from the last to the
-      // first (each piece a big-endian integer; digits that are constant over all rows cost nothing).  Short keys -- the
-      // usual case -- take one piece.
-      auto sort_piece = [&](int piece, unsigned long long* bits_or) {
-        const unsigned long long init[2] = {0ull, ~0ull};
-        unsigned long long oa[2] = {0, 0};
-        copy_h2d(ctx, d_or_and.get(), init, sizeof init);
-        launch_string_piece_keys(ctx, (const uint64_t*)kc.data.get(), perm, nrows, piece, keys, d_or_and.get());
-        copy_d2h(ctx, oa, d_or_and.get(), sizeof oa);
-        sync_stream(ctx);
-        if (bits_or) *bits_or = oa[0];
-        const uint64_t varying = nrows ? (oa[0] ^ oa[1]) : 0;
-        if (varying) segmented_sort_pairs(ctx, &out->plan, keys, keys_alt, perm, perm_alt, varying);
-      };
-      unsigned long long len_or = 0;
-      sort_piece(-1, &len_or);  // the OR of the lengths bounds the longest key from above
-      for (int piece = (int)((len_or + 7) / 8) - 1; piece >= 0; piece--) sort_piece(piece, nullptr);
-      if (kc.has_nulls) segmented_sort_pass_by_table(ctx, &out->plan, keys, keys_alt, perm, perm_alt, kc.valid.get());
-      continue;
-    }
-    unsigned long long or_and[2] = {0, 0};
-    if (from_raw && out->have_key_bits) {  // the partition's histogram pass has them already
-      or_and[0] = out->key_or_and[0];
-      or_and[1] = out->key_or_and[1];
-    } else {
-      const unsigned long long init[2] = {0ull, ~0ull};
-      copy_h2d(ctx, d_or_and.get(), init, sizeof init);
-      launch_encode_keys(ctx, kc.data.get(), kc.type, from_raw ? nullptr : perm, nrows, from_raw ? nullptr : keys, d_or_and.get());
-      copy_d2h(ctx, or_and, d_or_and.get(), sizeof or_and);
-      sync_stream(ctx);
-    }
-    const uint64_t varying = nrows ? (or_and[0] ^ or_and[1]) : 0;
-    // Keys with more than four varying bytes: LSD passes over the top four varying bytes only, then fix up the (rare,
-    // short) runs of rows that agree on those bytes.  Falls back to full passes when a run is long (low-entropy high bytes).
-    // How many high bytes: enough that a bucket's rows spread over more prefixes than it has rows (expected rows per
-    // prefix <= 0.5 for uniformly spread keys), at least 2.  5 M-row buckets -> 3 bytes, 125 M-row buckets -> 4.
-    uint64_t max_bucket = 1;
-    for (int b = 0; b < num_buckets; b++) max_bucket = std::max<uint64_t>(max_bucket, out->bucket_offsets[b + 1] - out->bucket_offsets[b]);
-    int want_bytes = 2;
-    while (want_bytes < 8 && (double)max_bucket / std::pow(256.0, want_bytes) > 0.5) want_bytes++;
-    int nbytes = 0, fourth_from_top = 0;
-    for (int b = 7, seen = 0; b >= 0; b--)
-      if ((varying >> (8 * b)) & 0xff) {
-        nbytes++;
-        if (++seen == want_bytes) fourth_from_top = b;
-      }
-    static const bool full_sort_only = getenv("HS_FULL_SORT") != nullptr;
-    const RawKeyColumn raw{kc.data.get(), kc.type, kc.width};
-    const RawKeyColumn* first_src = from_raw ? &raw : nullptr;
-    if (from_raw && (varying == 0 || nrows == 0)) {  // nothing to sort on: materialise the pairs as they stand
-      launch_iota_u32(ctx, perm, nrows);
-      launch_encode_keys(ctx, kc.data.get(), kc.type, nullptr, nrows, keys, d_or_and.get());
-      first_src = nullptr;
-    }
-    // A null-free fixed-width first column is sorted completely in shared memory (k_local_sort): straight from the raw
-    // column when every bucket fits one CTA, else after one MSD pass on the 8 bits below the highest varying bit, as long as
-    // the (bucket, digit) sub-buckets fit -- two HBM passes instead of one per varying byte.  Buckets with more than ~0.85 x
-    // 256 x kLocalSortCap rows would rarely pass the sub-bucket check, so they skip the MSD histogram.
-    // HS_LSD_SORT=1: LSD passes (+ tie-run fix-up) only (A/B switch).
-    const bool lsd_only = getenv("HS_LSD_SORT") != nullptr;
-    if (first_src && !kc.has_nulls && !lsd_only && !full_sort_only) {
-      bool local_done = false;
-      if (max_bucket <= (uint64_t)kLocalSortCap) {
-        segmented_sort_local(ctx, out->bucket_offsets.data(), num_buckets, raw, out->keys.get(), out->perm.get());
-        local_done = true;
-      } else if (nbytes > 2 && max_bucket <= (uint64_t)(0.85 * 256 * kLocalSortCap)) {
-        const int shift = std::max(0, 63 - __builtin_clzll(varying) - 7);
-        local_done = segmented_sort_msd_local(ctx, &out->plan, raw, shift, out->keys.get(), out->keys_alt.get(),
-                                              out->perm.get(), out->perm_alt.get());
-      }
-      if (local_done) {
-        keys = out->keys.get();
-        perm = out->perm.get();
-        keys_alt = out->keys_alt.get();
-        perm_alt = out->perm_alt.get();
-        // a single key column is the last thing this function sorts: the caller need not wait for it
-        sort_deferred = defer_settle && nkeys == 1;
-        continue;  // (null-free: no validity pass)
-      }
-    }
-    if (nbytes > want_bytes && !full_sort_only) {
-      const uint64_t high_mask = ~0ull << (8 * fourth_from_top);
-      const uint64_t low_mask = ~high_mask;
-      segmented_sort_pairs(ctx, &out->plan, keys, keys_alt, perm, perm_alt, varying & high_mask, first_src);
-      out->d_fix_flag.alloc(ctx, 1);
-      fill_bytes(ctx, out->d_fix_flag.get(), 0, 4);
-      launch_fix_runs(ctx, &out->plan, keys, perm, high_mask, low_mask, 64, out->d_fix_flag.get());
-      out->fix_flag = 0;
-      out->fix_varying = varying;
-      out->fix_queued_at = ctx->sync_count;
-      out->fix_pending = true;
-      copy_d2h(ctx, &out->fix_flag, out->d_fix_flag.get(), 4);
-      // a single, null-free key column is the last thing this function sorts: the verdict can wait for the caller's next
-      // synchronisation (the encoder plans its pages on the host meanwhile); otherwise later passes build on this order
-      if (!(defer_settle && nkeys == 1 && !kc.has_nulls)) {
-        out->sorted_keys = keys;
-        out->sorted_perm = perm;
-        settle_sort(ctx, out, stats);
-        keys = out->sorted_keys;
-        perm = out->sorted_perm;
-        keys_alt = keys == out->keys.get() ? out->keys_alt.get() : out->keys.get();
-        perm_alt = perm == out->perm.get() ? out->perm_alt.get() : out->perm.get();
-      }
-    } else {
-      segmented_sort_pairs(ctx, &out->plan, keys, keys_alt, perm, perm_alt, varying, first_src);
-    }
-    if (kc.has_nulls)  // nulls first: one more stable pass on the validity byte (0 = null)
-      segmented_sort_pass_by_table(ctx, &out->plan, keys, keys_alt, perm, perm_alt, kc.valid.get());
+  std::vector<KeyColumn> keys(nkeys);
+  for (int k = 0; k < nkeys; k++) {
+    const DevColumn& c = out->part.cols[k];
+    keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width};
   }
-  out->sorted_keys = keys;
-  out->sorted_perm = perm;
+  sort_rows(ctx, &out->plan, keys.data(), nkeys, out->have_key_bits ? out->key_or_and : nullptr, defer_settle, &out->sorted);
   t_sort->stop();
-  if (out->fix_pending || sort_deferred) {  // no synchronisation here: the stage timers are read in settle_sort
+  if (out->sorted.queued) {  // no synchronisation here: the stage timers are read in settle_sort
     out->pending_timers.push_back(IndexedRows::DeferredTimer{std::move(t_sort), &hs_stats::ms_sort});
     return;
   }
@@ -1089,25 +964,13 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
 }
 
 bool settle_sort(hs_ctx* ctx, IndexedRows* out, hs_stats* stats) {
-  bool again = false;
-  if (out->fix_pending) {
-    if (ctx->sync_count <= out->fix_queued_at) sync_stream(ctx);  // the flag has not been delivered yet
-    out->fix_pending = false;
-    if (out->fix_flag) {
-      StageTimer t(ctx);
-      t.start();
-      uint64_t* keys = out->sorted_keys;
-      uint32_t* perm = out->sorted_perm;
-      uint64_t* keys_alt = keys == out->keys.get() ? out->keys_alt.get() : out->keys.get();
-      uint32_t* perm_alt = perm == out->perm.get() ? out->perm_alt.get() : out->perm.get();
-      segmented_sort_pairs(ctx, &out->plan, keys, keys_alt, perm, perm_alt, out->fix_varying);
-      out->sorted_keys = keys;
-      out->sorted_perm = perm;
-      t.stop();
-      sync_stream(ctx);
-      stats->ms_sort += t.ms();
-      again = true;
-    }
+  StageTimer t(ctx);
+  t.start();
+  const bool again = settle_sorted_rows(ctx, &out->plan, &out->sorted);
+  t.stop();
+  if (again) {
+    sync_stream(ctx);
+    stats->ms_sort += t.ms();
   }
   for (auto& d : out->pending_timers) stats->*(d.field) += d.t->ms();
   out->pending_timers.clear();

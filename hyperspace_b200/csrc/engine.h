@@ -79,13 +79,12 @@ struct IndexedRows {
   std::vector<uint64_t> bucket_offsets;  // host, nb+1
   Buf<uint64_t> d_bucket_offsets;     // device copy
   SortPlan plan;
-  Buf<uint64_t> keys, keys_alt;       // sorted encoded first-key column (keys) + scratch
-  Buf<uint32_t> perm, perm_alt;       // perm[p] = partitioned row at sorted position p
+  // sorted.perm()[p] = partitioned row at sorted position p.  radix_sort.cu (sort_rows) chooses how the rows are sorted
+  // and keeps what a sort left queued needs; settle_sort() settles it
+  SortedRows sorted;
   // OR / AND of the sort-encoded last indexed column, when the partition's histogram pass already computed them
   bool have_key_bits = false;
   unsigned long long key_or_and[2] = {0, ~0ull};
-  uint64_t* sorted_keys = nullptr;    // points into keys or keys_alt
-  uint32_t* sorted_perm = nullptr;
   // stage timers whose events are read at the call's next synchronisation (reading one synchronises)
   struct DeferredTimer {
     std::unique_ptr<StageTimer> t;
@@ -93,13 +92,6 @@ struct IndexedRows {
   };
   std::vector<DeferredTimer> pending_timers;
   std::unique_ptr<DictProbe> probe;   // see DictProbe
-  // deferred verdict of the tie fix-up (sort_partitioned_rows(..., defer_settle)): k_fix_runs raises the flag when a run of
-  // equal prefixes is too long for it; the flag travels with the call's next synchronisation and settle_sort() re-sorts
-  // with full passes if it is set (never for keys that spread over their high bytes)
-  Buf<uint32_t> d_fix_flag;
-  uint32_t fix_flag = 0;
-  uint64_t fix_queued_at = 0, fix_varying = 0;
-  bool fix_pending = false;
 };
 
 struct OutFile {
@@ -140,7 +132,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
                     const CarryOptions* carry = nullptr);
 
 // K2-K4 on a decoded table whose first nkeys columns are the indexed columns.
-// defer_settle: see IndexedRows::fix_pending -- the caller must call settle_sort() after its next synchronisation
+// defer_settle: the sort may be left queued (sort_rows' may_defer) -- the caller must call settle_sort() after its next
+// synchronisation
 void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false);
 
 // K5+K6: encode every segment (bucket or source file) as one Parquet file image inside one device arena.
@@ -178,7 +171,8 @@ bool p2p_exchange_supported(hs_ctx* ctx, int num_buckets);
 void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats);
 // K4 only: sorts out->part (already bucket-major, offsets in out->bucket_offsets) on the first nkeys columns.
 void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false);
-// true when the rows had to be sorted again (whatever was derived from sorted_keys / sorted_perm must be redone)
+// settle_sorted_rows() plus the stage timers: true when the rows had to be sorted again (whatever was derived from
+// sorted.keys() / sorted.perm() must be redone)
 bool settle_sort(hs_ctx* ctx, IndexedRows* out, hs_stats* stats);
 void launch_dictionary_probes(hs_ctx* ctx, const Table& part, bool use_dictionary, std::unique_ptr<DictProbe>* out);
 

@@ -211,6 +211,7 @@ struct SortTile {
   uint32_t count;
   uint64_t start;  // global position of the tile's first pair
 };
+struct SortChunk;  // radix_sort.cu
 struct SortPlan {
   int64_t n = 0;
   int64_t ntiles = 0;
@@ -221,42 +222,40 @@ struct SortPlan {
   Buf<uint32_t> tile_hist;      // device, ntiles x 256
   Buf<uint32_t> tile_dst;       // device, ntiles x 256: destination of every (tile, digit) for the current pass
   std::vector<uint32_t> h_seg_tile_begin;  // host mirror of seg_tile_begin
+  std::vector<uint64_t> h_seg_start;       // host mirror of seg_start
+  int64_t nchunks = 0;          // the per-segment scan of a pass works on chunks of up to 128 tiles of one segment:
+  Buf<SortChunk> chunks;        // device, nchunks
+  Buf<uint32_t> seg_chunk_begin;// device, nseg+1: first chunk of each segment
+  Buf<uint32_t> chunk_sums;     // device, nchunks x 256
 };
 // seg_offsets: host array of nseg+1 global offsets
 void build_sort_plan(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, SortPlan* plan);
-// Stable LSD radix sort of (key, val) pairs within each segment on the key bits set in `bit_mask` (bytes whose bits
-// are all constant are skipped).  Result is left in (keys, vals); (keys_alt, vals_alt) are scratch of the same size.
-// first_pass_source (optional): the pairs have not been materialised yet -- the first pass that runs reads the raw key
-// column (position p holds the value of row p) and uses p itself as the row index.  bit_mask must then select at least
-// one byte.
-struct RawKeyColumn {
-  const void* data;
-  int type, width;
+// The rows of a SortPlan in sorted order: at sorted position p, keys()[p] is the sort encoding of the first key column and
+// perm()[p] the row (the position in the plan's input order).
+struct SortedRows {
+  Buf<uint64_t> keys_buf[2];  // the pairs and scratch pairs of the same size: the sort passes move them back and forth
+  Buf<uint32_t> perm_buf[2];
+  int cur = 0;                // the pairs are in keys_buf[cur] / perm_buf[cur]
+  uint64_t* keys() const { return keys_buf[cur].get(); }
+  uint32_t* perm() const { return perm_buf[cur].get(); }
+  // queued, not yet settled (sort_rows with may_defer): the sort may still be running, and settle_sorted_rows() says
+  // whether the rows had to be sorted again
+  bool queued = false;
+  // the tie fix-up's verdict while it is outstanding (resort_bits != 0): gave_up arrives with the first synchronisation
+  // after ctx->sync_count was queued_at; if it is set, the rows are sorted again on resort_bits
+  uint64_t resort_bits = 0, queued_at = 0;
+  uint32_t gave_up = 0;
 };
-void segmented_sort_pairs(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t*& keys_alt, uint32_t*& vals,
-                          uint32_t*& vals_alt, uint64_t bit_mask, const RawKeyColumn* first_pass_source = nullptr);
-// After sorting on the bits of high_mask: stable insertion sort of every run of equal (key & high_mask) on (key & low_mask);
-// *d_flag is set when a run is longer than max_run (the caller then runs the remaining passes instead).
-void launch_fix_runs(hs_ctx* ctx, SortPlan* plan, uint64_t* keys, uint32_t* vals, uint64_t high_mask, uint64_t low_mask,
-                     uint32_t max_run, uint32_t* d_flag);
-// Local sort (k_local_sort): one CTA sorts up to kLocalSortCap pairs completely and stably in shared memory.
-constexpr int kLocalSortCap = 12288;
-struct LocalSortItem {
-  uint32_t start, count;  // a range of pairs that is sorted as a whole
-};
-// Every segment (at most kLocalSortCap rows each) sorted completely on the raw key column in one HBM pass; the result
-// (encoded keys, partition-order row positions) is written to (keys, vals).
-void segmented_sort_local(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, const RawKeyColumn& raw, uint64_t* keys,
-                          uint32_t* vals);
-// Complete sort of the raw key column within every segment in two HBM passes: one stable MSD pass on digit
-// (key >> shift) & 255 into (keys_alt, vals_alt), then k_local_sort of every (segment, digit) sub-bucket into (keys, vals).
-// The bits above shift + 7 must be constant over the input.  Returns false, having queued only the MSD histogram, when a
-// sub-bucket holds more than kLocalSortCap rows; the caller then sorts some other way.  Synchronises the stream once.
-bool segmented_sort_msd_local(hs_ctx* ctx, SortPlan* plan, const RawKeyColumn& raw, int shift, uint64_t* keys,
-                              uint64_t* keys_alt, uint32_t* vals, uint32_t* vals_alt);
-// One extra stable pass on an external 8-bit digit: digit = digits[vals[i]]  (null flags for nullable 64-bit keys)
-void segmented_sort_pass_by_table(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t*& keys_alt, uint32_t*& vals,
-                                  uint32_t*& vals_alt, const uint8_t* digits);
+// Sorts the rows within every segment of `plan` stably by cols[0], then cols[1], ... (nulls first); row r of a column
+// is the row at position r of the plan's input.  Chooses the sort path (radix_sort.cu).  last_or_and (optional): OR / AND
+// of the sort encoding of cols[ncols - 1], when the caller has them already.  may_defer: the sort of a single null-free
+// key column may be left queued (out->queued) -- the host does not wait for it, and settle_sorted_rows() must run before
+// out is read, best after the caller's next synchronisation.  Otherwise the result is final in stream order.
+void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, const unsigned long long* last_or_and,
+               bool may_defer, SortedRows* out);
+// Settles a queued sort (a no-op otherwise).  True when the rows had to be sorted again: whatever was derived from
+// keys() / perm() must be redone.
+bool settle_sorted_rows(hs_ctx* ctx, SortPlan* plan, SortedRows* s);
 
 // ---- gather + Parquet encode (gather_encode.cu) -----------------------------------------------------------------
 struct GatherColumn {

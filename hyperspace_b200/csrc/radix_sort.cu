@@ -11,10 +11,23 @@
 //
 // k_local_sort finishes ranges that fit one CTA in shared memory: whole small segments straight from the raw column, or
 // the (segment, digit) sub-buckets of one MSD pass -- two HBM passes for keys whose LSD sort would take three or more.
+//
+// sort_rows() is the module's one entry point and makes every choice between these paths, from shapes the host knows:
+// a null-free int32 / int64 / float / double first key column takes k_local_sort when it can (HS_LSD_SORT=1 turns that
+// off for A/B measurements); other keys take LSD passes over their top varying bytes plus k_fix_runs, or over every
+// varying byte.  When k_fix_runs gives up on a long run, the rows are sorted again with full passes -- at once, or in
+// settle_sorted_rows() when the caller let the verdict wait for its next synchronisation.
+#include <cmath>
+
 #include "device_utils.cuh"
 #include "kernels.h"
 
 namespace hs {
+
+struct SortChunk {  // up to kChunkTiles consecutive tiles of one segment: the unit of the per-segment scan
+  uint32_t seg;
+  uint32_t tile_begin, tile_end;
+};
 
 namespace {
 
@@ -24,11 +37,6 @@ constexpr int kItems = kSortTile / kThreads;   // 8
 constexpr int kWarpRows = kSortTile / kWarps;  // 256 consecutive pairs per warp
 constexpr int kChunkTiles = 128;
 constexpr int kHistThreads = 256;
-
-struct SortChunk {
-  uint32_t seg;
-  uint32_t tile_begin, tile_end;
-};
 
 struct DigitShift {
   int shift;
@@ -134,6 +142,52 @@ __global__ void __launch_bounds__(1024) k_seg_apply(const SortChunk* __restrict_
   }
 }
 
+// Stable ranking of a tile's items on their 8-bit digits, shared by k_sort_scatter and local_pass.  W warps, I items per
+// lane: item j of a lane is the tile's item warp * I * 32 + j * 32 + lane, with digit bin(j).  On return rank[j] is the
+// item's rank among its warp's earlier items with the same digit and cnt[w][d] the first tile position of (warp w,
+// digit d); the result is the first tile position of digit threadIdx.x (threads below 256).  cnt must be zero, and the
+// block synchronised since it was zeroed.  kGuard: only items below `count` are ranked, tested per warp row (warp-
+// uniform); otherwise every slot is, and slots past the end must carry the digit 255 (see k_sort_scatter).
+template <int W, int I, bool kGuard, typename Bin>
+__device__ __forceinline__ uint32_t rank_tile(uint16_t (&cnt)[W][256], uint32_t* warp_sums, Bin bin, uint32_t count,
+                                              uint32_t (&rank)[I]) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1;
+  uint16_t* wcnt = cnt[warp];
+#pragma unroll
+  for (int j = 0; j < I; j++) {
+    rank[j] = 0;
+    if (!kGuard || warp * (I * 32) + j * 32 < count) {
+      const uint32_t b = bin(j);
+      const unsigned peers = match_any_full<8>(b);
+      const uint32_t before = __popc(peers & lt);
+      const uint32_t pre = wcnt[b];   // every peer reads the same counter (broadcast)
+      __syncwarp();
+      if (before == 0) wcnt[b] = (uint16_t)(pre + __popc(peers));
+      __syncwarp();
+      rank[j] = pre + before;
+    }
+  }
+  __syncthreads();
+  // per digit: exclusive prefix over warps and digits -> first in-tile position of every (warp, digit)
+  uint32_t total = 0;
+  if (threadIdx.x < 256) {
+#pragma unroll
+    for (int w = 0; w < W; w++) total += cnt[w][threadIdx.x];
+  }
+  const uint32_t start = block_exclusive_scan(total, warp_sums, nullptr);
+  if (threadIdx.x < 256) {
+    uint32_t run = start;
+#pragma unroll
+    for (int w = 0; w < W; w++) {
+      const uint16_t c = cnt[w][threadIdx.x];
+      cnt[w][threadIdx.x] = (uint16_t)run;
+      run += c;
+    }
+  }
+  return start;
+}
+
 struct ScatterShared {
   uint64_t keys[kSortTile];
   uint32_t vals[kSortTile];
@@ -153,7 +207,6 @@ __global__ void __launch_bounds__(kThreads, 2) k_sort_scatter(const SortTile* __
   extern __shared__ __align__(16) uint8_t smem_raw[];
   ScatterShared& sm = *reinterpret_cast<ScatterShared*>(smem_raw);
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned lt = (1u << lane) - 1;
   {
     uint32_t* z = reinterpret_cast<uint32_t*>(&sm.cnt[0][0]);
 #pragma unroll
@@ -176,39 +229,12 @@ __global__ void __launch_bounds__(kThreads, 2) k_sort_scatter(const SortTile* __
     bin[j] = a ? digit(k[j], v[j]) : 255u;
   }
   __syncthreads();
-  // stable rank of every item among the warp's earlier items with the same digit
-  uint16_t* cnt = sm.cnt[warp];
   uint32_t rank[kItems];
-#pragma unroll
-  for (int j = 0; j < kItems; j++) {
-    const unsigned peers = match_any_full<8>(bin[j]);
-    const uint32_t before = __popc(peers & lt);
-    const uint32_t pre = cnt[bin[j]];   // every peer reads the same counter (broadcast)
-    __syncwarp();
-    if (before == 0) cnt[bin[j]] = (uint16_t)(pre + __popc(peers));
-    __syncwarp();
-    rank[j] = pre + before;
-  }
-  __syncthreads();
-  // per digit: exclusive prefix over warps and digits -> first in-tile position of every (warp, digit)
-  uint32_t total = 0;
-  if (threadIdx.x < 256) {
-#pragma unroll
-    for (int w = 0; w < kWarps; w++) total += sm.cnt[w][threadIdx.x];
-  }
-  const uint32_t start = block_exclusive_scan(total, sm.warp_sums, nullptr);
-  if (threadIdx.x < 256) {
-    uint32_t run = start;
-#pragma unroll
-    for (int w = 0; w < kWarps; w++) {
-      const uint16_t c = sm.cnt[w][threadIdx.x];
-      sm.cnt[w][threadIdx.x] = (uint16_t)run;
-      run += c;
-    }
-    sm.out_adj[threadIdx.x] = dst0 - start;
-  }
+  const uint32_t start = rank_tile<kWarps, kItems, false>(sm.cnt, sm.warp_sums, [&](int j) { return bin[j]; }, 0, rank);
+  if (threadIdx.x < 256) sm.out_adj[threadIdx.x] = dst0 - start;
   __syncthreads();
   // exchange: digit-sorted order inside the tile
+  const uint16_t* cnt = sm.cnt[warp];
 #pragma unroll
   for (int j = 0; j < kItems; j++) {
     const uint32_t pos = cnt[bin[j]] + rank[j];
@@ -240,6 +266,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_sort_scatter(const SortTile* __
 // run of two or more" -- a straight-line compare against both neighbours -- and the heads are compacted into a list in
 // shared memory; (2) the threads walk that list, one run each.  With 24 sorted bits and 5 M-row buckets about a quarter
 // of the rows head such a run; testing and sorting in the same loop left three quarters of every warp idle.
+constexpr uint32_t kFixMaxRun = 64;
 __global__ void __launch_bounds__(256) k_fix_runs(const SortTile* __restrict__ tiles, const uint64_t* __restrict__ seg_start,
                                                    uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
                                                    uint64_t high_mask, uint64_t low_mask, uint32_t max_run,
@@ -374,6 +401,10 @@ __global__ void __launch_bounds__(256) k_fix_runs(const SortTile* __restrict__ t
 // (short, rare) runs of rows that share that prefix are insertion-sorted on the whole key.  When a run is longer than
 // kLocalMaxRun (low-entropy high bits, heavy ties), the item is sorted again from its load order with LSD passes over all of
 // its varying digits: the result is the same stable order either way.
+constexpr int kLocalSortCap = 12288;
+struct LocalSortItem {
+  uint32_t start, count;  // a range of pairs that is sorted as a whole
+};
 constexpr int kLocalThreads = 1024;
 constexpr int kLocalWarps = kLocalThreads / 32;
 constexpr int kLocalItems = kLocalSortCap / kLocalThreads;  // 12 slots per thread
@@ -395,7 +426,6 @@ struct LocalShared {
 // all lie past the end skip it (their counters stay zero), so small items cost little.
 __device__ __forceinline__ void local_pass(LocalShared& sm, uint32_t count, int shift) {
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned lt = (1u << lane) - 1;
   {
     uint32_t* z = reinterpret_cast<uint32_t*>(&sm.cnt[0][0]);
 #pragma unroll
@@ -410,38 +440,9 @@ __device__ __forceinline__ void local_pass(LocalShared& sm, uint32_t count, int 
     slot_bin[j] = s << 8 | (pos < count ? (uint32_t)(sm.keys[s] >> shift) & 255u : 255u);
   }
   __syncthreads();
-  uint16_t* cnt = sm.cnt[warp];
-#pragma unroll
-  for (int j = 0; j < kLocalItems; j++) {
-    rank[j] = 0;
-    if (warp * kLocalWarpRows + j * 32 < count) {  // warp-uniform
-      const uint32_t bin = slot_bin[j] & 255u;
-      const unsigned peers = match_any_full<8>(bin);
-      const uint32_t before = __popc(peers & lt);
-      const uint32_t pre = cnt[bin];
-      __syncwarp();
-      if (before == 0) cnt[bin] = (uint16_t)(pre + __popc(peers));
-      __syncwarp();
-      rank[j] = pre + before;
-    }
-  }
+  rank_tile<kLocalWarps, kLocalItems, true>(sm.cnt, sm.warp_sums, [&](int j) { return slot_bin[j] & 255u; }, count, rank);
   __syncthreads();
-  uint32_t total = 0;
-  if (threadIdx.x < 256) {
-#pragma unroll
-    for (int w = 0; w < kLocalWarps; w++) total += sm.cnt[w][threadIdx.x];
-  }
-  const uint32_t start = block_exclusive_scan(total, sm.warp_sums, nullptr);
-  if (threadIdx.x < 256) {
-    uint32_t run = start;
-#pragma unroll
-    for (int w = 0; w < kLocalWarps; w++) {
-      const uint16_t c = sm.cnt[w][threadIdx.x];
-      sm.cnt[w][threadIdx.x] = (uint16_t)run;
-      run += c;
-    }
-  }
-  __syncthreads();
+  const uint16_t* cnt = sm.cnt[warp];
 #pragma unroll
   for (int j = 0; j < kLocalItems; j++)
     if (warp * kLocalWarpRows + j * 32 < count) sm.slot[cnt[slot_bin[j] & 255u] + rank[j]] = (uint16_t)(slot_bin[j] >> 8);
@@ -576,8 +577,7 @@ void launch_local_sort(hs_ctx* ctx, const std::vector<LocalSortItem>& items, Src
 
 // histogram of one pass and the (segment, digit) bases; digit_base (optional) receives the bases, see k_seg_scan
 template <typename Src, typename Digit>
-void run_hist(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, const uint32_t* seg_chunk_begin,
-              uint32_t* chunk_sums, Src src, Digit digit, uint32_t* digit_base) {
+void run_hist(hs_ctx* ctx, SortPlan* plan, Src src, Digit digit, uint32_t* digit_base) {
   {
     KernelScope _ks(ctx, "k_sort_hist");
     k_sort_hist<Src, Digit><<<(unsigned)plan->ntiles, kHistThreads, 0, ctx->stream>>>(plan->tiles.get(), src, digit,
@@ -585,19 +585,21 @@ void run_hist(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchu
     HS_LAUNCH_CHECK(ctx);
   }
   KernelScope _ks(ctx, "k_seg_scan");
-  k_seg_chunk_sums<<<(unsigned)nchunks, 256, 0, ctx->stream>>>(chunks, plan->tile_hist.get(), chunk_sums);
+  k_seg_chunk_sums<<<(unsigned)plan->nchunks, 256, 0, ctx->stream>>>(plan->chunks.get(), plan->tile_hist.get(),
+                                                                     plan->chunk_sums.get());
   HS_LAUNCH_CHECK(ctx);
-  k_seg_scan<<<(unsigned)plan->nseg, 256, 0, ctx->stream>>>(seg_chunk_begin, plan->seg_start.get(), chunk_sums, digit_base);
+  k_seg_scan<<<(unsigned)plan->nseg, 256, 0, ctx->stream>>>(plan->seg_chunk_begin.get(), plan->seg_start.get(),
+                                                            plan->chunk_sums.get(), digit_base);
   HS_LAUNCH_CHECK(ctx);
 }
 
 // the scatter of a pass whose histogram run_hist queued
 template <typename Src, typename Digit>
-void run_scatter(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, uint32_t* chunk_sums, Src src,
-                 uint64_t* out_keys, uint32_t* out_vals, Digit digit) {
+void run_scatter(hs_ctx* ctx, SortPlan* plan, Src src, Digit digit, uint64_t* out_keys, uint32_t* out_vals) {
   {
     KernelScope _ks(ctx, "k_seg_scan");
-    k_seg_apply<<<(unsigned)nchunks, 1024, 0, ctx->stream>>>(chunks, plan->tile_hist.get(), plan->tile_dst.get(), chunk_sums);
+    k_seg_apply<<<(unsigned)plan->nchunks, 1024, 0, ctx->stream>>>(plan->chunks.get(), plan->tile_hist.get(),
+                                                                   plan->tile_dst.get(), plan->chunk_sums.get());
     HS_LAUNCH_CHECK(ctx);
   }
   static DeviceOnce attr_once;  // one per (Src, Digit) instantiation
@@ -613,40 +615,88 @@ void run_scatter(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t n
   HS_LAUNCH_CHECK(ctx);
 }
 
+// one whole pass into the scratch pairs, which then hold the sorted pairs
 template <typename Src, typename Digit>
-void run_pass(hs_ctx* ctx, SortPlan* plan, const SortChunk* chunks, int64_t nchunks, const uint32_t* seg_chunk_begin,
-              uint32_t* chunk_sums, Src src, uint64_t* out_keys, uint32_t* out_vals, Digit digit) {
-  run_hist(ctx, plan, chunks, nchunks, seg_chunk_begin, chunk_sums, src, digit, nullptr);
-  run_scatter(ctx, plan, chunks, nchunks, chunk_sums, src, out_keys, out_vals, digit);
+void run_pass(hs_ctx* ctx, SortPlan* plan, Src src, Digit digit, SortedRows* s) {
+  run_hist(ctx, plan, src, digit, nullptr);
+  run_scatter(ctx, plan, src, digit, s->keys_buf[s->cur ^ 1].get(), s->perm_buf[s->cur ^ 1].get());
+  s->cur ^= 1;
 }
 
-struct ChunkPlan {
-  Buf<SortChunk> chunks;
-  Buf<uint32_t> seg_chunk_begin;
-  Buf<uint32_t> chunk_sums;
-  int64_t nchunks = 0;
-};
-
-// chunk lists are derived from the plan's host-side segment -> tile mapping
-ChunkPlan build_chunks(hs_ctx* ctx, const std::vector<uint32_t>& seg_tile_begin) {
-  ChunkPlan cp;
-  const int nseg = (int)seg_tile_begin.size() - 1;
-  std::vector<SortChunk> chunks;
-  std::vector<uint32_t> scb(nseg + 1);
-  for (int s = 0; s < nseg; s++) {
-    scb[s] = (uint32_t)chunks.size();
-    for (uint32_t t = seg_tile_begin[s]; t < seg_tile_begin[s + 1]; t += kChunkTiles)
-      chunks.push_back(SortChunk{(uint32_t)s, t, std::min<uint32_t>(t + kChunkTiles, seg_tile_begin[s + 1])});
+// f(SrcRaw<T>{...}) for the column's type
+template <typename F>
+void with_raw_source(const KeyColumn& raw, F&& f) {
+  switch (raw.type) {
+    case HS_TYPE_INT32: f(SrcRaw<HS_TYPE_INT32>{raw.data}); break;
+    case HS_TYPE_INT64: f(SrcRaw<HS_TYPE_INT64>{raw.data}); break;
+    case HS_TYPE_FLOAT: f(SrcRaw<HS_TYPE_FLOAT>{raw.data}); break;
+    case HS_TYPE_DOUBLE: f(SrcRaw<HS_TYPE_DOUBLE>{raw.data}); break;
+    default: fail(HS_EUNSUPPORTED, "sort: key type %d", raw.type);
   }
-  scb[nseg] = (uint32_t)chunks.size();
-  cp.nchunks = (int64_t)chunks.size();
-  cp.chunks.alloc(ctx, std::max<size_t>(1, chunks.size()));
-  cp.seg_chunk_begin.alloc(ctx, scb.size());
-  cp.chunk_sums.alloc(ctx, std::max<size_t>(1, chunks.size()) * 256);
-  if (!chunks.empty())
-    copy_h2d(ctx, cp.chunks.get(), chunks.data(), chunks.size() * sizeof(SortChunk));
-  copy_h2d(ctx, cp.seg_chunk_begin.get(), scb.data(), scb.size() * 4);  // (snapshots: the vectors may go out of scope)
-  return cp;
+}
+
+// Stable LSD passes on the key bytes that `bits` selects (a byte constant over the input costs nothing).  raw (optional):
+// the pairs have not been materialised yet -- the first pass reads the raw key column (position p holds the value of row
+// p) and uses p itself as the row index.  bits must then select at least one byte.
+void lsd_passes(hs_ctx* ctx, SortPlan* plan, SortedRows* s, uint64_t bits, const KeyColumn* raw) {
+  if (plan->ntiles == 0) return;
+  bool first = raw != nullptr;
+  for (int pass = 0; pass < 8; pass++) {
+    if (((bits >> (pass * 8)) & 0xff) == 0) continue;  // digit constant over the whole input
+    const DigitShift digit{pass * 8};
+    if (first)
+      with_raw_source(*raw, [&](auto src) { run_pass(ctx, plan, src, digit, s); });
+    else
+      run_pass(ctx, plan, SrcPairs{s->keys(), s->perm()}, digit, s);
+    first = false;
+  }
+  if (first) fail(HS_EINVAL, "sort: raw first-pass source given but no pass ran");
+}
+
+// Every segment (at most kLocalSortCap rows each) sorted completely on the raw key column in one HBM pass.
+void local_sort_segments(hs_ctx* ctx, const SortPlan& plan, const KeyColumn& raw, SortedRows* s) {
+  std::vector<LocalSortItem> items;
+  for (int g = 0; g < plan.nseg; g++) {
+    const uint64_t n = plan.h_seg_start[g + 1] - plan.h_seg_start[g];
+    if (n) items.push_back(LocalSortItem{(uint32_t)plan.h_seg_start[g], (uint32_t)n});
+  }
+  with_raw_source(raw, [&](auto src) { launch_local_sort(ctx, items, src, s->keys(), s->perm()); });
+}
+
+// Complete sort of the raw key column within every segment in two HBM passes: one stable MSD pass on digit
+// (key >> shift) & 255 into the scratch pairs, then k_local_sort of every (segment, digit) sub-bucket back into the sorted
+// pairs.  The bits above shift + 7 must be constant over the input.  Returns false, having queued only the MSD histogram,
+// when a sub-bucket holds more than kLocalSortCap rows.  Synchronises the stream once.
+bool msd_local_sort(hs_ctx* ctx, SortPlan* plan, const KeyColumn& raw, int shift, SortedRows* s) {
+  if (plan->ntiles == 0) return false;
+  const size_t nsub = (size_t)plan->nseg * 256;
+  Buf<uint32_t> d_base(ctx, nsub);
+  const DigitShift digit{shift};
+  with_raw_source(raw, [&](auto src) { run_hist(ctx, plan, src, digit, d_base.get()); });
+  std::vector<uint32_t> base(nsub + 1);
+  copy_d2h(ctx, base.data(), d_base.get(), nsub * 4);
+  sync_stream(ctx);
+  base[nsub] = (uint32_t)plan->n;
+  // work items: consecutive whole sub-buckets of one segment, up to kLocalSortCap rows
+  std::vector<LocalSortItem> items;
+  for (int g = 0; g < plan->nseg; g++) {
+    LocalSortItem cur{base[(size_t)g * 256], 0};
+    for (size_t d = (size_t)g * 256; d < (size_t)(g + 1) * 256; d++) {
+      const uint32_t sz = base[d + 1] - base[d];
+      if (sz > (uint32_t)kLocalSortCap) return false;
+      if (cur.count + sz > (uint32_t)kLocalSortCap) {
+        items.push_back(cur);
+        cur = LocalSortItem{base[d], 0};
+      }
+      cur.count += sz;
+    }
+    if (cur.count) items.push_back(cur);
+  }
+  uint64_t* keys_alt = s->keys_buf[s->cur ^ 1].get();
+  uint32_t* perm_alt = s->perm_buf[s->cur ^ 1].get();
+  with_raw_source(raw, [&](auto src) { run_scatter(ctx, plan, src, digit, keys_alt, perm_alt); });
+  launch_local_sort(ctx, items, SrcPairs{keys_alt, perm_alt}, s->keys(), s->perm());
+  return true;
 }
 
 }  // namespace
@@ -665,144 +715,169 @@ __global__ void k_build_tiles(const uint64_t* __restrict__ seg_start, const uint
 }
 
 void build_sort_plan(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, SortPlan* plan) {
-  std::vector<uint32_t> stb(nseg + 1);
+  std::vector<uint32_t> stb(nseg + 1), scb(nseg + 1);
   std::vector<uint64_t> sstart(nseg + 1);
+  std::vector<SortChunk> chunks;
   uint64_t ntiles = 0;
   for (int s = 0; s < nseg; s++) {
     stb[s] = (uint32_t)ntiles;
     sstart[s] = seg_offsets[s];
     ntiles += ceil_div(seg_offsets[s + 1] - seg_offsets[s], (uint64_t)kSortTile);
+    scb[s] = (uint32_t)chunks.size();
+    for (uint32_t t = stb[s]; t < ntiles; t += kChunkTiles)
+      chunks.push_back(SortChunk{(uint32_t)s, t, (uint32_t)std::min<uint64_t>(t + kChunkTiles, ntiles)});
   }
   stb[nseg] = (uint32_t)ntiles;
   sstart[nseg] = seg_offsets[nseg];
+  scb[nseg] = (uint32_t)chunks.size();
   if (seg_offsets[nseg] >= (1ull << 32)) fail(HS_EUNSUPPORTED, "more than 2^32-1 rows per GPU per call");
   plan->n = (int64_t)seg_offsets[nseg];
   plan->ntiles = (int64_t)ntiles;
   plan->nseg = nseg;
+  plan->nchunks = (int64_t)chunks.size();
   plan->tiles.alloc(ctx, std::max<size_t>(1, ntiles));
   plan->seg_tile_begin.alloc(ctx, stb.size());
   plan->seg_start.alloc(ctx, sstart.size());
   plan->tile_hist.alloc(ctx, std::max<size_t>(1, ntiles) * 256);
   plan->tile_dst.alloc(ctx, std::max<size_t>(1, ntiles) * 256);
+  plan->chunks.alloc(ctx, std::max<size_t>(1, chunks.size()));
+  plan->seg_chunk_begin.alloc(ctx, scb.size());
+  plan->chunk_sums.alloc(ctx, std::max<size_t>(1, chunks.size()) * 256);
   copy_h2d(ctx, plan->seg_tile_begin.get(), stb.data(), stb.size() * 4);
   copy_h2d(ctx, plan->seg_start.get(), sstart.data(), sstart.size() * 8);
+  if (!chunks.empty()) copy_h2d(ctx, plan->chunks.get(), chunks.data(), chunks.size() * sizeof(SortChunk));
+  copy_h2d(ctx, plan->seg_chunk_begin.get(), scb.data(), scb.size() * 4);
   if (nseg > 0 && ntiles > 0) {
     k_build_tiles<<<nseg, 256, 0, ctx->stream>>>(plan->seg_start.get(), plan->seg_tile_begin.get(), plan->tiles.get());
     HS_LAUNCH_CHECK(ctx);
   }
-  plan->h_seg_tile_begin = stb;  // (copy_h2d took snapshots of the host vectors)
+  plan->h_seg_tile_begin = std::move(stb);  // (copy_h2d took snapshots of the host vectors)
+  plan->h_seg_start = std::move(sstart);
 }
 
-void segmented_sort_pairs(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t*& keys_alt, uint32_t*& vals,
-                          uint32_t*& vals_alt, uint64_t bit_mask, const RawKeyColumn* first_pass_source) {
-  if (plan->ntiles == 0) return;
-  ChunkPlan cp = build_chunks(ctx, plan->h_seg_tile_begin);
-  bool first = first_pass_source != nullptr;
-  for (int pass = 0; pass < 8; pass++) {
-    if (((bit_mask >> (pass * 8)) & 0xff) == 0) continue;  // digit constant over the whole input
-    if (first) {
-      const void* raw = first_pass_source->data;
-      const DigitShift digit{pass * 8};
-#define HS_RAW_PASS(T)                                                                                                   \
-  run_pass(ctx, plan, cp.chunks.get(), cp.nchunks, cp.seg_chunk_begin.get(), cp.chunk_sums.get(), SrcRaw<T>{raw}, keys_alt, \
-           vals_alt, digit)
-      switch (first_pass_source->type) {
-        case HS_TYPE_INT32: HS_RAW_PASS(HS_TYPE_INT32); break;
-        case HS_TYPE_INT64: HS_RAW_PASS(HS_TYPE_INT64); break;
-        case HS_TYPE_FLOAT: HS_RAW_PASS(HS_TYPE_FLOAT); break;
-        case HS_TYPE_DOUBLE: HS_RAW_PASS(HS_TYPE_DOUBLE); break;
-        default: fail(HS_EUNSUPPORTED, "sort: key type %d", first_pass_source->type);
-      }
-#undef HS_RAW_PASS
-      first = false;
+void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, const unsigned long long* last_or_and,
+               bool may_defer, SortedRows* out) {
+  const int64_t nrows = plan->n;
+  for (auto& b : out->keys_buf) b.alloc(ctx, std::max<int64_t>(1, nrows));
+  for (auto& b : out->perm_buf) b.alloc(ctx, std::max<int64_t>(1, nrows));
+  out->cur = 0;
+  out->queued = false;
+  out->resort_bits = 0;
+  Buf<unsigned long long> d_or_and(ctx, 2);
+  unsigned long long or_and[2] = {0, 0};
+  // or_and = OR / AND of the encoded keys that launch(d_or_and) reduces, on the host (synchronises)
+  auto reduce = [&](auto launch) {
+    const unsigned long long init[2] = {0ull, ~0ull};
+    copy_h2d(ctx, d_or_and.get(), init, sizeof init);
+    launch(d_or_and.get());
+    copy_d2h(ctx, or_and, d_or_and.get(), sizeof or_and);
+    sync_stream(ctx);
+  };
+  uint64_t max_seg = 1;
+  for (int g = 0; g < plan->nseg; g++) max_seg = std::max<uint64_t>(max_seg, plan->h_seg_start[g + 1] - plan->h_seg_start[g]);
+  // How many high bytes the tie fix-up sorts on: enough that a segment's rows spread over more prefixes than it has rows
+  // (expected rows per prefix <= 0.5 for uniformly spread keys), at least 2.  5 M-row segments -> 3 bytes, 125 M-row -> 4.
+  int want_bytes = 2;
+  while (want_bytes < 8 && (double)max_seg / std::pow(256.0, want_bytes) > 0.5) want_bytes++;
+  const bool lsd_only = getenv("HS_LSD_SORT") != nullptr;
+  for (int k = ncols - 1; k >= 0; k--) {
+    const KeyColumn& kc = cols[k];
+    // The first column sorted (the last key column) starts from rows in input order: its first radix pass reads the raw
+    // column and encodes on the fly, so neither the identity permutation nor the encoded keys are written out beforehand;
+    // only the OR / AND of the encoded keys is needed to pick the passes.
+    const bool from_raw = k == ncols - 1 && kc.type >= HS_TYPE_INT32 && kc.type <= HS_TYPE_DOUBLE;
+    if (k == ncols - 1 && !from_raw) launch_iota_u32(ctx, out->perm(), nrows);
+    if (kc.type == HS_TYPE_STRING) {
+      // A string key is sorted piecewise: stable LSD passes on the length, then on its 8-byte pieces from the last to the
+      // first (each piece a big-endian integer; digits that are constant over all rows cost nothing).  Short keys -- the
+      // usual case -- take one piece.
+      auto sort_piece = [&](int piece) {
+        reduce([&](unsigned long long* d) {
+          launch_string_piece_keys(ctx, (const uint64_t*)kc.data, out->perm(), nrows, piece, out->keys(), d);
+        });
+        lsd_passes(ctx, plan, out, or_and[0] ^ or_and[1], nullptr);
+      };
+      sort_piece(-1);
+      const unsigned long long len_or = or_and[0];  // the OR of the lengths bounds the longest key from above
+      for (int piece = (int)((len_or + 7) / 8) - 1; piece >= 0; piece--) sort_piece(piece);
     } else {
-      run_pass(ctx, plan, cp.chunks.get(), cp.nchunks, cp.seg_chunk_begin.get(), cp.chunk_sums.get(), SrcPairs{keys, vals},
-               keys_alt, vals_alt, DigitShift{pass * 8});
-    }
-    std::swap(keys, keys_alt);
-    std::swap(vals, vals_alt);
-  }
-  if (first) fail(HS_EINVAL, "segmented_sort_pairs: raw first-pass source given but no pass ran");
-}
-
-namespace {
-// f(SrcRaw<T>{...}) for the column's type
-template <typename F>
-void with_raw_source(const RawKeyColumn& raw, F&& f) {
-  switch (raw.type) {
-    case HS_TYPE_INT32: f(SrcRaw<HS_TYPE_INT32>{raw.data}); break;
-    case HS_TYPE_INT64: f(SrcRaw<HS_TYPE_INT64>{raw.data}); break;
-    case HS_TYPE_FLOAT: f(SrcRaw<HS_TYPE_FLOAT>{raw.data}); break;
-    case HS_TYPE_DOUBLE: f(SrcRaw<HS_TYPE_DOUBLE>{raw.data}); break;
-    default: fail(HS_EUNSUPPORTED, "sort: key type %d", raw.type);
-  }
-}
-}  // namespace
-
-void segmented_sort_local(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, const RawKeyColumn& raw, uint64_t* keys,
-                          uint32_t* vals) {
-  std::vector<LocalSortItem> items;
-  for (int s = 0; s < nseg; s++) {
-    const uint64_t n = seg_offsets[s + 1] - seg_offsets[s];
-    if (n > (uint64_t)kLocalSortCap) fail(HS_EINVAL, "segmented_sort_local: segment of %llu rows", (unsigned long long)n);
-    if (n) items.push_back(LocalSortItem{(uint32_t)seg_offsets[s], (uint32_t)n});
-  }
-  with_raw_source(raw, [&](auto src) { launch_local_sort(ctx, items, src, keys, vals); });
-}
-
-bool segmented_sort_msd_local(hs_ctx* ctx, SortPlan* plan, const RawKeyColumn& raw, int shift, uint64_t* keys,
-                              uint64_t* keys_alt, uint32_t* vals, uint32_t* vals_alt) {
-  if (plan->ntiles == 0) return false;
-  ChunkPlan cp = build_chunks(ctx, plan->h_seg_tile_begin);
-  const size_t nsub = (size_t)plan->nseg * 256;
-  Buf<uint32_t> d_base(ctx, nsub);
-  const DigitShift digit{shift};
-  with_raw_source(raw, [&](auto src) {
-    run_hist(ctx, plan, cp.chunks.get(), cp.nchunks, cp.seg_chunk_begin.get(), cp.chunk_sums.get(), src, digit, d_base.get());
-  });
-  std::vector<uint32_t> base(nsub + 1);
-  copy_d2h(ctx, base.data(), d_base.get(), nsub * 4);
-  sync_stream(ctx);
-  base[nsub] = (uint32_t)plan->n;
-  // work items: consecutive whole sub-buckets of one segment, up to kLocalSortCap rows
-  std::vector<LocalSortItem> items;
-  for (int s = 0; s < plan->nseg; s++) {
-    LocalSortItem cur{base[(size_t)s * 256], 0};
-    for (size_t d = (size_t)s * 256; d < (size_t)(s + 1) * 256; d++) {
-      const uint32_t sz = base[d + 1] - base[d];
-      if (sz > (uint32_t)kLocalSortCap) return false;
-      if (cur.count + sz > (uint32_t)kLocalSortCap) {
-        items.push_back(cur);
-        cur = LocalSortItem{base[d], 0};
+      if (from_raw && last_or_and) {
+        or_and[0] = last_or_and[0];
+        or_and[1] = last_or_and[1];
+      } else {
+        reduce([&](unsigned long long* d) {
+          launch_encode_keys(ctx, kc.data, kc.type, from_raw ? nullptr : out->perm(), nrows, from_raw ? nullptr : out->keys(), d);
+        });
       }
-      cur.count += sz;
+      const uint64_t varying = nrows ? (or_and[0] ^ or_and[1]) : 0;
+      int nbytes = 0, lowest_high_byte = 0;  // varying bytes; the lowest of the top want_bytes of them
+      for (int b = 7, seen = 0; b >= 0; b--)
+        if ((varying >> (8 * b)) & 0xff) {
+          nbytes++;
+          if (++seen == want_bytes) lowest_high_byte = b;
+        }
+      const KeyColumn* raw = from_raw ? &kc : nullptr;
+      if (from_raw && varying == 0) {  // nothing to sort on: materialise the pairs as they stand
+        launch_iota_u32(ctx, out->perm(), nrows);
+        launch_encode_keys(ctx, kc.data, kc.type, nullptr, nrows, out->keys(), d_or_and.get());
+        raw = nullptr;
+      }
+      // nothing is sorted after a single null-free key column, so the caller need not wait for its sort
+      const bool defer = may_defer && ncols == 1 && !kc.valid;
+      // A null-free fixed-width first column is sorted completely in shared memory (k_local_sort): straight from the raw
+      // column when every segment fits one CTA, else after one MSD pass on the 8 bits below the highest varying bit, as long
+      // as the (segment, digit) sub-buckets fit -- two HBM passes instead of one per varying byte.  Segments with more than
+      // ~0.85 x 256 x kLocalSortCap rows would rarely pass the sub-bucket check, so they skip the MSD histogram.
+      bool local = false;
+      if (raw && !kc.valid && !lsd_only) {
+        if (max_seg <= (uint64_t)kLocalSortCap) {
+          local_sort_segments(ctx, *plan, kc, out);
+          local = true;
+        } else if (nbytes > 2 && max_seg <= (uint64_t)(0.85 * 256 * kLocalSortCap)) {
+          local = msd_local_sort(ctx, plan, kc, std::max(0, 63 - __builtin_clzll(varying) - 7), out);
+        }
+      }
+      if (local) {
+        out->queued = defer;
+      } else if (nbytes > want_bytes) {
+        // LSD passes over the top want_bytes varying bytes only, then k_fix_runs sorts the (rare, short) runs of rows that
+        // agree on those bytes.  Its verdict travels with the next synchronisation: the caller's when it may wait (the
+        // encoder plans its pages on the host meanwhile), else at once, since later passes build on this order.
+        const uint64_t high_mask = ~0ull << (8 * lowest_high_byte);
+        lsd_passes(ctx, plan, out, varying & high_mask, raw);
+        Buf<uint32_t> d_gave_up(ctx, 1);
+        fill_bytes(ctx, d_gave_up.get(), 0, 4);
+        {
+          KernelScope _ks(ctx, "k_fix_runs");
+          k_fix_runs<<<(unsigned)plan->ntiles, 256, 0, ctx->stream>>>(plan->tiles.get(), plan->seg_start.get(), out->keys(),
+                                                                      out->perm(), high_mask, ~high_mask, kFixMaxRun,
+                                                                      d_gave_up.get());
+          HS_LAUNCH_CHECK(ctx);
+        }
+        out->gave_up = 0;
+        out->resort_bits = varying;
+        out->queued_at = ctx->sync_count;
+        out->queued = true;
+        copy_d2h(ctx, &out->gave_up, d_gave_up.get(), 4);
+        if (!defer) settle_sorted_rows(ctx, plan, out);
+      } else {
+        lsd_passes(ctx, plan, out, varying, raw);
+      }
     }
-    if (cur.count) items.push_back(cur);
+    if (kc.valid && plan->ntiles)  // nulls first: one more stable pass on the validity byte (0 = null)
+      run_pass(ctx, plan, SrcPairs{out->keys(), out->perm()}, DigitTable{kc.valid}, out);
   }
-  with_raw_source(raw, [&](auto src) {
-    run_scatter(ctx, plan, cp.chunks.get(), cp.nchunks, cp.chunk_sums.get(), src, keys_alt, vals_alt, digit);
-  });
-  launch_local_sort(ctx, items, SrcPairs{keys_alt, vals_alt}, keys, vals);
+}
+
+bool settle_sorted_rows(hs_ctx* ctx, SortPlan* plan, SortedRows* s) {
+  const uint64_t bits = s->resort_bits;
+  s->queued = false;
+  s->resort_bits = 0;
+  if (bits == 0) return false;                            // no fix-up verdict outstanding
+  if (ctx->sync_count <= s->queued_at) sync_stream(ctx);  // the verdict has not been delivered yet
+  if (!s->gave_up) return false;
+  lsd_passes(ctx, plan, s, bits, nullptr);  // a run was too long for k_fix_runs: full passes
   return true;
-}
-
-void launch_fix_runs(hs_ctx* ctx, SortPlan* plan, uint64_t* keys, uint32_t* vals, uint64_t high_mask, uint64_t low_mask,
-                     uint32_t max_run, uint32_t* d_flag) {
-  KernelScope _ks(ctx, "k_fix_runs");
-  if (plan->ntiles == 0) return;
-  k_fix_runs<<<(unsigned)plan->ntiles, 256, 0, ctx->stream>>>(plan->tiles.get(), plan->seg_start.get(), keys, vals, high_mask,
-                                                              low_mask, max_run, d_flag);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void segmented_sort_pass_by_table(hs_ctx* ctx, SortPlan* plan, uint64_t*& keys, uint64_t*& keys_alt, uint32_t*& vals,
-                                  uint32_t*& vals_alt, const uint8_t* digits) {
-  if (plan->ntiles == 0) return;
-  ChunkPlan cp = build_chunks(ctx, plan->h_seg_tile_begin);
-  run_pass(ctx, plan, cp.chunks.get(), cp.nchunks, cp.seg_chunk_begin.get(), cp.chunk_sums.get(), SrcPairs{keys, vals},
-           keys_alt, vals_alt, DigitTable{digits});
-  std::swap(keys, keys_alt);
-  std::swap(vals, vals_alt);
 }
 
 }  // namespace hs

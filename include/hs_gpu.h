@@ -17,7 +17,6 @@
  *   HS_EXCHANGE=nccl   multi-GPU: NCCL all-to-all instead of the fused partition + NVLink peer stores
  *   HS_NO_CARRY=1      decode dictionary-encoded included columns to values instead of carrying 16-bit codes
  *                      (on several GPUs all ranks must agree)
- *   HS_FULL_SORT=1     radix-sort every varying key byte instead of the high bytes + tie fix-up (implies HS_LSD_SORT=1)
  *   HS_LSD_SORT=1      sort the first key column with LSD passes over its high bytes + tie fix-up instead of the
  *                      shared-memory local sort (directly, or after one MSD pass)
  *   HS_PART_REHASH=1   partition kernel hashes the keys again instead of reading the stored bucket ids
