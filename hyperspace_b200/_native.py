@@ -71,6 +71,13 @@ class ScanSpec(C.Structure):
                 ("lo_bytes", C.c_char_p), ("hi_bytes", C.c_char_p), ("lo_len", C.c_uint32), ("hi_len", C.c_uint32)]
 
 
+class PredicateSpec(C.Structure):
+    _fields_ = [("column", C.c_char_p), ("literal_type", C.c_int32), ("has_lo", C.c_int32), ("has_hi", C.c_int32),
+                ("lo_strict", C.c_int32), ("hi_strict", C.c_int32), ("reserved", C.c_int32),
+                ("lo_i", C.c_int64), ("hi_i", C.c_int64), ("lo_f", C.c_double), ("hi_f", C.c_double),
+                ("lo_bytes", C.c_char_p), ("hi_bytes", C.c_char_p), ("lo_len", C.c_uint32), ("hi_len", C.c_uint32)]
+
+
 class JoinSpec(C.Structure):
     _fields_ = [("left_files", C.POINTER(SourceFile)), ("n_left", C.c_int32),
                 ("right_files", C.POINTER(SourceFile)), ("n_right", C.c_int32),
@@ -104,7 +111,7 @@ EXPORTED_SYMBOLS = [
     "hs_k_bucket_ids", "hs_k_sort_perm", "hs_synth_table",
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
-    "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets",
+    "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -151,6 +158,9 @@ def load_library() -> C.CDLL:
     L.hs_result_free.argtypes = [C.c_void_p]
     L.hs_filter_scan.restype = C.c_int
     L.hs_filter_scan.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    L.hs_filter_scan_where.restype = C.c_int
+    L.hs_filter_scan_where.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32, C.POINTER(C.c_void_p),
+                                       C.POINTER(Stats), *err]
     L.hs_bucket_join.restype = C.c_int
     L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_batch_num_rows.restype = C.c_int64
@@ -227,6 +237,31 @@ class FileImage:
     size: int = 0
     file_id: int = -1
     on_device: bool = False
+
+
+def _literal_type(lo, hi) -> int:
+    """HS_TYPE_* of a predicate's literals: str / bytes -> string, int -> long (it must fit in 64 bits), float -> double."""
+    kinds = set()
+    for v in (lo, hi):
+        if v is None:
+            continue
+        if isinstance(v, (bool, np.bool_)):
+            raise ValueError("a boolean literal cannot bound a range")
+        if isinstance(v, (str, bytes, bytearray)):
+            kinds.add(HS_TYPE_STRING)
+        elif isinstance(v, (int, np.integer)):
+            if not -2**63 <= int(v) < 2**63:
+                raise ValueError(f"integer literal {v} does not fit in a long")
+            kinds.add(HS_TYPE_INT64)
+        elif isinstance(v, (float, np.floating)):
+            kinds.add(HS_TYPE_DOUBLE)
+        else:
+            raise ValueError(f"unsupported literal {v!r}")
+    if not kinds:
+        raise ValueError("a predicate needs a lower or an upper bound")
+    if HS_TYPE_STRING in kinds and len(kinds) > 1:
+        raise ValueError("a predicate cannot mix string and numeric bounds")
+    return HS_TYPE_DOUBLE if HS_TYPE_DOUBLE in kinds else kinds.pop()
 
 
 def _source_array(files: Sequence[FileImage]):
@@ -612,6 +647,50 @@ class Context:
         res, st = C.c_void_p(), Stats()
         err = C.create_string_buffer(1024)
         _check(L.hs_filter_scan(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
+    def filter_scan_where(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
+                          sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (), output: int = HS_OUT_HOST
+                          ) -> Tuple[Batch, Dict[str, float]]:
+        """hs_filter_scan_where: rows where every predicate holds.  A predicate is ``(column, lo, lo_strict, hi, hi_strict)``
+        with None for a missing bound; the literal type follows the Python value (int -> long, float -> double, str / bytes
+        -> string) and the engine applies Spark's comparison coercion."""
+        L = load_library()
+        src, keep = _source_array(files)
+        pc = _cstr_array(projected)
+        spec = ScanSpec()
+        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
+        spec.key_column = key.encode() if key else None
+        spec.projected_columns, spec.n_projected = pc, len(projected)
+        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
+        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
+        spec.output = output
+        split = []  # an int bound and a float bound are two comparisons, each in its own type
+        for column, lo, lo_strict, hi, hi_strict in predicates:
+            if lo is not None and hi is not None and {_literal_type(lo, None), _literal_type(None, hi)} == {HS_TYPE_INT64, HS_TYPE_DOUBLE}:
+                split += [(column, lo, lo_strict, None, False), (column, None, False, hi, hi_strict)]
+            else:
+                split.append((column, lo, lo_strict, hi, hi_strict))
+        preds = (PredicateSpec * max(1, len(split)))()
+        for p, (column, lo, lo_strict, hi, hi_strict) in zip(preds, split):
+            p.column = column.encode()
+            p.literal_type = _literal_type(lo, hi)
+            p.has_lo, p.has_hi = int(lo is not None), int(hi is not None)
+            p.lo_strict, p.hi_strict = int(bool(lo_strict)), int(bool(hi_strict))
+            for side, v in (("lo", lo), ("hi", hi)):
+                if v is None:
+                    continue
+                if p.literal_type == HS_TYPE_STRING:
+                    b = v.encode("utf-8") if isinstance(v, str) else bytes(v)
+                    setattr(p, side + "_bytes", b)
+                    setattr(p, side + "_len", len(b))
+                elif p.literal_type == HS_TYPE_INT64:
+                    setattr(p, side + "_i", int(v))
+                else:
+                    setattr(p, side + "_f", float(v))
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_filter_scan_where(self._h, C.byref(spec), preds, len(split), C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     def bucket_join(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],

@@ -164,7 +164,7 @@ void drop_deleted_rows(hs_ctx* ctx, Table& t, const int64_t* deleted, int ndelet
   copy_d2h(ctx, &kept, offs.get() + n, 8);
   sync_stream(ctx);
   Buf<uint32_t> idx(ctx, std::max<uint64_t>(1, kept));
-  launch_compact_indices(ctx, mask.get(), offs.get(), n, idx.get());
+  launch_compact_indices(ctx, mask.get(), offs.get(), n, nullptr, idx.get());
   gather_table(ctx, t, idx.get(), (int64_t)kept);
 }
 
@@ -825,15 +825,17 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
       if (is_str) bc.offsets = std::move(d_offsets[i]);
       if (c.has_nulls) bc.valid = std::move(d_valid[i]);
     } else {
+      // result columns go straight to their pinned buffers on the copy engine (the ring of copy_d2h would stage results of
+      // up to 16 MB through a host memcpy)
       bc.data.alloc(ctx, std::max<size_t>(1, data_bytes), true);
-      if (data_bytes) copy_d2h(ctx, bc.data.get(), d_data[i].get(), data_bytes);
+      if (data_bytes) copy_d2h_engine(ctx, bc.data.get(), d_data[i].get(), data_bytes);
       if (is_str) {
         bc.offsets.alloc(ctx, (size_t)n_out + 1, true);
-        copy_d2h(ctx, bc.offsets.get(), d_offsets[i].get(), 8 * ((size_t)n_out + 1));
+        copy_d2h_engine(ctx, bc.offsets.get(), d_offsets[i].get(), 8 * ((size_t)n_out + 1));
       }
       if (c.has_nulls) {
         bc.valid.alloc(ctx, (size_t)std::max<int64_t>(1, n_out), true);
-        if (n_out) copy_d2h(ctx, bc.valid.get(), d_valid[i].get(), (size_t)n_out);
+        if (n_out) copy_d2h_engine(ctx, bc.valid.get(), d_valid[i].get(), (size_t)n_out);
       }
     }
     b->cols.push_back(std::move(bc));
@@ -842,7 +844,7 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
   b->nrows = n_out;
 }
 
-// int32 keys are widened once so that the comparison kernels (range bounds, predicate mask, join probes) stay int64-only
+// int32 join keys are widened once so that the join probes stay int64-only
 __global__ void k_widen_i32(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ out) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
@@ -870,8 +872,183 @@ __global__ void k_ranges_to_indices(const int64_t* __restrict__ bounds, const ui
   for (int64_t i = first + threadIdx.x; i < last; i += blockDim.x) out_idx[o + (i - first)] = (uint32_t)(base + i);
 }
 
-int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
-  if (!ctx || !spec || !out) return HS_EINVAL;
+}  // extern "C"
+
+// ---- predicates: Spark 3.1's binary-comparison coercion, decided once on the host ---------------------------------------
+// Every predicate becomes a PredRange (kernels.h): numeric columns get an inclusive range of sort_encode values, found by
+// binary search over the encoded domain with the comparison Spark would evaluate -- in the wider of the column's and the
+// literal's types (int < long < float < double), with SQLOrderingUtil's order (NaN == NaN, NaN above +inf, -0.0 == 0.0).
+// Every cast on the way (int/long -> double, float -> double, long -> float) is monotone, so the rows satisfying a bound
+// are one end of the encoded order, and rounding casts (long -> double beyond 2^53) are followed exactly.
+
+template <typename F>
+static int spark_compare(F a, F b) {  // SQLOrderingUtil.compareDoubles / compareFloats
+  const bool na = a != a, nb = b != b;
+  if (na || nb) return na == nb ? 0 : (na ? 1 : -1);
+  return a < b ? -1 : (a > b ? 1 : 0);
+}
+
+// the column value whose sort_encode is e, compared with the literal (lit_i when lit_type is HS_TYPE_INT64, else lit_f)
+static int compare_encoded(int col_type, uint64_t e, int lit_type, int64_t lit_i, double lit_f) {
+  const bool lit_long = lit_type == HS_TYPE_INT64;
+  switch (col_type) {
+    case HS_TYPE_INT32:
+    case HS_TYPE_INT64: {
+      const int64_t v = col_type == HS_TYPE_INT32 ? (int64_t)(int32_t)((uint32_t)e ^ 0x80000000u) : (int64_t)(e ^ 0x8000000000000000ull);
+      if (lit_long) return v < lit_i ? -1 : (v > lit_i ? 1 : 0);
+      return spark_compare((double)v, lit_f);
+    }
+    case HS_TYPE_FLOAT: {
+      const uint32_t u = (uint32_t)e, bits = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+      float f;
+      memcpy(&f, &bits, 4);
+      return lit_long ? spark_compare(f, (float)lit_i) : spark_compare((double)f, lit_f);
+    }
+    default: {
+      const uint64_t bits = (e & 0x8000000000000000ull) ? (e & 0x7fffffffffffffffull) : ~e;
+      double d;
+      memcpy(&d, &bits, 8);
+      return spark_compare(d, lit_long ? (double)lit_i : lit_f);
+    }
+  }
+}
+
+// encoded values of a column type, lowest to highest (floating point: -inf .. the NaNs above +inf)
+static void encoded_domain(int col_type, uint64_t* lo, uint64_t* hi) {
+  switch (col_type) {
+    case HS_TYPE_INT32: *lo = 0, *hi = 0xffffffffull; return;
+    case HS_TYPE_INT64: *lo = 0, *hi = ~0ull; return;
+    case HS_TYPE_FLOAT: *lo = 0x007fffffull, *hi = 0xffffffffull; return;   // ~bits(-inf)
+    default: *lo = 0x000fffffffffffffull, *hi = ~0ull; return;             // ~bits(-inf)
+  }
+}
+
+struct ResolvedPredicate {
+  int col = -1;  // index into the scan's decoded columns
+  PredRange r{};
+  const uint8_t* lo_host = nullptr;  // string bounds, for intersecting them on the host
+  const uint8_t* hi_host = nullptr;
+  uint32_t lo_len = 0, hi_len = 0;
+};
+
+// p.literal_type < 0 (hs_filter_scan): the literal type follows the column -- int64 bounds on an integer column, bytes on a
+// string column.  The bytes of string bounds are copied to `holder` (device).
+static PredRange resolve_predicate(hs_ctx* ctx, const hs_predicate& p, const DevColumn& c, std::vector<Buf<uint8_t>>* holder,
+                                   ResolvedPredicate* rp) {
+  const bool str_col = c.type == HS_TYPE_STRING;
+  int lit = p.literal_type;
+  if (lit < 0) {
+    if (!str_col && c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64) fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
+    lit = str_col ? HS_TYPE_STRING : HS_TYPE_INT64;
+  }
+  if (c.type == HS_TYPE_BOOL) fail(HS_EUNSUPPORTED, "filter scan: predicates on the boolean column '%s' are not handled", c.name.c_str());
+  if (c.type < HS_TYPE_INT32 || c.type > HS_TYPE_STRING) fail(HS_EUNSUPPORTED, "filter scan: column '%s' has an unhandled type", c.name.c_str());
+  if (str_col != (lit == HS_TYPE_STRING))
+    fail(HS_EUNSUPPORTED, "filter scan: a %s literal cannot be compared with the %s column '%s'", lit == HS_TYPE_STRING ? "string" : "numeric",
+         str_col ? "string" : "numeric", c.name.c_str());
+  PredRange r{};
+  r.type = c.type;
+  r.has_lo = p.has_lo != 0;
+  r.has_hi = p.has_hi != 0;
+  if (str_col) {
+    if ((p.has_lo && p.lo_len && !p.lo_bytes) || (p.has_hi && p.hi_len && !p.hi_bytes))
+      fail(HS_EINVAL, "filter scan: string column '%s' needs lo_bytes / hi_bytes", c.name.c_str());
+    if (p.lo_len > kMaxStringLen || p.hi_len > kMaxStringLen) fail(HS_EUNSUPPORTED, "string bound longer than 65535 bytes");
+    const uint32_t ll = p.has_lo ? p.lo_len : 0, hl = p.has_hi ? p.hi_len : 0;
+    holder->emplace_back(ctx, (size_t)ll + hl + 16);
+    uint8_t* d = holder->back().get();
+    if (ll) copy_h2d(ctx, d, p.lo_bytes, ll);
+    if (hl) copy_h2d(ctx, d + ll, p.hi_bytes, hl);
+    r.lo = string_ref(d, ll);
+    r.hi = string_ref(d + ll, hl);
+    r.lo_strict = r.has_lo && p.lo_strict;
+    r.hi_strict = r.has_hi && p.hi_strict;
+    rp->lo_host = (const uint8_t*)p.lo_bytes, rp->lo_len = ll;
+    rp->hi_host = (const uint8_t*)p.hi_bytes, rp->hi_len = hl;
+    return r;
+  }
+  uint64_t emin, emax;
+  encoded_domain(c.type, &emin, &emax);
+  auto cmp = [&](uint64_t e, bool hi_side) {
+    return compare_encoded(c.type, e, lit, hi_side ? p.hi_i : p.lo_i, hi_side ? p.hi_f : p.lo_f);
+  };
+  bool empty = false;
+  if (r.has_lo) {  // smallest e with value >= lo (> lo when strict)
+    const int t = p.lo_strict ? 1 : 0;
+    if (cmp(emax, false) < t) {
+      empty = true;
+    } else {
+      uint64_t a = emin, b = emax;
+      while (a < b) {
+        const uint64_t mid = a + ((b - a) >> 1);
+        if (cmp(mid, false) >= t) b = mid;
+        else a = mid + 1;
+      }
+      r.lo = a;
+    }
+  }
+  if (r.has_hi) {  // largest e with value <= hi (< hi when strict)
+    const int t = p.hi_strict ? -1 : 0;
+    if (cmp(emin, true) > t) {
+      empty = true;
+    } else {
+      uint64_t a = emin, b = emax;
+      while (a < b) {
+        const uint64_t mid = b - ((b - a) >> 1);
+        if (cmp(mid, true) <= t) a = mid;
+        else b = mid - 1;
+      }
+      r.hi = a;
+    }
+  }
+  if (empty) r.has_lo = r.has_hi = 1, r.lo = 1, r.hi = 0;
+  return r;
+}
+
+static int host_string_compare(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  const int c = memcmp(a, b, std::min(la, lb));
+  if (c) return c < 0 ? -1 : 1;
+  return la == lb ? 0 : (la < lb ? -1 : 1);
+}
+
+// the conjunction of predicates on one column as one range (the window search takes one range per file)
+static PredRange intersect_ranges(int type, const std::vector<ResolvedPredicate>& ps) {
+  PredRange r{};
+  r.type = type;
+  const uint8_t *lo_b = nullptr, *hi_b = nullptr;
+  uint32_t lo_l = 0, hi_l = 0;
+  for (const ResolvedPredicate& p : ps) {
+    if (p.r.has_lo) {
+      bool take = !r.has_lo;
+      if (!take && type == HS_TYPE_STRING) {
+        const int c = host_string_compare(p.lo_host, p.lo_len, lo_b, lo_l);
+        take = c > 0 || (c == 0 && p.r.lo_strict);
+      } else if (!take) {
+        take = p.r.lo > r.lo;
+      }
+      if (take) r.has_lo = 1, r.lo = p.r.lo, r.lo_strict = p.r.lo_strict, lo_b = p.lo_host, lo_l = p.lo_len;
+    }
+    if (p.r.has_hi) {
+      bool take = !r.has_hi;
+      if (!take && type == HS_TYPE_STRING) {
+        const int c = host_string_compare(p.hi_host, p.hi_len, hi_b, hi_l);
+        take = c < 0 || (c == 0 && p.r.hi_strict);
+      } else if (!take) {
+        take = p.r.hi < r.hi;
+      }
+      if (take) r.has_hi = 1, r.hi = p.r.hi, r.hi_strict = p.r.hi_strict, hi_b = p.hi_host, hi_l = p.hi_len;
+    }
+  }
+  return r;
+}
+
+// The one filter scan: the sorted path binary-searches the key column's windows and decodes the other columns only inside
+// them, then evaluates the predicates on other columns over the window rows; the unsorted path (source files, Hybrid
+// Scan's appended files, the lineage NOT-IN) evaluates every predicate over all rows.
+// legacy (hs_filter_scan): predicates may have no bound (the row's key must then not be null, as that call always did),
+// literal types follow the column, and floating-point keys are refused (the call's bounds are int64).
+static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int n_preds, bool legacy,
+                            hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   *out = nullptr;
   hs_stats st;
   memset(&st, 0, sizeof st);
@@ -881,61 +1058,48 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
   int rc = guarded(ctx, err, errlen, [&] {
     StageTimer total(ctx);
     total.start();
-    if (!spec->key_column) fail(HS_EINVAL, "key_column is required");
-    // columns to decode: key first, then the projection, then lineage when deletes must be filtered
-    std::vector<std::string> cols{spec->key_column};
-    std::vector<int> proj_idx;
-    for (int i = 0; i < spec->n_projected; i++) {
-      std::string nm = spec->projected_columns[i];
-      auto it = std::find(cols.begin(), cols.end(), nm);
-      if (it == cols.end()) {
-        cols.push_back(nm);
-        proj_idx.push_back((int)cols.size() - 1);
-      } else {
-        proj_idx.push_back((int)(it - cols.begin()));
-      }
-    }
-    int lineage_col = -1;
-    if (spec->n_deleted_file_ids > 0) {
-      auto it = std::find(cols.begin(), cols.end(), std::string("_data_file_id"));
-      if (it == cols.end()) {
-        cols.push_back("_data_file_id");
-        lineage_col = (int)cols.size() - 1;
-      } else {
-        lineage_col = (int)(it - cols.begin());
-      }
-    }
     const bool try_sorted = spec->sorted_on_key && spec->n_deleted_file_ids == 0;
+    if (try_sorted && !spec->key_column) fail(HS_EINVAL, "key_column is required");
+    // columns to decode: the key first (sorted path), then the projection, the predicate columns, and lineage when
+    // deletes must be filtered
+    std::vector<std::string> cols;
+    auto col_of = [&](const std::string& nm) {
+      auto it = std::find(cols.begin(), cols.end(), nm);
+      if (it != cols.end()) return (int)(it - cols.begin());
+      cols.push_back(nm);
+      return (int)cols.size() - 1;
+    };
+    if (try_sorted) col_of(spec->key_column);
+    std::vector<int> proj_idx;
+    for (int i = 0; i < spec->n_projected; i++) proj_idx.push_back(col_of(spec->projected_columns[i]));
+    std::vector<int> pred_col(n_preds);
+    for (int i = 0; i < n_preds; i++) pred_col[i] = col_of(preds[i].column);
+    const int lineage_col = spec->n_deleted_file_ids > 0 ? col_of("_data_file_id") : -1;
     SourceSet src;
     open_sources(ctx, spec->files, spec->n_files, &src, &st);
     Table t;
-    if (try_sorted) {
-      // phase 1: only the key column; the other columns are decoded after the binary search, restricted to the pages
-      // that hold qualifying rows
-      decode_sources(ctx, src, {cols[0]}, nullptr, &t, &st);
-    } else {
-      decode_sources(ctx, src, cols, nullptr, &t, &st);
-    }
-    const bool str_key = t.cols[0].type == HS_TYPE_STRING;
-    if (!str_key && t.cols[0].type != HS_TYPE_INT64 && t.cols[0].type != HS_TYPE_INT32)
+    // phase 1 (sorted path): only the key column; the other columns are decoded after the binary search, restricted to
+    // the pages that hold rows inside the windows
+    if (try_sorted) decode_sources(ctx, src, {cols[0]}, nullptr, &t, &st);
+    else decode_sources(ctx, src, cols, nullptr, &t, &st);
+    if (legacy && try_sorted && t.cols[0].type != HS_TYPE_STRING && t.cols[0].type != HS_TYPE_INT64 && t.cols[0].type != HS_TYPE_INT32)
       fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
     const int64_t n = t.nrows;
-    Buf<int64_t> k64;
-    const int64_t* d_keys = str_key ? nullptr : widened_key(ctx, t.cols[0], n, &k64);
-    // string bounds: device copies of the bytes, addressed like every string value (a reference)
-    Buf<uint8_t> d_bound_bytes;
-    uint64_t lo_ref = 0, hi_ref = 0;
-    if (str_key) {
-      if ((spec->has_lo && spec->lo_len && !spec->lo_bytes) || (spec->has_hi && spec->hi_len && !spec->hi_bytes))
-        fail(HS_EINVAL, "filter scan: string key '%s' needs lo_bytes / hi_bytes", t.cols[0].name.c_str());
-      if (spec->lo_len > kMaxStringLen || spec->hi_len > kMaxStringLen) fail(HS_EUNSUPPORTED, "string bound longer than 65535 bytes");
-      const uint32_t ll = spec->has_lo ? spec->lo_len : 0, hl = spec->has_hi ? spec->hi_len : 0;
-      d_bound_bytes.alloc(ctx, (size_t)ll + hl + 16);
-      if (ll) copy_h2d(ctx, d_bound_bytes.get(), spec->lo_bytes, ll);
-      if (hl) copy_h2d(ctx, d_bound_bytes.get() + ll, spec->hi_bytes, hl);
-      lo_ref = string_ref(d_bound_bytes.get(), ll);
-      hi_ref = string_ref(d_bound_bytes.get() + ll, hl);
-    }
+    std::vector<Buf<uint8_t>> bound_bytes;
+    std::vector<ResolvedPredicate> rps(n_preds);
+    auto resolve = [&](int i) {
+      rps[i].col = pred_col[i];
+      rps[i].r = resolve_predicate(ctx, preds[i], t.cols[pred_col[i]], &bound_bytes, &rps[i]);
+    };
+    auto residual_set = [&](bool skip_key) {
+      PredSet ps;
+      for (int i = 0; i < n_preds; i++) {
+        if (skip_key && pred_col[i] == 0) continue;
+        const DevColumn& c = t.cols[rps[i].col];
+        ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, rps[i].r};
+      }
+      return ps;
+    };
     StageTimer t_scan(ctx);
     t_scan.start();
     Buf<uint32_t> idx;
@@ -945,21 +1109,26 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
       Table full;
       decode_sources(ctx, src, cols, nullptr, &full, &st);
       t = std::move(full);
-      if (!str_key) d_keys = widened_key(ctx, t.cols[0], n, &k64);
     }
     if (sorted) {
-      // K7: two binary searches per file
+      // K7: two binary searches per file, on the intersection of the predicates on the key
+      const int ktype = t.cols[0].type;
+      if (ktype < HS_TYPE_INT32 || ktype > HS_TYPE_STRING || ktype == HS_TYPE_BOOL)
+        fail(HS_EUNSUPPORTED, "filter scan: the sorted key column '%s' must be int32 / int64 / float / double / string", cols[0].c_str());
+      std::vector<ResolvedPredicate> on_key;
+      for (int i = 0; i < n_preds; i++)
+        if (pred_col[i] == 0) {
+          resolve(i);
+          on_key.push_back(rps[i]);
+        }
+      const PredRange key_range = intersect_ranges(ktype, on_key);
       const int nseg = spec->n_files;
       std::vector<uint64_t> seg(nseg + 1);
       for (int f = 0; f <= nseg; f++) seg[f] = (uint64_t)t.file_row_begin[f];
       Buf<uint64_t> d_seg(ctx, nseg + 1);
       Buf<int64_t> d_bounds(ctx, 2 * std::max(1, nseg));
       copy_h2d(ctx, d_seg.get(), seg.data(), 8 * (nseg + 1));
-      if (str_key)
-        launch_range_bounds_strings(ctx, (const uint64_t*)t.cols[0].data.get(), d_seg.get(), nseg, spec->has_lo, lo_ref, spec->has_hi,
-                                    hi_ref, d_bounds.get());
-      else
-        launch_range_bounds(ctx, d_keys, d_seg.get(), nseg, spec->has_lo, spec->lo, spec->has_hi, spec->hi, d_bounds.get());
+      launch_range_bounds(ctx, t.cols[0].data.get(), key_range, d_seg.get(), nseg, d_bounds.get());
       std::vector<int64_t> bounds(2 * std::max(1, nseg));
       copy_d2h(ctx, bounds.data(), d_bounds.get(), 16 * nseg);
       sync_stream(ctx);
@@ -973,25 +1142,40 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
         decode_sources(ctx, src, rest, &windows, &others, &st);
         for (auto& c : others.cols) t.cols.push_back(std::move(c));
       }
-      n_out = (int64_t)oo[nseg];
+      const int64_t n_cand = (int64_t)oo[nseg];
       Buf<uint64_t> d_oo(ctx, nseg + 1);
       copy_h2d(ctx, d_oo.get(), oo.data(), 8 * (nseg + 1));
-      idx.alloc(ctx, std::max<int64_t>(1, n_out));
+      idx.alloc(ctx, std::max<int64_t>(1, n_cand));
       if (nseg) {
         k_ranges_to_indices<<<nseg, 256, 0, ctx->stream>>>(d_bounds.get(), d_seg.get(), d_oo.get(), nseg, idx.get());
         HS_LAUNCH_CHECK(ctx);
       }
+      n_out = n_cand;
+      if ((int)on_key.size() < n_preds) {
+        // residual: the predicates on other columns, over the window rows, compacted through the candidate list
+        for (int i = 0; i < n_preds; i++)
+          if (pred_col[i] != 0) resolve(i);
+        const PredSet ps = residual_set(true);
+        Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n_cand));
+        Buf<uint64_t> offs(ctx, n_cand + 1);
+        launch_predicate_mask(ctx, ps, idx.get(), n_cand, mask.get());
+        exclusive_scan_u32_u64(ctx, mask.get(), n_cand, offs.get());
+        uint64_t kept = 0;
+        copy_d2h(ctx, &kept, offs.get() + n_cand, 8);
+        sync_stream(ctx);
+        n_out = (int64_t)kept;
+        Buf<uint32_t> kept_idx(ctx, std::max<int64_t>(1, n_out));
+        launch_compact_indices(ctx, mask.get(), offs.get(), n_cand, idx.get(), kept_idx.get());
+        idx = std::move(kept_idx);
+      }
       sync_stream(ctx);
     } else {
-      // full predicate scan (appended source files under Hybrid Scan, or lineage NOT-IN filter)
+      // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
+      for (int i = 0; i < n_preds; i++) resolve(i);
+      const PredSet ps = residual_set(false);
       Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
       Buf<uint64_t> offs(ctx, n + 1);
-      if (str_key)
-        launch_filter_mask_strings(ctx, (const uint64_t*)t.cols[0].data.get(), t.cols[0].has_nulls ? t.cols[0].valid.get() : nullptr, n,
-                                   spec->has_lo, lo_ref, spec->has_hi, hi_ref, mask.get());
-      else
-        launch_filter_mask(ctx, d_keys, t.cols[0].has_nulls ? t.cols[0].valid.get() : nullptr, n, spec->has_lo, spec->lo,
-                           spec->has_hi, spec->hi, mask.get());
+      launch_predicate_mask(ctx, ps, nullptr, n, mask.get());
       if (spec->n_deleted_file_ids > 0) {
         Buf<int64_t> d_del(ctx, spec->n_deleted_file_ids);
         copy_h2d(ctx, d_del.get(), spec->deleted_file_ids, 8 * spec->n_deleted_file_ids);
@@ -1004,14 +1188,18 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
       sync_stream(ctx);
       n_out = (int64_t)kept;
       idx.alloc(ctx, std::max<int64_t>(1, n_out));
-      launch_compact_indices(ctx, mask.get(), offs.get(), n, idx.get());
+      launch_compact_indices(ctx, mask.get(), offs.get(), n, nullptr, idx.get());
       sync_stream(ctx);
     }
     t_scan.stop();
+    StageTimer t_gather(ctx);
+    t_gather.start();
     batch_from_gather(ctx, t, proj_idx, idx.get(), n_out, res.get());
+    t_gather.stop();
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_scan.ms();
+    st.ms_gather += t_gather.ms();
     st.rows_out = n_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;
@@ -1019,6 +1207,49 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
   if (stats) *stats = st;
   if (rc == HS_OK) *out = res.release();
   return rc;
+}
+
+extern "C" {
+
+int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  if (!ctx || !spec || !out) return HS_EINVAL;
+  *out = nullptr;
+  if (!spec->key_column) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "key_column is required");
+    return HS_EINVAL;
+  }
+  // one predicate on the key, its literal type following the column
+  hs_predicate p;
+  memset(&p, 0, sizeof p);
+  p.column = spec->key_column;
+  p.literal_type = -1;
+  p.has_lo = spec->has_lo, p.has_hi = spec->has_hi;
+  p.lo_i = spec->lo, p.hi_i = spec->hi;
+  p.lo_bytes = spec->lo_bytes, p.hi_bytes = spec->hi_bytes;
+  p.lo_len = spec->lo_len, p.hi_len = spec->hi_len;
+  return filter_scan_core(ctx, spec, &p, 1, true, out, stats, err, errlen);
+}
+
+int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
+                         hs_stats* stats, char* err, size_t errlen) {
+  if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds)) return HS_EINVAL;
+  *out = nullptr;
+  auto refuse = [&](int code, const char* msg, const char* what) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, msg, what);
+    return code;
+  };
+  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
+  if (spec->has_lo || spec->has_hi) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
+  for (int i = 0; i < n_preds; i++) {
+    const hs_predicate& p = preds[i];
+    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
+    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
+    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING)
+      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
+  }
+  return filter_scan_core(ctx, spec, preds, n_preds, false, out, stats, err, errlen);
 }
 
 // Orders the decoded rows of one join side bucket-major and key-sorted.  When every bucket holds exactly one file the

@@ -172,6 +172,9 @@ namespace hs {
 // through sync_stream; error paths use xfer_abort (synchronises, drops undelivered results).
 void copy_h2d(hs_ctx* ctx, void* dst_dev, const void* src_host, size_t bytes);
 void copy_d2h(hs_ctx* ctx, void* dst_host, const void* src_dev, size_t bytes);
+// Always on the copy engine, whatever the size: for results copied into pinned memory the caller owns (copy_d2h sends
+// copies up to 16 MB through the small-transfer ring: a copy kernel writing over PCIe, then a host memcpy at sync_stream).
+void copy_d2h_engine(hs_ctx* ctx, void* dst_host, const void* src_dev, size_t bytes);
 void fill_bytes(hs_ctx* ctx, void* dst, int value, size_t bytes);  // cudaMemsetAsync without a copy engine
 void sync_stream(hs_ctx* ctx);
 void xfer_abort(hs_ctx* ctx);

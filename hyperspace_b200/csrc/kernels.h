@@ -345,9 +345,31 @@ void launch_copy_blobs(hs_ctx* ctx, const BlobCopy* blobs, int64_t n, const uint
 void launch_synth_column(hs_ctx* ctx, int col, int64_t first_row, int64_t n, void* out);
 
 // ---- read side (read_side.cu) ---------------------------------------------------------------------------
-// per segment s: bounds[2s] = first index with key >= lo, bounds[2s+1] = first index with key > hi (segment-relative)
-void launch_range_bounds(hs_ctx* ctx, const int64_t* keys, const uint64_t* seg_offsets, int nseg, int has_lo,
-                         int64_t lo, int has_hi, int64_t hi, int64_t* bounds);
+// A filter scan's comparisons (api.cu resolves Spark's coercion into these ranges).  One range on one column of type `type`:
+// numeric columns compare sort_encode(type, value) with the inclusive encoded bounds lo / hi (lo_strict = hi_strict = 0;
+// lo > hi is an empty range); string / binary columns compare the value with the references lo / hi (device copies of the
+// bound bytes) in UTF8String byte order, strictly where lo_strict / hi_strict say so.
+constexpr int kMaxPredicates = 16;
+struct PredRange {
+  int32_t type;
+  int32_t has_lo, has_hi, lo_strict, hi_strict;
+  uint64_t lo, hi;
+};
+struct PredDesc {
+  const void* data;      // column values (string references for strings)
+  const uint8_t* valid;  // nullptr: no nulls; a null never satisfies a predicate
+  PredRange r;
+};
+struct PredSet {
+  PredDesc p[kMaxPredicates];
+  int n = 0;
+};
+// per sorted segment s (ascending on `keys`): bounds[2s] = first row inside r, bounds[2s+1] = first row above r
+// (segment-relative)
+void launch_range_bounds(hs_ctx* ctx, const void* keys, const PredRange& r, const uint64_t* seg_offsets, int nseg,
+                         int64_t* bounds);
+// mask[i] = every predicate of `preds` holds for row cand[i] (row i when cand is nullptr)
+void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, uint32_t* mask);
 // match counts of every left row against the right rows of the same bucket
 // string_keys: lkeys / rkeys hold string references (device_utils.cuh) compared in byte order
 void launch_join_count(hs_ctx* ctx, const int64_t* lkeys, const uint64_t* lseg, const int64_t* rkeys,
@@ -356,21 +378,14 @@ void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first
                       int64_t nl, uint32_t* out_li, uint32_t* out_ri);
 // exclusive scan of uint32 counts into uint64 offsets (n+1 entries; last = total)
 void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t* out);
-// mask[i] = lo <= keys[i] <= hi (and file id not deleted); compaction index list
-void launch_filter_mask(hs_ctx* ctx, const int64_t* keys, const uint8_t* valid, int64_t n, int has_lo, int64_t lo,
-                        int has_hi, int64_t hi, uint32_t* mask);
-// string / binary keys (values are references into the source images, device_utils.cuh: string_ref): the bounds are
-// references to device copies of the bound bytes; order = unsigned byte order, shorter first on a common prefix
-void launch_range_bounds_strings(hs_ctx* ctx, const uint64_t* refs, const uint64_t* seg_offsets, int nseg, int has_lo,
-                                 uint64_t lo_ref, int has_hi, uint64_t hi_ref, int64_t* bounds);
-void launch_filter_mask_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, int64_t n, int has_lo,
-                                uint64_t lo_ref, int has_hi, uint64_t hi_ref, uint32_t* mask);
 // lens[i] = length of refs[idx[i]] (0 for a null);  then, with offsets = exclusive scan of lens: out[offsets[i] ..] = bytes
 void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                            uint32_t* lens);
 void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                          const uint64_t* offsets, uint8_t* out);
-void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, uint32_t* out_idx);
+// out_idx[offsets[i]] = cand[i] (i when cand is nullptr) for every i with mask[i]
+void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, const uint32_t* cand,
+                            uint32_t* out_idx);
 void launch_not_in_mask(hs_ctx* ctx, const int64_t* file_ids, int64_t n, const int64_t* deleted, int ndeleted,
                         uint32_t* mask /* and-ed in place */);
 

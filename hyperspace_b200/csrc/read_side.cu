@@ -33,16 +33,80 @@ __device__ __forceinline__ int64_t upper_bound_i64(const int64_t* a, int64_t n, 
   return lo;
 }
 
-__global__ void k_range_bounds(const int64_t* __restrict__ keys, const uint64_t* __restrict__ seg_offsets, int nseg,
-                               int has_lo, int64_t lo, int has_hi, int64_t hi, int64_t* __restrict__ bounds) {
+// ---- predicate evaluation (kernels.h: PredRange) -------------------------------------------------------------------
+// value i of a column of type KT against a bound: -1 / 0 / +1.  Numeric values are compared as sort_encode(KT, value)
+// with an encoded bound (Spark's order: NaN greatest, -0.0 == 0.0); strings as references in UTF8String byte order.
+template <int KT>
+__device__ __forceinline__ int cmp_bound(const void* __restrict__ col, int64_t i, uint64_t bound) {
+  if constexpr (KT == HS_TYPE_STRING) {
+    return string_compare(((const uint64_t*)col)[i], bound);
+  } else {
+    uint64_t raw;
+    if constexpr (KT == HS_TYPE_INT32 || KT == HS_TYPE_FLOAT) raw = ((const uint32_t*)col)[i];
+    else raw = ((const uint64_t*)col)[i];
+    const uint64_t e = sort_encode(KT, raw);
+    return e < bound ? -1 : (e > bound ? 1 : 0);
+  }
+}
+
+// first row of the ascending rows [b, b + n) with cmp_bound(row, bound) >= t (segment-relative)
+template <int KT>
+__device__ __forceinline__ int64_t first_at_least(const void* col, int64_t b, int64_t n, uint64_t bound, int t) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (cmp_bound<KT>(col, b + mid, bound) < t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// K7 window search, one thread per sorted file: bounds[2s] = first row inside the range, bounds[2s+1] = first row above it.
+// Numeric bounds are inclusive (strictness is folded in on the host); string bounds carry their strictness.
+template <int KT>
+__global__ void k_range_bounds(const void* __restrict__ keys, PredRange r, const uint64_t* __restrict__ seg_offsets, int nseg,
+                               int64_t* __restrict__ bounds) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= nseg) return;
   const int64_t b = (int64_t)seg_offsets[s], n = (int64_t)seg_offsets[s + 1] - b;
-  int64_t first = has_lo ? lower_bound_i64(keys + b, n, lo) : 0;
-  int64_t last = has_hi ? upper_bound_i64(keys + b, n, hi) : n;
+  int64_t first = r.has_lo ? first_at_least<KT>(keys, b, n, r.lo, r.lo_strict ? 1 : 0) : 0;
+  int64_t last = r.has_hi ? first_at_least<KT>(keys, b, n, r.hi, r.hi_strict ? 0 : 1) : n;
   if (last < first) last = first;
   bounds[2 * s] = first;
   bounds[2 * s + 1] = last;
+}
+
+template <int KT>
+__device__ __forceinline__ bool in_range(const void* col, int64_t i, const PredRange& r) {
+  if (r.has_lo && cmp_bound<KT>(col, i, r.lo) < (r.lo_strict ? 1 : 0)) return false;
+  if (r.has_hi && cmp_bound<KT>(col, i, r.hi) > (r.hi_strict ? -1 : 0)) return false;
+  return true;
+}
+
+// The residual conjunction, one thread per candidate row: mask[i] = every predicate holds for row cand[i] (row i without a
+// candidate list).  Inside a window the candidates are consecutive rows, so the predicate columns are read coalesced.
+__global__ void k_predicate_mask(const __grid_constant__ PredSet ps, const uint32_t* __restrict__ cand, int64_t n,
+                                 uint32_t* __restrict__ mask) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int64_t row = cand ? (int64_t)cand[i] : i;
+    bool ok = true;
+    for (int p = 0; p < ps.n && ok; p++) {
+      const PredDesc& d = ps.p[p];
+      if (d.valid && !d.valid[row]) {  // a null never satisfies a comparison
+        ok = false;
+        continue;
+      }
+      switch (d.r.type) {
+        case HS_TYPE_INT32: ok = in_range<HS_TYPE_INT32>(d.data, row, d.r); break;
+        case HS_TYPE_INT64: ok = in_range<HS_TYPE_INT64>(d.data, row, d.r); break;
+        case HS_TYPE_FLOAT: ok = in_range<HS_TYPE_FLOAT>(d.data, row, d.r); break;
+        case HS_TYPE_DOUBLE: ok = in_range<HS_TYPE_DOUBLE>(d.data, row, d.r); break;
+        default: ok = in_range<HS_TYPE_STRING>(d.data, row, d.r); break;
+      }
+    }
+    mask[i] = ok ? 1u : 0u;
+  }
 }
 
 // one thread per left row; the segment of a row is found by binary search over the (few hundred) segment offsets
@@ -176,18 +240,6 @@ __global__ void __launch_bounds__(kScanThreads) k_scan_apply(const uint32_t* __r
   }
 }
 
-__global__ void k_filter_mask(const int64_t* __restrict__ keys, const uint8_t* __restrict__ valid, int64_t n, int has_lo,
-                              int64_t lo, int has_hi, int64_t hi, uint32_t* __restrict__ mask) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const int64_t k = keys[i];
-    bool ok = !valid || valid[i];  // a null key never satisfies a comparison
-    if (has_lo) ok = ok && k >= lo;
-    if (has_hi) ok = ok && k <= hi;
-    mask[i] = ok ? 1u : 0u;
-  }
-}
-
 __global__ void k_not_in_mask(const int64_t* __restrict__ ids, int64_t n, const int64_t* __restrict__ deleted,
                               int ndeleted, uint32_t* __restrict__ mask) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -200,61 +252,16 @@ __global__ void k_not_in_mask(const int64_t* __restrict__ ids, int64_t n, const 
 }
 
 __global__ void k_compact(const uint32_t* __restrict__ mask, const uint64_t* __restrict__ offsets, int64_t n,
-                          uint32_t* __restrict__ out_idx) {
+                          const uint32_t* __restrict__ cand, uint32_t* __restrict__ out_idx) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    if (mask[i]) out_idx[offsets[i]] = (uint32_t)i;
+    if (mask[i]) out_idx[offsets[i]] = cand ? cand[i] : (uint32_t)i;
 }
 
 inline int grid_for(hs_ctx* ctx, int64_t n, int threads, int per_sm) {
   int64_t want = ceil_div(n, threads);
   int64_t cap = (int64_t)ctx->sm_count * per_sm;
   return (int)std::max<int64_t>(1, std::min(want, cap));
-}
-
-// ---- string keys: the same scans over references, compared in UTF8String byte order ------------------------------------
-__global__ void k_range_bounds_str(const uint64_t* __restrict__ refs, const uint64_t* __restrict__ seg_offsets, int nseg,
-                                   int has_lo, uint64_t lo_ref, int has_hi, uint64_t hi_ref, int64_t* __restrict__ bounds) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= nseg) return;
-  const int64_t b = (int64_t)seg_offsets[s], n = (int64_t)seg_offsets[s + 1] - b;
-  const uint64_t* a = refs + b;
-  int64_t first = 0, last = n;
-  if (has_lo) {  // first row with value >= lo
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo) >> 1);
-      if (string_compare(a[mid], lo_ref) < 0) lo = mid + 1;
-      else hi = mid;
-    }
-    first = lo;
-  }
-  if (has_hi) {  // first row with value > hi
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo) >> 1);
-      if (string_compare(a[mid], hi_ref) <= 0) lo = mid + 1;
-      else hi = mid;
-    }
-    last = lo;
-  }
-  if (last < first) last = first;
-  bounds[2 * s] = first;
-  bounds[2 * s + 1] = last;
-}
-
-__global__ void k_filter_mask_str(const uint64_t* __restrict__ refs, const uint8_t* __restrict__ valid, int64_t n, int has_lo,
-                                  uint64_t lo_ref, int has_hi, uint64_t hi_ref, uint32_t* __restrict__ mask) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    bool ok = !valid || valid[i];  // a null key never satisfies a comparison
-    if (ok) {
-      const uint64_t r = refs[i];
-      if (has_lo) ok = string_compare(r, lo_ref) >= 0;
-      if (ok && has_hi) ok = string_compare(r, hi_ref) <= 0;
-    }
-    mask[i] = ok ? 1u : 0u;
-  }
 }
 
 __global__ void k_string_lengths(const uint64_t* __restrict__ refs, const uint8_t* __restrict__ valid,
@@ -284,20 +291,6 @@ __global__ void k_copy_strings(const uint64_t* __restrict__ refs, const uint8_t*
 
 }  // namespace
 
-void launch_range_bounds_strings(hs_ctx* ctx, const uint64_t* refs, const uint64_t* seg_offsets, int nseg, int has_lo,
-                                 uint64_t lo_ref, int has_hi, uint64_t hi_ref, int64_t* bounds) {
-  if (nseg == 0) return;
-  k_range_bounds_str<<<(nseg + 127) / 128, 128, 0, ctx->stream>>>(refs, seg_offsets, nseg, has_lo, lo_ref, has_hi, hi_ref, bounds);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_filter_mask_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, int64_t n, int has_lo,
-                                uint64_t lo_ref, int has_hi, uint64_t hi_ref, uint32_t* mask) {
-  if (n == 0) return;
-  k_filter_mask_str<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(refs, valid, n, has_lo, lo_ref, has_hi, hi_ref, mask);
-  HS_LAUNCH_CHECK(ctx);
-}
-
 void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                            uint32_t* lens) {
   if (n == 0) return;
@@ -312,10 +305,26 @@ void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid
   HS_LAUNCH_CHECK(ctx);
 }
 
-void launch_range_bounds(hs_ctx* ctx, const int64_t* keys, const uint64_t* seg_offsets, int nseg, int has_lo,
-                         int64_t lo, int has_hi, int64_t hi, int64_t* bounds) {
+void launch_range_bounds(hs_ctx* ctx, const void* keys, const PredRange& r, const uint64_t* seg_offsets, int nseg,
+                         int64_t* bounds) {
+  KernelScope _ks(ctx, "k_range_bounds");
   if (nseg == 0) return;
-  k_range_bounds<<<(nseg + 127) / 128, 128, 0, ctx->stream>>>(keys, seg_offsets, nseg, has_lo, lo, has_hi, hi, bounds);
+  const int grid = (nseg + 127) / 128;
+  switch (r.type) {
+    case HS_TYPE_INT32: k_range_bounds<HS_TYPE_INT32><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
+    case HS_TYPE_INT64: k_range_bounds<HS_TYPE_INT64><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
+    case HS_TYPE_FLOAT: k_range_bounds<HS_TYPE_FLOAT><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
+    case HS_TYPE_DOUBLE: k_range_bounds<HS_TYPE_DOUBLE><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
+    case HS_TYPE_STRING: k_range_bounds<HS_TYPE_STRING><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
+    default: fail(HS_EUNSUPPORTED, "range search over a column of type %d", r.type);
+  }
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, uint32_t* mask) {
+  KernelScope _ks(ctx, "k_predicate_mask");
+  if (n == 0) return;
+  k_predicate_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(preds, cand, n, mask);
   HS_LAUNCH_CHECK(ctx);
 }
 
@@ -352,16 +361,10 @@ void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t
   }
 }
 
-void launch_filter_mask(hs_ctx* ctx, const int64_t* keys, const uint8_t* valid, int64_t n, int has_lo, int64_t lo,
-                        int has_hi, int64_t hi, uint32_t* mask) {
+void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, const uint32_t* cand,
+                            uint32_t* out_idx) {
   if (n == 0) return;
-  k_filter_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(keys, valid, n, has_lo, lo, has_hi, hi, mask);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, uint32_t* out_idx) {
-  if (n == 0) return;
-  k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask, offsets, n, out_idx);
+  k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask, offsets, n, cand, out_idx);
   HS_LAUNCH_CHECK(ctx);
 }
 

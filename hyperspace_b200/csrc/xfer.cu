@@ -8,7 +8,7 @@
 // write directly over PCIe (unified addressing makes pinned host memory device-accessible): host data is snapshot into the
 // ring at once (the caller's buffer may die immediately -- no "keep the vector alive" synchronisation), a copy kernel on the
 // ctx stream moves it; device -> host results land in the ring and are handed to their destination by sync_stream().
-// Large transfers (file images, query results) still use the copy engines, which is what they are for.
+// Large transfers (file images) and query results (copy_d2h_engine, any size) use the copy engines, which is what they are for.
 #include "hs_common.h"
 
 namespace hs {
@@ -85,6 +85,11 @@ void copy_d2h(hs_ctx* ctx, void* dst_host, const void* src_dev, size_t bytes) {
   uint8_t* slot = ring_slot(ctx, bytes);
   launch_xfer(ctx, slot, src_dev, bytes);
   ctx->xfer_pending.push_back(hs_ctx::PendingD2H{dst_host, slot, bytes});
+}
+
+void copy_d2h_engine(hs_ctx* ctx, void* dst_host, const void* src_dev, size_t bytes) {
+  if (bytes == 0) return;
+  HS_CUDA(cudaMemcpyAsync(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
 }
 
 // cudaMemsetAsync may be served by a copy engine too: the build path fills with a kernel

@@ -7,7 +7,7 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan (K1 + K7) and hs_bucket_join (K1 + K8).
+Physical execution is the C ABI: hs_filter_scan_where (K1 + K7) and hs_bucket_join (K1 + K8).
 """
 from __future__ import annotations
 
@@ -185,7 +185,8 @@ def _host_column(d: np.ndarray) -> np.ndarray:
 
 
 class ScanExec:
-    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- always hs_filter_scan."""
+    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- always hs_filter_scan_where
+    with the filter's comparisons as its predicates."""
 
     def __init__(self, session, lin: Linear, cand: Optional[Candidate]):
         self.session, self.lin, self.cand = session, lin, cand
@@ -199,36 +200,29 @@ class ScanExec:
             extra = f", hybridScan(appended={len(self.cand.appended)}, deletedIds={self.cand.deleted_ids})"
         return f"GpuIndexScan(Hyperspace(Type: CI, Name: {e.name}, LogVersion: {e.id}), files={len(e.index_files)}{extra})"
 
-    def _bounds(self, key: str):
-        if not self.lin.predicate or key not in self.lin.predicate.bounds:
-            return None, None
-        return self.lin.predicate.bounds[key]
-
     def _scan(self, files, key, out_cols, sorted_on_key, deleted_ids=()):
-        lo, hi = self._bounds(key)
-        batch, _ = self.session.gpu.filter_scan(files, key, out_cols, lo=lo, hi=hi, sorted_on_key=sorted_on_key,
-                                                deleted_file_ids=list(deleted_ids))
+        preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
+        batch, _ = self.session.gpu.filter_scan_where(files, key, out_cols, preds, sorted_on_key=sorted_on_key,
+                                                      deleted_file_ids=list(deleted_ids))
         out = {n: _host_column(d) for n, d, _ in batch.columns}
         batch.free()
         return out
 
     def execute(self) -> Dict[str, np.ndarray]:
         out_cols = self.lin.output
-        pred_cols = self.lin.predicate.columns if self.lin.predicate else []
-        if len(pred_cols) > 1:
-            raise LE.HyperspaceException("the GPU scan handles range predicates on one integer or string column")
         if self.cand is None:
-            key = pred_cols[0] if pred_cols else self.lin.relation.column_names[0]
-            return self._scan(_file_images([f[0] for f in self.lin.relation.files]), key, out_cols, False)
+            return self._scan(_file_images([f[0] for f in self.lin.relation.files]), None, out_cols, False)
         e = self.cand.entry
-        key = pred_cols[0] if pred_cols else e.indexedColumns[0]
+        first = e.indexedColumns[0]
+        pred_cols = self.lin.predicate.columns if self.lin.predicate else []
+        key = next((c for c in pred_cols if c.lower() == first.lower()), first)
         parts = []
         if self.cand.deleted_ids:  # NOT (_data_file_id IN deleted): CoveringIndexRuleUtils.scala:244-253
             parts.append(self._scan(_file_images(e.index_files), key, out_cols, False, self.cand.deleted_ids))
-        else:
-            parts.append(self._scan(_file_images(e.index_files), key, out_cols, key.lower() == e.indexedColumns[0].lower()))
+        else:  # index files are sorted on the first indexed column: binary search when the filter bounds it
+            parts.append(self._scan(_file_images(e.index_files), key, out_cols, key in pred_cols))
         if self.cand.appended:     # appended source files are scanned raw and unioned: CoveringIndexRuleUtils.scala:191-212
-            parts.append(self._scan(_file_images([f[0] for f in self.cand.appended]), key, out_cols, False))
+            parts.append(self._scan(_file_images([f[0] for f in self.cand.appended]), None, out_cols, False))
         return _concat(parts, out_cols)
 
 

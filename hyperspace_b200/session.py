@@ -88,10 +88,17 @@ class RuntimeConf:
 # expressions
 # ---------------------------------------------------------------------------------------------------------------------
 
+# comparison operator of a term -> (lower bound?, strict?) sides it sets
+_TERM_SIDES = {">=": ((False,), ()), ">": ((True,), ()), "<=": ((), (False,)), "<": ((), (True,)), "==": ((False,), (False,))}
+
+
 @dataclass
 class Predicate:
-    """Conjunction of inclusive integer bounds per column: {column: (lo or None, hi or None)}."""
+    """Conjunction of comparisons with literals.  ``bounds`` is the inclusive integer (or byte-string) range per column, which
+    the plan layer uses to pick an index; ``terms`` are the comparisons as written -- (column, operator, literal) with the
+    operator one of >=, >, <=, <, == -- which the engine evaluates with Spark's type coercion."""
     bounds: Dict[str, Tuple[Optional[int], Optional[int]]]
+    terms: List[Tuple[str, str, object]] = field(default_factory=list)
 
     def __and__(self, other: "Predicate") -> "Predicate":
         out = dict(self.bounds)
@@ -101,11 +108,42 @@ class Predicate:
                 lo = l0 if lo is None else (lo if l0 is None else max(lo, l0))
                 hi = h0 if hi is None else (hi if h0 is None else min(hi, h0))
             out[c] = (lo, hi)
-        return Predicate(out)
+        return Predicate(out, self._as_terms() + other._as_terms())
+
+    def _as_terms(self) -> List[Tuple[str, str, object]]:
+        """The comparisons; a Predicate built from bounds alone states them as inclusive bounds, so that a conjunction with
+        one that has terms keeps both sides' conditions."""
+        if self.terms:
+            return list(self.terms)
+        out = []
+        for c, (lo, hi) in self.bounds.items():
+            if lo is not None:
+                out.append((c, ">=", lo))
+            if hi is not None:
+                out.append((c, "<=", hi))
+        return out
 
     @property
     def columns(self) -> List[str]:
         return list(self.bounds)
+
+    def conjuncts(self) -> List[Tuple[str, object, bool, object, bool]]:
+        """The comparisons as (column, lo, lo_strict, hi, hi_strict) ranges for Context.filter_scan_where (a Predicate
+        built from bounds alone gives its inclusive bounds)."""
+        out = []
+        for c, op, v in self._as_terms():
+            lo_side, hi_side = _TERM_SIDES[op]
+            out.append((c, v if lo_side else None, lo_side[0] if lo_side else False, v if hi_side else None,
+                        hi_side[0] if hi_side else False))
+        return out
+
+
+def _ceil(v):  # NaN and infinities (floating-point columns) stay as they are in the bounds
+    return math.ceil(v) if math.isfinite(v) else v
+
+
+def _floor(v):
+    return math.floor(v) if math.isfinite(v) else v
 
 
 def _as_bytes(v) -> bytes:
@@ -121,35 +159,36 @@ class Column:
     # `col("Query") == "facebook"` is the predicate of the reference's own filter-rule tests (T/index/E2EHyperspaceRulesTest.scala).
     def __ge__(self, v):
         if isinstance(v, (str, bytes)):
-            return Predicate({self.name: (_as_bytes(v), None)})
-        return Predicate({self.name: (math.ceil(v), None)})
+            return Predicate({self.name: (_as_bytes(v), None)}, [(self.name, ">=", v)])
+        return Predicate({self.name: (_ceil(v), None)}, [(self.name, ">=", v)])
 
     def __gt__(self, v):
         if isinstance(v, (str, bytes)):
-            return Predicate({self.name: (_as_bytes(v) + b"\x00", None)})  # the smallest value above v
-        return Predicate({self.name: (math.floor(v) + 1, None)})
+            return Predicate({self.name: (_as_bytes(v) + b"\x00", None)}, [(self.name, ">", v)])  # the smallest value above v
+        return Predicate({self.name: (_floor(v) + 1, None)}, [(self.name, ">", v)])
 
     def __le__(self, v):
         if isinstance(v, (str, bytes)):
-            return Predicate({self.name: (None, _as_bytes(v))})
-        return Predicate({self.name: (None, math.floor(v))})
+            return Predicate({self.name: (None, _as_bytes(v))}, [(self.name, "<=", v)])
+        return Predicate({self.name: (None, _floor(v))}, [(self.name, "<=", v)])
 
     def __lt__(self, v):
         if isinstance(v, (str, bytes)):
             raise ValueError("a strict upper bound on a string column has no inclusive form: use <= or between")
-        return Predicate({self.name: (None, math.ceil(v) - 1)})
+        return Predicate({self.name: (None, _ceil(v) - 1)}, [(self.name, "<", v)])
 
     def __eq__(self, v):  # noqa: A003
         if isinstance(v, (str, bytes)):
-            return Predicate({self.name: (_as_bytes(v), _as_bytes(v))})
-        if v != math.floor(v):
-            return Predicate({self.name: (1, 0)})  # an integer never equals a fraction: empty range
-        return Predicate({self.name: (int(v), int(v))})
+            return Predicate({self.name: (_as_bytes(v), _as_bytes(v))}, [(self.name, "==", v)])
+        if not math.isfinite(v) or v != math.floor(v):
+            return Predicate({self.name: (1, 0)}, [(self.name, "==", v)])  # an integer never equals a fraction: empty range
+        return Predicate({self.name: (int(v), int(v))}, [(self.name, "==", v)])
 
     def between(self, lo, hi):
+        terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
         if isinstance(lo, (str, bytes)) or isinstance(hi, (str, bytes)):
-            return Predicate({self.name: (_as_bytes(lo), _as_bytes(hi))})
-        return Predicate({self.name: (math.ceil(lo), math.floor(hi))})
+            return Predicate({self.name: (_as_bytes(lo), _as_bytes(hi))}, terms)
+        return Predicate({self.name: (_ceil(lo), _floor(hi))}, terms)
 
 
 def col(name: str) -> Column:
@@ -261,7 +300,8 @@ class DataFrame:
         return name if name in hits else hits[0]
 
     def filter(self, predicate: Predicate) -> "DataFrame":
-        resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()})
+        resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
+                             [(self._resolve(c), op, v) for c, op, v in predicate.terms])
         return DataFrame(self.session, FilterNode(self.plan, resolved))
 
     where = filter

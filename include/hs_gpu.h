@@ -58,8 +58,8 @@ extern "C" {
 #define HS_TYPE_FLOAT 2
 #define HS_TYPE_DOUBLE 3
 #define HS_TYPE_BOOL 4
-#define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): write path (keys and included columns, one GPU); the index
-                            scans and joins do not read it yet -> HS_EUNSUPPORTED */
+#define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): indexed and included columns (one GPU), filter scan keys and
+                            predicates, single-column join keys; compared in UTF8String byte order */
 
 typedef struct hs_ctx hs_ctx;
 typedef struct hs_index_result hs_index_result;
@@ -236,6 +236,36 @@ typedef struct {
 /* Executes the scan FilterIndexRule.applyIndex substitutes for the source scan
  * (index/covering/FilterIndexRule.scala:135-149; CoveringIndexRuleUtils.scala:98-130). */
 int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
+/* One comparison range on one column, a conjunct of a filter: lo <= column <= hi (strict where lo_strict / hi_strict say
+ * so; has_lo / has_hi say which bounds exist, at least one must).  literal_type says which fields hold the bounds:
+ * HS_TYPE_INT64 -> lo_i / hi_i, HS_TYPE_DOUBLE -> lo_f / hi_f, HS_TYPE_STRING -> lo_bytes / hi_bytes (lo_len / hi_len bytes,
+ * at most 65535).  The comparison is Spark 3.1's after its binary-comparison coercion: it happens in the wider of the
+ * column's and the literal's types (int < long < float < double), so `int_col > 1.5` is `int_col >= 2`, a float column
+ * against a double literal compares (double)f, and a float column against a long literal casts the literal to float;
+ * NaN equals NaN and is greater than +inf, -0.0 equals 0.0 (SQLOrderingUtil.compareDoubles).  String columns take
+ * HS_TYPE_STRING literals only, numeric columns numeric ones; boolean columns are not handled (HS_EUNSUPPORTED). */
+typedef struct {
+  const char* column;            /* any column of the files: int32 / int64 / float / double / string */
+  int32_t literal_type;          /* HS_TYPE_INT64, HS_TYPE_DOUBLE or HS_TYPE_STRING */
+  int32_t has_lo, has_hi;
+  int32_t lo_strict, hi_strict;  /* 1: lo < x / x < hi; 0: inclusive */
+  int32_t reserved;
+  int64_t lo_i, hi_i;
+  double lo_f, hi_f;
+  const void* lo_bytes;
+  const void* hi_bytes;
+  uint32_t lo_len, hi_len;
+} hs_predicate;
+
+/* The scan FilterIndexRule substitutes (FilterIndexRule.scala:58-101), with the conjunction of preds (at most 16) as the
+ * filter: a row qualifies when every predicate holds, and a null never satisfies a bound.  spec gives files, sorted_on_key,
+ * key_column (the column the files are sorted on; may be NULL when sorted_on_key is 0), projection, deleted_file_ids and
+ * output; its own bounds (has_lo / has_hi) must be 0.  Sorted files are binary-searched on the predicates over key_column,
+ * and the other predicates are evaluated over the rows inside those windows only.  Float and double keys are handled here
+ * (hs_filter_scan, whose bounds are int64, refuses them). */
+int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
+                         hs_stats* stats, char* err, size_t errlen);
 
 typedef struct {
   const hs_source_file* left_files;  /* index files of the left side, any order; bucket id parsed from the name */
