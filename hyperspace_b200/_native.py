@@ -112,6 +112,7 @@ EXPORTED_SYMBOLS = [
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
+    "hs_bucket_join_where",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -163,6 +164,10 @@ def load_library() -> C.CDLL:
                                        C.POINTER(Stats), *err]
     L.hs_bucket_join.restype = C.c_int
     L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    L.hs_bucket_join_where.restype = C.c_int
+    L.hs_bucket_join_where.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
+                                       C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateSpec), C.c_int32,
+                                       C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_batch_num_rows.restype = C.c_int64
     L.hs_batch_num_rows.argtypes = [C.c_void_p]
     L.hs_batch_on_device.restype = C.c_int32
@@ -262,6 +267,35 @@ def _literal_type(lo, hi) -> int:
     if HS_TYPE_STRING in kinds and len(kinds) > 1:
         raise ValueError("a predicate cannot mix string and numeric bounds")
     return HS_TYPE_DOUBLE if HS_TYPE_DOUBLE in kinds else kinds.pop()
+
+
+def _predicate_array(predicates: Sequence[tuple]):
+    """``(column, lo, lo_strict, hi, hi_strict)`` tuples -> (hs_predicate array, count).  A range with an int bound and a
+    float bound becomes two comparisons, each in its own type."""
+    split = []
+    for column, lo, lo_strict, hi, hi_strict in predicates:
+        if lo is not None and hi is not None and {_literal_type(lo, None), _literal_type(None, hi)} == {HS_TYPE_INT64, HS_TYPE_DOUBLE}:
+            split += [(column, lo, lo_strict, None, False), (column, None, False, hi, hi_strict)]
+        else:
+            split.append((column, lo, lo_strict, hi, hi_strict))
+    preds = (PredicateSpec * max(1, len(split)))()
+    for p, (column, lo, lo_strict, hi, hi_strict) in zip(preds, split):
+        p.column = column.encode()
+        p.literal_type = _literal_type(lo, hi)
+        p.has_lo, p.has_hi = int(lo is not None), int(hi is not None)
+        p.lo_strict, p.hi_strict = int(bool(lo_strict)), int(bool(hi_strict))
+        for side, v in (("lo", lo), ("hi", hi)):
+            if v is None:
+                continue
+            if p.literal_type == HS_TYPE_STRING:
+                b = v.encode("utf-8") if isinstance(v, str) else bytes(v)
+                setattr(p, side + "_bytes", b)
+                setattr(p, side + "_len", len(b))
+            elif p.literal_type == HS_TYPE_INT64:
+                setattr(p, side + "_i", int(v))
+            else:
+                setattr(p, side + "_f", float(v))
+    return preds, len(split)
 
 
 def _source_array(files: Sequence[FileImage]):
@@ -665,39 +699,14 @@ class Context:
         dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
         spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
         spec.output = output
-        split = []  # an int bound and a float bound are two comparisons, each in its own type
-        for column, lo, lo_strict, hi, hi_strict in predicates:
-            if lo is not None and hi is not None and {_literal_type(lo, None), _literal_type(None, hi)} == {HS_TYPE_INT64, HS_TYPE_DOUBLE}:
-                split += [(column, lo, lo_strict, None, False), (column, None, False, hi, hi_strict)]
-            else:
-                split.append((column, lo, lo_strict, hi, hi_strict))
-        preds = (PredicateSpec * max(1, len(split)))()
-        for p, (column, lo, lo_strict, hi, hi_strict) in zip(preds, split):
-            p.column = column.encode()
-            p.literal_type = _literal_type(lo, hi)
-            p.has_lo, p.has_hi = int(lo is not None), int(hi is not None)
-            p.lo_strict, p.hi_strict = int(bool(lo_strict)), int(bool(hi_strict))
-            for side, v in (("lo", lo), ("hi", hi)):
-                if v is None:
-                    continue
-                if p.literal_type == HS_TYPE_STRING:
-                    b = v.encode("utf-8") if isinstance(v, str) else bytes(v)
-                    setattr(p, side + "_bytes", b)
-                    setattr(p, side + "_len", len(b))
-                elif p.literal_type == HS_TYPE_INT64:
-                    setattr(p, side + "_i", int(v))
-                else:
-                    setattr(p, side + "_f", float(v))
+        preds, n_preds = _predicate_array(predicates)
         res, st = C.c_void_p(), Stats()
         err = C.create_string_buffer(1024)
-        _check(L.hs_filter_scan_where(self._h, C.byref(spec), preds, len(split), C.byref(res), C.byref(st), err, len(err)), err)
+        _check(L.hs_filter_scan_where(self._h, C.byref(spec), preds, n_preds, C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
-    def bucket_join(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
-                    right_buckets: Sequence[int], num_buckets: int, left_key: str, right_key: str,
-                    left_columns: Sequence[str], right_columns: Sequence[str], output: int = HS_OUT_HOST
-                    ) -> Tuple[Batch, Dict[str, float]]:
-        L = load_library()
+    def _join_spec(self, left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns, right_columns,
+                   output):
         ls, k1 = _source_array(left)
         rs, k2 = _source_array(right)
         lc, rc = _cstr_array(left_columns), _cstr_array(right_columns)
@@ -706,13 +715,45 @@ class Context:
         spec = JoinSpec()
         spec.left_files, spec.n_left, spec.right_files, spec.n_right = ls, len(left), rs, len(right)
         spec.left_buckets, spec.right_buckets, spec.num_buckets = lb, rb, num_buckets
-        spec.left_key, spec.right_key = left_key.encode(), right_key.encode()
+        spec.left_key = left_key.encode() if left_key is not None else None
+        spec.right_key = right_key.encode() if right_key is not None else None
         spec.left_columns, spec.n_left_columns = lc, len(left_columns)
         spec.right_columns, spec.n_right_columns = rc, len(right_columns)
         spec.output = output
+        return spec, (ls, k1, rs, k2, lc, rc, lb, rb)
+
+    def bucket_join(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                    right_buckets: Sequence[int], num_buckets: int, left_key: str, right_key: str,
+                    left_columns: Sequence[str], right_columns: Sequence[str], output: int = HS_OUT_HOST
+                    ) -> Tuple[Batch, Dict[str, float]]:
+        L = load_library()
+        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns,
+                                     right_columns, output)
         res, st = C.c_void_p(), Stats()
         err = C.create_string_buffer(1024)
         _check(L.hs_bucket_join(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
+    def bucket_join_where(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                          right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                          left_columns: Sequence[str], right_columns: Sequence[str], left_predicates: Sequence[tuple] = (),
+                          right_predicates: Sequence[tuple] = (), output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_where: inner join on left_keys[k] == right_keys[k] for every k (in the order of the indexes' indexed
+        columns), keeping on each side only the rows where every predicate of that side holds.  Predicates are
+        filter_scan_where's ``(column, lo, lo_strict, hi, hi_strict)`` tuples.  Rows with a null key join nothing.  The
+        side selection's time is in ``ms_exchange``."""
+        L = load_library()
+        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
+                                     right_columns, output)
+        lk, rk = _cstr_array(left_keys), _cstr_array(right_keys)
+        if len(left_keys) != len(right_keys):
+            raise ValueError("left_keys and right_keys must pair up")
+        lp, nlp = _predicate_array(left_predicates)
+        rp, nrp = _predicate_array(right_predicates)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_bucket_join_where(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, rp, nrp, C.byref(res), C.byref(st),
+                                      err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------

@@ -850,12 +850,12 @@ __global__ void k_widen_i32(const int32_t* __restrict__ in, int64_t n, int64_t* 
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
 }
 
-static const int64_t* widened_key(hs_ctx* ctx, const DevColumn& c, int64_t n, Buf<int64_t>* hold) {
-  if (c.type == HS_TYPE_INT64) return (const int64_t*)c.data.get();
+static const int64_t* widened_key(hs_ctx* ctx, const DevColumn& c, const void* data, int64_t n, Buf<int64_t>* hold) {
+  if (c.type == HS_TYPE_INT64) return (const int64_t*)data;
   if (c.type != HS_TYPE_INT32) fail(HS_EUNSUPPORTED, "key column '%s' must be int32 or int64 on the read side", c.name.c_str());
   hold->alloc(ctx, std::max<int64_t>(1, n));
   if (n) {
-    k_widen_i32<<<(int)std::min<int64_t>(ceil_div(n, 256), ctx->sm_count * 16), 256, 0, ctx->stream>>>((const int32_t*)c.data.get(), n,
+    k_widen_i32<<<(int)std::min<int64_t>(ceil_div(n, 256), ctx->sm_count * 16), 256, 0, ctx->stream>>>((const int32_t*)data, n,
                                                                                                       hold->get());
     HS_LAUNCH_CHECK(ctx);
   }
@@ -1209,6 +1209,25 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
   return rc;
 }
 
+// The refusals of a predicate list that need no data (hs_filter_scan_where, hs_bucket_join_where): HS_OK or the code,
+// with stats zeroed and the message in err
+static int check_predicates(const hs_predicate* preds, int n_preds, hs_stats* stats, char* err, size_t errlen) {
+  auto refuse = [&](int code, const char* msg, const char* what) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, msg, what);
+    return code;
+  };
+  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
+  for (int i = 0; i < n_preds; i++) {
+    const hs_predicate& p = preds[i];
+    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
+    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
+    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING)
+      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
+  }
+  return HS_OK;
+}
+
 extern "C" {
 
 int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
@@ -1242,23 +1261,32 @@ int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predica
   };
   if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
   if (spec->has_lo || spec->has_hi) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
-  for (int i = 0; i < n_preds; i++) {
-    const hs_predicate& p = preds[i];
-    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
-    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
-    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING)
-      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
-  }
+  const int rc = check_predicates(preds, n_preds, stats, err, errlen);
+  if (rc != HS_OK) return rc;
   return filter_scan_core(ctx, spec, preds, n_preds, false, out, stats, err, errlen);
 }
 
+}  // extern "C"
+
+// One side of a bucket join: its rows bucket-major and ascending on the key columns.  perm maps a sorted position to a
+// row of t (nullptr: the identity, every bucket is one index file); after the side selection it lists only the rows
+// that can take part in the join, still in sorted order, and seg holds the buckets' new boundaries.
+struct JoinSide {
+  SourceSet src;  // string values are references into the file images: kept alive until the result batch exists
+  Table t;
+  IndexedRows rows;
+  std::vector<uint64_t> seg;  // nb+1 sorted positions
+  const uint32_t* perm = nullptr;
+  Buf<uint32_t> iota, kept;
+  int64_t n = 0;  // rows in sorted order
+};
+
 // Orders the decoded rows of one join side bucket-major and key-sorted.  When every bucket holds exactly one file the
 // files are already sorted (they are index files) and only need to be visited in bucket order; otherwise the rows go
-// through K2-K4 again, which is what Spark's SortExec does for multi-file buckets.
-static void prepare_join_side(hs_ctx* ctx, SourceSet* src, const hs_source_file* files, int n_files, const int32_t* buckets, int nb,
-                              const std::vector<std::string>& cols, Table* t, IndexedRows* rows, hs_stats* st,
-                              std::vector<uint64_t>* seg, const int64_t** d_keys, const uint32_t** d_perm, Buf<uint32_t>* iota,
-                              Buf<int64_t>* k64) {
+// through K2-K4 again on all n_keys key columns, which is what Spark's SortExec does for multi-file buckets.
+// cols: the n_keys key columns first, then the projected and the predicate columns.
+static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file* files, int n_files, const int32_t* buckets, int nb,
+                              const std::vector<std::string>& cols, int n_keys, bool nulls_refused, hs_stats* st) {
   // reorder files by bucket so the decoded table is bucket-major
   std::vector<int> order(n_files);
   for (int i = 0; i < n_files; i++) order[i] = i;
@@ -1270,49 +1298,60 @@ static void prepare_join_side(hs_ctx* ctx, SourceSet* src, const hs_source_file*
     if (buckets[order[i]] < 0 || buckets[order[i]] >= nb) fail(HS_EINVAL, "bucket id %d out of range", buckets[order[i]]);
     per_bucket[buckets[order[i]]]++;
   }
-  // string values are references into the file images: the caller's SourceSet keeps those alive until the result batch exists
-  open_sources(ctx, sorted_files.data(), n_files, src, st);
-  decode_sources(ctx, *src, cols, nullptr, t, st);
-  if (!t->has_strings) src->release_images();
-  const bool str_key = t->cols[0].type == HS_TYPE_STRING;
-  if (!str_key && t->cols[0].type != HS_TYPE_INT64 && t->cols[0].type != HS_TYPE_INT32)
-    fail(HS_EUNSUPPORTED, "bucket join: key column must be int32, int64 or string");
-  if (t->cols[0].has_nulls) fail(HS_EUNSUPPORTED, "bucket join: null join keys are not handled yet");
+  Table* t = &side->t;
+  open_sources(ctx, sorted_files.data(), n_files, &side->src, st);
+  decode_sources(ctx, side->src, cols, nullptr, t, st);
+  if (!t->has_strings) side->src.release_images();
+  for (int k = 0; k < n_keys; k++) {
+    const int ty = t->cols[k].type;
+    if (ty != HS_TYPE_STRING && ty != HS_TYPE_INT64 && ty != HS_TYPE_INT32)
+      fail(HS_EUNSUPPORTED, "bucket join: key column must be int32, int64 or string");
+    if (nulls_refused && t->cols[k].has_nulls) fail(HS_EUNSUPPORTED, "bucket join: null join keys are not handled yet");
+  }
   const bool single = std::all_of(per_bucket.begin(), per_bucket.end(), [](int c) { return c <= 1; });
   if (single) {
-    seg->assign(nb + 1, 0);
+    side->seg.assign(nb + 1, 0);
     int fi = 0;
     for (int b = 0; b < nb; b++) {
-      (*seg)[b] = (uint64_t)t->file_row_begin[fi];
+      side->seg[b] = (uint64_t)t->file_row_begin[fi];
       if (per_bucket[b]) fi++;
     }
-    (*seg)[nb] = (uint64_t)t->nrows;
-    *d_keys = str_key ? (const int64_t*)t->cols[0].data.get() : widened_key(ctx, t->cols[0], t->nrows, k64);
-    iota->alloc(ctx, std::max<int64_t>(1, t->nrows));
-    launch_iota_u32(ctx, iota->get(), t->nrows);
-    *d_perm = iota->get();
+    side->seg[nb] = (uint64_t)t->nrows;
   } else {
-    index_rows(ctx, *t, 1, nb, rows, st);
-    *seg = rows->bucket_offsets;
-    // materialise the sorted key column
-    const int kw = rows->part.cols[0].width;
-    const int ktype = rows->part.cols[0].type;
-    Buf<uint8_t> sk(ctx, (size_t)std::max<int64_t>(1, rows->part.nrows) * kw);
-    launch_gather_plain(ctx, rows->part.cols[0].data.get(), rows->sorted.perm(), rows->part.nrows, kw, sk.get());
+    IndexedRows* rows = &side->rows;
+    index_rows(ctx, *t, n_keys, nb, rows, st);
+    side->seg = rows->bucket_offsets;
     rows->sorted.keys_buf[rows->sorted.cur ^ 1].release();  // the sort's scratch keys
     t->cols.clear();
     t->cols = std::move(rows->part.cols);
     t->nrows = rows->part.nrows;
-    // keep the sorted keys in a column appended at the end
-    DevColumn kc;
-    kc.name = "__sorted_key";
-    kc.type = ktype;
-    kc.width = kw;
-    kc.data = std::move(sk);
-    t->cols.push_back(std::move(kc));
-    *d_keys = str_key ? (const int64_t*)t->cols.back().data.get() : widened_key(ctx, t->cols.back(), t->nrows, k64);
-    *d_perm = rows->sorted.perm();
+    side->perm = rows->sorted.perm();
   }
+  side->n = t->nrows;
+}
+
+// Side selection: keeps the rows whose key columns are all non-null and where every predicate of the side holds.  The
+// predicates run over the sorted positions as their candidate list, so the compacted rows stay in sorted order and a
+// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps is empty.
+static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, int nb) {
+  if (ps.n == 0) return;
+  const int64_t n = side->n;
+  Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
+  Buf<uint64_t> offs(ctx, n + 1);
+  launch_predicate_mask(ctx, ps, side->perm, n, mask.get());
+  exclusive_scan_u32_u64(ctx, mask.get(), n, offs.get());
+  std::vector<uint32_t> bounds(nb + 1);
+  for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
+  Buf<uint32_t> d_bounds(ctx, nb + 1);
+  Buf<uint64_t> d_seg(ctx, nb + 1);
+  copy_h2d(ctx, d_bounds.get(), bounds.data(), 4 * (nb + 1));
+  launch_gather_plain(ctx, offs.get(), d_bounds.get(), nb + 1, 8, d_seg.get());
+  copy_d2h(ctx, side->seg.data(), d_seg.get(), 8 * (nb + 1));
+  sync_stream(ctx);
+  side->n = (int64_t)side->seg[nb];
+  side->kept.alloc(ctx, std::max<int64_t>(1, side->n));
+  launch_compact_indices(ctx, mask.get(), offs.get(), n, side->perm, side->kept.get());
+  side->perm = side->kept.get();
 }
 
 __global__ void k_compose_u32(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, int64_t n, uint32_t* out) {
@@ -1321,9 +1360,12 @@ __global__ void k_compose_u32(const uint32_t* __restrict__ a, const uint32_t* __
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = a[b[i]];
 }
 
-int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
-  if (!ctx || !spec || !out) return HS_EINVAL;
-  *out = nullptr;
+// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  A one-key join
+// probes with k_join_count over int64 (int32 keys widened) or string references; several keys go through
+// k_join_count_keys over sort_encode values and references.
+static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                            int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
+                            int n_right_preds, bool legacy, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   hs_stats st;
   memset(&st, 0, sizeof st);
   std::unique_ptr<hs_batch> res(new hs_batch());
@@ -1334,44 +1376,118 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
     total.start();
     const int nb = spec->num_buckets;
     if (nb < 1) fail(HS_EINVAL, "num_buckets must be positive");
-    std::vector<std::string> lcols{spec->left_key}, rcols{spec->right_key};
-    std::vector<int> lproj, rproj;
-    for (int i = 0; i < spec->n_left_columns; i++) {
-      std::string nm = spec->left_columns[i];
-      auto it = std::find(lcols.begin(), lcols.end(), nm);
-      if (it == lcols.end()) { lcols.push_back(nm); lproj.push_back((int)lcols.size() - 1); }
-      else lproj.push_back((int)(it - lcols.begin()));
-    }
-    for (int i = 0; i < spec->n_right_columns; i++) {
-      std::string nm = spec->right_columns[i];
-      auto it = std::find(rcols.begin(), rcols.end(), nm);
-      if (it == rcols.end()) { rcols.push_back(nm); rproj.push_back((int)rcols.size() - 1); }
-      else rproj.push_back((int)(it - rcols.begin()));
-    }
-    Table lt, rt;
-    IndexedRows lrows, rrows;
-    std::vector<uint64_t> lseg, rseg;
-    const int64_t *lkeys = nullptr, *rkeys = nullptr;
-    const uint32_t *lperm = nullptr, *rperm = nullptr;
-    Buf<uint32_t> liota, riota;
+    // columns to decode: the keys first, then the projection, then the predicate columns
+    auto side_columns = [&](const char* const* keys, const char* const* proj, int n_proj, const hs_predicate* preds, int n_preds,
+                            std::vector<int>* proj_idx, std::vector<int>* pred_idx) {
+      std::vector<std::string> cols;
+      for (int k = 0; k < n_keys; k++) {
+        if (!keys[k]) fail(HS_EINVAL, "bucket join: missing key column");
+        if (std::find(cols.begin(), cols.end(), keys[k]) != cols.end()) fail(HS_EINVAL, "bucket join: key column '%s' given twice", keys[k]);
+        cols.push_back(keys[k]);
+      }
+      auto col_of = [&](const std::string& nm) {
+        auto it = std::find(cols.begin(), cols.end(), nm);
+        if (it != cols.end()) return (int)(it - cols.begin());
+        cols.push_back(nm);
+        return (int)cols.size() - 1;
+      };
+      for (int i = 0; i < n_proj; i++) proj_idx->push_back(col_of(proj[i]));
+      for (int i = 0; i < n_preds; i++) pred_idx->push_back(col_of(preds[i].column));
+      return cols;
+    };
+    std::vector<int> lproj, rproj, lpred, rpred;
+    const std::vector<std::string> lcols = side_columns(left_keys, spec->left_columns, spec->n_left_columns, left_preds, n_left_preds, &lproj, &lpred);
+    const std::vector<std::string> rcols = side_columns(right_keys, spec->right_columns, spec->n_right_columns, right_preds, n_right_preds, &rproj, &rpred);
+    JoinSide L, R;
+    prepare_join_side(ctx, &L, spec->left_files, spec->n_left, spec->left_buckets, nb, lcols, n_keys, legacy, &st);
+    prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, n_keys, legacy, &st);
+    // hashInt and hashLong put equal values into different buckets: both sides must have been bucketed on the same types
+    // (JoinIndexRule only pairs indexes whose indexed columns have the same data types)
+    for (int k = 0; k < n_keys; k++)
+      if (L.t.cols[k].type != R.t.cols[k].type) {
+        if (n_keys == 1) fail(HS_EUNSUPPORTED, "bucket join: key columns have different types");
+        fail(HS_EUNSUPPORTED, "bucket join: key columns '%s' and '%s' have different types", left_keys[k], right_keys[k]);
+      }
+    if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
+    // side selection: IS NOT NULL on the nullable key columns, then the side's predicates
+    std::vector<Buf<uint8_t>> bound_bytes;
+    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx) {
+      PredSet ps;
+      for (int k = 0; k < n_keys; k++) {
+        const DevColumn& c = s.t.cols[k];
+        if (c.has_nulls) {
+          PredDesc d{};
+          d.data = c.data.get(), d.valid = c.valid.get(), d.r.type = c.type;
+          ps.p[ps.n++] = d;
+        }
+      }
+      for (size_t i = 0; i < pred_idx.size(); i++) {
+        const DevColumn& c = s.t.cols[pred_idx[i]];
+        ResolvedPredicate rp;
+        const PredRange r = resolve_predicate(ctx, preds[i], c, &bound_bytes, &rp);
+        ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, r};
+      }
+      return ps;
+    };
+    const PredSet lps = side_preds(L, left_preds, lpred), rps = side_preds(R, right_preds, rpred);
+    StageTimer t_sel(ctx);
+    t_sel.start();
+    select_join_side(ctx, &L, lps, nb);
+    select_join_side(ctx, &R, rps, nb);
+    t_sel.stop();
+    // the key columns in (selected) sorted order
+    Buf<uint8_t> lsorted, rsorted;
     Buf<int64_t> lk64, rk64;
-    SourceSet lsrc, rsrc;
-    prepare_join_side(ctx, &lsrc, spec->left_files, spec->n_left, spec->left_buckets, nb, lcols, &lt, &lrows, &st, &lseg, &lkeys, &lperm, &liota, &lk64);
-    prepare_join_side(ctx, &rsrc, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, &rt, &rrows, &st, &rseg, &rkeys, &rperm, &riota, &rk64);
-    // hashInt and hashLong put equal values into different buckets: both sides must have been bucketed on the same type
-    // (JoinIndexRule only pairs indexes whose indexed columns have the same data type)
-    if (lt.cols[0].type != rt.cols[0].type) fail(HS_EUNSUPPORTED, "bucket join: key columns have different types");
-    const int64_t nl = lt.nrows, nr = rt.nrows;
-    if (nr >= (1ll << 32) || nl >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
+    std::vector<Buf<uint64_t>> key_bufs;
+    Buf<unsigned long long> or_and(ctx, 2);  // k_encode_keys reduces into it; unused here
+    auto one_key = [&](const JoinSide& s, Buf<uint8_t>* sorted, Buf<int64_t>* k64) {
+      const DevColumn& c = s.t.cols[0];
+      const void* data = c.data.get();
+      if (s.perm) {  // materialise the sorted key column
+        sorted->alloc(ctx, (size_t)std::max<int64_t>(1, s.n) * c.width);
+        launch_gather_plain(ctx, data, s.perm, s.n, c.width, sorted->get());
+        data = sorted->get();
+      }
+      return c.type == HS_TYPE_STRING ? (const int64_t*)data : widened_key(ctx, c, data, s.n, k64);
+    };
+    auto key_tuples = [&](const JoinSide& s) {
+      JoinKeyCols kc{};
+      kc.n = n_keys;
+      for (int k = 0; k < n_keys; k++) {
+        const DevColumn& c = s.t.cols[k];
+        if (c.type == HS_TYPE_STRING) {
+          kc.str_mask |= 1u << k;
+          if (!s.perm) {
+            kc.col[k] = (const uint64_t*)c.data.get();
+            continue;
+          }
+          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n));
+          launch_gather_plain(ctx, c.data.get(), s.perm, s.n, 8, key_bufs.back().get());
+        } else {
+          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n));
+          launch_encode_keys(ctx, c.data.get(), c.type, s.perm, s.n, key_bufs.back().get(), or_and.get());
+        }
+        kc.col[k] = key_bufs.back().get();
+      }
+      return kc;
+    };
+    const int64_t nl = L.n;
     StageTimer t_join(ctx);
     t_join.start();
     Buf<uint64_t> d_lseg(ctx, nb + 1), d_rseg(ctx, nb + 1);
-    copy_h2d(ctx, d_lseg.get(), lseg.data(), 8 * (nb + 1));
-    copy_h2d(ctx, d_rseg.get(), rseg.data(), 8 * (nb + 1));
+    copy_h2d(ctx, d_lseg.get(), L.seg.data(), 8 * (nb + 1));
+    copy_h2d(ctx, d_rseg.get(), R.seg.data(), 8 * (nb + 1));
     Buf<uint32_t> counts(ctx, std::max<int64_t>(1, nl)), first(ctx, std::max<int64_t>(1, nl));
     Buf<uint64_t> offs(ctx, nl + 1);
-    launch_join_count(ctx, lkeys, d_lseg.get(), rkeys, d_rseg.get(), nb, nl, counts.get(), first.get(),
-                      lt.cols[0].type == HS_TYPE_STRING);
+    if (n_keys == 1) {
+      const int64_t* lkeys = one_key(L, &lsorted, &lk64);
+      const int64_t* rkeys = one_key(R, &rsorted, &rk64);
+      launch_join_count(ctx, lkeys, d_lseg.get(), rkeys, d_rseg.get(), nb, nl, counts.get(), first.get(),
+                        L.t.cols[0].type == HS_TYPE_STRING);
+    } else {
+      const JoinKeyCols lk = key_tuples(L), rk = key_tuples(R);
+      launch_join_count_keys(ctx, lk, d_lseg.get(), rk, d_rseg.get(), nb, nl, counts.get(), first.get());
+    }
     exclusive_scan_u32_u64(ctx, counts.get(), nl, offs.get());
     uint64_t total_out = 0;
     copy_d2h(ctx, &total_out, offs.get() + nl, 8);
@@ -1379,21 +1495,28 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
     if (total_out >= (1ull << 32)) fail(HS_EUNSUPPORTED, "join output larger than 2^32-1 rows per call");
     Buf<uint32_t> li(ctx, std::max<uint64_t>(1, total_out)), ri(ctx, std::max<uint64_t>(1, total_out));
     launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, li.get(), ri.get());
-    // positions in sorted order -> rows of the partitioned tables
+    // positions in sorted order -> rows of the decoded (or partitioned) tables
+    for (JoinSide* s : {&L, &R})
+      if (!s->perm) {
+        s->iota.alloc(ctx, std::max<int64_t>(1, s->n));
+        launch_iota_u32(ctx, s->iota.get(), s->n);
+        s->perm = s->iota.get();
+      }
     Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
     if (total_out) {
       const int grid = (int)std::min<int64_t>(ceil_div((int64_t)total_out, 256), ctx->sm_count * 16);
-      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(lperm, li.get(), (int64_t)total_out, lrow.get());
+      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(L.perm, li.get(), (int64_t)total_out, lrow.get());
       HS_LAUNCH_CHECK(ctx);
-      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(rperm, ri.get(), (int64_t)total_out, rrow.get());
+      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(R.perm, ri.get(), (int64_t)total_out, rrow.get());
       HS_LAUNCH_CHECK(ctx);
     }
     t_join.stop();
-    batch_from_gather(ctx, lt, lproj, lrow.get(), (int64_t)total_out, res.get());
-    batch_from_gather(ctx, rt, rproj, rrow.get(), (int64_t)total_out, res.get());
+    batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
+    batch_from_gather(ctx, R.t, rproj, rrow.get(), (int64_t)total_out, res.get());
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
+    if (lps.n || rps.n) st.ms_exchange += t_sel.ms();
     st.rows_out = (int64_t)total_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;
@@ -1401,6 +1524,36 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
   if (stats) *stats = st;
   if (rc == HS_OK) *out = res.release();
   return rc;
+}
+
+extern "C" {
+
+int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  if (!ctx || !spec || !out) return HS_EINVAL;
+  *out = nullptr;
+  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, true, out, stats, err, errlen);
+}
+
+int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                         int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate* right_preds,
+                         int32_t n_right_preds, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
+      (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
+    return HS_EINVAL;
+  *out = nullptr;
+  auto refuse = [&](int code, const char* msg) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "%s", msg);
+    return code;
+  };
+  if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
+  if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
+  if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
+  int rc = check_predicates(left_preds, n_left_preds, stats, err, errlen);
+  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, stats, err, errlen);
+  if (rc != HS_OK) return rc;
+  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, false,
+                          out, stats, err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

@@ -350,6 +350,7 @@ void launch_synth_column(hs_ctx* ctx, int col, int64_t first_row, int64_t n, voi
 // lo > hi is an empty range); string / binary columns compare the value with the references lo / hi (device copies of the
 // bound bytes) in UTF8String byte order, strictly where lo_strict / hi_strict say so.
 constexpr int kMaxPredicates = 16;
+constexpr int kMaxJoinKeys = 8;
 struct PredRange {
   int32_t type;
   int32_t has_lo, has_hi, lo_strict, hi_strict;
@@ -358,10 +359,10 @@ struct PredRange {
 struct PredDesc {
   const void* data;      // column values (string references for strings)
   const uint8_t* valid;  // nullptr: no nulls; a null never satisfies a predicate
-  PredRange r;
+  PredRange r;           // neither bound: the row only has to be non-null (a join side's key columns)
 };
 struct PredSet {
-  PredDesc p[kMaxPredicates];
+  PredDesc p[kMaxPredicates + kMaxJoinKeys];  // a join side: its predicates plus one IS NOT NULL per nullable key column
   int n = 0;
 };
 // per sorted segment s (ascending on `keys`): bounds[2s] = first row inside r, bounds[2s+1] = first row above r
@@ -374,6 +375,15 @@ void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* ca
 // string_keys: lkeys / rkeys hold string references (device_utils.cuh) compared in byte order
 void launch_join_count(hs_ctx* ctx, const int64_t* lkeys, const uint64_t* lseg, const int64_t* rkeys,
                        const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match, bool string_keys = false);
+// the same over several key columns (k_join_count_keys): col[k][p] is key column k at sorted position p, a sort_encode
+// value, or a string reference when bit k of str_mask is set; the tuples compare column by column
+struct JoinKeyCols {
+  const uint64_t* col[kMaxJoinKeys];
+  int32_t n;
+  uint32_t str_mask;
+};
+void launch_join_count_keys(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
+                            const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match);
 void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
                       int64_t nl, uint32_t* out_li, uint32_t* out_ri);
 // exclusive scan of uint32 counts into uint64 offsets (n+1 entries; last = total)

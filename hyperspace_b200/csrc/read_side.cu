@@ -6,7 +6,8 @@
 // K8 replaces the bucketed scan + SortMergeJoinExec (no ShuffleExchangeExec) Spark plans after
 // JoinIndexRule.applyIndex (index/covering/JoinIndexRule.scala:653-687): bucket b of the left index joins bucket b of
 // the right index; every left row binary-searches its match range in the right bucket, a scan turns match counts into
-// output offsets, and a second kernel emits the (left row, right row) pairs in (left, right) order.
+// output offsets, and a second kernel emits the (left row, right row) pairs in (left, right) order.  A join on several
+// key columns searches on the key tuples, compared column by column (k_join_count_keys).
 #include "device_utils.cuh"
 #include "kernels.h"
 
@@ -147,6 +148,48 @@ __global__ void k_join_count(const int64_t* __restrict__ lkeys, const uint64_t* 
       l = upper_bound_i64(rkeys + rb, rn, k);
     }
     counts[i] = (uint32_t)(l - f);
+    first_match[i] = (uint32_t)(rb + f);
+  }
+}
+
+// left row i against right row j on every key column, in order: -1 / 0 / +1
+__device__ __forceinline__ int compare_key_tuples(const JoinKeyCols& l, int64_t i, const JoinKeyCols& r, int64_t j) {
+  for (int k = 0; k < l.n; k++) {
+    const uint64_t a = l.col[k][i], b = r.col[k][j];
+    const int c = (l.str_mask >> k) & 1u ? string_compare(a, b) : (a < b ? -1 : (a > b ? 1 : 0));
+    if (c) return c;
+  }
+  return 0;
+}
+
+// k_join_count over several key columns: the right rows of a bucket are ascending on the key tuples, so the matches of a
+// left row are the range between two lexicographic binary searches
+__global__ void k_join_count_keys(const __grid_constant__ JoinKeyCols lk, const uint64_t* __restrict__ lseg,
+                                  const __grid_constant__ JoinKeyCols rk, const uint64_t* __restrict__ rseg, int nseg,
+                                  int64_t nl, uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
+    int lo = 0, hi = nseg;  // last segment with lseg[s] <= i
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (lseg[mid] <= (uint64_t)i) lo = mid;
+      else hi = mid;
+    }
+    const int64_t rb = (int64_t)rseg[lo], rn = (int64_t)rseg[lo + 1] - rb;
+    int64_t x = 0, y = rn;  // first right row >= the left tuple
+    while (x < y) {
+      const int64_t mid = x + ((y - x) >> 1);
+      if (compare_key_tuples(lk, i, rk, rb + mid) > 0) x = mid + 1;
+      else y = mid;
+    }
+    const int64_t f = x;
+    y = rn;  // first right row > the left tuple
+    while (x < y) {
+      const int64_t mid = x + ((y - x) >> 1);
+      if (compare_key_tuples(lk, i, rk, rb + mid) >= 0) x = mid + 1;
+      else y = mid;
+    }
+    counts[i] = (uint32_t)(x - f);
     first_match[i] = (uint32_t)(rb + f);
   }
 }
@@ -336,6 +379,14 @@ void launch_join_count(hs_ctx* ctx, const int64_t* lkeys, const uint64_t* lseg, 
     k_join_count<true><<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
   else
     k_join_count<false><<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_join_count_keys(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
+                            const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
+  KernelScope _ks(ctx, "k_join_count_keys");
+  if (nl == 0) return;
+  k_join_count_keys<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
   HS_LAUNCH_CHECK(ctx);
 }
 

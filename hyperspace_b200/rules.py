@@ -7,7 +7,7 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan_where (K1 + K7) and hs_bucket_join (K1 + K8).
+Physical execution is the C ABI: hs_filter_scan_where (K1 + K7) and hs_bucket_join_where (K1 + K8).
 """
 from __future__ import annotations
 
@@ -227,11 +227,15 @@ class ScanExec:
 
 
 class BucketJoinExec:
-    """Join of two index scans bucket by bucket (no exchange), or of two on-the-fly bucketed sides when no index applies."""
+    """Join of two index scans bucket by bucket (no exchange), or of two on-the-fly bucketed sides when no index applies.
+    ``keys`` are the (left, right) key pairs in the order both sides are bucketed and sorted on: the left index's indexed
+    columns when the indexes serve, the condition's order otherwise; None when the condition is not a one-to-one equi-join
+    between the two sides, which the GPU join cannot run.  A filter below a side becomes that side's predicates."""
 
-    def __init__(self, session, left: Linear, right: Linear, lkey: str, rkey: str, lcand: Optional[Candidate],
-                 rcand: Optional[Candidate]):
-        self.session, self.left, self.right, self.lkey, self.rkey, self.lcand, self.rcand = session, left, right, lkey, rkey, lcand, rcand
+    def __init__(self, session, left: Linear, right: Linear, keys: Optional[List[Tuple[str, str]]], lcand: Optional[Candidate],
+                 rcand: Optional[Candidate], condition: Optional[List[Tuple[str, str]]] = None):
+        self.session, self.left, self.right, self.keys, self.lcand, self.rcand = session, left, right, keys, lcand, rcand
+        self.condition = condition if condition is not None else keys
 
     def describe(self) -> str:
         def side(c, lin):
@@ -239,17 +243,21 @@ class BucketJoinExec:
                 return f"GpuShuffle(files={len(lin.relation.files)})"
             return f"Hyperspace(Type: CI, Name: {c.entry.name}, LogVersion: {c.entry.id})"
 
-        return f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, exchange=none)"
+        keys = ", ".join(f"{l} = {r}" for l, r in (self.keys or self.condition or []))
+        filters = "".join(f", {n}Filter={lin.predicate.conjuncts()}" for n, lin in (("left", self.left), ("right", self.right))
+                          if lin.predicate)
+        return f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, keys=[{keys}]{filters}, exchange=none)"
 
-    def _side(self, lin: Linear, cand: Optional[Candidate], key: str, nb: int):
+    def _side(self, lin: Linear, cand: Optional[Candidate], keys: List[str], nb: int):
         """(file images, bucket ids, temporaries to free)."""
         from . import _native
 
         ctx = self.session.gpu
         temps = []
-        cols = [c for c in lin.referenced() if c.lower() != key.lower()]
+        low = {k.lower() for k in keys}
+        cols = [c for c in lin.referenced() if c.lower() not in low]
         if cand is None:
-            res, _ = ctx.create_index(_file_images([f[0] for f in lin.relation.files]), [key], cols, nb, output=_native.HS_OUT_DEVICE)
+            res, _ = ctx.create_index(_file_images([f[0] for f in lin.relation.files]), keys, cols, nb, output=_native.HS_OUT_DEVICE)
             temps.append(res)
             return res.as_sources(), [f.bucket for f in res.files], temps
         files = list(cand.entry.index_files)
@@ -258,20 +266,24 @@ class BucketJoinExec:
         if cand.deleted_ids:
             raise LE.HyperspaceException("join over an index with deleted source files needs refreshIndex first")
         if cand.appended:  # BucketUnion(index scan, repartitioned appended rows): CoveringIndexRuleUtils.scala:256-284
-            res, _ = ctx.create_index(_file_images([f[0] for f in cand.appended]), [key], cols, nb, output=_native.HS_OUT_DEVICE)
+            res, _ = ctx.create_index(_file_images([f[0] for f in cand.appended]), keys, cols, nb, output=_native.HS_OUT_DEVICE)
             temps.append(res)
             images += res.as_sources()
             buckets += [f.bucket for f in res.files]
         return images, buckets, temps
 
     def execute(self) -> Dict[str, np.ndarray]:
+        if self.keys is None:
+            raise LE.HyperspaceException(f"join condition {self.condition} is not a one-to-one equi-join between the two sides")
         nb = self.lcand.entry.numBuckets if self.lcand else (self.rcand.entry.numBuckets if self.rcand else self.session.conf.num_buckets)
-        li, lb, lt = self._side(self.left, self.lcand, self.lkey, nb)
-        ri, rb, rt = self._side(self.right, self.rcand, self.rkey, nb)
+        lkeys, rkeys = [l for l, _ in self.keys], [r for _, r in self.keys]
+        li, lb, lt = self._side(self.left, self.lcand, lkeys, nb)
+        ri, rb, rt = self._side(self.right, self.rcand, rkeys, nb)
         try:
-            lcols = self.left.output
-            rcols = self.right.output
-            batch, _ = self.session.gpu.bucket_join(li, lb, ri, rb, nb, self.lkey, self.rkey, lcols, rcols)
+            lp = self.left.predicate.conjuncts() if self.left.predicate else []
+            rp = self.right.predicate.conjuncts() if self.right.predicate else []
+            batch, _ = self.session.gpu.bucket_join_where(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                          lp, rp)
         finally:
             for t in lt + rt:
                 t.free()
@@ -342,29 +354,60 @@ def filter_index_rule(session, lin: Linear) -> Optional[Candidate]:
     return rank_filter_candidates(session, good)
 
 
-def join_index_rule(session, left: Linear, right: Linear, lkey: str, rkey: str):
-    """JoinIndexRule: join columns == indexed columns on both sides, each index covers its side's referenced columns
-    (JoinIndexRule.scala:325-513); pairs ranked by rank_join_pairs.  The GPU merge join needs both sides bucketed alike,
-    so only the best EQUAL-bucket pair is used (the reference would re-shuffle one side of an unequal pair; here the
-    query then runs without indexes)."""
+def join_key_pairs(left: Linear, right: Linear, pairs: Sequence[Tuple[str, str]]) -> Optional[List[Tuple[str, str]]]:
+    """JoinAttributeFilter (JoinIndexRule.scala:164-170, 262-301): every equality must compare a column of the left side
+    with one of the right side, in either orientation, and the columns must map one to one; repeated equalities collapse
+    (names match case-insensitively).  Returns the (left, right) pairs in condition order, or None."""
+    lcols = {c.lower(): c for c in left.relation.column_names}
+    rcols = {c.lower(): c for c in right.relation.column_names}
+    out, seen, l2r, r2l = [], set(), {}, {}
+    for a, b in pairs:
+        if a.lower() in lcols and b.lower() in rcols:
+            l, r = lcols[a.lower()], rcols[b.lower()]
+        elif b.lower() in lcols and a.lower() in rcols:
+            l, r = lcols[b.lower()], rcols[a.lower()]
+        else:
+            return None  # both columns on one side (or unknown)
+        if l2r.setdefault(l.lower(), r.lower()) != r.lower() or r2l.setdefault(r.lower(), l.lower()) != l.lower():
+            return None  # not one-to-one
+        if (l.lower(), r.lower()) not in seen:
+            seen.add((l.lower(), r.lower()))
+            out.append((l, r))
+    return out
+
+
+def join_index_rule(session, left: Linear, right: Linear, keys: Sequence[Tuple[str, str]]):
+    """JoinIndexRule over the (left, right) key pairs of join_key_pairs: JoinColumnFilter -- an index's indexed columns
+    equal its side's key columns as a set, and it covers every column its side references, filter columns included
+    (JoinIndexRule.scala:399-463); JoinRankFilter -- a pair is compatible only when the right index's indexed columns are
+    the left index's, mapped through the keys, in the same order (JoinIndexRule.scala:569-616); pairs ranked by
+    rank_join_pairs.  The GPU merge join needs both sides bucketed alike, so only the best EQUAL-bucket pair is used (the
+    reference would re-shuffle one side of an unequal pair; here the query then runs without indexes)."""
     # (an index whose source lost files would need the lineage NOT-IN filter below the merge join, which the GPU join does
     # not apply: such a candidate is skipped and the query falls back to the next pair / to no index, as the fail-open rule
     # layer of the reference would -- ApplyHyperspace.scala:57-64)
+    lset, rset = {l.lower() for l, _ in keys}, {r.lower() for _, r in keys}
+    l2r = {l.lower(): r.lower() for l, r in keys}
     lc = [c for c in candidates_for(session, left.relation)
-          if [x.lower() for x in c.entry.indexedColumns] == [lkey.lower()] and _covers(c.entry, left.referenced())
-          and not c.deleted_ids]
+          if {x.lower() for x in c.entry.indexedColumns} == lset and len(c.entry.indexedColumns) == len(lset)
+          and _covers(c.entry, left.referenced()) and not c.deleted_ids]
     rc = [c for c in candidates_for(session, right.relation)
-          if [x.lower() for x in c.entry.indexedColumns] == [rkey.lower()] and _covers(c.entry, right.referenced())
-          and not c.deleted_ids]
+          if {x.lower() for x in c.entry.indexedColumns} == rset and len(c.entry.indexedColumns) == len(rset)
+          and _covers(c.entry, right.referenced()) and not c.deleted_ids]
+
     # Spark's analyzer puts a Cast on one side when the key types differ, and a condition over a Cast is not the plain
     # attribute equality the rule asks for (JoinIndexRule.scala:143-163): no index then.  It also matters physically:
     # hashInt and hashLong (and hashUnsafeBytes) send equal values to different buckets.
     def key_type(lin: Linear, key: str):
         return next((t for n, t in lin.relation.schema if n.lower() == key.lower()), None)
 
-    if key_type(left, lkey) != key_type(right, rkey):
+    if any(key_type(left, l) != key_type(right, r) for l, r in keys):
         return None
-    ranked = rank_join_pairs(session, [(a, b) for a in lc for b in rc])
+
+    def compatible(a: Candidate, b: Candidate) -> bool:
+        return [l2r[x.lower()] for x in a.entry.indexedColumns] == [x.lower() for x in b.entry.indexedColumns]
+
+    ranked = rank_join_pairs(session, [(a, b) for a in lc for b in rc if compatible(a, b)])
     if not ranked or ranked[0][0].entry.numBuckets != ranked[0][1].entry.numBuckets:
         return None
     return ranked[0]
@@ -382,19 +425,24 @@ def plan_query(session, plan):
         l, r = _linear(node.left), _linear(node.right)
         if l is None or r is None:
             raise LE.HyperspaceException("only joins of linear plans (Project?(Filter?(Relation))) are handled")
-        if l.predicate or r.predicate:
-            raise LE.HyperspaceException("filters below a join are not handled by the GPU join yet")
-        if post_project is not None:  # column pruning: each side scans only what the final projection needs + its key
+        keys = join_key_pairs(l, r, node.pairs)
+        if post_project is not None:  # column pruning: each side outputs only what the final projection needs + its keys
             lout, rout = l.output, r.output
             lneed = [c for c in post_project if c in lout]
             rneed = [c for c in post_project if c not in lout and c in rout]
             missing = [c for c in post_project if c not in lout and c not in rout]
             if missing:
                 raise LE.HyperspaceException(f"cannot resolve columns {missing}")
-            l = Linear(l.relation, None, lneed + ([node.left_key] if node.left_key not in lneed else []))
-            r = Linear(r.relation, None, rneed + ([node.right_key] if node.right_key not in rneed else []))
-        pair = join_index_rule(session, l, r, node.left_key, node.right_key) if enabled else None
-        op = BucketJoinExec(session, l, r, node.left_key, node.right_key, pair[0] if pair else None, pair[1] if pair else None)
+            # the filter stays on its side: its columns are read, not output
+            lk = [a for a, _ in keys] if keys else []
+            rk = [b for _, b in keys] if keys else []
+            l = Linear(l.relation, l.predicate, lneed + [k for k in lk if k not in lneed])
+            r = Linear(r.relation, r.predicate, rneed + [k for k in rk if k not in rneed])
+        pair = join_index_rule(session, l, r, keys) if enabled and keys else None
+        if pair:  # both sides bucketed and sorted in the left index's column order
+            order = [x.lower() for x in pair[0].entry.indexedColumns]
+            keys = sorted(keys, key=lambda p: order.index(p[0].lower()))
+        op = BucketJoinExec(session, l, r, keys, pair[0] if pair else None, pair[1] if pair else None, list(node.pairs))
         if post_project is not None:
             return _Projected(op, post_project)
         return op

@@ -11,6 +11,7 @@ notebooks of the shape used in the reference's docs/tests to run unchanged again
     session.enableHyperspace()
     df.filter(col("k").between(0, 100)).select("k", "v1").collect()
     a.join(b, on="k").select(...).collect()
+    a.filter(col("v") > 0).join(b, on=[("k1", "k1"), ("k2", "key2")]).collect()
 
 Every scan, filter and join runs on the GPU through the C ABI (no CPU fallback); the plan layer only decides which
 files the native call reads -- the same decision FilterIndexRule / JoinIndexRule make (hyperspace_b200/rules.py).
@@ -233,10 +234,11 @@ class ProjectNode:
 
 @dataclass
 class JoinNode:
+    """Inner equi-join on the AND of ``left column == right column`` for every pair (a pair may name its columns in
+    either order; rules.join_key_pairs orients them)."""
     left: object
     right: object
-    left_key: str
-    right_key: str
+    pairs: List[Tuple[str, str]]
 
 
 _SPARK_TYPE_OF_ARROW = {"int32": "integer", "int64": "long", "float": "float", "double": "double", "bool": "boolean",
@@ -313,8 +315,28 @@ class DataFrame:
     def join(self, other: "DataFrame", on, how: str = "inner") -> "DataFrame":
         if how != "inner":
             raise LE.HyperspaceException("only inner equi-joins are handled by the GPU path")
-        lk, rk = (on, on) if isinstance(on, str) else on
-        return DataFrame(self.session, JoinNode(self.plan, other.plan, self._resolve(lk), other._resolve(rk)))
+        if isinstance(on, str):
+            pairs = [(on, on)]
+        elif isinstance(on, tuple) and len(on) == 2 and all(isinstance(c, str) for c in on):
+            pairs = [on]
+        else:
+            pairs = list(on)
+            if not pairs or not all(isinstance(p, (tuple, list)) and len(p) == 2 for p in pairs):
+                raise LE.HyperspaceException("join `on` takes a column name, a (left, right) pair or a list of such pairs")
+        return DataFrame(self.session, JoinNode(self.plan, other.plan, [self._join_pair(other, a, b) for a, b in pairs]))
+
+    def _join_pair(self, other: "DataFrame", a: str, b: str) -> Tuple[str, str]:
+        """Resolves one equality of a join condition: (this side, other side) when it reads so, else swapped, else (for a
+        pair whose columns are on the same side, which no index can serve) both on the side that has them."""
+        def has(df, c):
+            return any(x.lower() == c.lower() for x in df.columns)
+
+        if has(self, a) and has(other, b):
+            return self._resolve(a), other._resolve(b)
+        if has(other, a) and has(self, b):
+            return self._resolve(b), other._resolve(a)
+        side = self if has(self, a) and has(self, b) else other
+        return side._resolve(a), side._resolve(b)
 
     # ---- introspection ------------------------------------------------------------------------------------
     @property

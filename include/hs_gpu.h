@@ -59,7 +59,7 @@ extern "C" {
 #define HS_TYPE_DOUBLE 3
 #define HS_TYPE_BOOL 4
 #define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): indexed and included columns (one GPU), filter scan keys and
-                            predicates, single-column join keys; compared in UTF8String byte order */
+                            predicates, join keys (alone or with other key columns); compared in UTF8String byte order */
 
 typedef struct hs_ctx hs_ctx;
 typedef struct hs_index_result hs_index_result;
@@ -288,6 +288,22 @@ typedef struct {
  * after JoinIndexRule.applyIndex (index/covering/JoinIndexRule.scala:653-687; T/index/E2EHyperspaceRulesTest.scala:487-512).
  * Buckets holding several files (after an incremental refresh) are merged first, as Spark's SortExec would. */
 int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
+/* The same join on n_keys (1..8) AND-ed equalities left_keys[k] == right_keys[k], with a filter below each side -- the
+ * joins JoinIndexRule rewrites (JoinIndexRule.scala:164-170 conditions, 569-616 column orders; T/index/covering/
+ * JoinIndexRuleTest.scala:84-95 puts a Filter under both sides).  The keys come in the order of the indexes' indexed
+ * columns: the left index's order, and the right columns they map to; both sides must have been bucketed and sorted on
+ * the keys in that order.  Key columns are int32 / int64 / string, of the same type at each position (float, double and
+ * boolean keys: HS_EUNSUPPORTED; n_keys > 8: HS_EUNSUPPORTED; n_keys < 1: HS_EINVAL).  A row whose key has a null in any
+ * column joins nothing, as in Spark's inner join.  left_preds / right_preds (at most 16 each) are conjunctions with the
+ * semantics and refusals of hs_filter_scan_where; a row joins only when every predicate of its side holds.  Files,
+ * buckets, projection and output come from spec, whose left_key / right_key must be NULL.  Output: the pairs in (bucket,
+ * left sorted position, right sorted position) order, as hs_bucket_join.  With one key, no predicates and no nulls in the
+ * keys this runs exactly what hs_bucket_join runs.  stats->ms_exchange (a one-GPU join exchanges nothing) reports the
+ * side selection: the null and predicate masks and the compaction of both sides. */
+int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                         int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate* right_preds,
+                         int32_t n_right_preds, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
 
 int64_t hs_batch_num_rows(const hs_batch* b);
 int32_t hs_batch_on_device(const hs_batch* b); /* != 0: the column pointers are device pointers (output = HS_OUT_DEVICE) */
