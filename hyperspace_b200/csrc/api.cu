@@ -614,26 +614,10 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
       if (spec->lineage) fill_lineage(ctx, table, spec->files, spec->n_files);
       if (spec->n_deleted_file_ids > 0) drop_deleted_rows(ctx, table, spec->deleted_file_ids, spec->n_deleted_file_ids);
       IndexedRows rows;
-      if (p2p_exchange_supported(ctx, spec->num_buckets)) {
-        // partition + exchange fused over NVLink peer memory, then the local sort
-        exchange_partition_p2p(ctx, table, spec->n_indexed, spec->num_buckets, &rows, &st);
-        sort_partitioned_rows(ctx, spec->n_indexed, spec->num_buckets, &rows, &st, /*defer_settle=*/true);
-      } else {
-        if (ctx->world > 1) exchange_rows(ctx, table, spec->n_indexed, spec->num_buckets, &st);  // NCCL all-to-all
-        index_rows(ctx, table, spec->n_indexed, spec->num_buckets, &rows, &st, /*defer_settle=*/true);
-      }
-      // From here to the end of encode_segments the host does not wait for the GPU unless it has to: the sort kernels are
-      // queued, the verdict of the tie fix-up is on its way (settle_sort below), and the encoder lays the pages out on the
-      // host while the rows are still being sorted.
-      if (!has_strings) src.release_images();  // every column is materialised bucket-major now (string
-                                                         // references keep pointing into the images until the encode)
-
       EncodeRequest req;
       req.table = &rows.part;
-      req.d_perm = rows.sorted.perm();
-      req.d_sorted_keys = rows.sorted.keys();
+      req.key_sorted = true;
       req.plan = &rows.plan;
-      req.seg_offsets = rows.bucket_offsets;
       req.rows_per_page = spec->rows_per_page;
       req.rows_per_row_group = spec->rows_per_row_group;
       req.use_dictionary = spec->disable_dictionary == 0;
@@ -649,8 +633,37 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
         snprintf(nm, sizeof nm, "part-%05d-%s_%05d.c000%s.parquet", b, uuid.c_str(), b, req.codec == pq::SNAPPY ? ".snappy" : "");
         req.seg_names[b] = nm;
       }
-      req.probe = rows.probe.get();
-      encode_segments(ctx, req, &enc, &st);  // synchronises the stream before it returns
+      // The files are laid out before the sort when their layout does not depend on the sorted order: a local sort of a
+      // single integer key then stores the key straight into its pages (the sort calls this while its MSD scatter runs).
+      // Otherwise the host lays the pages out below, while the GPU still sorts.
+      EncodeLayout lay;
+      const KeyPagesFn layout_before_sort = [&]() -> const KeyPageDest* {
+        if (layout_needs_sorted_rows(rows.part)) return nullptr;
+        req.seg_offsets = rows.bucket_offsets;
+        req.probe = rows.probe.get();
+        layout_segments(ctx, req, &lay, &enc, &st);
+        return key_page_dest(lay, req, &enc);
+      };
+      if (p2p_exchange_supported(ctx, spec->num_buckets)) {
+        // partition + exchange fused over NVLink peer memory, then the local sort
+        exchange_partition_p2p(ctx, table, spec->n_indexed, spec->num_buckets, &rows, &st);
+        sort_partitioned_rows(ctx, spec->n_indexed, spec->num_buckets, &rows, &st, /*defer_settle=*/true, &layout_before_sort);
+      } else {
+        if (ctx->world > 1) exchange_rows(ctx, table, spec->n_indexed, spec->num_buckets, &st);  // NCCL all-to-all
+        index_rows(ctx, table, spec->n_indexed, spec->num_buckets, &rows, &st, /*defer_settle=*/true, &layout_before_sort);
+      }
+      // From here to the end of write_segments the host does not wait for the GPU unless it has to: the sort kernels are
+      // queued and the verdict of the tie fix-up is on its way (settle_sort below).
+      if (!has_strings) src.release_images();  // every column is materialised bucket-major now (string
+                                                         // references keep pointing into the images until the encode)
+      req.d_perm = rows.sorted.perm();
+      if (!rows.sorted.key_pages_written) req.d_sorted_keys = rows.sorted.keys();
+      if (!lay.impl) {
+        req.seg_offsets = rows.bucket_offsets;
+        req.probe = rows.probe.get();
+        layout_segments(ctx, req, &lay, &enc, &st);
+      }
+      write_segments(ctx, req, lay, rows.sorted.key_pages_written, &enc, &st);  // synchronises the stream before it returns
       if (settle_sort(ctx, &rows, &st)) {    // (rare) the fix-up gave up on a long run of equal key prefixes: the rows were sorted
         req.probe = nullptr;                 // again with full passes, so the pages are gathered again
         req.d_perm = rows.sorted.perm();

@@ -136,6 +136,10 @@ HS_HD uint64_t sort_encode(int type, uint64_t raw) {
   }
   return raw;
 }
+// inverse of sort_encode for the integer types (type 1: int64, else int32)
+__device__ __forceinline__ uint64_t sort_decode_int(int type, uint64_t e) {
+  return type == 1 ? (e ^ 0x8000000000000000ull) : (uint64_t)((uint32_t)e ^ 0x80000000u);
+}
 
 // Fibonacci hashing of a dictionary value's raw bits: one 64-bit multiply; the top bits of the product depend on every
 // input bit.  Shared by the device hash sets / look-up tables and the host code that builds the compact look-up table.

@@ -824,7 +824,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
 
 // ---------------------------------------------------------------------------------------------------------------------
 
-void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle) {
+void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle,
+                const KeyPagesFn* key_pages) {
   const int64_t nrows = table.nrows;
   const int ncols = (int)table.cols.size();
   if (num_buckets < 1 || num_buckets > kMaxBuckets)
@@ -931,10 +932,11 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
 
   stats->ms_hash += t_hash.ms();
   stats->ms_partition += t_part.ms();
-  sort_partitioned_rows(ctx, nkeys, num_buckets, out, stats, defer_settle);
+  sort_partitioned_rows(ctx, nkeys, num_buckets, out, stats, defer_settle, key_pages);
 }
 
-void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle) {
+void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle,
+                           const KeyPagesFn* key_pages) {
   auto t_sort = std::make_unique<StageTimer>(ctx);
   // ---- K4: segmented sort on the indexed columns (radix_sort.cu) -----------------------------------------------
   if (defer_settle && !out->probe) {
@@ -951,7 +953,8 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
     const DevColumn& c = out->part.cols[k];
     keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width};
   }
-  sort_rows(ctx, &out->plan, keys.data(), nkeys, out->have_key_bits ? out->key_or_and : nullptr, defer_settle, &out->sorted);
+  sort_rows(ctx, &out->plan, keys.data(), nkeys, out->have_key_bits ? out->key_or_and : nullptr, defer_settle, &out->sorted,
+            key_pages);
   t_sort->stop();
   if (out->sorted.queued) {  // no synchronisation here: the stage timers are read in settle_sort
     out->pending_timers.push_back(IndexedRows::DeferredTimer{std::move(t_sort), &hs_stats::ms_sort});
@@ -1007,20 +1010,96 @@ void launch_dictionary_probes(hs_ctx* ctx, const Table& part, bool use_dictionar
 
 // ---------------------------------------------------------------------------------------------------------------------
 
+namespace {
+
+struct ColDict {
+  bool use = false;
+  uint32_t bw = 0, ndict = 0, empty_index = 0, mask = 0;
+  Buf<unsigned long long> keys;       // owned when the set was built here
+  const unsigned long long* keys_ptr = nullptr;  // the hash set in use (own or the column's ready-made one)
+  Buf<uint8_t> entries;               // value -> code look-up table, 16-byte entries (upload_lookup_table)
+  size_t skel_off = 0, skel_len = 0;  // [dictionary page header][PLAIN values] inside the skeleton
+  std::vector<uint64_t> values;       // sorted dictionary (raw bits)
+};
+// every page of every file, in file order (needed only when the pages are compressed afterwards)
+struct PagePlan {
+  uint64_t hdr_off;   // arena offset of the page header
+  uint32_t hdr_len;   // Thrift header bytes
+  uint32_t body_len;  // page bytes behind the header
+};
+struct FilePlan {
+  int seg = 0;
+  int64_t rows = 0;
+  std::vector<pq::OutRowGroup> rgs;
+  std::vector<std::pair<size_t, size_t>> chunk_pages;  // per (row group, column): first page, page count
+};
+
+}  // namespace
+
+// what layout_segments decided and uploaded, for write_segments
+struct EncodeLayout::Impl {
+  explicit Impl(hs_ctx* ctx) : t_plan(ctx) {}
+  StageTimer t_plan;  // read at the end of write_segments (reading it synchronises)
+  int64_t P = 0;      // rows per page
+  std::vector<pq::SchemaColumn> schema;
+  std::string schema_json;
+  std::vector<std::vector<uint64_t>> tile_val_off, tile_def_off;  // nullable and string columns
+  std::vector<ColDict> dicts;
+  std::vector<int> carried_cols;  // by record slot
+  std::vector<StatPatch> stat_patches;
+  std::vector<uint8_t> skeleton;
+  std::vector<ByteCopy> copies;
+  bool compress = false;
+  std::vector<PagePlan> page_plans;
+  std::vector<FilePlan> file_plans;
+  uint64_t cursor = 0;
+  uint32_t page_counter = 0;
+  Buf<uint8_t> d_skel;
+  Buf<ByteCopy> d_copies;
+  Buf<uint32_t> d_page_begin;
+  Buf<uint64_t> d_pvo;  // ncols x page_counter
+  KeyPageDest key_dest{};
+};
+
+bool layout_needs_sorted_rows(const Table& table) {
+  for (const DevColumn& dc : table.cols)
+    if (dc.has_nulls || dc.type == HS_TYPE_STRING) return true;
+  return false;
+}
+
 void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, hs_stats* stats) {
+  EncodeLayout lay;
+  layout_segments(ctx, req, &lay, out, stats);
+  write_segments(ctx, req, lay, false, out, stats);
+}
+
+const KeyPageDest* key_page_dest(EncodeLayout& lay, const EncodeRequest& req, EncodedFiles* out) {
+  EncodeLayout::Impl& L = *lay.impl;
+  const DevColumn& dc = req.table->cols[0];
+  if (dc.has_nulls || L.dicts[0].use || (dc.type != HS_TYPE_INT32 && dc.type != HS_TYPE_INT64) || L.P > (int64_t)UINT32_MAX)
+    return nullptr;
+  L.key_dest = KeyPageDest{out->arena.get(), L.d_page_begin.get(), L.d_pvo.get(), (uint32_t)L.P, dc.width, dc.type};
+  return &L.key_dest;
+}
+
+void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, EncodedFiles* out, hs_stats* stats) {
+  (void)stats;
+  lay->impl = std::make_shared<EncodeLayout::Impl>(ctx);
+  EncodeLayout::Impl& L = *lay->impl;
   const Table& table = *req.table;
   const int ncols = (int)table.cols.size();
   const int nseg = (int)req.seg_offsets.size() - 1;
   int64_t P = req.rows_per_page > 0 ? req.rows_per_page : 131072;
   P = (int64_t)round_up((size_t)P, kSortTile);
-  StageTimer t_plan(ctx), t_enc(ctx);
-  t_plan.start();
+  L.P = P;
+  L.t_plan.start();
   for (int c = 0; c < ncols; c++) {
     const DevColumn& dc = table.cols[c];
     if (dc.width != 4 && dc.width != 8)
       fail(HS_EUNSUPPORTED, "column '%s': %d-byte values cannot be written by the GPU encoder yet", dc.name.c_str(), dc.width);
   }
-  std::vector<pq::SchemaColumn> schema(ncols);
+  std::vector<pq::SchemaColumn>& schema = L.schema;
+  schema.resize(ncols);
   for (int c = 0; c < ncols; c++) {
     schema[c] = table.cols[c].schema;
     schema[c].repetition = pq::OPTIONAL;  // Spark writes every column of a DataFrame read from Parquet as optional
@@ -1033,13 +1112,17 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
       case HS_TYPE_STRING: schema[c].type = pq::BYTE_ARRAY; break;  // converted type (UTF8 or none) comes from the source
     }
   }
-  const std::string schema_json = pq::spark_schema_json(schema);
+  L.schema_json = pq::spark_schema_json(schema);
+  const std::string& schema_json = L.schema_json;
 
   // nullable columns: per-tile non-null counts (tiles are kSortTile-aligned inside a segment and P is a multiple of
   // kSortTile, so a tile never straddles a page)
   const int64_t ntiles = req.plan->ntiles;
   std::vector<std::vector<uint32_t>> tile_valid(ncols), tile_bytes(ncols);  // tile_bytes: string columns only
-  std::vector<std::vector<uint64_t>> tile_val_off(ncols), tile_def_off(ncols);
+  std::vector<std::vector<uint64_t>>& tile_val_off = L.tile_val_off;
+  std::vector<std::vector<uint64_t>>& tile_def_off = L.tile_def_off;
+  tile_val_off.resize(ncols);
+  tile_def_off.resize(ncols);
   {
     std::vector<Buf<uint32_t>> d_counts(ncols), d_bytes(ncols);
     bool any = false;
@@ -1075,18 +1158,11 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
   const std::vector<uint32_t>& seg_tile_begin = req.plan->h_seg_tile_begin;
 
   // ---- dictionary analysis: distinct values of every non-null column, capped at kMaxDictEntries ---------------------
-  struct ColDict {
-    bool use = false;
-    uint32_t bw = 0, ndict = 0, empty_index = 0, mask = 0;
-    Buf<unsigned long long> keys;       // owned when the set was built here
-    const unsigned long long* keys_ptr = nullptr;  // the hash set in use (own or the column's ready-made one)
-    Buf<uint8_t> entries;               // value -> code look-up table, 16-byte entries (upload_lookup_table)
-    size_t skel_off = 0, skel_len = 0;  // [dictionary page header][PLAIN values] inside the skeleton
-    std::vector<uint64_t> values;       // sorted dictionary (raw bits)
-  };
-  std::vector<ColDict> dicts(ncols);
+  std::vector<ColDict>& dicts = L.dicts;
+  dicts.resize(ncols);
   const int64_t total_rows = table.nrows;
-  std::vector<int> carried_cols(kMaxCarried, -1);  // by record slot
+  std::vector<int>& carried_cols = L.carried_cols;
+  carried_cols.assign(kMaxCarried, -1);
   for (int c = 0; c < ncols; c++) {
     const DevColumn& dc = table.cols[c];
     if (!dc.carried) continue;  // late-materialised: the dictionary and the codes were fixed when the sources were decoded
@@ -1177,26 +1253,15 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
     }
   }
 
-  const bool stats_on_key = req.d_sorted_keys != nullptr && !table.cols[0].has_nulls &&
+  const bool stats_on_key = req.key_sorted && !table.cols[0].has_nulls &&
                             (table.cols[0].type == HS_TYPE_INT32 || table.cols[0].type == HS_TYPE_INT64);
-  std::vector<StatPatch> stat_patches;
-  std::vector<uint8_t> skeleton;
-  std::vector<ByteCopy> copies;
-  // every page of every file, in file order (needed only when the pages are compressed afterwards)
-  struct PagePlan {
-    uint64_t hdr_off;   // arena offset of the page header
-    uint32_t hdr_len;   // Thrift header bytes
-    uint32_t body_len;  // page bytes behind the header
-  };
-  struct FilePlan {
-    int seg = 0;
-    int64_t rows = 0;
-    std::vector<pq::OutRowGroup> rgs;
-    std::vector<std::pair<size_t, size_t>> chunk_pages;  // per (row group, column): first page, page count
-  };
-  const bool compress = req.codec == pq::SNAPPY;
-  std::vector<PagePlan> page_plans;
-  std::vector<FilePlan> file_plans;
+  std::vector<StatPatch>& stat_patches = L.stat_patches;
+  std::vector<uint8_t>& skeleton = L.skeleton;
+  std::vector<ByteCopy>& copies = L.copies;
+  L.compress = req.codec == pq::SNAPPY;
+  const bool compress = L.compress;
+  std::vector<PagePlan>& page_plans = L.page_plans;
+  std::vector<FilePlan>& file_plans = L.file_plans;
   auto header_len_at = [&](size_t skel_pos) -> uint32_t {  // length of the Thrift struct (page header) that starts there
     thrift::Reader r(skeleton.data() + skel_pos, skeleton.data() + skeleton.size());
     r.skip(thrift::T_STRUCT);
@@ -1205,8 +1270,8 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
   };
   std::vector<uint32_t> seg_page_begin(nseg + 1, 0);
   std::vector<std::vector<uint64_t>> page_value_offset(ncols);
-  uint64_t cursor = 0;
-  uint32_t page_counter = 0;
+  uint64_t& cursor = L.cursor;
+  uint32_t& page_counter = L.page_counter;
   auto emit = [&](uint64_t dst, size_t skel_begin) {
     copies.push_back(ByteCopy{dst, (uint32_t)skel_begin, (uint32_t)(skeleton.size() - skel_begin)});
   };
@@ -1392,19 +1457,47 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
   out->arena.alloc(ctx, std::max<uint64_t>(cursor, 16) + 64);
 
   // upload the plan
-  Buf<uint8_t> d_skel(ctx, std::max<size_t>(1, skeleton.size()));
-  Buf<ByteCopy> d_copies(ctx, std::max<size_t>(1, copies.size()));
-  Buf<uint32_t> d_page_begin(ctx, seg_page_begin.size());
-  Buf<uint64_t> d_pvo(ctx, std::max<size_t>(1, (size_t)ncols * page_counter));
+  L.d_skel.alloc(ctx, std::max<size_t>(1, skeleton.size()));
+  L.d_copies.alloc(ctx, std::max<size_t>(1, copies.size()));
+  L.d_page_begin.alloc(ctx, seg_page_begin.size());
+  L.d_pvo.alloc(ctx, std::max<size_t>(1, (size_t)ncols * page_counter));
   if (!skeleton.empty())
-    copy_h2d(ctx, d_skel.get(), skeleton.data(), skeleton.size());
+    copy_h2d(ctx, L.d_skel.get(), skeleton.data(), skeleton.size());
   if (!copies.empty())
-    copy_h2d(ctx, d_copies.get(), copies.data(), copies.size() * sizeof(ByteCopy));
-  copy_h2d(ctx, d_page_begin.get(), seg_page_begin.data(), seg_page_begin.size() * 4);
+    copy_h2d(ctx, L.d_copies.get(), copies.data(), copies.size() * sizeof(ByteCopy));
+  copy_h2d(ctx, L.d_page_begin.get(), seg_page_begin.data(), seg_page_begin.size() * 4);
   for (int c = 0; c < ncols; c++)
     if (page_counter)
-      copy_h2d(ctx, d_pvo.get() + (size_t)c * page_counter, page_value_offset[c].data(), (size_t)page_counter * 8);
-  t_plan.stop();
+      copy_h2d(ctx, L.d_pvo.get() + (size_t)c * page_counter, page_value_offset[c].data(), (size_t)page_counter * 8);
+  L.t_plan.stop();
+}
+
+void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bool key_pages_written, EncodedFiles* out,
+                    hs_stats* stats) {
+  EncodeLayout::Impl& L = *lay.impl;
+  const Table& table = *req.table;
+  const int ncols = (int)table.cols.size();
+  const int64_t ntiles = req.plan->ntiles;
+  const int64_t P = L.P;
+  const std::vector<pq::SchemaColumn>& schema = L.schema;
+  const std::string& schema_json = L.schema_json;
+  const std::vector<std::vector<uint64_t>>& tile_val_off = L.tile_val_off;
+  const std::vector<std::vector<uint64_t>>& tile_def_off = L.tile_def_off;
+  const std::vector<ColDict>& dicts = L.dicts;
+  const std::vector<int>& carried_cols = L.carried_cols;
+  const std::vector<StatPatch>& stat_patches = L.stat_patches;
+  const std::vector<uint8_t>& skeleton = L.skeleton;
+  const std::vector<ByteCopy>& copies = L.copies;
+  const bool compress = L.compress;
+  const std::vector<PagePlan>& page_plans = L.page_plans;
+  std::vector<FilePlan>& file_plans = L.file_plans;
+  uint64_t& cursor = L.cursor;
+  const uint32_t page_counter = L.page_counter;
+  const Buf<uint8_t>& d_skel = L.d_skel;
+  const Buf<ByteCopy>& d_copies = L.d_copies;
+  const Buf<uint32_t>& d_page_begin = L.d_page_begin;
+  const Buf<uint64_t>& d_pvo = L.d_pvo;
+  StageTimer t_enc(ctx);
 
   // ---- K5+K6 -----------------------------------------------------------------------------------------
   t_enc.start();
@@ -1438,6 +1531,7 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
                                     d_voff.get(), d_doff.get(), out->arena.get());
       continue;
     }
+    if (c == 0 && key_pages_written) continue;  // the sort stored the key into its pages
     if (c == 0 && req.d_sorted_keys && (dc.type == HS_TYPE_INT32 || dc.type == HS_TYPE_INT64)) gc.sorted_keys = req.d_sorted_keys;
     launch_gather_encode(ctx, req.plan->tiles.get(), req.plan->ntiles, req.plan->seg_start.get(), req.d_perm, gc,
                          d_page_begin.get(), P, out->arena.get());
@@ -1445,7 +1539,7 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
   if (!stat_patches.empty()) {
     Buf<StatPatch> d_sp(ctx, stat_patches.size());
     copy_h2d(ctx, d_sp.get(), stat_patches.data(), sizeof(StatPatch) * stat_patches.size());
-    launch_patch_key_stats(ctx, d_sp.get(), (int64_t)stat_patches.size(), req.d_sorted_keys, table.cols[0].type, out->arena.get());
+    launch_patch_key_stats(ctx, d_sp.get(), (int64_t)stat_patches.size(), req.d_perm, table.cols[0].data.get(), out->arena.get());
   }
   {  // dictionary columns, up to 8 per launch pair
     std::vector<int> dcols;
@@ -1650,7 +1744,7 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
     if (!patches2.empty()) {
       Buf<StatPatch> d_sp(ctx, patches2.size());
       copy_h2d(ctx, d_sp.get(), patches2.data(), sizeof(StatPatch) * patches2.size());
-      launch_patch_key_stats(ctx, d_sp.get(), (int64_t)patches2.size(), req.d_sorted_keys, table.cols[0].type, arena2.get());
+      launch_patch_key_stats(ctx, d_sp.get(), (int64_t)patches2.size(), req.d_perm, table.cols[0].data.get(), arena2.get());
     }
     sync_stream(ctx);  // (large plan arrays may have gone through cudaMemcpyAsync: keep them alive until here)
     out->arena = std::move(arena2);
@@ -1660,10 +1754,11 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
   }
   t_enc.stop();
   sync_stream(ctx);  // host plan vectors are about to go out of scope
-  stats->ms_plan += t_plan.ms();
+  stats->ms_plan += L.t_plan.ms();
   stats->ms_encode += t_enc.ms();
   stats->bytes_out += (int64_t)cursor;
   stats->files_out += (int32_t)out->files.size();
+  lay.impl.reset();
 }
 
 }  // namespace hs

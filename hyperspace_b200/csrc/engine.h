@@ -133,14 +133,17 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
 
 // K2-K4 on a decoded table whose first nkeys columns are the indexed columns.
 // defer_settle: the sort may be left queued (sort_rows' may_defer) -- the caller must call settle_sort() after its next
-// synchronisation
-void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false);
+// synchronisation.  key_pages (optional): passed on to sort_rows (kernels.h)
+void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false,
+                const KeyPagesFn* key_pages = nullptr);
 
 // K5+K6: encode every segment (bucket or source file) as one Parquet file image inside one device arena.
 struct EncodeRequest {
   const Table* table = nullptr;            // column values (indexed by perm)
   const uint32_t* d_perm = nullptr;        // sorted position -> row of `table`
-  const uint64_t* d_sorted_keys = nullptr; // optional: sorted encoded values of column 0 (integer key)
+  // optional: sorted encoded values of column 0 (integer key), streamed into its pages instead of gathered through d_perm
+  const uint64_t* d_sorted_keys = nullptr;
+  bool key_sorted = false;                 // column 0 is sorted inside every segment: its row groups carry min / max
   const SortPlan* plan = nullptr;          // tiles over the segments
   std::vector<uint64_t> seg_offsets;       // host, nseg+1
   std::vector<std::string> seg_names;      // file name per segment (empty segments produce no file)
@@ -158,6 +161,22 @@ struct EncodedFiles {
   std::vector<OutFile> files;
 };
 void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, hs_stats* stats);
+// encode_segments in two halves, so that an index build can lay its files out before it sorts and let the sort store the
+// key into its pages.  layout_segments: the dictionary decisions, the host page plan and skeleton, the arena (out->arena,
+// out->files) and the upload of the page tables; it needs the bucket sizes and req.plan, and the sorted rows (req.d_perm)
+// only for a table where layout_needs_sorted_rows() holds (nullable or string columns: their page sizes depend on the
+// order).  write_segments: the kernels that fill the pages, footer statistics and SNAPPY; key_pages_written: the sort
+// has stored column 0 already (to key_page_dest()).
+struct EncodeLayout {
+  struct Impl;  // engine.cu
+  std::shared_ptr<Impl> impl;
+};
+bool layout_needs_sorted_rows(const Table& table);
+void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, EncodedFiles* out, hs_stats* stats);
+// where column 0's PLAIN page bodies lie, or nullptr when it has none to store into (nulls, a dictionary, not an integer)
+const KeyPageDest* key_page_dest(EncodeLayout& lay, const EncodeRequest& req, EncodedFiles* out);
+void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bool key_pages_written, EncodedFiles* out,
+                    hs_stats* stats);
 
 // multi-GPU exchange (exchange.cu): redistributes the rows of `table` so that this rank holds exactly the rows of
 // the buckets it owns (owner(b) = b % world).  No-op when world == 1.
@@ -170,7 +189,8 @@ void comm_allgather_host(hs_ctx* ctx, const void* in, size_t bytes, void* out);
 bool p2p_exchange_supported(hs_ctx* ctx, int num_buckets);
 void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats);
 // K4 only: sorts out->part (already bucket-major, offsets in out->bucket_offsets) on the first nkeys columns.
-void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false);
+void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false,
+                           const KeyPagesFn* key_pages = nullptr);
 // settle_sorted_rows() plus the stage timers: true when the rows had to be sorted again (whatever was derived from
 // sorted.keys() / sorted.perm() must be redone)
 bool settle_sort(hs_ctx* ctx, IndexedRows* out, hs_stats* stats);

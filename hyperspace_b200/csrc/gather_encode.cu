@@ -16,11 +16,6 @@ namespace {
 
 constexpr int kThreads = 256;
 
-// inverse of sort_encode for the integer types
-__device__ __forceinline__ uint64_t sort_decode_int(int type, uint64_t e) {
-  return type == 1 ? (e ^ 0x8000000000000000ull) : (uint64_t)((uint32_t)e ^ 0x80000000u);
-}
-
 template <int W>
 __global__ void __launch_bounds__(kThreads) k_gather_encode(const SortTile* __restrict__ tiles,
                                                              const uint64_t* __restrict__ seg_start,
@@ -268,14 +263,16 @@ __global__ void __launch_bounds__(256) k_copy_blobs(const BlobCopy* __restrict__
 }
 
 // min / max statistics of the (sorted) indexed column: first and last key of every row group, written over the
-// placeholders the host left in the footer
-__global__ void k_patch_key_stats(const StatPatch* __restrict__ patches, int64_t n, const uint64_t* __restrict__ sorted_keys,
-                                  int key_type, uint8_t* __restrict__ arena) {
+// placeholders the host left in the footer.  The values come from the partitioned column through the permutation, which
+// every sort path writes (the page bodies would hold codes when the key is dictionary-encoded).
+__global__ void k_patch_key_stats(const StatPatch* __restrict__ patches, int64_t n, const uint32_t* __restrict__ perm,
+                                  const void* __restrict__ keys, uint8_t* __restrict__ arena) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const StatPatch p = patches[i];
-  const uint64_t vmin = sort_decode_int(key_type, sorted_keys[p.first_pos]);
-  const uint64_t vmax = sort_decode_int(key_type, sorted_keys[p.last_pos]);
+  const uint32_t rmin = perm[p.first_pos], rmax = perm[p.last_pos];
+  const uint64_t vmin = p.width == 8 ? ((const uint64_t*)keys)[rmin] : ((const uint32_t*)keys)[rmin];
+  const uint64_t vmax = p.width == 8 ? ((const uint64_t*)keys)[rmax] : ((const uint32_t*)keys)[rmax];
   for (int b = 0; b < p.width; b++) {
     const uint8_t lo = (uint8_t)(vmin >> (8 * b)), hi = (uint8_t)(vmax >> (8 * b));
     arena[p.min_off[0] + b] = lo;
@@ -399,10 +396,10 @@ void launch_scatter_bytes(hs_ctx* ctx, const ByteCopy* copies, int64_t n, const 
   HS_LAUNCH_CHECK(ctx);
 }
 
-void launch_patch_key_stats(hs_ctx* ctx, const StatPatch* patches, int64_t n, const uint64_t* sorted_keys, int key_type,
+void launch_patch_key_stats(hs_ctx* ctx, const StatPatch* patches, int64_t n, const uint32_t* perm, const void* keys,
                             uint8_t* arena) {
   if (n == 0) return;
-  k_patch_key_stats<<<(unsigned)ceil_div(n, 128), 128, 0, ctx->stream>>>(patches, n, sorted_keys, key_type, arena);
+  k_patch_key_stats<<<(unsigned)ceil_div(n, 128), 128, 0, ctx->stream>>>(patches, n, perm, keys, arena);
   HS_LAUNCH_CHECK(ctx);
 }
 

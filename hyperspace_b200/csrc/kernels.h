@@ -1,5 +1,7 @@
 // kernels.h -- host-callable launchers of the CUDA kernels (one .cu per stage).
 #pragma once
+#include <functional>
+
 #include "hs_common.h"
 
 namespace hs {
@@ -230,8 +232,20 @@ struct SortPlan {
 };
 // seg_offsets: host array of nseg+1 global offsets
 void build_sort_plan(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, SortPlan* plan);
+// Where the PLAIN page bodies of a single int32 / int64 key column lie in the encoder's arena, laid out before the sort:
+// the value at position lr of segment s goes to arena + page_value_offset[seg_page_begin[s] + lr / rows_per_page]
+// + (lr % rows_per_page) * width.  The local sort writes the decoded keys there itself (see sort_rows).
+struct KeyPageDest {
+  uint8_t* arena;
+  const uint32_t* seg_page_begin;     // device, per segment: its first page
+  const uint64_t* page_value_offset;  // device, per page: arena offset of the first value byte
+  uint32_t rows_per_page;             // a multiple of kSortTile
+  int32_t width;                      // 4 or 8
+  int32_t type;                       // HS_TYPE_INT32 / HS_TYPE_INT64
+};
 // The rows of a SortPlan in sorted order: at sorted position p, keys()[p] is the sort encoding of the first key column and
-// perm()[p] the row (the position in the plan's input order).
+// perm()[p] the row (the position in the plan's input order).  When the sort wrote the key pages (key_pages_written),
+// the final keys are not materialised and keys() is not valid.
 struct SortedRows {
   Buf<uint64_t> keys_buf[2];  // the pairs and scratch pairs of the same size: the sort passes move them back and forth
   Buf<uint32_t> perm_buf[2];
@@ -245,14 +259,21 @@ struct SortedRows {
   // after ctx->sync_count was queued_at; if it is set, the rows are sorted again on resort_bits
   uint64_t resort_bits = 0, queued_at = 0;
   uint32_t gave_up = 0;
+  bool key_pages_written = false;  // the sort stored the key into the pages of a KeyPageDest
 };
+// Lays the key's pages out on request: called at most once, by a sort that can store the key into its pages, as soon as
+// the sort has queued the work that does not depend on them.  Returns the destinations, or nullptr to have the sort
+// write keys() as usual.
+using KeyPagesFn = std::function<const KeyPageDest*()>;
 // Sorts the rows within every segment of `plan` stably by cols[0], then cols[1], ... (nulls first); row r of a column
 // is the row at position r of the plan's input.  Chooses the sort path (radix_sort.cu).  last_or_and (optional): OR / AND
 // of the sort encoding of cols[ncols - 1], when the caller has them already.  may_defer: the sort of a single null-free
 // key column may be left queued (out->queued) -- the host does not wait for it, and settle_sorted_rows() must run before
 // out is read, best after the caller's next synchronisation.  Otherwise the result is final in stream order.
+// key_pages (optional): a single null-free int32 / int64 key that takes k_local_sort asks it for the key's page
+// destinations and stores the decoded keys there instead of into keys() (out->key_pages_written).
 void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, const unsigned long long* last_or_and,
-               bool may_defer, SortedRows* out);
+               bool may_defer, SortedRows* out, const KeyPagesFn* key_pages = nullptr);
 // Settles a queued sort (a no-op otherwise).  True when the rows had to be sorted again: whatever was derived from
 // keys() / perm() must be redone.
 bool settle_sorted_rows(hs_ctx* ctx, SortPlan* plan, SortedRows* s);
@@ -327,7 +348,8 @@ struct StatPatch {        // min/max of the sorted key column of one row group
   uint64_t min_off[2], max_off[2];  // arena offsets of the footer placeholders
   int32_t width, pad;
 };
-void launch_patch_key_stats(hs_ctx* ctx, const StatPatch* patches, int64_t n, const uint64_t* sorted_keys, int key_type,
+// min / max = the key values (width bytes each, in `keys`) of the rows perm[first_pos] and perm[last_pos]
+void launch_patch_key_stats(hs_ctx* ctx, const StatPatch* patches, int64_t n, const uint32_t* perm, const void* keys,
                             uint8_t* arena);
 struct ByteCopy {
   uint64_t dst;  // arena offset

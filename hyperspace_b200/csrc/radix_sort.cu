@@ -404,6 +404,7 @@ __global__ void __launch_bounds__(256) k_fix_runs(const SortTile* __restrict__ t
 constexpr int kLocalSortCap = 12288;
 struct LocalSortItem {
   uint32_t start, count;  // a range of pairs that is sorted as a whole
+  uint32_t seg, seg_row;  // its segment, and the position of its first pair inside the segment
 };
 constexpr int kLocalThreads = 1024;
 constexpr int kLocalWarps = kLocalThreads / 32;
@@ -449,10 +450,12 @@ __device__ __forceinline__ void local_pass(LocalShared& sm, uint32_t count, int 
   __syncthreads();
 }
 
+// out_keys == nullptr: each sorted key is decoded and stored into its PLAIN page body instead (KeyPageDest).  Bodies are
+// width-aligned except on tiny pages (Thrift headers have odd sizes), where the value is stored byte by byte.
 template <typename Src>
 __global__ void __launch_bounds__(kLocalThreads, 1) k_local_sort(const LocalSortItem* __restrict__ items, Src src,
                                                                  uint64_t* __restrict__ out_keys,
-                                                                 uint32_t* __restrict__ out_vals) {
+                                                                 uint32_t* __restrict__ out_vals, KeyPageDest pages) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   LocalShared& sm = *reinterpret_cast<LocalShared*>(smem_raw);
   const LocalSortItem it = items[blockIdx.x];
@@ -546,21 +549,52 @@ __global__ void __launch_bounds__(kLocalThreads, 1) k_local_sort(const LocalSort
     }
   }
   __syncthreads();
+  if (out_keys) {
+#pragma unroll
+    for (int j = 0; j < kLocalItems; j++) {
+      const uint32_t i = j * kLocalThreads + threadIdx.x;
+      if (i < count) {
+        const uint32_t s = sm.slot[i];
+        out_keys[(uint64_t)it.start + i] = sm.keys[s];
+        out_vals[(uint64_t)it.start + i] = sm.vals[s];
+      }
+    }
+    return;
+  }
+  const uint64_t* pvo = pages.page_value_offset + pages.seg_page_begin[it.seg];
+  const uint32_t P = pages.rows_per_page;
 #pragma unroll
   for (int j = 0; j < kLocalItems; j++) {
     const uint32_t i = j * kLocalThreads + threadIdx.x;
     if (i < count) {
       const uint32_t s = sm.slot[i];
-      out_keys[(uint64_t)it.start + i] = sm.keys[s];
       out_vals[(uint64_t)it.start + i] = sm.vals[s];
+      const uint32_t lr = it.seg_row + i, page = lr / P;
+      uint8_t* dst = pages.arena + pvo[page] + (uint64_t)(lr - page * P) * pages.width;
+      const uint64_t v = sort_decode_int(pages.type, sm.keys[s]);
+      if (((uintptr_t)dst & (pages.width - 1)) != 0) {
+        for (int b = 0; b < pages.width; b++) dst[b] = (uint8_t)(v >> (8 * b));
+      } else if (pages.width == 8) {
+        *reinterpret_cast<uint64_t*>(dst) = v;
+      } else {
+        *reinterpret_cast<uint32_t*>(dst) = (uint32_t)v;
+      }
     }
   }
 }
 
+// pages != nullptr: the keys go into their pages, out_keys is not written
 template <typename Src>
 void launch_local_sort(hs_ctx* ctx, const std::vector<LocalSortItem>& items, Src src, uint64_t* out_keys,
-                       uint32_t* out_vals) {
+                       uint32_t* out_vals, const KeyPageDest* pages) {
   if (items.empty()) return;
+  KeyPageDest dest{};
+  if (pages) {
+    dest = *pages;
+    out_keys = nullptr;
+  } else if (!out_keys) {
+    fail(HS_EINVAL, "internal: local sort without a key destination");
+  }
   Buf<LocalSortItem> d_items(ctx, items.size());
   copy_h2d(ctx, d_items.get(), items.data(), items.size() * sizeof(LocalSortItem));
   static DeviceOnce attr_once;  // one per Src instantiation
@@ -571,7 +605,7 @@ void launch_local_sort(hs_ctx* ctx, const std::vector<LocalSortItem>& items, Src
   }
   KernelScope _ks(ctx, "k_local_sort");
   k_local_sort<Src><<<(unsigned)items.size(), kLocalThreads, sizeof(LocalShared), ctx->stream>>>(d_items.get(), src,
-                                                                                                 out_keys, out_vals);
+                                                                                                 out_keys, out_vals, dest);
   HS_LAUNCH_CHECK(ctx);
 }
 
@@ -653,21 +687,40 @@ void lsd_passes(hs_ctx* ctx, SortPlan* plan, SortedRows* s, uint64_t bits, const
   if (first) fail(HS_EINVAL, "sort: raw first-pass source given but no pass ran");
 }
 
+// The final sorted keys (keys_buf[cur]), allocated on first use: a sort that writes the key pages never needs them.
+uint64_t* final_keys(hs_ctx* ctx, SortedRows* s, int64_t n) {
+  Buf<uint64_t>& b = s->keys_buf[s->cur];
+  if (!b) b.alloc(ctx, std::max<int64_t>(1, n));
+  return b.get();
+}
+
+// The local sort's destinations: the key pages when key_pages (optional, see sort_rows) gives them, else the final keys.
+const KeyPageDest* key_destination(hs_ctx* ctx, const KeyPagesFn* key_pages, SortedRows* s, int64_t n) {
+  const KeyPageDest* pages = key_pages ? (*key_pages)() : nullptr;
+  if (!pages) final_keys(ctx, s, n);
+  s->key_pages_written = pages != nullptr;
+  return pages;
+}
+
 // Every segment (at most kLocalSortCap rows each) sorted completely on the raw key column in one HBM pass.
-void local_sort_segments(hs_ctx* ctx, const SortPlan& plan, const KeyColumn& raw, SortedRows* s) {
+void local_sort_segments(hs_ctx* ctx, const SortPlan& plan, const KeyColumn& raw, SortedRows* s,
+                         const KeyPagesFn* key_pages) {
   std::vector<LocalSortItem> items;
   for (int g = 0; g < plan.nseg; g++) {
     const uint64_t n = plan.h_seg_start[g + 1] - plan.h_seg_start[g];
-    if (n) items.push_back(LocalSortItem{(uint32_t)plan.h_seg_start[g], (uint32_t)n});
+    if (n) items.push_back(LocalSortItem{(uint32_t)plan.h_seg_start[g], (uint32_t)n, (uint32_t)g, 0});
   }
-  with_raw_source(raw, [&](auto src) { launch_local_sort(ctx, items, src, s->keys(), s->perm()); });
+  const KeyPageDest* pages = key_destination(ctx, key_pages, s, plan.n);
+  with_raw_source(raw, [&](auto src) { launch_local_sort(ctx, items, src, s->keys(), s->perm(), pages); });
 }
 
 // Complete sort of the raw key column within every segment in two HBM passes: one stable MSD pass on digit
 // (key >> shift) & 255 into the scratch pairs, then k_local_sort of every (segment, digit) sub-bucket back into the sorted
 // pairs.  The bits above shift + 7 must be constant over the input.  Returns false, having queued only the MSD histogram,
-// when a sub-bucket holds more than kLocalSortCap rows.  Synchronises the stream once.
-bool msd_local_sort(hs_ctx* ctx, SortPlan* plan, const KeyColumn& raw, int shift, SortedRows* s) {
+// when a sub-bucket holds more than kLocalSortCap rows.  Synchronises the stream once.  key_pages (optional, see sort_rows)
+// is asked for the page destinations while the MSD scatter runs, so that the caller's host work overlaps it.
+bool msd_local_sort(hs_ctx* ctx, SortPlan* plan, const KeyColumn& raw, int shift, SortedRows* s,
+                    const KeyPagesFn* key_pages) {
   if (plan->ntiles == 0) return false;
   const size_t nsub = (size_t)plan->nseg * 256;
   Buf<uint32_t> d_base(ctx, nsub);
@@ -680,13 +733,14 @@ bool msd_local_sort(hs_ctx* ctx, SortPlan* plan, const KeyColumn& raw, int shift
   // work items: consecutive whole sub-buckets of one segment, up to kLocalSortCap rows
   std::vector<LocalSortItem> items;
   for (int g = 0; g < plan->nseg; g++) {
-    LocalSortItem cur{base[(size_t)g * 256], 0};
+    const uint32_t seg_begin = base[(size_t)g * 256];
+    LocalSortItem cur{seg_begin, 0, (uint32_t)g, 0};
     for (size_t d = (size_t)g * 256; d < (size_t)(g + 1) * 256; d++) {
       const uint32_t sz = base[d + 1] - base[d];
       if (sz > (uint32_t)kLocalSortCap) return false;
       if (cur.count + sz > (uint32_t)kLocalSortCap) {
         items.push_back(cur);
-        cur = LocalSortItem{base[d], 0};
+        cur = LocalSortItem{base[d], 0, (uint32_t)g, base[d] - seg_begin};
       }
       cur.count += sz;
     }
@@ -695,7 +749,8 @@ bool msd_local_sort(hs_ctx* ctx, SortPlan* plan, const KeyColumn& raw, int shift
   uint64_t* keys_alt = s->keys_buf[s->cur ^ 1].get();
   uint32_t* perm_alt = s->perm_buf[s->cur ^ 1].get();
   with_raw_source(raw, [&](auto src) { run_scatter(ctx, plan, src, digit, keys_alt, perm_alt); });
-  launch_local_sort(ctx, items, SrcPairs{keys_alt, perm_alt}, s->keys(), s->perm());
+  const KeyPageDest* pages = key_destination(ctx, key_pages, s, plan->n);
+  launch_local_sort(ctx, items, SrcPairs{keys_alt, perm_alt}, s->keys(), s->perm(), pages);
   return true;
 }
 
@@ -756,13 +811,22 @@ void build_sort_plan(hs_ctx* ctx, const uint64_t* seg_offsets, int nseg, SortPla
 }
 
 void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, const unsigned long long* last_or_and,
-               bool may_defer, SortedRows* out) {
+               bool may_defer, SortedRows* out, const KeyPagesFn* key_pages) {
   const int64_t nrows = plan->n;
-  for (auto& b : out->keys_buf) b.alloc(ctx, std::max<int64_t>(1, nrows));
-  for (auto& b : out->perm_buf) b.alloc(ctx, std::max<int64_t>(1, nrows));
+  const bool lsd_only = getenv("HS_LSD_SORT") != nullptr;
+  // only a single null-free integer key can leave its final keys in the pages (sort_decode_int inverts its encoding)
+  if (ncols != 1 || cols[0].valid || (cols[0].type != HS_TYPE_INT32 && cols[0].type != HS_TYPE_INT64) || lsd_only)
+    key_pages = nullptr;
+  // the final keys (keys_buf[0]) are allocated once it is known that the sort does not write the key pages
   out->cur = 0;
+  out->keys_buf[1].alloc(ctx, std::max<int64_t>(1, nrows));
+  out->keys_buf[0].release();
+  auto need_keys = [&] { final_keys(ctx, out, nrows); };
+  if (!key_pages) need_keys();
+  for (auto& b : out->perm_buf) b.alloc(ctx, std::max<int64_t>(1, nrows));
   out->queued = false;
   out->resort_bits = 0;
+  out->key_pages_written = false;
   Buf<unsigned long long> d_or_and(ctx, 2);
   unsigned long long or_and[2] = {0, 0};
   // or_and = OR / AND of the encoded keys that launch(d_or_and) reduces, on the host (synchronises)
@@ -779,7 +843,6 @@ void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, co
   // (expected rows per prefix <= 0.5 for uniformly spread keys), at least 2.  5 M-row segments -> 3 bytes, 125 M-row -> 4.
   int want_bytes = 2;
   while (want_bytes < 8 && (double)max_seg / std::pow(256.0, want_bytes) > 0.5) want_bytes++;
-  const bool lsd_only = getenv("HS_LSD_SORT") != nullptr;
   for (int k = ncols - 1; k >= 0; k--) {
     const KeyColumn& kc = cols[k];
     // The first column sorted (the last key column) starts from rows in input order: its first radix pass reads the raw
@@ -818,6 +881,7 @@ void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, co
         }
       const KeyColumn* raw = from_raw ? &kc : nullptr;
       if (from_raw && varying == 0) {  // nothing to sort on: materialise the pairs as they stand
+        need_keys();
         launch_iota_u32(ctx, out->perm(), nrows);
         launch_encode_keys(ctx, kc.data, kc.type, nullptr, nrows, out->keys(), d_or_and.get());
         raw = nullptr;
@@ -831,12 +895,13 @@ void sort_rows(hs_ctx* ctx, SortPlan* plan, const KeyColumn* cols, int ncols, co
       bool local = false;
       if (raw && !kc.valid && !lsd_only) {
         if (max_seg <= (uint64_t)kLocalSortCap) {
-          local_sort_segments(ctx, *plan, kc, out);
+          local_sort_segments(ctx, *plan, kc, out, key_pages);
           local = true;
         } else if (nbytes > 2 && max_seg <= (uint64_t)(0.85 * 256 * kLocalSortCap)) {
-          local = msd_local_sort(ctx, plan, kc, std::max(0, 63 - __builtin_clzll(varying) - 7), out);
+          local = msd_local_sort(ctx, plan, kc, std::max(0, 63 - __builtin_clzll(varying) - 7), out, key_pages);
         }
       }
+      if (!out->key_pages_written) need_keys();
       if (local) {
         out->queued = defer;
       } else if (nbytes > want_bytes) {
