@@ -4,7 +4,7 @@
 
   (1) one key, k = k, SELECT L.v1, R.v2, through hs_bucket_join and through hs_bucket_join_where, alternating
   (2) two key columns (k, v3) = (k, v3): v3 = row % 100 is a function of the row like k, so the pairs and the 125 M-row
-      output are those of (1); the indexes are built on (k, v3) and the probe is k_join_count_keys
+      output are those of (1); the indexes are built on (k, v3) and k_join_count compares both columns
   (3) one key with a filter below each side: L.v3 < 10 and R.v1 < 100 (about 10 % of each side)
 
 Each workload runs --reps times; (1)'s two entry points alternate inside one process.  For each it reports ms per join,

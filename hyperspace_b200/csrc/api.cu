@@ -117,10 +117,6 @@ __global__ void k_fill_u64(uint64_t* out, int64_t n, uint64_t v) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = v;
 }
-__global__ void k_fill_u32(uint32_t* out, int64_t n, uint32_t v) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = v;
-}
 
 // CoveringIndex.createIndexData lineage (index/covering/CoveringIndex.scala:152-186): every row carries the id of the
 // source file it came from.
@@ -150,22 +146,10 @@ void drop_deleted_rows(hs_ctx* ctx, Table& t, const int64_t* deleted, int ndelet
   for (size_t c = 0; c < t.cols.size(); c++)
     if (t.cols[c].name == "_data_file_id") lc = (int)c;
   if (lc < 0) fail(HS_EINVAL, "deleted_file_ids given but the source has no _data_file_id column (index built without lineage)");
-  const int64_t n = t.nrows;
-  if (n == 0) return;
-  Buf<uint32_t> mask(ctx, n);
-  Buf<uint64_t> offs(ctx, n + 1);
-  Buf<int64_t> d_del(ctx, ndeleted);
-  copy_h2d(ctx, d_del.get(), deleted, sizeof(int64_t) * ndeleted);
-  k_fill_u32<<<(int)std::min<int64_t>(ceil_div(n, 256), ctx->sm_count * 8), 256, 0, ctx->stream>>>(mask.get(), n, 1u);
-  HS_LAUNCH_CHECK(ctx);
-  launch_not_in_mask(ctx, (const int64_t*)t.cols[lc].data.get(), n, d_del.get(), ndeleted, mask.get());
-  exclusive_scan_u32_u64(ctx, mask.get(), n, offs.get());
-  uint64_t kept = 0;
-  copy_d2h(ctx, &kept, offs.get() + n, 8);
-  sync_stream(ctx);
-  Buf<uint32_t> idx(ctx, std::max<uint64_t>(1, kept));
-  launch_compact_indices(ctx, mask.get(), offs.get(), n, nullptr, idx.get());
-  gather_table(ctx, t, idx.get(), (int64_t)kept);
+  if (t.nrows == 0) return;
+  Buf<uint32_t> idx;
+  const int64_t kept = select_rows(ctx, PredSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
+  gather_table(ctx, t, idx.get(), kept);
 }
 
 std::vector<std::string> names_of(const char* const* a, int na, const char* const* b, int nb) {
@@ -857,24 +841,6 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
   b->nrows = n_out;
 }
 
-// int32 join keys are widened once so that the join probes stay int64-only
-__global__ void k_widen_i32(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ out) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
-}
-
-static const int64_t* widened_key(hs_ctx* ctx, const DevColumn& c, const void* data, int64_t n, Buf<int64_t>* hold) {
-  if (c.type == HS_TYPE_INT64) return (const int64_t*)data;
-  if (c.type != HS_TYPE_INT32) fail(HS_EUNSUPPORTED, "key column '%s' must be int32 or int64 on the read side", c.name.c_str());
-  hold->alloc(ctx, std::max<int64_t>(1, n));
-  if (n) {
-    k_widen_i32<<<(int)std::min<int64_t>(ceil_div(n, 256), ctx->sm_count * 16), 256, 0, ctx->stream>>>((const int32_t*)data, n,
-                                                                                                      hold->get());
-    HS_LAUNCH_CHECK(ctx);
-  }
-  return hold->get();
-}
-
 __global__ void k_ranges_to_indices(const int64_t* __restrict__ bounds, const uint64_t* __restrict__ seg_offsets,
                                     const uint64_t* __restrict__ out_offsets, int nseg, uint32_t* __restrict__ out_idx) {
   // one CTA per segment
@@ -1168,42 +1134,17 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
         // residual: the predicates on other columns, over the window rows, compacted through the candidate list
         for (int i = 0; i < n_preds; i++)
           if (pred_col[i] != 0) resolve(i);
-        const PredSet ps = residual_set(true);
-        Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n_cand));
-        Buf<uint64_t> offs(ctx, n_cand + 1);
-        launch_predicate_mask(ctx, ps, idx.get(), n_cand, mask.get());
-        exclusive_scan_u32_u64(ctx, mask.get(), n_cand, offs.get());
-        uint64_t kept = 0;
-        copy_d2h(ctx, &kept, offs.get() + n_cand, 8);
-        sync_stream(ctx);
-        n_out = (int64_t)kept;
-        Buf<uint32_t> kept_idx(ctx, std::max<int64_t>(1, n_out));
-        launch_compact_indices(ctx, mask.get(), offs.get(), n_cand, idx.get(), kept_idx.get());
-        idx = std::move(kept_idx);
+        Buf<uint32_t> kept;
+        n_out = select_rows(ctx, residual_set(true), idx.get(), n_cand, nullptr, nullptr, 0, &kept);
+        idx = std::move(kept);
       }
-      sync_stream(ctx);
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
       for (int i = 0; i < n_preds; i++) resolve(i);
-      const PredSet ps = residual_set(false);
-      Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
-      Buf<uint64_t> offs(ctx, n + 1);
-      launch_predicate_mask(ctx, ps, nullptr, n, mask.get());
-      if (spec->n_deleted_file_ids > 0) {
-        Buf<int64_t> d_del(ctx, spec->n_deleted_file_ids);
-        copy_h2d(ctx, d_del.get(), spec->deleted_file_ids, 8 * spec->n_deleted_file_ids);
-        launch_not_in_mask(ctx, (const int64_t*)t.cols[lineage_col].data.get(), n, d_del.get(), spec->n_deleted_file_ids, mask.get());
-        sync_stream(ctx);
-      }
-      exclusive_scan_u32_u64(ctx, mask.get(), n, offs.get());
-      uint64_t kept = 0;
-      copy_d2h(ctx, &kept, offs.get() + n, 8);
-      sync_stream(ctx);
-      n_out = (int64_t)kept;
-      idx.alloc(ctx, std::max<int64_t>(1, n_out));
-      launch_compact_indices(ctx, mask.get(), offs.get(), n, nullptr, idx.get());
-      sync_stream(ctx);
+      const int64_t* file_ids = lineage_col >= 0 ? (const int64_t*)t.cols[lineage_col].data.get() : nullptr;
+      n_out = select_rows(ctx, residual_set(false), nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
     }
+    sync_stream(ctx);
     t_scan.stop();
     StageTimer t_gather(ctx);
     t_gather.start();
@@ -1223,14 +1164,17 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
 }
 
 // The refusals of a predicate list that need no data (hs_filter_scan_where, hs_bucket_join_where): HS_OK or the code,
-// with stats zeroed and the message in err
-static int check_predicates(const hs_predicate* preds, int n_preds, hs_stats* stats, char* err, size_t errlen) {
+// with stats zeroed and the message in err.  bounds_in_spec: hs_filter_scan_where was also given the bounds of
+// hs_filter_scan.
+static int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_in_spec, hs_stats* stats, char* err,
+                            size_t errlen) {
   auto refuse = [&](int code, const char* msg, const char* what) {
     if (stats) memset(stats, 0, sizeof *stats);
     if (err && errlen) snprintf(err, errlen, msg, what);
     return code;
   };
   if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
+  if (bounds_in_spec) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
   for (int i = 0; i < n_preds; i++) {
     const hs_predicate& p = preds[i];
     if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
@@ -1267,14 +1211,7 @@ int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predica
                          hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds)) return HS_EINVAL;
   *out = nullptr;
-  auto refuse = [&](int code, const char* msg, const char* what) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, msg, what);
-    return code;
-  };
-  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
-  if (spec->has_lo || spec->has_hi) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
-  const int rc = check_predicates(preds, n_preds, stats, err, errlen);
+  const int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
   if (rc != HS_OK) return rc;
   return filter_scan_core(ctx, spec, preds, n_preds, false, out, stats, err, errlen);
 }
@@ -1290,7 +1227,7 @@ struct JoinSide {
   IndexedRows rows;
   std::vector<uint64_t> seg;  // nb+1 sorted positions
   const uint32_t* perm = nullptr;
-  Buf<uint32_t> iota, kept;
+  Buf<uint32_t> kept;
   int64_t n = 0;  // rows in sorted order
 };
 
@@ -1348,11 +1285,9 @@ static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file*
 // bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps is empty.
 static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, int nb) {
   if (ps.n == 0) return;
-  const int64_t n = side->n;
-  Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
-  Buf<uint64_t> offs(ctx, n + 1);
-  launch_predicate_mask(ctx, ps, side->perm, n, mask.get());
-  exclusive_scan_u32_u64(ctx, mask.get(), n, offs.get());
+  Buf<uint64_t> offs;
+  side->n = select_rows(ctx, ps, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
+  side->perm = side->kept.get();
   std::vector<uint32_t> bounds(nb + 1);
   for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
   Buf<uint32_t> d_bounds(ctx, nb + 1);
@@ -1361,21 +1296,10 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, int
   launch_gather_plain(ctx, offs.get(), d_bounds.get(), nb + 1, 8, d_seg.get());
   copy_d2h(ctx, side->seg.data(), d_seg.get(), 8 * (nb + 1));
   sync_stream(ctx);
-  side->n = (int64_t)side->seg[nb];
-  side->kept.alloc(ctx, std::max<int64_t>(1, side->n));
-  launch_compact_indices(ctx, mask.get(), offs.get(), n, side->perm, side->kept.get());
-  side->perm = side->kept.get();
 }
 
-__global__ void k_compose_u32(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, int64_t n, uint32_t* out) {
-  // out[i] = a[b[i]]
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = a[b[i]];
-}
-
-// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  A one-key join
-// probes with k_join_count over int64 (int32 keys widened) or string references; several keys go through
-// k_join_count_keys over sort_encode values and references.
+// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  k_join_count
+// probes on the key columns where they lie: the decoded columns, or their gather through the side's permutation.
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                             int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
                             int n_right_preds, bool legacy, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
@@ -1449,38 +1373,19 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     select_join_side(ctx, &R, rps, nb);
     t_sel.stop();
     // the key columns in (selected) sorted order
-    Buf<uint8_t> lsorted, rsorted;
-    Buf<int64_t> lk64, rk64;
-    std::vector<Buf<uint64_t>> key_bufs;
-    Buf<unsigned long long> or_and(ctx, 2);  // k_encode_keys reduces into it; unused here
-    auto one_key = [&](const JoinSide& s, Buf<uint8_t>* sorted, Buf<int64_t>* k64) {
-      const DevColumn& c = s.t.cols[0];
-      const void* data = c.data.get();
-      if (s.perm) {  // materialise the sorted key column
-        sorted->alloc(ctx, (size_t)std::max<int64_t>(1, s.n) * c.width);
-        launch_gather_plain(ctx, data, s.perm, s.n, c.width, sorted->get());
-        data = sorted->get();
-      }
-      return c.type == HS_TYPE_STRING ? (const int64_t*)data : widened_key(ctx, c, data, s.n, k64);
-    };
-    auto key_tuples = [&](const JoinSide& s) {
+    std::vector<Buf<uint8_t>> key_bufs;
+    auto key_cols = [&](const JoinSide& s) {
       JoinKeyCols kc{};
       kc.n = n_keys;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
-        if (c.type == HS_TYPE_STRING) {
-          kc.str_mask |= 1u << k;
-          if (!s.perm) {
-            kc.col[k] = (const uint64_t*)c.data.get();
-            continue;
-          }
-          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n));
-          launch_gather_plain(ctx, c.data.get(), s.perm, s.n, 8, key_bufs.back().get());
-        } else {
-          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n));
-          launch_encode_keys(ctx, c.data.get(), c.type, s.perm, s.n, key_bufs.back().get(), or_and.get());
+        kc.type[k] = c.type;
+        kc.col[k] = c.data.get();
+        if (s.perm) {
+          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n) * c.width);
+          launch_gather_plain(ctx, c.data.get(), s.perm, s.n, c.width, key_bufs.back().get());
+          kc.col[k] = key_bufs.back().get();
         }
-        kc.col[k] = key_bufs.back().get();
       }
       return kc;
     };
@@ -1492,37 +1397,15 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     copy_h2d(ctx, d_rseg.get(), R.seg.data(), 8 * (nb + 1));
     Buf<uint32_t> counts(ctx, std::max<int64_t>(1, nl)), first(ctx, std::max<int64_t>(1, nl));
     Buf<uint64_t> offs(ctx, nl + 1);
-    if (n_keys == 1) {
-      const int64_t* lkeys = one_key(L, &lsorted, &lk64);
-      const int64_t* rkeys = one_key(R, &rsorted, &rk64);
-      launch_join_count(ctx, lkeys, d_lseg.get(), rkeys, d_rseg.get(), nb, nl, counts.get(), first.get(),
-                        L.t.cols[0].type == HS_TYPE_STRING);
-    } else {
-      const JoinKeyCols lk = key_tuples(L), rk = key_tuples(R);
-      launch_join_count_keys(ctx, lk, d_lseg.get(), rk, d_rseg.get(), nb, nl, counts.get(), first.get());
-    }
+    const JoinKeyCols lk = key_cols(L), rk = key_cols(R);
+    launch_join_count(ctx, lk, d_lseg.get(), rk, d_rseg.get(), nb, nl, counts.get(), first.get());
     exclusive_scan_u32_u64(ctx, counts.get(), nl, offs.get());
     uint64_t total_out = 0;
     copy_d2h(ctx, &total_out, offs.get() + nl, 8);
     sync_stream(ctx);
     if (total_out >= (1ull << 32)) fail(HS_EUNSUPPORTED, "join output larger than 2^32-1 rows per call");
-    Buf<uint32_t> li(ctx, std::max<uint64_t>(1, total_out)), ri(ctx, std::max<uint64_t>(1, total_out));
-    launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, li.get(), ri.get());
-    // positions in sorted order -> rows of the decoded (or partitioned) tables
-    for (JoinSide* s : {&L, &R})
-      if (!s->perm) {
-        s->iota.alloc(ctx, std::max<int64_t>(1, s->n));
-        launch_iota_u32(ctx, s->iota.get(), s->n);
-        s->perm = s->iota.get();
-      }
     Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
-    if (total_out) {
-      const int grid = (int)std::min<int64_t>(ceil_div((int64_t)total_out, 256), ctx->sm_count * 16);
-      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(L.perm, li.get(), (int64_t)total_out, lrow.get());
-      HS_LAUNCH_CHECK(ctx);
-      k_compose_u32<<<grid, 256, 0, ctx->stream>>>(R.perm, ri.get(), (int64_t)total_out, rrow.get());
-      HS_LAUNCH_CHECK(ctx);
-    }
+    launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, L.perm, R.perm, lrow.get(), rrow.get());
     t_join.stop();
     batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
     batch_from_gather(ctx, R.t, rproj, rrow.get(), (int64_t)total_out, res.get());
@@ -1562,8 +1445,8 @@ int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* cons
   if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
   if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
   if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
-  int rc = check_predicates(left_preds, n_left_preds, stats, err, errlen);
-  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, stats, err, errlen);
+  int rc = check_predicates(left_preds, n_left_preds, false, stats, err, errlen);
+  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
   if (rc != HS_OK) return rc;
   return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, false,
                           out, stats, err, errlen);

@@ -393,21 +393,21 @@ void launch_range_bounds(hs_ctx* ctx, const void* keys, const PredRange& r, cons
                          int64_t* bounds);
 // mask[i] = every predicate of `preds` holds for row cand[i] (row i when cand is nullptr)
 void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, uint32_t* mask);
-// match counts of every left row against the right rows of the same bucket
-// string_keys: lkeys / rkeys hold string references (device_utils.cuh) compared in byte order
-void launch_join_count(hs_ctx* ctx, const int64_t* lkeys, const uint64_t* lseg, const int64_t* rkeys,
-                       const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match, bool string_keys = false);
-// the same over several key columns (k_join_count_keys): col[k][p] is key column k at sorted position p, a sort_encode
-// value, or a string reference when bit k of str_mask is set; the tuples compare column by column
+// The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its
+// type's width (type[k]: HS_TYPE_INT32 / HS_TYPE_INT64, or HS_TYPE_STRING for string references).  The tuples compare
+// column by column, integers as signed values, strings in byte order.
 struct JoinKeyCols {
-  const uint64_t* col[kMaxJoinKeys];
+  const void* col[kMaxJoinKeys];
+  int32_t type[kMaxJoinKeys];
   int32_t n;
-  uint32_t str_mask;
 };
-void launch_join_count_keys(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
-                            const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match);
+// match counts of every left position against the right positions of the same bucket (k_join_count)
+void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
+                       const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match);
+// the (left row, right row) pairs at out_offsets (the scan of counts); a sorted position p is row perm[p] of its side
+// (perm nullptr: row p)
 void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
-                      int64_t nl, uint32_t* out_li, uint32_t* out_ri);
+                      int64_t nl, const uint32_t* lperm, const uint32_t* rperm, uint32_t* out_lrow, uint32_t* out_rrow);
 // exclusive scan of uint32 counts into uint64 offsets (n+1 entries; last = total)
 void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t* out);
 // lens[i] = length of refs[idx[i]] (0 for a null);  then, with offsets = exclusive scan of lens: out[offsets[i] ..] = bytes
@@ -415,10 +415,11 @@ void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* val
                            uint32_t* lens);
 void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                          const uint64_t* offsets, uint8_t* out);
-// out_idx[offsets[i]] = cand[i] (i when cand is nullptr) for every i with mask[i]
-void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, const uint32_t* cand,
-                            uint32_t* out_idx);
-void launch_not_in_mask(hs_ctx* ctx, const int64_t* file_ids, int64_t n, const int64_t* deleted, int ndeleted,
-                        uint32_t* mask /* and-ed in place */);
+// Row selection over n candidates (cand[i], or row i when cand is nullptr): keeps those where every predicate of `preds`
+// holds and, when ndeleted > 0, whose file_ids[i] is not in the host array `deleted`.  The kept candidates go to *kept in
+// their order; returns how many there are (after a stream synchronisation).  offsets, when given, receives the exclusive
+// scan of the keep mask (n+1 entries): offsets[i] is the number of kept candidates before i.
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, const int64_t* file_ids,
+                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets = nullptr);
 
 }  // namespace hs

@@ -6,33 +6,14 @@
 // K8 replaces the bucketed scan + SortMergeJoinExec (no ShuffleExchangeExec) Spark plans after
 // JoinIndexRule.applyIndex (index/covering/JoinIndexRule.scala:653-687): bucket b of the left index joins bucket b of
 // the right index; every left row binary-searches its match range in the right bucket, a scan turns match counts into
-// output offsets, and a second kernel emits the (left row, right row) pairs in (left, right) order.  A join on several
-// key columns searches on the key tuples, compared column by column (k_join_count_keys).
+// output offsets, and a second kernel emits the (left row, right row) pairs in (left, right) order.  The key tuples of
+// 1-8 columns are compared column by column (k_join_count).
 #include "device_utils.cuh"
 #include "kernels.h"
 
 namespace hs {
 
 namespace {
-
-__device__ __forceinline__ int64_t lower_bound_i64(const int64_t* a, int64_t n, int64_t v) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = lo + ((hi - lo) >> 1);
-    if (a[mid] < v) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
-__device__ __forceinline__ int64_t upper_bound_i64(const int64_t* a, int64_t n, int64_t v) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = lo + ((hi - lo) >> 1);
-    if (a[mid] <= v) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
 
 // ---- predicate evaluation (kernels.h: PredRange) -------------------------------------------------------------------
 // value i of a column of type KT against a bound: -1 / 0 / +1.  Numeric values are compared as sort_encode(KT, value)
@@ -110,11 +91,38 @@ __global__ void k_predicate_mask(const __grid_constant__ PredSet ps, const uint3
   }
 }
 
-// one thread per left row; the segment of a row is found by binary search over the (few hundred) segment offsets
-template <bool STR>
-__global__ void k_join_count(const int64_t* __restrict__ lkeys, const uint64_t* __restrict__ lseg,
-                             const int64_t* __restrict__ rkeys, const uint64_t* __restrict__ rseg, int nseg, int64_t nl,
-                             uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
+// a key value at position p, read at its type's width: int32 sign-extended, int64 as it is, a string as its reference
+template <int KT>
+__device__ __forceinline__ int64_t key_value(const void* col, int64_t p) {
+  if constexpr (KT == HS_TYPE_INT32) return ((const int32_t*)col)[p];
+  else return ((const int64_t*)col)[p];
+}
+
+// -1 / 0 / +1: integers as signed values, strings in UTF8String byte order
+template <int KT>
+__device__ __forceinline__ int compare_keys(int64_t a, int64_t b) {
+  if constexpr (KT == HS_TYPE_STRING) return string_compare((uint64_t)a, (uint64_t)b);
+  else return a < b ? -1 : (a > b ? 1 : 0);
+}
+
+// key column k of left position i against right position j
+__device__ __forceinline__ int compare_column(const JoinKeyCols& l, int64_t i, const JoinKeyCols& r, int64_t j, int k) {
+  switch (r.type[k]) {
+    case HS_TYPE_INT32: return compare_keys<HS_TYPE_INT32>(key_value<HS_TYPE_INT32>(l.col[k], i), key_value<HS_TYPE_INT32>(r.col[k], j));
+    case HS_TYPE_INT64: return compare_keys<HS_TYPE_INT64>(key_value<HS_TYPE_INT64>(l.col[k], i), key_value<HS_TYPE_INT64>(r.col[k], j));
+    default: return compare_keys<HS_TYPE_STRING>(key_value<HS_TYPE_STRING>(l.col[k], i), key_value<HS_TYPE_STRING>(r.col[k], j));
+  }
+}
+
+// One thread per left position; the segment of a position is found by binary search over the (few hundred) segment
+// offsets.  The right positions of a bucket are ascending on the key tuples, so the matches of a left position are the
+// range between two lexicographic binary searches.  The leading key column, KT0 its type, decides almost every step: its
+// left value stays in a register and its comparison is compiled in, so a step is one load and a branch-free compare.  The
+// later columns are compared only where the leading ones tie.
+template <int KT0>
+__device__ __forceinline__ void join_count_rows(const JoinKeyCols& lk, const uint64_t* __restrict__ lseg, const JoinKeyCols& rk,
+                                                const uint64_t* __restrict__ rseg, int nseg, int64_t nl,
+                                                uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
     int lo = 0, hi = nseg;  // last segment with lseg[s] <= i
@@ -123,70 +131,24 @@ __global__ void k_join_count(const int64_t* __restrict__ lkeys, const uint64_t* 
       if (lseg[mid] <= (uint64_t)i) lo = mid;
       else hi = mid;
     }
-    const int64_t rb = (int64_t)rseg[lo], rn = (int64_t)rseg[lo + 1] - rb;
-    int64_t f, l;
-    if (STR) {  // keys are string references: the same two searches in byte order
-      const uint64_t k = (uint64_t)lkeys[i];
-      const uint64_t* a = (const uint64_t*)rkeys + rb;
-      int64_t x = 0, y = rn;
-      while (x < y) {
-        const int64_t mid = x + ((y - x) >> 1);
-        if (string_compare(a[mid], k) < 0) x = mid + 1;
-        else y = mid;
-      }
-      f = x;
-      y = rn;
-      while (x < y) {
-        const int64_t mid = x + ((y - x) >> 1);
-        if (string_compare(a[mid], k) <= 0) x = mid + 1;
-        else y = mid;
-      }
-      l = x;
-    } else {
-      const int64_t k = lkeys[i];
-      f = lower_bound_i64(rkeys + rb, rn, k);
-      l = upper_bound_i64(rkeys + rb, rn, k);
-    }
-    counts[i] = (uint32_t)(l - f);
-    first_match[i] = (uint32_t)(rb + f);
-  }
-}
-
-// left row i against right row j on every key column, in order: -1 / 0 / +1
-__device__ __forceinline__ int compare_key_tuples(const JoinKeyCols& l, int64_t i, const JoinKeyCols& r, int64_t j) {
-  for (int k = 0; k < l.n; k++) {
-    const uint64_t a = l.col[k][i], b = r.col[k][j];
-    const int c = (l.str_mask >> k) & 1u ? string_compare(a, b) : (a < b ? -1 : (a > b ? 1 : 0));
-    if (c) return c;
-  }
-  return 0;
-}
-
-// k_join_count over several key columns: the right rows of a bucket are ascending on the key tuples, so the matches of a
-// left row are the range between two lexicographic binary searches
-__global__ void k_join_count_keys(const __grid_constant__ JoinKeyCols lk, const uint64_t* __restrict__ lseg,
-                                  const __grid_constant__ JoinKeyCols rk, const uint64_t* __restrict__ rseg, int nseg,
-                                  int64_t nl, uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
-    int lo = 0, hi = nseg;  // last segment with lseg[s] <= i
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (lseg[mid] <= (uint64_t)i) lo = mid;
-      else hi = mid;
-    }
+    const int64_t l0 = key_value<KT0>(lk.col[0], i);
+    auto compare = [&](int64_t j) {  // the left tuple against right position j
+      int c = compare_keys<KT0>(l0, key_value<KT0>(rk.col[0], j));
+      for (int k = 1; k < rk.n && c == 0; k++) c = compare_column(lk, i, rk, j, k);
+      return c;
+    };
     const int64_t rb = (int64_t)rseg[lo], rn = (int64_t)rseg[lo + 1] - rb;
     int64_t x = 0, y = rn;  // first right row >= the left tuple
     while (x < y) {
       const int64_t mid = x + ((y - x) >> 1);
-      if (compare_key_tuples(lk, i, rk, rb + mid) > 0) x = mid + 1;
+      if (compare(rb + mid) > 0) x = mid + 1;
       else y = mid;
     }
     const int64_t f = x;
-    y = rn;  // first right row > the left tuple
+    x = 0, y = rn;  // first right row > the left tuple (from the start again: the same path, so cached)
     while (x < y) {
       const int64_t mid = x + ((y - x) >> 1);
-      if (compare_key_tuples(lk, i, rk, rb + mid) >= 0) x = mid + 1;
+      if (compare(rb + mid) >= 0) x = mid + 1;
       else y = mid;
     }
     counts[i] = (uint32_t)(x - f);
@@ -194,17 +156,30 @@ __global__ void k_join_count_keys(const __grid_constant__ JoinKeyCols lk, const 
   }
 }
 
+__global__ void k_join_count(const __grid_constant__ JoinKeyCols lk, const uint64_t* __restrict__ lseg,
+                             const __grid_constant__ JoinKeyCols rk, const uint64_t* __restrict__ rseg, int nseg, int64_t nl,
+                             uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
+  switch (lk.type[0]) {
+    case HS_TYPE_INT32: join_count_rows<HS_TYPE_INT32>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
+    case HS_TYPE_INT64: join_count_rows<HS_TYPE_INT64>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
+    default: join_count_rows<HS_TYPE_STRING>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
+  }
+}
+
+// the matches of left position i are right positions [first_match[i], + counts[i]); both go through their side's
+// permutation (nullptr: the identity) to rows
 __global__ void k_join_emit(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ first_match,
-                            const uint64_t* __restrict__ out_offsets, int64_t nl, uint32_t* __restrict__ out_li,
-                            uint32_t* __restrict__ out_ri) {
+                            const uint64_t* __restrict__ out_offsets, int64_t nl, const uint32_t* __restrict__ lperm,
+                            const uint32_t* __restrict__ rperm, uint32_t* __restrict__ out_lrow, uint32_t* __restrict__ out_rrow) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
     const uint32_t c = counts[i];
     const uint64_t o = out_offsets[i];
     const uint32_t f = first_match[i];
+    const uint32_t lrow = lperm ? lperm[i] : (uint32_t)i;
     for (uint32_t j = 0; j < c; j++) {
-      out_li[o + j] = (uint32_t)i;
-      out_ri[o + j] = f + j;
+      out_lrow[o + j] = lrow;
+      out_rrow[o + j] = rperm ? rperm[f + j] : f + j;
     }
   }
 }
@@ -371,30 +346,20 @@ void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* ca
   HS_LAUNCH_CHECK(ctx);
 }
 
-void launch_join_count(hs_ctx* ctx, const int64_t* lkeys, const uint64_t* lseg, const int64_t* rkeys,
-                       const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match, bool string_keys) {
+void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
+                       const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
   KernelScope _ks(ctx, "k_join_count");
   if (nl == 0) return;
-  if (string_keys)
-    k_join_count<true><<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
-  else
-    k_join_count<false><<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_join_count_keys(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
-                            const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
-  KernelScope _ks(ctx, "k_join_count_keys");
-  if (nl == 0) return;
-  k_join_count_keys<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
+  k_join_count<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lseg, rkeys, rseg, nseg, nl, counts, first_match);
   HS_LAUNCH_CHECK(ctx);
 }
 
 void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
-                      int64_t nl, uint32_t* out_li, uint32_t* out_ri) {
+                      int64_t nl, const uint32_t* lperm, const uint32_t* rperm, uint32_t* out_lrow, uint32_t* out_rrow) {
   KernelScope _ks(ctx, "k_join_emit");
   if (nl == 0) return;
-  k_join_emit<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(counts, first_match, out_offsets, nl, out_li, out_ri);
+  k_join_emit<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(counts, first_match, out_offsets, nl, lperm, rperm,
+                                                                      out_lrow, out_rrow);
   HS_LAUNCH_CHECK(ctx);
 }
 
@@ -412,18 +377,30 @@ void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t
   }
 }
 
-void launch_compact_indices(hs_ctx* ctx, const uint32_t* mask, const uint64_t* offsets, int64_t n, const uint32_t* cand,
-                            uint32_t* out_idx) {
-  if (n == 0) return;
-  k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask, offsets, n, cand, out_idx);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_not_in_mask(hs_ctx* ctx, const int64_t* file_ids, int64_t n, const int64_t* deleted, int ndeleted,
-                        uint32_t* mask) {
-  if (n == 0 || ndeleted == 0) return;
-  k_not_in_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(file_ids, n, deleted, ndeleted, mask);
-  HS_LAUNCH_CHECK(ctx);
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, const int64_t* file_ids,
+                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets) {
+  Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
+  Buf<uint64_t> own_offsets;
+  if (!offsets) offsets = &own_offsets;
+  offsets->alloc(ctx, n + 1);
+  launch_predicate_mask(ctx, preds, cand, n, mask.get());
+  Buf<int64_t> d_deleted;
+  if (n > 0 && ndeleted > 0) {
+    d_deleted.alloc(ctx, ndeleted);
+    copy_h2d(ctx, d_deleted.get(), deleted, sizeof(int64_t) * ndeleted);
+    k_not_in_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(file_ids, n, d_deleted.get(), ndeleted, mask.get());
+    HS_LAUNCH_CHECK(ctx);
+  }
+  exclusive_scan_u32_u64(ctx, mask.get(), n, offsets->get());
+  uint64_t count = 0;
+  copy_d2h(ctx, &count, offsets->get() + n, 8);
+  sync_stream(ctx);
+  kept->alloc(ctx, std::max<uint64_t>(1, count));
+  if (n > 0) {
+    k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask.get(), offsets->get(), n, cand, kept->get());
+    HS_LAUNCH_CHECK(ctx);
+  }
+  return (int64_t)count;
 }
 
 }  // namespace hs

@@ -90,6 +90,11 @@ def _tables(kind, nl, nr, seed):
     def one(n, idname):
         if kind == "i64_i32":
             cols = {"a": rng.integers(0, 60, n).astype(np.int64), "b": rng.integers(-20, 20, n).astype(np.int32)}
+        elif kind == "i64_i32_extremes":  # signed order at both ends of each range and around zero
+            i64, i32 = np.iinfo(np.int64), np.iinfo(np.int32)
+            a = np.concatenate([[i64.min, i64.min + 1, -1, 0, 1, i64.max - 1, i64.max], rng.integers(-2**62, 2**62, 33)])
+            b = np.concatenate([[i32.min, i32.min + 1, -1, 0, 1, i32.max - 1, i32.max], rng.integers(-2**30, 2**30, 33)])
+            cols = {"a": a.astype(np.int64)[rng.integers(0, len(a), n)], "b": b.astype(np.int32)[rng.integers(0, len(b), n)]}
         elif kind == "i32_str":  # the reference fixture's types: (int, string)
             cols = {"a": rng.integers(0, 40, n).astype(np.int32),
                     "b": np.array([WORDS[i] for i in rng.integers(0, len(WORDS), n)], dtype=object)}
@@ -113,11 +118,14 @@ KINDS = ["i64_i32", "i32_str", "i64_3"]
 
 
 @pytest.mark.parametrize("nb", [12, 200])
-@pytest.mark.parametrize("kind", KINDS)
+@pytest.mark.parametrize("kind", KINDS + ["i64_i32_extremes"])
 def test_composite_keys(ctx, kind, nb):
     L, R, keys = _tables(kind, 12_000, 9_000, 1)
     n, _ = _check(ctx, L, R, nb, keys, keys)
     assert n > 0
+    if kind == "i64_i32_extremes":  # each key alone: the int64 and the int32 extremes on both sides
+        for k in keys:
+            assert _check(ctx, L, R, nb, [k], [k])[0] > 0
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -261,7 +269,8 @@ def test_one_key_without_predicates_is_hs_bucket_join(ctx, ktype):
         b, sb = ctx.bucket_join_where(lf, lb, rf, rb, nb, ["k"], ["k"], ["k", "lid", "s"], ["v", "rid"])
         pb = _profile(ctx)
         ctx.profile_enable(False)
-        assert pa_ == pb and "k_join_count" in pa_ and "k_join_count_keys" not in pb and "k_predicate_mask" not in pb
+        assert pa_ == pb and pb.get("k_join_count") == 1 and "k_predicate_mask" not in pb
+        assert split is not None or "k_encode_keys" not in pb  # (multi-file buckets are re-sorted, which may encode keys)
         assert sa["gpu_launches"] == sb["gpu_launches"]
         assert a.num_rows == b.num_rows > 0
         for (na, va, ma), (nb_, vb, mb) in zip(a.columns, b.columns):
@@ -277,14 +286,20 @@ def test_one_key_without_predicates_is_hs_bucket_join(ctx, ktype):
             r.free()
 
 
-def test_composite_join_runs_the_tuple_search(ctx):
+def test_composite_join_runs_one_probe_without_key_encoding(ctx):
     L, R, keys = _tables("i64_i32", 5_000, 5_000, 11)
+    lres, rres = [_index(ctx, L, None, keys, 12, "l")], [_index(ctx, R, None, keys, 12, "r")]
     ctx.profile_enable(True)
     ctx.profile_report()
-    _check(ctx, L, R, 12, keys, keys)
+    batch, _ = _run(ctx, lres, rres, 12, keys, keys)  # the join alone: createIndex encodes keys for its sort
     prof = _profile(ctx)
     ctx.profile_enable(False)
-    assert prof.get("k_join_count_keys") == 1 and "k_join_count" not in prof and "k_predicate_mask" not in prof
+    li, ri = J.bucket_join(L, R, 12, keys, keys)
+    assert np.array_equal(batch.column("lid"), L["lid"][li]) and np.array_equal(batch.column("rid"), R["rid"][ri])
+    assert prof.get("k_join_count") == 1 and "k_encode_keys" not in prof and "k_predicate_mask" not in prof
+    batch.free()
+    for r in lres + rres:
+        r.free()
 
 
 # ---- refusals ----------------------------------------------------------------------------------------------------------
