@@ -6,6 +6,8 @@ library is missing, or no CUDA device is visible, every entry point raises.
 from __future__ import annotations
 
 import ctypes as C
+import datetime
+import decimal
 import os
 import weakref
 from dataclasses import dataclass
@@ -19,6 +21,7 @@ LIB_PATH = os.environ.get("HS_GPU_LIB") or os.path.join(_HERE, "lib", "libhs_gpu
 
 HS_OK, HS_EINVAL, HS_ENODEVICE, HS_ECUDA, HS_EFORMAT, HS_EIO, HS_EUNSUPPORTED, HS_ENOMEM, HS_ECOMM = 0, -1, -2, -3, -4, -5, -6, -7, -8
 HS_TYPE_INT32, HS_TYPE_INT64, HS_TYPE_FLOAT, HS_TYPE_DOUBLE, HS_TYPE_BOOL, HS_TYPE_STRING = range(6)
+HS_TYPE_DECIMAL = 6  # predicate literals only: unscaled value in lo_i / hi_i, scale in `scale`
 HS_SAVE_OVERWRITE, HS_SAVE_APPEND = 0, 1
 HS_OUT_FILES, HS_OUT_HOST, HS_OUT_DEVICE = 0, 1, 2
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY = 0, 1
@@ -73,7 +76,7 @@ class ScanSpec(C.Structure):
 
 class PredicateSpec(C.Structure):
     _fields_ = [("column", C.c_char_p), ("literal_type", C.c_int32), ("has_lo", C.c_int32), ("has_hi", C.c_int32),
-                ("lo_strict", C.c_int32), ("hi_strict", C.c_int32), ("reserved", C.c_int32),
+                ("lo_strict", C.c_int32), ("hi_strict", C.c_int32), ("scale", C.c_int32),
                 ("lo_i", C.c_int64), ("hi_i", C.c_int64), ("lo_f", C.c_double), ("hi_f", C.c_double),
                 ("lo_bytes", C.c_char_p), ("hi_bytes", C.c_char_p), ("lo_len", C.c_uint32), ("hi_len", C.c_uint32)]
 
@@ -244,15 +247,44 @@ class FileImage:
     on_device: bool = False
 
 
+_EPOCH = datetime.datetime(1970, 1, 1, tzinfo=datetime.timezone.utc)
+
+
+def timestamp_micros(v: datetime.datetime) -> int:
+    """A Spark timestamp literal's value: microseconds since the epoch (a naive datetime is UTC)."""
+    if v.tzinfo is None:
+        v = v.replace(tzinfo=datetime.timezone.utc)
+    return (v - _EPOCH) // datetime.timedelta(microseconds=1)
+
+
+def decimal_unscaled(v: decimal.Decimal) -> Tuple[int, int]:
+    """(unscaled value, scale) of a finite decimal literal; the unscaled value must fit in 64 bits."""
+    if not v.is_finite():
+        raise ValueError(f"decimal literal {v} is not finite")
+    sign, digits, exp = v.as_tuple()
+    unscaled = int("".join(map(str, digits)) or "0") * (-1 if sign else 1)
+    if exp > 0:
+        unscaled, exp = unscaled * 10 ** exp, 0
+    if not -2**63 <= unscaled < 2**63:
+        raise ValueError(f"decimal literal {v} has more than 18 significant digits")
+    return unscaled, -exp
+
+
 def _literal_type(lo, hi) -> int:
-    """HS_TYPE_* of a predicate's literals: str / bytes -> string, int -> long (it must fit in 64 bits), float -> double."""
+    """HS_TYPE_* of a predicate's literals: str / bytes -> string, int / datetime -> long (it must fit in 64 bits; a datetime
+    is a timestamp's micros), float -> double, decimal.Decimal -> decimal (an int beside a Decimal is a decimal of scale 0)."""
     kinds = set()
     for v in (lo, hi):
         if v is None:
             continue
         if isinstance(v, (bool, np.bool_)):
             raise ValueError("a boolean literal cannot bound a range")
-        if isinstance(v, (str, bytes, bytearray)):
+        if isinstance(v, datetime.datetime):
+            kinds.add(HS_TYPE_INT64)
+        elif isinstance(v, decimal.Decimal):
+            decimal_unscaled(v)
+            kinds.add(HS_TYPE_DECIMAL)
+        elif isinstance(v, (str, bytes, bytearray)):
             kinds.add(HS_TYPE_STRING)
         elif isinstance(v, (int, np.integer)):
             if not -2**63 <= int(v) < 2**63:
@@ -266,15 +298,22 @@ def _literal_type(lo, hi) -> int:
         raise ValueError("a predicate needs a lower or an upper bound")
     if HS_TYPE_STRING in kinds and len(kinds) > 1:
         raise ValueError("a predicate cannot mix string and numeric bounds")
-    return HS_TYPE_DOUBLE if HS_TYPE_DOUBLE in kinds else kinds.pop()
+    if HS_TYPE_DOUBLE in kinds:
+        return HS_TYPE_DOUBLE
+    return HS_TYPE_DECIMAL if HS_TYPE_DECIMAL in kinds else kinds.pop()
 
 
 def _predicate_array(predicates: Sequence[tuple]):
-    """``(column, lo, lo_strict, hi, hi_strict)`` tuples -> (hs_predicate array, count).  A range with an int bound and a
-    float bound becomes two comparisons, each in its own type."""
+    """``(column, lo, lo_strict, hi, hi_strict)`` tuples -> (hs_predicate array, count).  A range whose two bounds are
+    literals of different numeric types (int and float, decimal and float, int and decimal), or decimals of different
+    scales, becomes two comparisons, each in its own type."""
     split = []
     for column, lo, lo_strict, hi, hi_strict in predicates:
-        if lo is not None and hi is not None and {_literal_type(lo, None), _literal_type(None, hi)} == {HS_TYPE_INT64, HS_TYPE_DOUBLE}:
+        kinds = {_literal_type(lo, None), _literal_type(None, hi)} if lo is not None and hi is not None else set()
+        mixed = len(kinds) == 2 and HS_TYPE_STRING not in kinds
+        if kinds == {HS_TYPE_DECIMAL}:
+            mixed = decimal_unscaled(lo)[1] != decimal_unscaled(hi)[1]
+        if mixed:
             split += [(column, lo, lo_strict, None, False), (column, None, False, hi, hi_strict)]
         else:
             split.append((column, lo, lo_strict, hi, hi_strict))
@@ -292,7 +331,10 @@ def _predicate_array(predicates: Sequence[tuple]):
                 setattr(p, side + "_bytes", b)
                 setattr(p, side + "_len", len(b))
             elif p.literal_type == HS_TYPE_INT64:
-                setattr(p, side + "_i", int(v))
+                setattr(p, side + "_i", timestamp_micros(v) if isinstance(v, datetime.datetime) else int(v))
+            elif p.literal_type == HS_TYPE_DECIMAL:  # one scale per predicate: bounds of two scales were split above
+                unscaled, p.scale = decimal_unscaled(decimal.Decimal(v))
+                setattr(p, side + "_i", unscaled)
             else:
                 setattr(p, side + "_f", float(v))
     return preds, len(split)

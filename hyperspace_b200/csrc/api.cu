@@ -14,6 +14,7 @@
 
 #include "device_utils.cuh"
 #include "engine.h"
+#include "spark_types.h"
 
 using namespace hs;
 
@@ -867,14 +868,16 @@ static int spark_compare(F a, F b) {  // SQLOrderingUtil.compareDoubles / compar
   return a < b ? -1 : (a > b ? 1 : 0);
 }
 
-// the column value whose sort_encode is e, compared with the literal (lit_i when lit_type is HS_TYPE_INT64, else lit_f)
-static int compare_encoded(int col_type, uint64_t e, int lit_type, int64_t lit_i, double lit_f) {
-  const bool lit_long = lit_type == HS_TYPE_INT64;
+// the column value whose sort_encode is e, compared with the literal (lit_i when lit_type is HS_TYPE_INT64 or
+// HS_TYPE_DECIMAL, else lit_f).  Integer columns and integer / decimal literals compare as decimals of their scales
+// (col_scale: the column's, 0 unless it is a decimal; lit_scale: the literal's, 0 for HS_TYPE_INT64).
+static int compare_encoded(int col_type, uint64_t e, int lit_type, int64_t lit_i, double lit_f, int col_scale, int lit_scale) {
+  const bool lit_long = lit_type == HS_TYPE_INT64 || lit_type == HS_TYPE_DECIMAL;
   switch (col_type) {
     case HS_TYPE_INT32:
     case HS_TYPE_INT64: {
       const int64_t v = col_type == HS_TYPE_INT32 ? (int64_t)(int32_t)((uint32_t)e ^ 0x80000000u) : (int64_t)(e ^ 0x8000000000000000ull);
-      if (lit_long) return v < lit_i ? -1 : (v > lit_i ? 1 : 0);
+      if (lit_long) return compare_scaled(v, col_scale, lit_i, lit_scale);
       return spark_compare((double)v, lit_f);
     }
     case HS_TYPE_FLOAT: {
@@ -925,6 +928,17 @@ static PredRange resolve_predicate(hs_ctx* ctx, const hs_predicate& p, const Dev
   if (str_col != (lit == HS_TYPE_STRING))
     fail(HS_EUNSUPPORTED, "filter scan: a %s literal cannot be compared with the %s column '%s'", lit == HS_TYPE_STRING ? "string" : "numeric",
          str_col ? "string" : "numeric", c.name.c_str());
+  // Spark compares these in double: the caller keeps the conjunct in a Filter of its own
+  const bool dec_col = is_decimal(c.schema), ts_col = is_timestamp(c.schema);
+  if (lit == HS_TYPE_DOUBLE && (dec_col || ts_col))
+    fail(HS_EUNSUPPORTED, "filter scan: a double literal cannot be compared with the %s column '%s'", dec_col ? "decimal" : "timestamp",
+         c.name.c_str());
+  if (lit == HS_TYPE_DECIMAL && (ts_col || (c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64)))
+    fail(HS_EUNSUPPORTED, "filter scan: a decimal literal cannot be compared with the %s column '%s'",
+         ts_col ? "timestamp" : (c.type == HS_TYPE_STRING ? "string" : "floating-point"), c.name.c_str());
+  if (lit == HS_TYPE_DECIMAL && (p.scale < 0 || p.scale > 38))
+    fail(HS_EINVAL, "filter scan: decimal literal on '%s' has scale %d", c.name.c_str(), p.scale);
+  const int col_scale = dec_col ? c.schema.scale : 0, lit_scale = lit == HS_TYPE_DECIMAL ? p.scale : 0;
   PredRange r{};
   r.type = c.type;
   r.has_lo = p.has_lo != 0;
@@ -949,7 +963,7 @@ static PredRange resolve_predicate(hs_ctx* ctx, const hs_predicate& p, const Dev
   uint64_t emin, emax;
   encoded_domain(c.type, &emin, &emax);
   auto cmp = [&](uint64_t e, bool hi_side) {
-    return compare_encoded(c.type, e, lit, hi_side ? p.hi_i : p.lo_i, hi_side ? p.hi_f : p.lo_f);
+    return compare_encoded(c.type, e, lit, hi_side ? p.hi_i : p.lo_i, hi_side ? p.hi_f : p.lo_f, col_scale, lit_scale);
   };
   bool empty = false;
   if (r.has_lo) {  // smallest e with value >= lo (> lo when strict)
@@ -1179,7 +1193,8 @@ static int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_
     const hs_predicate& p = preds[i];
     if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
     if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
-    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING)
+    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING &&
+        p.literal_type != HS_TYPE_DECIMAL)
       return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
   }
   return HS_OK;
@@ -1340,8 +1355,13 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, n_keys, legacy, &st);
     // hashInt and hashLong put equal values into different buckets: both sides must have been bucketed on the same types
     // (JoinIndexRule only pairs indexes whose indexed columns have the same data types)
+    // the same holds for the decimals and timestamps riding on them: decimal(p <= 9) hashes as a long, an int32 as an int,
+    // and a decimal(9,2) equals a decimal(9,3) only after rescaling (other int32 / int64 / string pairs bucket alike)
+    auto spark_typed = [](const pq::SchemaColumn& s) { return is_decimal(s) || is_timestamp(s); };
     for (int k = 0; k < n_keys; k++)
-      if (L.t.cols[k].type != R.t.cols[k].type) {
+      if (L.t.cols[k].type != R.t.cols[k].type ||
+          ((spark_typed(L.t.cols[k].schema) || spark_typed(R.t.cols[k].schema)) &&
+           pq::spark_type_name(L.t.cols[k].schema) != pq::spark_type_name(R.t.cols[k].schema))) {
         if (n_keys == 1) fail(HS_EUNSUPPORTED, "bucket join: key columns have different types");
         fail(HS_EUNSUPPORTED, "bucket join: key columns '%s' and '%s' have different types", left_keys[k], right_keys[k]);
       }
@@ -1514,7 +1534,7 @@ int hs_k_bucket_ids(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int6
     upload_table(ctx, keys, nkeys, nrows, &t);
     std::vector<KeyColumn> h_keys(nkeys);
     for (int k = 0; k < nkeys; k++)
-      h_keys[k] = KeyColumn{t.cols[k].data.get(), t.cols[k].has_nulls ? t.cols[k].valid.get() : nullptr, t.cols[k].type, t.cols[k].width};
+      h_keys[k] = key_column_of(t.cols[k]);
     Buf<KeyColumn> d_keys(ctx, nkeys);
     copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
     const int64_t ntiles = ceil_div(nrows, kPartTile);

@@ -92,7 +92,11 @@ HS_HD uint64_t string_chunk(uint64_t ref, uint32_t chunk) {
   return v;
 }
 
-// raw bits of one key value (type = HS_TYPE_*), as stored in the decoded column
+// Hash kind of a Spark decimal(p <= 9) column: its unscaled value is an int32 in HBM, but Murmur3Hash hashes every decimal
+// of precision <= 18 as hashLong(unscaled) -- so the int32 is sign-extended and hashed as a long.
+constexpr int kHashDecimalInt = 6;
+
+// raw bits of one key value, as stored in the decoded column; type = HS_TYPE_* or kHashDecimalInt (KeyColumn::hash)
 HS_HD uint32_t mm3_hash_value(int type, uint64_t raw, uint32_t seed) {
   switch (type) {
     case 0: return mm3_hash_int((uint32_t)raw, seed);   // int32
@@ -111,6 +115,7 @@ HS_HD uint32_t mm3_hash_value(int type, uint64_t raw, uint32_t seed) {
     }
     case 4: return mm3_hash_int((raw & 0xff) ? 1u : 0u, seed);
     case 5: return mm3_hash_bytes(ref_ptr(raw), ref_len(raw), seed);  // string / binary: raw is a reference
+    case kHashDecimalInt: return mm3_hash_long((uint64_t)(int64_t)(int32_t)(uint32_t)raw, seed);
   }
   return seed;
 }

@@ -16,6 +16,7 @@
 
 #include "device_utils.cuh"
 #include "engine.h"
+#include "spark_types.h"
 
 namespace hs {
 
@@ -30,22 +31,6 @@ std::string make_uuid() {
 }
 
 namespace {
-
-int hs_type_of(const pq::SchemaColumn& c, const char* file) {
-  if (c.num_children > 0) fail(HS_EUNSUPPORTED, "%s: column '%s' is nested; only flat columns can be indexed", file, c.name.c_str());
-  if (c.repetition == pq::REPEATED) fail(HS_EUNSUPPORTED, "%s: column '%s' is repeated", file, c.name.c_str());
-  switch (c.type) {
-    case pq::BOOLEAN: return HS_TYPE_BOOL;
-    case pq::INT32: return HS_TYPE_INT32;
-    case pq::INT64: return HS_TYPE_INT64;
-    case pq::FLOAT: return HS_TYPE_FLOAT;
-    case pq::DOUBLE: return HS_TYPE_DOUBLE;
-    case pq::BYTE_ARRAY: return HS_TYPE_STRING;  // Spark string / binary
-    default:
-      fail(HS_EUNSUPPORTED, "%s: column '%s' has Parquet physical type %d; the GPU path handles BOOLEAN/INT32/INT64/FLOAT/DOUBLE/BYTE_ARRAY",
-           file, c.name.c_str(), c.type);
-  }
-}
 
 bool iequals(const std::string& a, const std::string& b) {
   if (a.size() != b.size()) return false;
@@ -73,6 +58,8 @@ const char* decode_error_text(uint32_t code) {
     case DERR_UNSUPPORTED_TYPE: return "unsupported physical type";
     case DERR_SNAPPY: return "corrupt snappy stream";
     case DERR_STRING_TOO_LONG: return "string / binary value longer than 65535 bytes";
+    case DERR_SPARK_RANGE: return "timestamp that Spark 3.1 does not read (an INT96 value before 1900-01-01T00:00:00Z, or millis beyond the int64 micros range)";
+    case DERR_DECIMAL_WIDTH: return "decimal value wider than its precision allows";
   }
   return "unknown decode error";
 }
@@ -376,27 +363,32 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
   std::vector<ChunkDesc> chunks;
   bool any_compressed = false;
   std::vector<bool> col_optional(ncols, false);
+  std::vector<bool> col_converted(ncols, false);  // some chunk's values are converted (ValueConv): the value path only
   int64_t nrows = 0;
   for (int f = 0; f < n_files; f++) {
     const pq::FileMeta& fm = imgs[f].meta;
     const char* what = imgs[f].what.c_str();
-    std::vector<int> idx(ncols);
+    std::vector<int> idx(ncols), conv(ncols);
     for (int c = 0; c < ncols; c++) {
       idx[c] = find_column(fm, columns[c]);
       if (idx[c] < 0) fail(HS_EINVAL, "%s: column '%s' not found", what, columns[c].c_str());
       const pq::SchemaColumn& sc = fm.columns[idx[c]];
       if (fm.nested) fail(HS_EUNSUPPORTED, "%s: nested schemas are not handled by the GPU path", what);
-      const int t = hs_type_of(sc, what);
+      const SourceType st = source_type_of(sc, what);
       DevColumn& dc = out->cols[c];
       if (dc.type < 0) {
         dc.name = columns[c];
-        dc.type = t;
-        dc.width = type_width(t);
-        dc.schema = sc;
+        dc.type = st.type;
+        dc.width = type_width(st.type);
+        dc.schema = st.schema;
         dc.schema.name = columns[c];
-      } else if (dc.type != t) {
+      } else if (dc.type != st.type ||
+                 ((is_decimal(dc.schema) || is_decimal(st.schema) || is_timestamp(dc.schema) || is_timestamp(st.schema)) &&
+                  pq::spark_type_name(dc.schema) != pq::spark_type_name(st.schema))) {
         fail(HS_EINVAL, "%s: column '%s' changes type between source files", what, columns[c].c_str());
       }
+      conv[c] = st.conv;
+      col_converted[c] = col_converted[c] || st.conv != CONV_NONE;
       if (sc.repetition == pq::OPTIONAL) col_optional[c] = true;
     }
     out->file_row_begin[f] = nrows;
@@ -424,6 +416,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
         cd.max_def = fm.columns[idx[c]].repetition == pq::OPTIONAL ? 1 : 0;
         cd.file_index = f;
         cd.codec = cm.codec;
+        cd.conv = conv[c];
+        cd.type_length = fm.columns[idx[c]].type_length;
         cd.pad = 0;
         chunks.push_back(cd);
       }
@@ -631,7 +625,7 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
       fill_bytes(ctx, d_cnt.get(), 0, 4 * (size_t)nspec);
       for (int i = 0; i < nspec; i++) {
         const DevColumn& dc = out->cols[spec[i]];
-        if ((dc.width != 4 && dc.width != 8) || dc.type == HS_TYPE_STRING) continue;
+        if ((dc.width != 4 && dc.width != 8) || dc.type == HS_TYPE_STRING || col_converted[spec[i]]) continue;
         sets[i].alloc(ctx, kDictCapacity);
         fill_bytes(ctx, sets[i].get(), 0xFF, sizeof(unsigned long long) * kDictCapacity);
         launch_dict_build_from_pages(ctx, d_pages.get(), n_pages, spec[i], dc.width, sets[i].get(), kDictCapacity, kMaxDictEntries,
@@ -660,7 +654,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
       m[0] = (uint64_t)(int64_t)dc.type;
       m[1] = dc.type == HS_TYPE_STRING ? 0ull : (uint64_t)dc.width;  // string references are not values: never carried
       m[2] = spec_state[4 * i];                                                    // distinct values in the set (excl. ~0)
-      m[3] = (spec_state[4 * i + 1] || spec_count[i] > kAgreeCap) ? 1 : 0;         // overflow: no carry for this column
+      // overflow, or a converted column (its dictionary pages hold stored values, not the engine's): no carry for this column
+      m[3] = (spec_state[4 * i + 1] || spec_count[i] > kAgreeCap || col_converted[spec[i]]) ? 1 : 0;
       m[4] = spec_state[4 * i + 2];                                                // the value ~0 occurs
       const uint32_t nv = std::min<uint32_t>(spec_count[i], kAgreeCap);
       for (uint32_t j = 0; j < nv; j++) m[5 + j] = spec_vals[(size_t)i * kAgreeCap + j];
@@ -749,7 +744,7 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
     for (int c = 0; c < ncols; c++) {
       DevColumn& dc = out->cols[c];
       const bool candidate = c >= carry->zc_first_col || (c == 0 && carry->zc_key && (dc.type == HS_TYPE_INT32 || dc.type == HS_TYPE_INT64));
-      if (!candidate || dc.carried || (dc.width != 4 && dc.width != 8)) continue;
+      if (!candidate || dc.carried || col_converted[c] || (dc.width != 4 && dc.width != 8)) continue;
       if (local_cls[c] & (PAGECLASS_NOT_IN_PLACE | PAGECLASS_MAYBE_NULLS)) continue;
       dc.zero_copy = true;
       dc.zc_tiles.alloc(ctx, (size_t)ceil_div(nrows, T));
@@ -779,16 +774,19 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
     sync_stream(ctx);
   }
   launch_decode_pages(ctx, d_pages.get(), n_pages, d_cols.get(), d_flags.get() + 1, file_windows ? d_window.get() : nullptr,
-                      d_flags.get());
+                      d_flags.get(), std::find(col_converted.begin(), col_converted.end(), true) != col_converted.end());
   std::vector<uint32_t> flags(1 + ncols);
   copy_d2h(ctx, flags.data(), d_flags.get(), sizeof(uint32_t) * (1 + ncols));
   t_dec.stop();
   sync_stream(ctx);
   if (flags[0]) {
     const uint32_t code = flags[0] >> 24, detail = flags[0] & 0xffffffu;
-    const int ecode = (code == DERR_COMPRESSED || code == DERR_UNSUPPORTED_ENCODING || code == DERR_UNSUPPORTED_TYPE || code == DERR_STRING_TOO_LONG)
+    const int ecode = (code == DERR_COMPRESSED || code == DERR_UNSUPPORTED_ENCODING || code == DERR_UNSUPPORTED_TYPE ||
+                       code == DERR_STRING_TOO_LONG || code == DERR_SPARK_RANGE)
                           ? HS_EUNSUPPORTED
                           : HS_EFORMAT;
+    if ((code == DERR_SPARK_RANGE || code == DERR_DECIMAL_WIDTH) && detail < (uint32_t)ncols)
+      fail(ecode, "Parquet decode failed: column '%s' holds a %s", columns[detail].c_str(), decode_error_text(code));
     fail(ecode, "Parquet decode failed: %s (detail %u)", decode_error_text(code), detail);
   }
   for (int c = 0; c < ncols; c++) out->cols[c].has_nulls = (flags[1 + c] & 1u) != 0;
@@ -799,7 +797,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
     fill_bytes(ctx, d_states.get(), 0, 16 * (size_t)std::max(1, ncols));
     for (int c = 0; c < ncols; c++) {
       DevColumn& dc = out->cols[c];
-      if (dc.carried || dc.zero_copy || dc.type == HS_TYPE_STRING || (flags[1 + c] & 2u) || (dc.width != 4 && dc.width != 8)) continue;
+      if (dc.carried || dc.zero_copy || dc.type == HS_TYPE_STRING || col_converted[c] || (flags[1 + c] & 2u) || (dc.width != 4 && dc.width != 8))
+        continue;
       dc.dict_keys.alloc(ctx, kDictCapacity);
       fill_bytes(ctx, dc.dict_keys.get(), 0xFF, sizeof(unsigned long long) * kDictCapacity);
       launch_dict_build_from_pages(ctx, d_pages.get(), n_pages, c, dc.width, dc.dict_keys.get(), kDictCapacity, kMaxDictEntries,
@@ -838,8 +837,7 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
   t_hash.start();
   std::vector<KeyColumn> h_keys(nkeys);
   for (int k = 0; k < nkeys; k++) {
-    DevColumn& c = table.cols[k];
-    h_keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width, c.zero_copy ? c.zc_tiles.get() : nullptr};
+    h_keys[k] = key_column_of(table.cols[k]);
   }
   Buf<KeyColumn> d_keys(ctx, nkeys);
   copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
@@ -949,10 +947,7 @@ void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows*
   t_sort->start();
   build_sort_plan(ctx, out->bucket_offsets.data(), num_buckets, &out->plan);
   std::vector<KeyColumn> keys(nkeys);
-  for (int k = 0; k < nkeys; k++) {
-    const DevColumn& c = out->part.cols[k];
-    keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width};
-  }
+  for (int k = 0; k < nkeys; k++) keys[k] = key_column_of(out->part.cols[k]);
   sort_rows(ctx, &out->plan, keys.data(), nkeys, out->have_key_bits ? out->key_or_and : nullptr, defer_settle, &out->sorted,
             key_pages);
   t_sort->stop();

@@ -4,6 +4,7 @@
 #include <string>
 #include <vector>
 
+#include "device_utils.cuh"
 #include "hs_common.h"
 #include "kernels.h"
 #include "parquet_meta.h"
@@ -40,6 +41,20 @@ struct DevColumn {
 };
 
 constexpr int kMaxCarried = 4;  // codes per record
+
+// Spark types that ride on an int32 / int64 column (DevColumn::schema holds the leaf the index file declares)
+inline bool is_decimal(const pq::SchemaColumn& s) { return s.converted_type == pq::CT_DECIMAL; }
+inline bool is_timestamp(const pq::SchemaColumn& s) {
+  return s.type == pq::INT64 && (s.converted_type == pq::CT_TIMESTAMP_MICROS || s.converted_type == pq::CT_TIMESTAMP_MILLIS);
+}
+
+// The hash and partition kernels' view of a key column.  The one place that decides how a key value is hashed: Spark
+// hashes a decimal(p <= 9) -- an int32 here -- as hashLong of the sign-extended unscaled value.
+inline KeyColumn key_column_of(const DevColumn& c) {
+  KeyColumn k{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width, c.zero_copy ? c.zc_tiles.get() : nullptr};
+  k.hash = c.type == HS_TYPE_INT32 && is_decimal(c.schema) ? kHashDecimalInt : c.type;
+  return k;
+}
 
 struct Table {
   int64_t nrows = 0;

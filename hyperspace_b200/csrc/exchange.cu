@@ -109,10 +109,7 @@ void exchange_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, hs_sta
   // ---- partition by owner rank (stable) -----------------------------------------------------------------------
   t_part.start();
   std::vector<KeyColumn> h_keys(nkeys);
-  for (int k = 0; k < nkeys; k++) {
-    DevColumn& c = table.cols[k];
-    h_keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width, c.zero_copy ? c.zc_tiles.get() : nullptr};
-  }
+  for (int k = 0; k < nkeys; k++) h_keys[k] = key_column_of(table.cols[k]);
   Buf<KeyColumn> d_keys(ctx, nkeys);
   copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
   const int64_t ntiles = ceil_div(nrows, fused_tile_rows(false));  // the send buffers are local memory
@@ -311,10 +308,7 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
   auto t_hash = std::make_unique<StageTimer>(ctx), t_x = std::make_unique<StageTimer>(ctx);
   t_hash->start();
   std::vector<KeyColumn> h_keys(nkeys);
-  for (int k = 0; k < nkeys; k++) {
-    DevColumn& c = table.cols[k];
-    h_keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width, c.zero_copy ? c.zc_tiles.get() : nullptr};
-  }
+  for (int k = 0; k < nkeys; k++) h_keys[k] = key_column_of(table.cols[k]);
   Buf<KeyColumn> d_keys(ctx, nkeys);
   copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
   const int64_t ntiles = ceil_div(nrows, fused_tile_rows(true));  // runs leave over NVLink: the large tile shape

@@ -37,7 +37,7 @@ __device__ __forceinline__ int32_t row_bucket(const KeyColumn* keys, int nkeys, 
   for (int k = 0; k < nkeys; k++) {
     const KeyColumn kc = keys[k];
     if (kc.valid && !kc.valid[row]) continue;  // null leaves the hash unchanged
-    h = mm3_hash_value(kc.type, load_raw(kc, row), h);
+    h = mm3_hash_value(key_hash_kind(kc), load_raw(kc, row), h);
   }
   return spark_pmod(h, nb);
 }
@@ -416,13 +416,14 @@ __device__ __forceinline__ uint32_t row_hash(const KeyColumn* keys, int nkeys, i
     if (kc.valid && !kc.valid[row]) continue;  // null leaves the hash unchanged
     const uint64_t raw = load_raw(kc, row);
     if (last_encoded && k == nkeys - 1) *last_encoded = sort_encode(kc.type, raw);
-    h = mm3_hash_value(kc.type, raw, h);
+    h = mm3_hash_value(key_hash_kind(kc), raw, h);
   }
   return h;
 }
 
 // KT >= 0: exactly one indexed column, of HS_TYPE KT and without nulls -- its descriptor is read once per thread and the
 // hash is straight-line code, so a thread's key loads issue back to back.  KT < 0: any number / type of key columns.
+// An int32 key may be a decimal(p <= 9), hashed as a long (KeyColumn::hash): read once, a branch uniform over the grid.
 // A single-key column may be zero-copy (KeyColumn::tiles): the tile's values then lie in at most two page bodies of the
 // source images, addressed by global row through rebased pointers (ZcTile); a decoded column is the same with one "page".
 template <int KT>
@@ -431,9 +432,12 @@ struct RowHasher {
   int nkeys;
   const uint8_t *p0, *p1;
   int64_t split;
-  __device__ __forceinline__ RowHasher(const KeyColumn* k, int n, int64_t tile) : keys(k), nkeys(n), p0(nullptr), p1(nullptr), split(INT64_MAX) {
+  bool decimal_hash;
+  __device__ __forceinline__ RowHasher(const KeyColumn* k, int n, int64_t tile)
+      : keys(k), nkeys(n), p0(nullptr), p1(nullptr), split(INT64_MAX), decimal_hash(false) {
     if (KT >= 0) {
       const KeyColumn kc = k[0];
+      decimal_hash = KT == HS_TYPE_INT32 && kc.hash == kHashDecimalInt;
       if (kc.tiles) {
         const ZcTile z = kc.tiles[tile];
         p0 = z.p0;
@@ -450,6 +454,7 @@ struct RowHasher {
       const uint64_t raw = (KT == HS_TYPE_INT64 || KT == HS_TYPE_DOUBLE) ? *(const uint64_t*)(b + row * 8)
                                                                          : (uint64_t) * (const uint32_t*)(b + row * 4);
       if (last_encoded) *last_encoded = sort_encode(KT, raw);
+      if (KT == HS_TYPE_INT32 && decimal_hash) return mm3_hash_value(kHashDecimalInt, raw, 42u);
       return mm3_hash_value(KT, raw, 42u);
     }
     return row_hash(keys, nkeys, row, last_encoded);

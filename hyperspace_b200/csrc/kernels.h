@@ -7,6 +7,16 @@
 namespace hs {
 
 // ---- Parquet decode (parquet_decode.cu) ---------------------------------------------------------------------------
+// How the decoder turns a stored value into the value the engine keeps for Spark's TimestampType / DecimalType
+// (engine.cu: source_type_of decides it per source column chunk).  Converted pages take the value path: never read in
+// place, never late-materialised.
+enum ValueConv : int32_t {
+  CONV_NONE = 0,
+  CONV_INT96 = 1,   // INT96 (8 B nanos of day, 4 B Julian day) -> int64 micros since the epoch; before 1900: DERR_SPARK_RANGE
+  CONV_MILLIS = 2,  // INT64 TIMESTAMP_MILLIS -> micros (x 1000); overflow: DERR_SPARK_RANGE
+  CONV_FLBA = 3,    // FIXED_LEN_BYTE_ARRAY decimal: big-endian two's complement -> int32 / int64 unscaled; DERR_DECIMAL_WIDTH
+  CONV_NARROW = 4,  // INT64 decimal(p <= 9) -> int32 unscaled; DERR_DECIMAL_WIDTH when it does not fit
+};
 struct ChunkDesc {          // one per (file, row group, projected column)
   const uint8_t* data;      // device pointer to the first page header of the chunk
   uint64_t size;            // chunk bytes
@@ -17,6 +27,8 @@ struct ChunkDesc {          // one per (file, row group, projected column)
   int32_t max_def;          // 0 (required) or 1 (optional)
   int32_t file_index;
   int32_t codec;            // pq::Codec of the chunk (UNCOMPRESSED or SNAPPY)
+  int32_t conv;             // ValueConv
+  int32_t type_length;      // FIXED_LEN_BYTE_ARRAY: bytes per value
   int32_t pad;
 };
 
@@ -39,6 +51,8 @@ struct PageDesc {           // one per data page
   int32_t is_compressed;      // this page's values are snappy-compressed
   int32_t codec;
   int32_t chunk;              // index of the column chunk (ChunkDesc) the page belongs to
+  int32_t conv;               // ValueConv of the chunk
+  int32_t type_length;        // FIXED_LEN_BYTE_ARRAY: bytes per value
 };
 
 struct ColumnOut {          // decoded column destination
@@ -77,7 +91,9 @@ void launch_fill_zc_tiles(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, Z
 // device error word: 0 = ok, else (code << 24 | detail)
 enum DecodeError : uint32_t {
   DERR_NONE = 0, DERR_BAD_HEADER = 1, DERR_UNSUPPORTED_ENCODING = 2, DERR_VALUE_COUNT = 3, DERR_COMPRESSED = 4,
-  DERR_OVERRUN = 5, DERR_DICT_INDEX = 6, DERR_UNSUPPORTED_TYPE = 7, DERR_SNAPPY = 8, DERR_STRING_TOO_LONG = 9
+  DERR_OVERRUN = 5, DERR_DICT_INDEX = 6, DERR_UNSUPPORTED_TYPE = 7, DERR_SNAPPY = 8, DERR_STRING_TOO_LONG = 9,
+  DERR_SPARK_RANGE = 10,    // a timestamp Spark 3.1 refuses to read: INT96 before 1900, MILLIS beyond int64 micros (detail: column)
+  DERR_DECIMAL_WIDTH = 11   // a decimal value wider than its precision's int32 / int64 (detail: column)
 };
 // BYTE_ARRAY dictionary pages -> tables of string references (device_utils.cuh: string_ref): one job per dictionary page,
 // walked by one thread (the entries are length-prefixed, so their positions are only found sequentially)
@@ -124,9 +140,10 @@ void launch_snappy_compress(hs_ctx* ctx, const SnappyFragment* frags, int64_t n,
 void launch_walk_pages(hs_ctx* ctx, const ChunkDesc* chunks, int n_chunks, int32_t* page_counts,
                        const int64_t* page_offsets, PageDesc* pages, uint32_t* d_error, int mode);
 // Decodes all pages into the column arrays.  row_window (optional, device, 2 x int64 per file: [lo, hi) global rows)
-// restricts decoding to pages that intersect the window of their file.
+// restricts decoding to pages that intersect the window of their file.  any_converted: some page has a ValueConv (those
+// are decoded by k_decode_converted_pages, launched right after k_decode_pages).
 void launch_decode_pages(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, const ColumnOut* cols,
-                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error);
+                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error, bool any_converted);
 
 // ---- hash / partition (hash_partition.cu) ---------------------------------------------------------------------------
 struct KeyColumn {
@@ -137,7 +154,12 @@ struct KeyColumn {
   // zero-copy column (data == nullptr): where each partition tile's values lie inside the source images.  Only a single
   // int32 / int64 key without nulls may come this way (the specialised hash kernels handle it).
   const ZcTile* tiles = nullptr;
+  // kind mm3_hash_value hashes the value as: kHashDecimalInt for a decimal(p <= 9) column, else the type (engine.h:
+  // key_column_of sets it; every site that buckets a row reads it through key_hash_kind)
+  int32_t hash = -1;
 };
+// -1 (a descriptor built without key_column_of) hashes by the type, as before decimals existed
+__host__ __device__ __forceinline__ int key_hash_kind(const KeyColumn& k) { return k.hash >= 0 ? k.hash : k.type; }
 
 constexpr int kPartTile = 4096;   // rows per partition tile (256 threads x 16)
 constexpr int kMaxBuckets = 4096;

@@ -9,6 +9,8 @@
 //   PLAIN fixed-width            unaligned little-endian loads -> coalesced stores
 //   PLAIN_/RLE_DICTIONARY        RLE/bit-packed hybrid index stream expanded warp-per-run, dictionary in smem
 //   definition levels (optional) same hybrid decoder at bit width 1, block scan -> dense value positions
+//   converted values (ValueConv) INT96 / MILLIS timestamps -> int64 micros, FIXED_LEN_BYTE_ARRAY / INT64 decimals -> their
+//                                unscaled int32 / int64, value by value (dictionary entries once, into the smem cache)
 // Supported: data page v1 and v2, UNCOMPRESSED codec, BOOLEAN/INT32/INT64/FLOAT/DOUBLE, flat schemas.
 #include "device_utils.cuh"
 #include "kernels.h"
@@ -108,7 +110,9 @@ __global__ void k_walk_pages(const ChunkDesc* __restrict__ chunks, int n_chunks,
       }
     } else if (h.type == pq::DICTIONARY_PAGE) {
       // dictionary entries are PLAIN values: all of them must lie inside the (decompressed) page
-      const int64_t vw = (ch.phys_type == pq::INT64 || ch.phys_type == pq::DOUBLE) ? 8 : (ch.phys_type == pq::BOOLEAN ? 0 : 4);
+      const int64_t vw = ch.phys_type == pq::INT96 ? 12
+                         : ch.phys_type == pq::FIXED_LEN_BYTE_ARRAY ? ch.type_length
+                         : (ch.phys_type == pq::INT64 || ch.phys_type == pq::DOUBLE) ? 8 : (ch.phys_type == pq::BOOLEAN ? 0 : 4);
       const int64_t need = vw ? (int64_t)h.num_values * vw : ((int64_t)h.num_values + 7) / 8;
       if (need > h.uncompressed_size) {
         set_error(d_error, DERR_BAD_HEADER, (uint32_t)c);
@@ -145,6 +149,8 @@ __global__ void k_walk_pages(const ChunkDesc* __restrict__ chunks, int n_chunks,
         // v1 pages of a compressed chunk are always compressed; v2 pages say so in their header
         pd.is_compressed = ch.codec != pq::UNCOMPRESSED && (h.type == pq::DATA_PAGE || h.is_compressed) ? 1 : 0;
         pd.chunk = c;
+        pd.conv = ch.conv;
+        pd.type_length = ch.type_length;
         pages[out + n_pages] = pd;
       }
       if (ch.codec == pq::UNCOMPRESSED && h.compressed_size != h.uncompressed_size) set_error(d_error, DERR_COMPRESSED, (uint32_t)c);
@@ -353,7 +359,7 @@ __global__ void k_classify_pages(const PageDesc* __restrict__ pages, int64_t n_p
   // readable in place?
   {
     const int W = (pg.phys_type == pq::INT64 || pg.phys_type == pq::DOUBLE) ? 8 : ((pg.phys_type == pq::INT32 || pg.phys_type == pq::FLOAT) ? 4 : 0);
-    bool in_place = W != 0 && pg.encoding == pq::ENC_PLAIN && !pg.is_compressed && pg.size == pg.uncompressed_size &&
+    bool in_place = W != 0 && pg.conv == CONV_NONE && pg.encoding == pq::ENC_PLAIN && !pg.is_compressed && pg.size == pg.uncompressed_size &&
                     (f & PAGECLASS_MAYBE_NULLS) == 0 && zc_tile_rows > 0 && pg.num_values >= zc_tile_rows;
     if (in_place) {
       const uint8_t* p = pg.data;
@@ -422,6 +428,66 @@ __device__ __forceinline__ void store_value(void* base, int64_t row, uint64_t v)
   else ((uint8_t*)base)[row] = (uint8_t)v;
 }
 
+// ---- converted values (ValueConv) ------------------------------------------------------------------------------------
+// bytes one stored value of a converted page takes
+__device__ __forceinline__ int conv_src_width(const PageDesc& pg) {
+  return pg.conv == CONV_INT96 ? 12 : (pg.conv == CONV_FLBA ? pg.type_length : 8);
+}
+
+constexpr int64_t kJulianDayOfEpoch = 2440588;          // DateTimeUtils.JULIAN_DAY_OF_EPOCH
+constexpr int64_t kMicrosPerDay = 86400000000ll;
+constexpr int64_t kMicros1900 = -2208988800000000ll;    // 1900-01-01T00:00:00Z: Spark 3.1 fails to load INT96 before it
+
+// The stored value at p as the engine keeps it (W bytes: int32 for a decimal(p <= 9), else int64).  A value Spark would
+// refuse, or that does not fit W, raises the conversion's error (detail: the column) and yields 0.
+template <int W>
+__device__ __forceinline__ uint64_t convert_value(const PageDesc& pg, const uint8_t* p, uint32_t* d_error) {
+  int64_t v;
+  switch (pg.conv) {
+    case CONV_INT96: {  // DateTimeUtils.fromJulianDay: (day - 2440588) * MICROS_PER_DAY + nanos / 1000 (truncating)
+      const int64_t nanos = (int64_t)load_le64_unaligned(p);
+      const int32_t day = (int32_t)load_le32_unaligned(p + 8);
+      v = (int64_t)((uint64_t)((int64_t)day - kJulianDayOfEpoch) * (uint64_t)kMicrosPerDay) + nanos / 1000;
+      if (v < kMicros1900) {
+        set_error(d_error, DERR_SPARK_RANGE, (uint32_t)pg.col);
+        return 0;
+      }
+      return (uint64_t)v;
+    }
+    case CONV_MILLIS: {  // Math.multiplyExact(millis, 1000)
+      const int64_t ms = (int64_t)load_le64_unaligned(p);
+      if (ms > INT64_MAX / 1000 || ms < INT64_MIN / 1000) {
+        set_error(d_error, DERR_SPARK_RANGE, (uint32_t)pg.col);
+        return 0;
+      }
+      return (uint64_t)(ms * 1000);
+    }
+    case CONV_FLBA: {  // big-endian two's complement of type_length bytes; the bytes above the low 8 only extend the sign
+      const int L = pg.type_length;
+      const int first = L > 8 ? L - 8 : 0;
+      uint64_t u = (p[first] & 0x80) ? ~0ull : 0ull;
+      for (int i = first; i < L; i++) u = (u << 8) | p[i];
+      v = (int64_t)u;
+      const uint8_t ext = v < 0 ? 0xff : 0x00;
+      bool ok = true;
+      for (int i = 0; i < first; i++) ok = ok && p[i] == ext;
+      if (!ok || (W == 4 && (v < INT32_MIN || v > INT32_MAX))) {
+        set_error(d_error, DERR_DECIMAL_WIDTH, (uint32_t)pg.col);
+        return 0;
+      }
+      return W == 4 ? (uint64_t)(uint32_t)(int32_t)v : (uint64_t)v;
+    }
+    default: {  // CONV_NARROW: INT64 decimal(p <= 9) -> int32
+      v = (int64_t)load_le64_unaligned(p);
+      if (v < INT32_MIN || v > INT32_MAX) {
+        set_error(d_error, DERR_DECIMAL_WIDTH, (uint32_t)pg.col);
+        return 0;
+      }
+      return (uint64_t)(uint32_t)(int32_t)v;
+    }
+  }
+}
+
 struct DecodeShared {
   HybridShared def;
   HybridShared idx;
@@ -434,9 +500,17 @@ struct DecodeShared {
 };
 
 // W = value width in bytes (8, 4) or 1 for BOOLEAN (bit-packed PLAIN, one output byte per row)
-template <int W>
+// CONV: the page's values are converted (pg.conv): W is the width kept, the stored values take conv_src_width bytes each
+template <int W, bool CONV = false>
 __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* col_has_nulls, uint32_t* d_error,
                             DecodeShared& sm) {
+  static_assert(!CONV || W == 4 || W == 8, "converted values are int32 / int64");
+  const int SW = CONV ? conv_src_width(pg) : W;  // bytes per stored value
+  // stored value i of the PLAIN run at base, as the column keeps it
+  auto load_at = [&](const uint8_t* base, int64_t i) -> uint64_t {
+    if (CONV) return convert_value<W>(pg, base + i * SW, d_error);
+    return load_value<W>(base + i * W);
+  };
   const int n = pg.num_values;
   const uint8_t* p = pg.data;
   const uint8_t* pend = pg.data + pg.size;
@@ -445,7 +519,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
     if (threadIdx.x == 0) set_error(d_error, DERR_UNSUPPORTED_ENCODING, (uint32_t)pg.encoding);
     return;
   }
-  const bool carry = W != 1 && co.carry != 0;  // emit 16-bit codes of the column-wide dictionary instead of values
+  const bool carry = W != 1 && !CONV && co.carry != 0;  // emit 16-bit codes of the column-wide dictionary instead of values
   if (carry && !is_dict) {  // the column was classified dictionary-only before decoding
     if (threadIdx.x == 0) set_error(d_error, DERR_UNSUPPORTED_ENCODING, (uint32_t)pg.encoding);
     return;
@@ -492,7 +566,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
       for (int i = threadIdx.x; i < pg.dict_count; i += blockDim.x) {
         uint64_t v;
         if (W == 1) v = (pg.dict[i >> 3] >> (i & 7)) & 1;
-        else v = load_value<W>(pg.dict + (size_t)i * W);
+        else v = load_at(pg.dict, i);
         if (carry) dict16[i] = (uint16_t)carry_code(co, v, d_error);
         else sm.dict[i] = v;
       }
@@ -511,7 +585,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
     if (carry) return dict_in_smem ? (uint64_t)dict16[ix] : (uint64_t)carry_code(co, load_value<W>(pg.dict + (size_t)ix * W), d_error);
     if (dict_in_smem) return sm.dict[ix];
     if (W == 1) return (pg.dict[ix >> 3] >> (ix & 7)) & 1;
-    return load_value<W>(pg.dict + (size_t)ix * W);
+    return load_at(pg.dict, ix);
   };
   auto emit = [&](int64_t row, uint64_t v) {
     if (carry) ((uint16_t*)co.data)[row] = (uint16_t)v;
@@ -531,6 +605,12 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
           return;
         }
         for (int i = threadIdx.x; i < n; i += blockDim.x) store_value<1>(co.data, row0 + i, (p[i >> 3] >> (i & 7)) & 1);
+      } else if (CONV) {
+        if ((int64_t)(pend - p) < (int64_t)n * SW) {
+          if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
+          return;
+        }
+        for (int i = threadIdx.x; i < n; i += kDecodeThreads) store_value<W>(co.data, row0 + i, load_at(p, i));
       } else {
         if ((int64_t)(pend - p) < (int64_t)n * W) {
           if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
@@ -689,7 +769,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
       }
     } else {  // the tile's dense PLAIN values must lie inside the page
       const int64_t have = (int64_t)(pend - p), upto = val_cursor + total;
-      if (W == 1 ? (upto + 7) / 8 > have : upto * W > have) {
+      if (W == 1 ? (upto + 7) / 8 > have : upto * SW > have) {
         if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
         return;
       }
@@ -703,7 +783,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
         else if (W == 1) {
           const int64_t bit = val_cursor + pos;
           v = (p[bit >> 3] >> (bit & 7)) & 1;
-        } else v = load_value<W>(p + (size_t)(val_cursor + pos) * W);
+        } else v = load_at(p, val_cursor + pos);
       }
       store_value<W>(co.data, row0 + base + i, v);
       co.valid[row0 + base + i] = valid ? 1 : 0;
@@ -841,7 +921,7 @@ __global__ void __launch_bounds__(kDecodeThreads) k_decode_pages(const PageDesc*
     if (pg.first_row + pg.num_values <= lo || pg.first_row >= hi) return;
   }
   const ColumnOut co = cols[pg.col];
-  if (co.skip) return;  // zero-copy column: read in place by the partition
+  if (co.skip || pg.conv != CONV_NONE) return;  // zero-copy column: read in place by the partition; converted: below
   switch (pg.phys_type) {
     case pq::INT64:
     case pq::DOUBLE: decode_page<8>(pg, co, col_has_nulls + pg.col, d_error, sm); break;
@@ -857,6 +937,27 @@ __global__ void __launch_bounds__(kDecodeThreads) k_decode_pages(const PageDesc*
     default:
       if (threadIdx.x == 0) set_error(d_error, DERR_UNSUPPORTED_TYPE, (uint32_t)pg.phys_type);
   }
+}
+
+// The pages whose values are converted (Spark timestamps and decimals, ValueConv), one CTA per page as above.  A kernel of
+// its own: the conversions inlined into k_decode_pages would raise its register count from 64 to 80 for every page.
+__global__ void __launch_bounds__(kDecodeThreads) k_decode_converted_pages(const PageDesc* __restrict__ pages,
+                                                                           const ColumnOut* __restrict__ cols,
+                                                                           uint32_t* col_has_nulls,
+                                                                           const int64_t* __restrict__ row_window,
+                                                                           uint32_t* d_error) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  DecodeShared& sm = *reinterpret_cast<DecodeShared*>(smem_raw);
+  const PageDesc pg = pages[blockIdx.x];
+  if (pg.conv == CONV_NONE) return;
+  if (row_window) {
+    const int64_t lo = row_window[2 * pg.file_index], hi = row_window[2 * pg.file_index + 1];
+    if (pg.first_row + pg.num_values <= lo || pg.first_row >= hi) return;
+  }
+  const ColumnOut co = cols[pg.col];
+  // the column's width, whatever the stored type
+  if (co.width == 8) decode_page<8, true>(pg, co, col_has_nulls + pg.col, d_error, sm);
+  else decode_page<4, true>(pg, co, col_has_nulls + pg.col, d_error, sm);
 }
 
 }  // namespace
@@ -894,18 +995,27 @@ void launch_fill_zc_tiles(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, Z
 }
 
 void launch_decode_pages(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, const ColumnOut* cols,
-                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error) {
-  KernelScope _ks(ctx, "k_decode_pages");
+                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error, bool any_converted) {
   if (n_pages == 0) return;
   static DeviceOnce attr_set_once;
   bool& attr_set = attr_set_once(ctx->device);
   if (!attr_set) {
     HS_CUDA(cudaFuncSetAttribute(k_decode_pages, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DecodeShared)));
+    HS_CUDA(cudaFuncSetAttribute(k_decode_converted_pages, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DecodeShared)));
     attr_set = true;
   }
-  k_decode_pages<<<(unsigned)n_pages, kDecodeThreads, sizeof(DecodeShared), ctx->stream>>>(pages, cols, col_has_nulls,
-                                                                                           row_window, d_error);
-  HS_LAUNCH_CHECK(ctx);
+  {
+    KernelScope _ks(ctx, "k_decode_pages");
+    k_decode_pages<<<(unsigned)n_pages, kDecodeThreads, sizeof(DecodeShared), ctx->stream>>>(pages, cols, col_has_nulls,
+                                                                                             row_window, d_error);
+    HS_LAUNCH_CHECK(ctx);
+  }
+  if (any_converted) {
+    KernelScope _ks(ctx, "k_decode_converted_pages");
+    k_decode_converted_pages<<<(unsigned)n_pages, kDecodeThreads, sizeof(DecodeShared), ctx->stream>>>(pages, cols, col_has_nulls,
+                                                                                                       row_window, d_error);
+    HS_LAUNCH_CHECK(ctx);
+  }
 }
 
 }  // namespace hs

@@ -28,7 +28,13 @@ struct SchemaColumn {
   int32_t converted_type = -1;  // carried through to the index file so Spark sees the same SQL type
   int32_t scale = -1, precision = -1;
   int32_t num_children = 0;
+  // LogicalType TIMESTAMP's unit (SchemaElement field 10): 1 millis, 2 micros, 3 nanos; 0 when the leaf has none.  NANOS
+  // has no converted type, so this is the only place it shows.
+  int32_t time_unit = 0;
 };
+
+// ConvertedType values the engine reads
+enum Converted : int32_t { CT_DECIMAL = 5, CT_DATE = 6, CT_TIMESTAMP_MILLIS = 9, CT_TIMESTAMP_MICROS = 10 };
 
 struct ColumnChunkMeta {
   int32_t type = -1;
@@ -81,6 +87,45 @@ inline std::string read_string(thrift::Reader& r) {
   return s;
 }
 
+// LogicalType union (SchemaElement field 10): DECIMAL and TIMESTAMP are mapped onto the converted type they stand for, so
+// that a leaf written with the logical type only reads like one written with both (pyarrow writes both, except for NANOS)
+inline void parse_logical_type(thrift::Reader& r, SchemaColumn& c) {
+  int16_t fid = 0;
+  for (;;) {
+    uint8_t t = r.field(fid);
+    if (t == thrift::T_STOP || r.bad) break;
+    if (t != thrift::T_STRUCT || (fid != 5 && fid != 8)) {
+      r.skip(t);
+      continue;
+    }
+    int32_t scale = 0, precision = -1, unit = 0;
+    int16_t f2 = 0;
+    for (;;) {
+      uint8_t t2 = r.field(f2);
+      if (t2 == thrift::T_STOP || r.bad) break;
+      if (fid == 5 && f2 == 1) scale = (int32_t)r.zigzag();
+      else if (fid == 5 && f2 == 2) precision = (int32_t)r.zigzag();
+      else if (fid == 8 && f2 == 2 && t2 == thrift::T_STRUCT) {  // TimeUnit union: the set member's id is the unit
+        int16_t f3 = 0;
+        for (;;) {
+          uint8_t t3 = r.field(f3);
+          if (t3 == thrift::T_STOP || r.bad) break;
+          unit = f3;
+          r.skip(t3);
+        }
+      } else r.skip(t2);
+    }
+    if (fid == 5) {
+      if (c.converted_type < 0) c.converted_type = CT_DECIMAL;
+      if (c.precision < 0) c.precision = precision, c.scale = scale;
+    } else {
+      c.time_unit = unit;
+      if (c.converted_type < 0 && unit == 1) c.converted_type = CT_TIMESTAMP_MILLIS;
+      if (c.converted_type < 0 && unit == 2) c.converted_type = CT_TIMESTAMP_MICROS;
+    }
+  }
+}
+
 inline void parse_schema_element(thrift::Reader& r, SchemaColumn& c) {
   int16_t fid = 0;
   for (;;) {
@@ -95,6 +140,10 @@ inline void parse_schema_element(thrift::Reader& r, SchemaColumn& c) {
       case 6: c.converted_type = (int32_t)r.zigzag(); break;
       case 7: c.scale = (int32_t)r.zigzag(); break;
       case 8: c.precision = (int32_t)r.zigzag(); break;
+      case 10:
+        if (t == thrift::T_STRUCT) parse_logical_type(r, c);
+        else r.skip(t);
+        break;
       default: r.skip(t);
     }
   }
@@ -531,9 +580,12 @@ inline std::vector<uint8_t> write_footer(const std::vector<SchemaColumn>& cols, 
 }
 
 // Spark SQL type name of a Parquet leaf (ParquetToSparkSchemaConverter) for the row.metadata JSON.
-inline const char* spark_type_name(const SchemaColumn& c) {
+inline std::string spark_type_name(const SchemaColumn& c) {
+  if (c.converted_type == CT_DECIMAL)
+    return "decimal(" + std::to_string(c.precision) + "," + std::to_string(c.scale < 0 ? 0 : c.scale) + ")";
   switch (c.type) {
     case BOOLEAN: return "boolean";
+    case INT96: return "timestamp";
     case INT32:
       if (c.converted_type == 6) return "date";
       if (c.converted_type == 15) return "byte";

@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(256) k_check_rows(const KeyColumn* __restrict_
     for (int k = 0; k < nkeys; k++) {
       const KeyColumn kc = keys[k];
       if (kc.valid && !kc.valid[i]) continue;
-      h = mm3_hash_value(kc.type, raw_value(kc.data, kc.width, i), h);
+      h = mm3_hash_value(key_hash_kind(kc), raw_value(kc.data, kc.width, i), h);
     }
     if (spark_pmod(h, nb) != file_bucket[lo]) bad_bucket++;
     if (i > file_row_begin[lo] && compare_rows(keys, nkeys, i - 1, i) > 0) bad_order++;
@@ -204,8 +204,7 @@ int hs_verify_index(hs_ctx* ctx, const hs_source_file* files, const int32_t* buc
     checksum_table(ctx, t, d_sums.get() + 2);
     std::vector<KeyColumn> h_keys(n_indexed);
     for (int k = 0; k < n_indexed; k++) {
-      DevColumn& c = t.cols[k];
-      h_keys[k] = KeyColumn{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, c.type, c.width};
+      h_keys[k] = key_column_of(t.cols[k]);
     }
     Buf<KeyColumn> d_keys(ctx, n_indexed);
     Buf<int64_t> d_frb(ctx, n_files + 1);

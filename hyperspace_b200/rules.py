@@ -19,7 +19,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import log_entry as LE
-from .session import FilterNode, JoinNode, Predicate, ProjectNode, RelationNode
+from .session import FilterNode, JoinNode, Predicate, ProjectNode, RelationNode, spark_values
 
 _BUCKET_RE = re.compile(r"_(\d+)(?:\..*)?$")  # Spark BucketingUtils.getBucketId
 
@@ -204,7 +204,8 @@ class ScanExec:
         preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
         batch, _ = self.session.gpu.filter_scan_where(files, key, out_cols, preds, sorted_on_key=sorted_on_key,
                                                       deleted_file_ids=list(deleted_ids))
-        out = {n: _host_column(d) for n, d, _ in batch.columns}
+        types = dict(self.lin.relation.schema)
+        out = {n: spark_values(_host_column(d), types.get(n)) for n, d, _ in batch.columns}
         batch.free()
         return out
 
@@ -288,9 +289,11 @@ class BucketJoinExec:
             for t in lt + rt:
                 t.free()
         out: Dict[str, np.ndarray] = {}
+        nleft = len(self.left.output)
         for i, (n, d, _) in enumerate(batch.columns):
             name = n if n not in out else f"{n}_right"
-            out[name] = _host_column(d)
+            types = dict((self.left if i < nleft else self.right).relation.schema)
+            out[name] = spark_values(_host_column(d), types.get(n))
         batch.free()
         return out
 

@@ -18,6 +18,8 @@ files the native call reads -- the same decision FilterIndexRule / JoinIndexRule
 """
 from __future__ import annotations
 
+import datetime
+import decimal
 import math
 import os
 from dataclasses import dataclass, field
@@ -139,11 +141,22 @@ class Predicate:
         return out
 
 
+def _number(v):
+    """A literal as a number for the bounds: a datetime is a timestamp's micros since the epoch (naive = UTC)."""
+    if isinstance(v, datetime.datetime):
+        from ._native import timestamp_micros
+
+        return timestamp_micros(v)
+    return v
+
+
 def _ceil(v):  # NaN and infinities (floating-point columns) stay as they are in the bounds
+    v = _number(v)
     return math.ceil(v) if math.isfinite(v) else v
 
 
 def _floor(v):
+    v = _number(v)
     return math.floor(v) if math.isfinite(v) else v
 
 
@@ -181,9 +194,10 @@ class Column:
     def __eq__(self, v):  # noqa: A003
         if isinstance(v, (str, bytes)):
             return Predicate({self.name: (_as_bytes(v), _as_bytes(v))}, [(self.name, "==", v)])
-        if not math.isfinite(v) or v != math.floor(v):
+        n = _number(v)
+        if not math.isfinite(n) or n != math.floor(n):
             return Predicate({self.name: (1, 0)}, [(self.name, "==", v)])  # an integer never equals a fraction: empty range
-        return Predicate({self.name: (int(v), int(v))}, [(self.name, "==", v)])
+        return Predicate({self.name: (int(n), int(n))}, [(self.name, "==", v)])
 
     def between(self, lo, hi):
         terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
@@ -246,6 +260,31 @@ _SPARK_TYPE_OF_ARROW = {"int32": "integer", "int64": "long", "float": "float", "
                         "int8": "byte", "int16": "short"}
 
 
+def spark_type_of_arrow(t) -> str:
+    """Spark SQL type name of a pyarrow field type, as ParquetToSparkSchemaConverter names the Parquet leaf: a timestamp of
+    any unit (INT96 included) is `timestamp`, a decimal `decimal(p,s)`."""
+    import pyarrow as pa
+
+    if pa.types.is_timestamp(t):
+        return "timestamp"
+    if pa.types.is_decimal(t):
+        return f"decimal({t.precision},{t.scale})"
+    return _SPARK_TYPE_OF_ARROW.get(str(t), str(t))
+
+
+def spark_values(d: np.ndarray, spark_type: Optional[str]) -> np.ndarray:
+    """A result column as the engine returns it (timestamps: int64 micros; decimals: unscaled int32 / int64) in the Python
+    form of its Spark type: datetime64[us], or an object array of decimal.Decimal."""
+    if spark_type == "timestamp" and d.dtype == np.int64:
+        return d.view("datetime64[us]")
+    if spark_type and spark_type.startswith("decimal(") and d.dtype in (np.int32, np.int64):
+        scale = int(spark_type[len("decimal("):-1].split(",")[1])
+        out = np.empty(len(d), dtype=object)
+        out[:] = [decimal.Decimal(int(v)).scaleb(-scale) for v in d.tolist()]
+        return out
+    return d
+
+
 def list_data_files(path: str) -> List[Tuple[str, int, int]]:
     p = LE.from_uri(path)
     out = []
@@ -268,7 +307,7 @@ def read_parquet_schema(path: str) -> List[Tuple[str, str]]:
     import pyarrow.parquet as pq
 
     sch = pq.ParquetFile(LE.from_uri(path)).schema_arrow
-    return [(f.name, _SPARK_TYPE_OF_ARROW.get(str(f.type), str(f.type))) for f in sch]
+    return [(f.name, spark_type_of_arrow(f.type)) for f in sch]
 
 
 class DataFrameReader:

@@ -60,6 +60,19 @@ extern "C" {
 #define HS_TYPE_BOOL 4
 #define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): indexed and included columns (one GPU), filter scan keys and
                             predicates, join keys (alone or with other key columns); compared in UTF8String byte order */
+#define HS_TYPE_DECIMAL 6 /* hs_predicate literal only: a decimal, unscaled value in lo_i / hi_i, scale in `scale` */
+
+/* Spark timestamps and decimals.  Columns keep an int32 / int64 storage type; their Spark type comes from the Parquet
+ * converted / logical type:
+ *   TimestampType (INT96, INT64 TIMESTAMP_MICROS, INT64 TIMESTAMP_MILLIS): HS_TYPE_INT64, microseconds since the epoch
+ *     (DateTimeUtils.fromJulianDay for INT96; millis x 1000); index files store INT64 TIMESTAMP_MICROS.  An INT96 value
+ *     before 1900-01-01T00:00:00Z, millis whose micros overflow, and TIMESTAMP(NANOS) are HS_EUNSUPPORTED, as Spark 3.1
+ *     refuses them.
+ *   DecimalType(p, s), p <= 18 (INT32, INT64 or FIXED_LEN_BYTE_ARRAY): the unscaled value, HS_TYPE_INT32 for p <= 9 and
+ *     HS_TYPE_INT64 above; index files store INT32 / INT64 DECIMAL(p, s).  Bucketed as Spark's Murmur3Hash does: hashLong
+ *     of the unscaled value at every precision.  p > 18: HS_EUNSUPPORTED.
+ * Result columns (hs_batch_column) come back as stored: int64 micros, int32 / int64 unscaled values; the caller knows the
+ * schema. */
 
 typedef struct hs_ctx hs_ctx;
 typedef struct hs_index_result hs_index_result;
@@ -218,7 +231,9 @@ typedef struct {
   const char* key_column;      /* predicate column (first indexed column, covering/FilterIndexRule.scala:33-103) */
   const char* const* projected_columns;
   int32_t n_projected;
-  int32_t has_lo, has_hi;      /* inclusive bounds lo <= key <= hi on an integer key */
+  int32_t has_lo, has_hi;      /* inclusive bounds lo <= key <= hi on an integer key.  A timestamp key compares them as
+                                  micros since the epoch; a decimal key as integer VALUES, rescaled to its scale (lo = 10 on a
+                                  decimal(9,2) key is 10.00, unscaled 1000), as Spark compares `price >= 10` */
   int64_t lo, hi;
   const int64_t* deleted_file_ids; /* Hybrid Scan: NOT (_data_file_id IN ids) (covering/CoveringIndexRuleUtils.scala:244-253) */
   int32_t n_deleted_file_ids;
@@ -240,17 +255,23 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
 /* One comparison range on one column, a conjunct of a filter: lo <= column <= hi (strict where lo_strict / hi_strict say
  * so; has_lo / has_hi say which bounds exist, at least one must).  literal_type says which fields hold the bounds:
  * HS_TYPE_INT64 -> lo_i / hi_i, HS_TYPE_DOUBLE -> lo_f / hi_f, HS_TYPE_STRING -> lo_bytes / hi_bytes (lo_len / hi_len bytes,
- * at most 65535).  The comparison is Spark 3.1's after its binary-comparison coercion: it happens in the wider of the
+ * at most 65535), HS_TYPE_DECIMAL -> lo_i / hi_i unscaled, with `scale`.
+ * Timestamp columns take HS_TYPE_INT64 literals, microseconds since the epoch (a Spark timestamp literal's value).  Decimal
+ * columns, and int32 / int64 columns against decimal literals, compare exactly, as Spark's decimal comparison does: an
+ * HS_TYPE_INT64 literal is an integer value (`price > 10` is `price > 10.00` on a decimal(p,2)), and a literal with more
+ * fractional digits than the column becomes the ceiling / floor bound with the right strictness.  Refused with
+ * HS_EUNSUPPORTED, so that the caller keeps the conjunct in a Spark Filter (Spark compares them in double): HS_TYPE_DOUBLE
+ * literals on decimal and timestamp columns, HS_TYPE_DECIMAL literals on float / double / timestamp / string columns.  The comparison is Spark 3.1's after its binary-comparison coercion: it happens in the wider of the
  * column's and the literal's types (int < long < float < double), so `int_col > 1.5` is `int_col >= 2`, a float column
  * against a double literal compares (double)f, and a float column against a long literal casts the literal to float;
  * NaN equals NaN and is greater than +inf, -0.0 equals 0.0 (SQLOrderingUtil.compareDoubles).  String columns take
  * HS_TYPE_STRING literals only, numeric columns numeric ones; boolean columns are not handled (HS_EUNSUPPORTED). */
 typedef struct {
-  const char* column;            /* any column of the files: int32 / int64 / float / double / string */
-  int32_t literal_type;          /* HS_TYPE_INT64, HS_TYPE_DOUBLE or HS_TYPE_STRING */
+  const char* column;            /* any column of the files: int32 / int64 / float / double / string / timestamp / decimal */
+  int32_t literal_type;          /* HS_TYPE_INT64, HS_TYPE_DOUBLE, HS_TYPE_STRING or HS_TYPE_DECIMAL */
   int32_t has_lo, has_hi;
   int32_t lo_strict, hi_strict;  /* 1: lo < x / x < hi; 0: inclusive */
-  int32_t reserved;
+  int32_t scale;                 /* HS_TYPE_DECIMAL: the literal's scale (0..38); ignored otherwise */
   int64_t lo_i, hi_i;
   double lo_f, hi_f;
   const void* lo_bytes;
@@ -276,7 +297,8 @@ typedef struct {
   const int32_t* right_buckets;
   int32_t num_buckets;
   int32_t output;                    /* HS_OUT_HOST (or 0) / HS_OUT_DEVICE, as in hs_scan_spec */
-  const char* left_key;              /* single join key on each side: int32 / int64 / string, the same type on both */
+  const char* left_key;              /* single join key on each side: int32 / int64 / string (timestamps and decimals too),
+                                        the same Spark type on both */
   const char* right_key;
   const char* const* left_columns;   /* projected from the left side */
   int32_t n_left_columns;
@@ -293,7 +315,9 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
  * joins JoinIndexRule rewrites (JoinIndexRule.scala:164-170 conditions, 569-616 column orders; T/index/covering/
  * JoinIndexRuleTest.scala:84-95 puts a Filter under both sides).  The keys come in the order of the indexes' indexed
  * columns: the left index's order, and the right columns they map to; both sides must have been bucketed and sorted on
- * the keys in that order.  Key columns are int32 / int64 / string, of the same type at each position (float, double and
+ * the keys in that order.  Key columns are int32 / int64 / string (timestamps, decimals of precision <= 18), of the same
+ * Spark type at each position -- a decimal's precision and scale included, and an int32 never pairs with a decimal(p <= 9)
+ * although both are int32 here (float, double and
  * boolean keys: HS_EUNSUPPORTED; n_keys > 8: HS_EUNSUPPORTED; n_keys < 1: HS_EINVAL).  A row whose key has a null in any
  * column joins nothing, as in Spark's inner join.  left_preds / right_preds (at most 16 each) are conjunctions with the
  * semantics and refusals of hs_filter_scan_where; a row joins only when every predicate of its side holds.  Files,
