@@ -577,16 +577,17 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
       // one GPU, or writing straight into the owners' memory on several), no rows to drop.  HS_NO_CARRY=1 switches it off
       // (A/B measurements; on several GPUs every rank must be given the same setting).
       const bool no_carry = getenv("HS_NO_CARRY") != nullptr;
+      // 0 above 1024 buckets: the partition there moves materialised columns only
+      const int part_tile_rows = partition_tile_rows(ctx, spec->num_buckets);
       CarryOptions carry;
-      if ((ctx->world == 1 || p2p_exchange_supported(ctx, spec->num_buckets)) && !spec->disable_dictionary &&
-          spec->n_deleted_file_ids == 0 && !no_carry && fused_partition_supported(spec->num_buckets)) {
+      if (part_tile_rows > 0 && !spec->disable_dictionary && spec->n_deleted_file_ids == 0 && !no_carry) {
         carry.first_col = spec->n_indexed;
         carry.num_segments = spec->num_buckets;
       }
       // PLAIN, null-free, value-aligned columns are not decoded either: hash and partition read them in place from the file
       // images (zero copy), which therefore stay alive until the rows have been partitioned.  HS_NO_ZEROCOPY=1: A/B switch.
-      if (fused_partition_supported(spec->num_buckets) && spec->n_deleted_file_ids == 0 && !getenv("HS_NO_ZEROCOPY")) {
-        carry.zc_tile_rows = fused_tile_rows(p2p_exchange_supported(ctx, spec->num_buckets));
+      if (part_tile_rows > 0 && spec->n_deleted_file_ids == 0 && !getenv("HS_NO_ZEROCOPY")) {
+        carry.zc_tile_rows = part_tile_rows;
         carry.zc_first_col = spec->n_indexed;
         carry.zc_key = spec->n_indexed == 1;
       }
@@ -629,7 +630,7 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
         layout_segments(ctx, req, &lay, &enc, &st);
         return key_page_dest(lay, req, &enc);
       };
-      if (p2p_exchange_supported(ctx, spec->num_buckets)) {
+      if (ctx->world > 1 && part_tile_rows > 0) {
         // partition + exchange fused over NVLink peer memory, then the local sort
         exchange_partition_p2p(ctx, table, spec->n_indexed, spec->num_buckets, &rows, &st);
         sort_partitioned_rows(ctx, spec->n_indexed, spec->num_buckets, &rows, &st, /*defer_settle=*/true, &layout_before_sort);
@@ -1535,16 +1536,12 @@ int hs_k_bucket_ids(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int6
     std::vector<KeyColumn> h_keys(nkeys);
     for (int k = 0; k < nkeys; k++)
       h_keys[k] = key_column_of(t.cols[k]);
-    Buf<KeyColumn> d_keys(ctx, nkeys);
-    copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
-    const int64_t ntiles = ceil_div(nrows, kPartTile);
-    Buf<uint16_t> bucket(ctx, std::max<int64_t>(1, nrows));
-    Buf<uint32_t> tile_hist(ctx, std::max<int64_t>(1, ntiles) * num_buckets);
     Buf<unsigned long long> ghist(ctx, num_buckets);
     fill_bytes(ctx, ghist.get(), 0, 8 * num_buckets);
-    launch_bucket_hist(ctx, d_keys.get(), nkeys, nrows, num_buckets, bucket.get(), tile_hist.get(), ghist.get());
+    HashedRows hashed;  // the hash step of index_rows
+    hash_rows(ctx, h_keys.data(), nkeys, nrows, num_buckets, 0, false, ghist.get(), nullptr, &hashed);
     std::vector<uint16_t> hb(nrows);
-    if (nrows) copy_d2h(ctx, hb.data(), bucket.get(), 2 * nrows);
+    if (nrows) copy_d2h(ctx, hb.data(), hashed.bin_ids.get(), 2 * nrows);
     if (out_hist) copy_d2h(ctx, out_hist, ghist.get(), 8 * num_buckets);
     sync_stream(ctx);
     if (out_bucket) for (int64_t i = 0; i < nrows; i++) out_bucket[i] = hb[i];

@@ -839,30 +839,17 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
   for (int k = 0; k < nkeys; k++) {
     h_keys[k] = key_column_of(table.cols[k]);
   }
-  Buf<KeyColumn> d_keys(ctx, nkeys);
-  copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
-  const bool fused = fused_partition_supported(num_buckets);
-  const int64_t ntiles = ceil_div(nrows, fused ? fused_tile_rows(false) : kPartTile);
-  Buf<uint16_t> bucket;
-  Buf<uint32_t> tile_hist(ctx, std::max<int64_t>(1, ntiles) * num_buckets);
   Buf<unsigned long long> ghist(ctx, num_buckets);
   out->d_bucket_offsets.alloc(ctx, num_buckets + 1);
   fill_bytes(ctx, ghist.get(), 0, sizeof(unsigned long long) * num_buckets);
   Buf<unsigned long long> d_key_bits(ctx, 2);
-  if (fused) {
-    const unsigned long long init[2] = {0ull, ~0ull};
-    copy_h2d(ctx, d_key_bits.get(), init, sizeof init);
-    static const bool rehash = getenv("HS_PART_REHASH") != nullptr;  // A/B: hash twice instead of storing 2 B/row
-    if (!rehash) bucket.alloc(ctx, std::max<int64_t>(1, nrows));
-    launch_tile_hist(ctx, d_keys.get(), nkeys, nrows, num_buckets, 0, tile_hist.get(), ghist.get(), d_key_bits.get(),
-                     single_key_type_of(h_keys.data(), nkeys), rehash ? nullptr : bucket.get());
-    copy_d2h(ctx, out->key_or_and, d_key_bits.get(), sizeof out->key_or_and);
-    out->have_key_bits = true;  // valid after the stream synchronisation below
-  } else {
-    bucket.alloc(ctx, std::max<int64_t>(1, nrows));
-    launch_bucket_hist(ctx, d_keys.get(), nkeys, nrows, num_buckets, bucket.get(), tile_hist.get(), ghist.get());
-  }
-  launch_tile_offsets(ctx, tile_hist.get(), ntiles, num_buckets, ghist.get(),
+  const unsigned long long init[2] = {0ull, ~0ull};
+  copy_h2d(ctx, d_key_bits.get(), init, sizeof init);
+  HashedRows hashed;
+  hash_rows(ctx, h_keys.data(), nkeys, nrows, num_buckets, 0, false, ghist.get(), d_key_bits.get(), &hashed);
+  copy_d2h(ctx, out->key_or_and, d_key_bits.get(), sizeof out->key_or_and);
+  out->have_key_bits = true;  // valid after the stream synchronisation below
+  launch_tile_offsets(ctx, hashed.tile_hist.get(), hashed.ntiles, num_buckets, ghist.get(),
                       (unsigned long long*)out->d_bucket_offsets.get());
   out->bucket_offsets.assign(num_buckets + 1, 0);
   copy_d2h(ctx, out->bucket_offsets.data(), out->d_bucket_offsets.get(), sizeof(uint64_t) * (num_buckets + 1));
@@ -888,7 +875,7 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
     memcpy(dst.dict_state, src.dict_state, sizeof dst.dict_state);
     dst.dict_ready = src.dict_ready;
     if (src.carried) {  // travels as a 16-bit code inside the row's code record
-      if (!fused || c < nkeys || pack.n >= kMaxCarried) fail(HS_EINVAL, "column '%s' cannot be late-materialised here", src.name.c_str());
+      if (c < nkeys || pack.n >= kMaxCarried) fail(HS_EINVAL, "column '%s' cannot be late-materialised here", src.name.c_str());
       dst.carried = true;
       dst.dict_values = std::move(src.dict_values);
       dst.dict_bw = src.dict_bw;
@@ -903,21 +890,11 @@ void index_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRo
       h_pc.push_back(PartColumn{src.valid.get(), dst.valid.get(), 1, 0});
     }
   }
-  Buf<uint32_t> dest;
-  Buf<PartColumn> d_pc(ctx, h_pc.size());
-  if (fused) {
-    copy_h2d(ctx, d_pc.get(), h_pc.data(), sizeof(PartColumn) * h_pc.size());
-    if (pack.n > 0) {
-      out->part.rec.alloc(ctx, (size_t)nrows * 8 + 16);
-      pack.out = out->part.rec.get();
-    }
-    launch_partition_rows(ctx, d_keys.get(), nkeys, nrows, num_buckets, 0, tile_hist.get(), d_pc.get(), (int)h_pc.size(),
-                          nullptr, 1, single_key_type_of(h_keys.data(), nkeys), &pack, bucket ? bucket.get() : nullptr);
-  } else {
-    dest.alloc(ctx, std::max<int64_t>(1, nrows));
-    launch_partition_dest(ctx, bucket.get(), nrows, num_buckets, tile_hist.get(), dest.get());
-    for (const PartColumn& pc : h_pc) launch_scatter_column(ctx, pc.in, pc.out, dest.get(), nrows, pc.width);
+  if (pack.n > 0) {
+    out->part.rec.alloc(ctx, (size_t)nrows * 8 + 16);
+    pack.out = out->part.rec.get();
   }
+  move_rows(ctx, hashed, h_pc.data(), (int)h_pc.size(), &pack);
   t_part.stop();
   if (defer_settle) launch_dictionary_probes(ctx, out->part, true, &out->probe);  // results ride on the synchronisation below
   sync_stream(ctx);  // h_pc is read by the async copy; bucket_offsets now valid on the host

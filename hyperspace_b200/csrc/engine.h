@@ -194,14 +194,15 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
                     hs_stats* stats);
 
 // multi-GPU exchange (exchange.cu): redistributes the rows of `table` so that this rank holds exactly the rows of
-// the buckets it owns (owner(b) = b % world).  No-op when world == 1.
+// the buckets it owns (owner(b) = b % world), with an NCCL all-to-all; index_rows partitions them by bucket afterwards.
+// The path above 1024 buckets.  No-op when world == 1.
 void exchange_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, hs_stats* stats);
 void comm_destroy(hs_ctx* ctx);
 // all-gather of a small host blob (out: world x bytes, rank-major); a plain copy on one GPU
 void comm_allgather_host(hs_ctx* ctx, const void* in, size_t bytes, void* out);
-// Fused alternative (NVLink peer memory): partitions by bucket and delivers every row to its final bucket-major position
-// on the owner GPU in one kernel; fills out->part / bucket_offsets so that sort_partitioned_rows can run next.
-bool p2p_exchange_supported(hs_ctx* ctx, int num_buckets);
+// Up to 1024 buckets (partition_tile_rows() > 0), over NVLink peer memory: partitions by bucket and delivers every row
+// to its final bucket-major position on the owner GPU in one kernel; fills out->part / bucket_offsets so that
+// sort_partitioned_rows can run next.
 void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats);
 // K4 only: sorts out->part (already bucket-major, offsets in out->bucket_offsets) on the first nkeys columns.
 void sort_partitioned_rows(hs_ctx* ctx, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats, bool defer_settle = false,

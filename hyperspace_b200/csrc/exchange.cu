@@ -2,9 +2,10 @@
 //
 // Replaces Spark's shuffle behind `indexData.repartition(numBuckets, indexedColumns)`
 // (index/covering/CoveringIndex.scala:60; on-the-fly variant covering/CoveringIndexRuleUtils.scala:413).
-// One process per GPU.  owner(bucket) = bucket % world.  Each rank partitions its decoded rows by owner with the same
-// stable counting sort as K3 (hash_partition.cu), all-gathers the world x world count matrix, and then moves every
-// column with ONE grouped ncclSend/ncclRecv all-to-all over NVLink.  NCCL is resolved with dlopen so that a
+// One process per GPU.  owner(bucket) = bucket % world.  Up to 1024 buckets the partition kernel itself stores every row
+// into its owner's memory (exchange_partition_p2p, below).  Above that, each rank partitions its decoded rows by owner
+// with the same stable counting sort as K3 (hash_partition.cu), all-gathers the world x world count matrix, and then
+// moves every column with ONE grouped ncclSend/ncclRecv all-to-all over NVLink.  NCCL is resolved with dlopen so that a
 // single-GPU deployment has no NCCL dependency and so that, inside a torch process, the already-loaded NCCL is used.
 #include <dlfcn.h>
 
@@ -110,16 +111,12 @@ void exchange_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, hs_sta
   t_part.start();
   std::vector<KeyColumn> h_keys(nkeys);
   for (int k = 0; k < nkeys; k++) h_keys[k] = key_column_of(table.cols[k]);
-  Buf<KeyColumn> d_keys(ctx, nkeys);
-  copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
-  const int64_t ntiles = ceil_div(nrows, fused_tile_rows(false));  // the send buffers are local memory
-  Buf<uint32_t> tile_hist(ctx, std::max<int64_t>(1, ntiles) * world);
   Buf<unsigned long long> ghist(ctx, world);
   Buf<uint64_t> d_send_off(ctx, world + 1);
   fill_bytes(ctx, ghist.get(), 0, 8 * world);
-  launch_tile_hist(ctx, d_keys.get(), nkeys, nrows, num_buckets, world, tile_hist.get(), ghist.get(), nullptr,
-                   single_key_type_of(h_keys.data(), nkeys));
-  launch_tile_offsets(ctx, tile_hist.get(), ntiles, world, ghist.get(), (unsigned long long*)d_send_off.get());
+  HashedRows owners;  // bins are the owner ranks; the send buffers are local memory
+  hash_rows(ctx, h_keys.data(), nkeys, nrows, num_buckets, world, false, ghist.get(), nullptr, &owners);
+  launch_tile_offsets(ctx, owners.tile_hist.get(), owners.ntiles, world, ghist.get(), (unsigned long long*)d_send_off.get());
   // ---- count matrix -----------------------------------------------------------------------------------------
   Buf<uint64_t> d_matrix(ctx, (size_t)world * world);  // row r = counts rank r sends to each destination
   HS_NCCL(nccl().AllGather(ghist.get(), d_matrix.get(), world, kNcclUint64, ctx->comm->comm, ctx->stream));
@@ -157,10 +154,7 @@ void exchange_rows(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, hs_sta
       else fill_bytes(ctx, send_valid[c].get(), 1, (size_t)nrows + 16);
     }
   }
-  Buf<PartColumn> d_pc(ctx, h_pc.size());
-  copy_h2d(ctx, d_pc.get(), h_pc.data(), sizeof(PartColumn) * h_pc.size());
-  launch_partition_rows(ctx, d_keys.get(), nkeys, nrows, num_buckets, world, tile_hist.get(), d_pc.get(), (int)h_pc.size(),
-                        nullptr, 1, single_key_type_of(h_keys.data(), nkeys));
+  move_rows(ctx, owners, h_pc.data(), (int)h_pc.size());
   sync_stream(ctx);
   for (int c = 0; c < ncols; c++) {
     table.cols[c].data.release();
@@ -292,13 +286,6 @@ void close_peer_mappings(hs_ctx* ctx) {
   cache.clear();
 }
 
-bool p2p_exchange_supported(hs_ctx* ctx, int num_buckets) {
-  if (ctx->world <= 1 || !fused_partition_supported(num_buckets)) return false;
-  const char* env = getenv("HS_EXCHANGE");
-  if (env && strcmp(env, "nccl") == 0) return false;
-  return true;
-}
-
 void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_buckets, IndexedRows* out, hs_stats* stats) {
   const int world = ctx->world, me = ctx->rank;
   if (!ctx->comm || !ctx->comm->comm) fail(HS_ECOMM, "hs_comm_init has not been called on this context");
@@ -309,10 +296,6 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
   t_hash->start();
   std::vector<KeyColumn> h_keys(nkeys);
   for (int k = 0; k < nkeys; k++) h_keys[k] = key_column_of(table.cols[k]);
-  Buf<KeyColumn> d_keys(ctx, nkeys);
-  copy_h2d(ctx, d_keys.get(), h_keys.data(), sizeof(KeyColumn) * nkeys);
-  const int64_t ntiles = ceil_div(nrows, fused_tile_rows(true));  // runs leave over NVLink: the large tile shape
-  Buf<uint32_t> tile_hist(ctx, std::max<int64_t>(1, ntiles) * nb);
 
   // ---- receive buffers, allocated BEFORE the ranks talk ---------------------------------------------------------------
   // Their capacity is a bound derived from the global row count the ranks exchanged while decoding (a uniform hash puts
@@ -380,9 +363,8 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
       memcpy(&h_mine[o_handles + (size_t)i * kHandleWords], &h, sizeof h);
     }
   copy_h2d(ctx, d_mine.get(), h_mine.data(), 8 * (size_t)msg);
-  Buf<uint16_t> bin_ids(ctx, std::max<int64_t>(1, nrows));  // bucket of every row: hashed once, read back by the partition
-  launch_tile_hist(ctx, d_keys.get(), nkeys, nrows, nb, 0, tile_hist.get(), d_mine.get(), d_mine.get() + o_bits,
-                   single_key_type_of(h_keys.data(), nkeys), bin_ids.get(), /*peer_tiles=*/true);
+  HashedRows hashed;  // the runs leave over NVLink
+  hash_rows(ctx, h_keys.data(), nkeys, nrows, nb, 0, true, d_mine.get(), d_mine.get() + o_bits, &hashed);
   HS_NCCL(nccl().AllGather(d_mine.get(), d_all.get(), msg, kNcclUint64, ctx->comm->comm, ctx->stream));
   copy_d2h(ctx, h_all.data(), d_all.get(), 8 * (size_t)msg * world);
   sync_stream(ctx);
@@ -433,7 +415,7 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
   // receives, which is all the sort needs to pick its passes (saves a pass over the received keys and a synchronisation)
   out->key_or_and[0] = key_or;
   out->key_or_and[1] = key_and;
-  out->have_key_bits = single_key_type_of(h_keys.data(), nkeys) >= 0 || nkeys >= 1;
+  out->have_key_bits = true;
 
   out->part.nrows = n_recv;
   std::vector<void*> h_peer;
@@ -495,24 +477,15 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
       for (int r = 0; r < world; r++)
         h_peer[(size_t)i * world + r] = (r == me) ? my_recv[i] : open_peer(ctx, all_handles[(size_t)r * nmoved + i]);
   }
-  // HS_DEBUG_LOCAL_PEERS=1 (timing experiments only, the index comes out WRONG): every run is written to this GPU's own
-  // buffers instead of its owner's -- the same kernel without the NVLink traffic
-  static const bool local_peers = getenv("HS_DEBUG_LOCAL_PEERS") != nullptr;
-  if (local_peers)
-    for (int i = 0; i < nmoved; i++)
-      for (int r = 0; r < world; r++) h_peer[(size_t)i * world + r] = my_recv[i];
 
   // ---- one kernel: partition + exchange ------------------------------------------------------------------------
   Buf<unsigned long long> d_base(ctx, nb);
-  Buf<PartColumn> d_pc(ctx, std::max(1, ncolmoved));
   Buf<void*> d_peer(ctx, (size_t)nmoved * world);
   copy_h2d(ctx, d_base.get(), my_base.data(), 8 * nb);
-  copy_h2d(ctx, d_pc.get(), h_pc.data(), sizeof(PartColumn) * ncolmoved);
   copy_h2d(ctx, d_peer.get(), h_peer.data(), sizeof(void*) * nmoved * world);
-  launch_tile_offsets(ctx, tile_hist.get(), ntiles, nb, d_mine.get(), nullptr, d_base.get());
+  launch_tile_offsets(ctx, hashed.tile_hist.get(), hashed.ntiles, nb, d_mine.get(), nullptr, d_base.get());
   // the peer table holds one row of `world` pointers per column round, then one row for the code records
-  launch_partition_rows(ctx, d_keys.get(), nkeys, nrows, nb, 0, tile_hist.get(), d_pc.get(), ncolmoved,
-                        (void* const*)d_peer.get(), world, single_key_type_of(h_keys.data(), nkeys), &pack, bin_ids.get());
+  move_rows(ctx, hashed, h_pc.data(), ncolmoved, &pack, (void* const*)d_peer.get());
   // closing barrier: nobody reads its receive buffers before every peer's kernel has completed.  Stream-ordered -- the
   // sort that follows is enqueued behind it, the host does not wait here.
   HS_NCCL(nccl().AllGather(d_mine.get(), d_all.get(), 1, kNcclUint64, ctx->comm->comm, ctx->stream));

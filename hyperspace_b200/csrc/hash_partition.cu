@@ -6,12 +6,13 @@
 // indices by bucket id.  Stability makes the whole build deterministic: rows with equal keys keep source order,
 // which is also the oracle's tie order.
 //
-// Per 4096-row tile (256 threads x 16 rows, each warp owns 512 consecutive rows):
-//   k_bucket_hist     hashes the key columns, stores the bucket id (u16), counts per-warp histograms in shared memory
-//                     with __match_any_sync aggregation, and writes the tile histogram M[tile][bucket].
-//   k_tile_offsets_*  turn M into exclusive per-(tile, bucket) destinations (column scan in 3 small kernels).
-//   k_partition_dest  re-ranks the tile's rows (same match_any walk) and emits dest[row].
-//   k_scatter_column  out[dest[i]] = in[i] for each projected column.
+// K2, every bucket count: k_tile_hist hashes the key columns, keeps every row's bin id (u16) and writes the tile histogram
+// M[tile][bin]; k_tile_offsets_* turn M into exclusive per-(tile, bin) destinations (column scan in 3 small kernels).
+// K3 up to kFusedMaxBins bins: k_partition_rows ranks each tile's rows and moves every column (the fused partition, below).
+// K3 above that, per 4096-row tile (256 threads x 16 rows, each warp owns 512 consecutive rows):
+//   k_partition_dest  ranks the tile's rows by bin id (__match_any_sync walk over per-warp counters) and emits dest[row].
+//   k_scatter         out[dest[i]] = in[i] for each projected column.
+// hash_rows and move_rows at the end of the file are the only entry points: they choose among these.
 #include "device_utils.cuh"
 #include "kernels.h"
 
@@ -19,10 +20,12 @@ namespace hs {
 
 namespace {
 
+constexpr int kFusedMaxBins = 1024;  // above this the per-warp counters no longer fit next to the exchange buffer
+
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kItems = kPartTile / kThreads;   // 16 rows per thread
-constexpr int kWarpRows = kPartTile / kWarps;  // 512 consecutive rows per warp
+constexpr int kItems = kFusedTileLocal / kThreads;   // 16 rows per thread
+constexpr int kWarpRows = kFusedTileLocal / kWarps;  // 512 consecutive rows per warp
 
 __device__ __forceinline__ uint64_t load_raw(const KeyColumn& k, int64_t row) {
   switch (k.width) {
@@ -30,16 +33,6 @@ __device__ __forceinline__ uint64_t load_raw(const KeyColumn& k, int64_t row) {
     case 4: return ((const uint32_t*)k.data)[row];
     default: return ((const uint8_t*)k.data)[row];
   }
-}
-
-__device__ __forceinline__ int32_t row_bucket(const KeyColumn* keys, int nkeys, int64_t row, int nb) {
-  uint32_t h = 42;
-  for (int k = 0; k < nkeys; k++) {
-    const KeyColumn kc = keys[k];
-    if (kc.valid && !kc.valid[row]) continue;  // null leaves the hash unchanged
-    h = mm3_hash_value(key_hash_kind(kc), load_raw(kc, row), h);
-  }
-  return spark_pmod(h, nb);
 }
 
 // Counts the warp's items into its private histogram with match_any aggregation and returns, for every item, its
@@ -60,43 +53,6 @@ __device__ __forceinline__ void warp_rank(const uint16_t (&bin)[ITEMS], const bo
       if ((peers & lt) == 0) cnt[bin[j]] = (uint16_t)(pre + __popc(peers));
     }
     __syncwarp();
-  }
-}
-
-// owner_mod > 0: bin = bucket % owner_mod (the rank that owns the bucket) and the histogram has owner_mod bins
-__global__ void __launch_bounds__(kThreads) k_bucket_hist(const KeyColumn* __restrict__ keys, int nkeys, int64_t nrows,
-                                                           int num_buckets, int owner_mod, uint16_t* __restrict__ bucket,
-                                                           uint32_t* __restrict__ tile_hist,
-                                                           unsigned long long* __restrict__ global_hist) {
-  extern __shared__ uint16_t s_cnt[];  // [kWarps][nb]
-  const int nb = owner_mod > 0 ? owner_mod : num_buckets;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < kWarps * nb; i += kThreads) s_cnt[i] = 0;
-  __syncthreads();
-  const int64_t tile = blockIdx.x;
-  const int64_t wbase = tile * kPartTile + (int64_t)warp * kWarpRows;
-  uint16_t bin[kItems], rank[kItems];
-  bool act[kItems];
-#pragma unroll
-  for (int j = 0; j < kItems; j++) {
-    const int64_t row = wbase + j * 32 + lane;
-    act[j] = row < nrows;
-    bin[j] = 0;
-    if (act[j]) {
-      int32_t b = row_bucket(keys, nkeys, row, num_buckets);
-      if (owner_mod > 0) b %= owner_mod;
-      bin[j] = (uint16_t)b;
-      bucket[row] = bin[j];
-    }
-  }
-  warp_rank<kItems>(bin, act, s_cnt + warp * nb, rank);
-  __syncthreads();
-  for (int b = threadIdx.x; b < nb; b += kThreads) {
-    uint32_t s = 0;
-#pragma unroll
-    for (int w = 0; w < kWarps; w++) s += s_cnt[w * nb + b];
-    tile_hist[tile * nb + b] = s;
-    if (s) atomicAdd(&global_hist[b], (unsigned long long)s);
   }
 }
 
@@ -165,7 +121,7 @@ __global__ void __launch_bounds__(kThreads) k_partition_dest(const uint16_t* __r
   for (int i = threadIdx.x; i < kWarps * nb; i += kThreads) s_cnt[i] = 0;
   __syncthreads();
   const int64_t tile = blockIdx.x;
-  const int64_t wbase = tile * kPartTile + (int64_t)warp * kWarpRows;
+  const int64_t wbase = tile * kFusedTileLocal + (int64_t)warp * kWarpRows;
   uint16_t bin[kItems], rank[kItems];
   bool act[kItems];
 #pragma unroll
@@ -263,35 +219,6 @@ inline int grid_for(hs_ctx* ctx, int64_t n, int threads, int per_sm) {
 
 }  // namespace
 
-void launch_bucket_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets,
-                        uint16_t* bucket, uint32_t* tile_hist, unsigned long long* global_hist) {
-  KernelScope _ks(ctx, "k_bucket_hist");
-  if (nrows == 0) return;
-  const int64_t ntiles = ceil_div(nrows, kPartTile);
-  const size_t smem = (size_t)kWarps * num_buckets * sizeof(uint16_t);
-  static DeviceOnce attr_once;
-  bool& attr = attr_once(ctx->device);
-  if (!attr) {
-    HS_CUDA(cudaFuncSetAttribute(k_bucket_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, kWarps * kMaxBuckets * 2));
-    HS_CUDA(cudaFuncSetAttribute(k_partition_dest, cudaFuncAttributeMaxDynamicSharedMemorySize, kWarps * kMaxBuckets * 2));
-    attr = true;
-  }
-  k_bucket_hist<<<(unsigned)ntiles, kThreads, smem, ctx->stream>>>(d_keys, nkeys, nrows, num_buckets, 0, bucket,
-                                                                   tile_hist, global_hist);
-  HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_owner_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int world,
-                       uint16_t* owner, uint32_t* tile_hist, unsigned long long* global_hist) {
-  KernelScope _ks(ctx, "k_bucket_hist");
-  if (nrows == 0) return;
-  const int64_t ntiles = ceil_div(nrows, kPartTile);
-  const size_t smem = (size_t)kWarps * world * sizeof(uint16_t);
-  k_bucket_hist<<<(unsigned)ntiles, kThreads, smem, ctx->stream>>>(d_keys, nkeys, nrows, num_buckets, world, owner,
-                                                                   tile_hist, global_hist);
-  HS_LAUNCH_CHECK(ctx);
-}
-
 void launch_tile_offsets(hs_ctx* ctx, uint32_t* tile_hist, int64_t ntiles, int num_buckets,
                          const unsigned long long* global_hist, unsigned long long* bucket_offsets,
                          const unsigned long long* explicit_base) {
@@ -310,17 +237,25 @@ void launch_tile_offsets(hs_ctx* ctx, uint32_t* tile_hist, int64_t ntiles, int n
   // the pool only hands it out again to work enqueued later on the same stream.
 }
 
-void launch_partition_dest(hs_ctx* ctx, const uint16_t* bucket, int64_t nrows, int num_buckets,
-                           const uint32_t* tile_offsets, uint32_t* dest) {
+// dest[row] = stable position of the row in bin-major order (tile_offsets: launch_tile_offsets of the 4096-row tiles)
+static void launch_partition_dest(hs_ctx* ctx, const uint16_t* bin_ids, int64_t nrows, int nbins,
+                                  const uint32_t* tile_offsets, uint32_t* dest) {
   KernelScope _ks(ctx, "k_partition_dest");
   if (nrows == 0) return;
-  const int64_t ntiles = ceil_div(nrows, kPartTile);
-  const size_t smem = (size_t)kWarps * num_buckets * sizeof(uint16_t);
-  k_partition_dest<<<(unsigned)ntiles, kThreads, smem, ctx->stream>>>(bucket, nrows, num_buckets, tile_offsets, dest);
+  const int64_t ntiles = ceil_div(nrows, kFusedTileLocal);
+  const size_t smem = (size_t)kWarps * nbins * sizeof(uint16_t);
+  static DeviceOnce attr_once;
+  bool& attr = attr_once(ctx->device);
+  if (!attr) {
+    HS_CUDA(cudaFuncSetAttribute(k_partition_dest, cudaFuncAttributeMaxDynamicSharedMemorySize, kWarps * kMaxBuckets * 2));
+    attr = true;
+  }
+  k_partition_dest<<<(unsigned)ntiles, kThreads, smem, ctx->stream>>>(bin_ids, nrows, nbins, tile_offsets, dest);
   HS_LAUNCH_CHECK(ctx);
 }
 
-void launch_scatter_column(hs_ctx* ctx, const void* in, void* out, const uint32_t* dest, int64_t nrows, int width) {
+// out[dest[i]] = in[i]
+static void launch_scatter_column(hs_ctx* ctx, const void* in, void* out, const uint32_t* dest, int64_t nrows, int width) {
   KernelScope _ks(ctx, "k_scatter_column");
   if (nrows == 0) return;
   const int grid = grid_for(ctx, nrows, 256, 16);
@@ -381,10 +316,10 @@ struct FusedCfg {
 };
 
 // CTAs per SM that __launch_bounds__ asks for, i.e. the register budget: 1024 threads per SM = 64 registers per thread.
-// Under sm_90a's register allocation the local tile's general-key and bulk-store instantiations spill at 64, so they get
-// three CTAs (up to 80 registers).  The peer tile (512 threads) keeps two: one CTA per SM would halve its occupancy.
-template <int KT, bool PEER, bool BULK>
-constexpr int partition_min_ctas() { return !PEER && (KT < 0 || BULK) ? 3 : FusedCfg<PEER>::kMinCtas; }
+// Under sm_90a's register allocation the local tile's general-key instantiations spill at 64, so they get three CTAs (up
+// to 80 registers).  The peer tile (512 threads) keeps two: one CTA per SM would halve its occupancy.
+template <int KT, bool PEER>
+constexpr int partition_min_ctas() { return !PEER && KT < 0 ? 3 : FusedCfg<PEER>::kMinCtas; }
 
 // pmod(hash, n) and bucket % world without an integer division per row: Lemire's fastmod (M = 2^64 / n + 1; exact for
 // 32-bit operands).  The signed Murmur3 value is shifted into unsigned range first and the shift is taken out again
@@ -538,14 +473,17 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 //
 // All warp collectives run with the full mask and outside any branch: slots past the end of the last tile carry the
 // last bin and, being the last slots of the tile, rank behind every real row of that bin; they are never written out.
-template <int BITS, int KT, bool PEER, bool BULK>
-__global__ void __launch_bounds__(FusedCfg<PEER>::kThreads, partition_min_ctas<KT, PEER, BULK>()) k_partition_rows(const KeyColumn* __restrict__ keys, int nkeys, int64_t nrows,
+//
+// PEER: the runs go to the owners' memory over NVLink -- the large tile, and every 8-byte run leaves as a bulk copy; the
+// local tile stores row by row into the dense layout.
+template <int BITS, int KT, bool PEER>
+__global__ void __launch_bounds__(FusedCfg<PEER>::kThreads, partition_min_ctas<KT, PEER>()) k_partition_rows(const KeyColumn* __restrict__ keys, int nkeys, int64_t nrows,
                                                                ModConst bucket_mod, ModConst owner_mod, int use_owner,
                                                                const uint32_t* __restrict__ tile_dst,
                                                                const PartColumn* __restrict__ cols, int ncols,
                                                                void* const* __restrict__ peer_out, int out_world,
                                                                CodePackRound pack, const uint16_t* __restrict__ bin_ids) {
-  constexpr bool bulk = BULK;  // compile-time: the plain-store instantiation carries none of the bulk layout's bookkeeping
+  constexpr bool bulk = PEER;  // compile-time: the plain-store instantiation carries none of the bulk layout's bookkeeping
   extern __shared__ __align__(16) uint8_t smem[];
   constexpr int kFThreads = FusedCfg<PEER>::kThreads, kFItems = FusedCfg<PEER>::kItems, kFusedTile = FusedCfg<PEER>::kTile;
   constexpr int kFWarps = FusedCfg<PEER>::kWarps, kFWarpRows = FusedCfg<PEER>::kWarpRows;
@@ -772,54 +710,37 @@ __global__ void __launch_bounds__(FusedCfg<PEER>::kThreads, partition_min_ctas<K
   }
 }
 
+
 template <bool PEER>
-size_t fused_smem_bytes(int nb, bool bulk = true) {
-  const size_t XN = (size_t)FusedCfg<PEER>::kTile + (bulk ? 2 * (size_t)nb + 2 : 0);
+size_t fused_smem_bytes(int nb) {
+  const size_t XN = (size_t)FusedCfg<PEER>::kTile + (PEER ? 2 * (size_t)nb + 2 : 0);
   size_t u16s = XN + (size_t)FusedCfg<PEER>::kWarps * nb;
   u16s += u16s & 1;
   return XN * 8 + u16s * 2 + (size_t)nb * 4 * 2 + (size_t)nb * 2 * 2 + 40 * 4;
 }
 
-}  // namespace
-
-bool fused_partition_supported(int nbins) { return nbins <= kFusedMaxBins; }
-
-// HS_PEER_TILE=small: experiments -- rows that leave over NVLink are partitioned with the local tile shape too
-bool peer_tile_shape() {
-  static const char* e = getenv("HS_PEER_TILE");
-  return !(e && strcmp(e, "small") == 0);
+// HS_TYPE_INT32 / HS_TYPE_INT64 when there is exactly one key column, of that type and without nulls (selects the kernels
+// with the hash inlined for it); -1 otherwise
+int single_key_type_of(const KeyColumn* keys, int nkeys) {
+  return nkeys == 1 && keys[0].valid == nullptr && (keys[0].type == HS_TYPE_INT32 || keys[0].type == HS_TYPE_INT64)
+             ? keys[0].type
+             : -1;
 }
-int fused_tile_rows(bool peer_tiles) { return peer_tiles && peer_tile_shape() ? kFusedTilePeer : kFusedTileLocal; }
 
 template <bool PEER>
-static void launch_tile_hist_t(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod,
-                               uint32_t* tile_hist, unsigned long long* global_hist, unsigned long long* key_or_and,
-                               int single_key_type, uint16_t* bin_ids) {
-  const int nb = owner_mod > 0 ? owner_mod : num_buckets;
-  const int64_t ntiles = ceil_div(nrows, FusedCfg<PEER>::kTile);
-  const ModConst bm = make_mod_const((uint32_t)num_buckets), om = make_mod_const((uint32_t)std::max(owner_mod, 1));
-  const int uo = owner_mod > 0 ? 1 : 0;
+void launch_tile_hist(hs_ctx* ctx, const HashedRows& h, unsigned long long* global_hist, unsigned long long* key_or_and) {
+  const ModConst bm = make_mod_const((uint32_t)h.num_buckets), om = make_mod_const((uint32_t)std::max(h.owner_mod, 1));
+  const int uo = h.owner_mod > 0 ? 1 : 0;
 #define HS_HIST(KT)                                                                                                       \
-  k_tile_hist<KT, PEER><<<(unsigned)ntiles, FusedCfg<PEER>::kThreads, (size_t)nb * 4, ctx->stream>>>(                     \
-      d_keys, nkeys, nrows, bm, om, uo, tile_hist, global_hist, key_or_and, bin_ids)
-  switch (single_key_type) {
+  k_tile_hist<KT, PEER><<<(unsigned)h.ntiles, FusedCfg<PEER>::kThreads, (size_t)h.nbins * 4, ctx->stream>>>(             \
+      h.keys.get(), h.nkeys, h.nrows, bm, om, uo, h.tile_hist.get(), global_hist, key_or_and, h.bin_ids.get())
+  switch (h.single_key_type) {
     case HS_TYPE_INT32: HS_HIST(HS_TYPE_INT32); break;
     case HS_TYPE_INT64: HS_HIST(HS_TYPE_INT64); break;
     default: HS_HIST(-1); break;
   }
 #undef HS_HIST
   HS_LAUNCH_CHECK(ctx);
-}
-
-void launch_tile_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod,
-                      uint32_t* tile_hist, unsigned long long* global_hist, unsigned long long* key_or_and,
-                      int single_key_type, uint16_t* bin_ids, bool peer_tiles) {
-  KernelScope _ks(ctx, "k_tile_hist");
-  if (nrows == 0) return;
-  if (peer_tiles && peer_tile_shape())
-    launch_tile_hist_t<true>(ctx, d_keys, nkeys, nrows, num_buckets, owner_mod, tile_hist, global_hist, key_or_and, single_key_type, bin_ids);
-  else
-    launch_tile_hist_t<false>(ctx, d_keys, nkeys, nrows, num_buckets, owner_mod, tile_hist, global_hist, key_or_and, single_key_type, bin_ids);
 }
 
 struct PartitionLaunch {
@@ -834,34 +755,27 @@ struct PartitionLaunch {
   int out_world;
   CodePackRound pack;
   const uint16_t* bin_ids;
-  int bulk;
 };
 
-template <int BITS, int KT, bool PEER, bool BULK>
-static void launch_partition_rows_tb(hs_ctx* ctx, const PartitionLaunch& a) {
+template <int BITS, int KT, bool PEER>
+void launch_partition_rows_t(hs_ctx* ctx, const PartitionLaunch& a) {
   const int nb = a.owner_mod > 0 ? a.owner_mod : a.num_buckets;
   const int64_t ntiles = ceil_div(a.nrows, FusedCfg<PEER>::kTile);
   static DeviceOnce attr_once;  // one per instantiation
   bool& attr = attr_once(ctx->device);
   if (!attr) {
-    HS_CUDA(cudaFuncSetAttribute(k_partition_rows<BITS, KT, PEER, BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)fused_smem_bytes<PEER>(kFusedMaxBins, BULK)));
+    HS_CUDA(cudaFuncSetAttribute(k_partition_rows<BITS, KT, PEER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)fused_smem_bytes<PEER>(kFusedMaxBins)));
     attr = true;
   }
-  k_partition_rows<BITS, KT, PEER, BULK><<<(unsigned)ntiles, FusedCfg<PEER>::kThreads, fused_smem_bytes<PEER>(nb, BULK), ctx->stream>>>(
+  k_partition_rows<BITS, KT, PEER><<<(unsigned)ntiles, FusedCfg<PEER>::kThreads, fused_smem_bytes<PEER>(nb), ctx->stream>>>(
       a.d_keys, a.nkeys, a.nrows, make_mod_const((uint32_t)a.num_buckets), make_mod_const((uint32_t)std::max(a.owner_mod, 1)),
       a.owner_mod > 0 ? 1 : 0, a.tile_dst, a.d_cols, a.ncols, a.d_peer_out, a.out_world, a.pack, a.bin_ids);
   HS_LAUNCH_CHECK(ctx);
 }
 
-template <int BITS, int KT, bool PEER>
-static void launch_partition_rows_t(hs_ctx* ctx, const PartitionLaunch& a) {
-  if (a.bulk) launch_partition_rows_tb<BITS, KT, PEER, true>(ctx, a);
-  else launch_partition_rows_tb<BITS, KT, PEER, false>(ctx, a);
-}
-
 template <int BITS, bool PEER>
-static void launch_partition_rows_bits(hs_ctx* ctx, const PartitionLaunch& a, int single_key_type) {
+void launch_partition_rows_bits(hs_ctx* ctx, const PartitionLaunch& a, int single_key_type) {
   switch (single_key_type) {
     case HS_TYPE_INT32: launch_partition_rows_t<BITS, HS_TYPE_INT32, PEER>(ctx, a); break;
     case HS_TYPE_INT64: launch_partition_rows_t<BITS, HS_TYPE_INT64, PEER>(ctx, a); break;
@@ -870,7 +784,7 @@ static void launch_partition_rows_bits(hs_ctx* ctx, const PartitionLaunch& a, in
 }
 
 template <bool PEER>
-static void launch_partition_rows_cfg(hs_ctx* ctx, const PartitionLaunch& a, int single_key_type) {
+void launch_partition_rows(hs_ctx* ctx, const PartitionLaunch& a, int single_key_type) {
   const int nb = a.owner_mod > 0 ? a.owner_mod : a.num_buckets;
   // the ranking votes once per bin-id bit: 4, 8 or 10 (kFusedMaxBins = 1024)
   if (nb <= 16) launch_partition_rows_bits<4, PEER>(ctx, a, single_key_type);
@@ -878,20 +792,58 @@ static void launch_partition_rows_cfg(hs_ctx* ctx, const PartitionLaunch& a, int
   else launch_partition_rows_bits<10, PEER>(ctx, a, single_key_type);
 }
 
-void launch_partition_rows(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod,
-                           const uint32_t* tile_dst, const PartColumn* d_cols, int ncols, void* const* d_peer_out,
-                           int out_world, int single_key_type, const CodePackRound* pack_round, const uint16_t* bin_ids) {
-  KernelScope _ks(ctx, "k_partition_rows");
+}  // namespace
+
+int partition_tile_rows(hs_ctx* ctx, int num_buckets) {
+  if (num_buckets > kFusedMaxBins) return 0;
+  return ctx->world > 1 ? kFusedTilePeer : kFusedTileLocal;
+}
+
+void hash_rows(hs_ctx* ctx, const KeyColumn* keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod, bool to_peers,
+               unsigned long long* global_hist, unsigned long long* key_or_and, HashedRows* out) {
+  HashedRows& h = *out;
+  h.nrows = nrows;
+  h.num_buckets = num_buckets;
+  h.owner_mod = owner_mod;
+  h.nbins = owner_mod > 0 ? owner_mod : num_buckets;
+  if (to_peers && h.nbins > kFusedMaxBins) fail(HS_EINVAL, "%d bins: rows go to peer GPUs only up to %d", h.nbins, kFusedMaxBins);
+  h.to_peers = to_peers;
+  h.single_key_type = single_key_type_of(keys, nkeys);
+  h.nkeys = nkeys;
+  h.keys.alloc(ctx, nkeys);
+  copy_h2d(ctx, h.keys.get(), keys, sizeof(KeyColumn) * nkeys);
+  // the unfused partition's tile is the local one: k_partition_dest ranks the rows k_tile_hist counted
+  h.ntiles = ceil_div(nrows, to_peers ? kFusedTilePeer : kFusedTileLocal);
+  h.tile_hist.alloc(ctx, std::max<int64_t>(1, h.ntiles) * h.nbins);
+  if (owner_mod == 0) h.bin_ids.alloc(ctx, std::max<int64_t>(1, nrows));
+  KernelScope _ks(ctx, "k_tile_hist");
   if (nrows == 0) return;
-  // HS_PART_BULK=0|1: plain 8-byte stores or cp.async.bulk runs (A/B switch; default: bulk when the runs leave over NVLink)
-  static const char* bulk_env = getenv("HS_PART_BULK");
-  const int bulk = bulk_env ? atoi(bulk_env) : (d_peer_out ? 1 : 0);
-  PartitionLaunch a{d_keys, nkeys, nrows, num_buckets, owner_mod, tile_dst, d_cols, ncols, d_peer_out, out_world, {}, bin_ids, bulk};
+  if (to_peers) launch_tile_hist<true>(ctx, h, global_hist, key_or_and);
+  else launch_tile_hist<false>(ctx, h, global_hist, key_or_and);
+}
+
+void move_rows(hs_ctx* ctx, const HashedRows& h, const PartColumn* cols, int ncols, const CodePackRound* pack,
+               void* const* peer_out) {
+  if ((peer_out != nullptr) != h.to_peers) fail(HS_EINVAL, "move_rows: a peer table is needed exactly when rows go to peers");
+  if (h.nbins > kFusedMaxBins) {  // bin ids -> destinations -> one scatter per column
+    if (pack && pack->n > 0) fail(HS_EINVAL, "%d bins: code records need at most %d bins", h.nbins, kFusedMaxBins);
+    for (int c = 0; c < ncols; c++)
+      if (cols[c].tiles) fail(HS_EINVAL, "%d bins: columns are read in place only up to %d bins", h.nbins, kFusedMaxBins);
+    Buf<uint32_t> dest(ctx, std::max<int64_t>(1, h.nrows));
+    launch_partition_dest(ctx, h.bin_ids.get(), h.nrows, h.nbins, h.tile_hist.get(), dest.get());
+    for (int c = 0; c < ncols; c++) launch_scatter_column(ctx, cols[c].in, cols[c].out, dest.get(), h.nrows, cols[c].width);
+    return;
+  }
+  Buf<PartColumn> d_cols(ctx, std::max(1, ncols));
+  copy_h2d(ctx, d_cols.get(), cols, sizeof(PartColumn) * ncols);
+  KernelScope _ks(ctx, "k_partition_rows");
+  if (h.nrows == 0) return;
+  PartitionLaunch a{h.keys.get(), h.nkeys, h.nrows, h.num_buckets, h.owner_mod, h.tile_hist.get(), d_cols.get(), ncols,
+                    peer_out, h.to_peers ? ctx->world : 1, {}, h.bin_ids.get()};
   memset(&a.pack, 0, sizeof a.pack);
-  if (pack_round) a.pack = *pack_round;
-  // tiles that leave over NVLink use the large shape (the tile histogram must have been taken with peer_tiles = true)
-  if (d_peer_out && peer_tile_shape()) launch_partition_rows_cfg<true>(ctx, a, single_key_type);
-  else launch_partition_rows_cfg<false>(ctx, a, single_key_type);
+  if (pack) a.pack = *pack;
+  if (h.to_peers) launch_partition_rows<true>(ctx, a, h.single_key_type);
+  else launch_partition_rows<false>(ctx, a, h.single_key_type);
 }
 
 }  // namespace hs

@@ -161,30 +161,39 @@ struct KeyColumn {
 // -1 (a descriptor built without key_column_of) hashes by the type, as before decimals existed
 __host__ __device__ __forceinline__ int key_hash_kind(const KeyColumn& k) { return k.hash >= 0 ? k.hash : k.type; }
 
-constexpr int kPartTile = 4096;   // rows per partition tile (256 threads x 16)
 constexpr int kMaxBuckets = 4096;
 
-// bucket id per row + per-tile histograms M[tile][nb] + global histogram + OR/AND of the first key's sort encoding
-void launch_bucket_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets,
-                        uint16_t* bucket, uint32_t* tile_hist, unsigned long long* global_hist);
-// same, but bins are the owner ranks (bucket % world) -- the map side of the multi-GPU exchange
-void launch_owner_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int world,
-                       uint16_t* owner, uint32_t* tile_hist, unsigned long long* global_hist);
+// The hash partition (K2 + K3): every row's bucket is pmod(murmur3(keys, seed 42), num_buckets); its bin is the bucket, or
+// the owner rank bucket % owner_mod.  The rows then move stably into bin-major order.  hash_rows and move_rows choose the
+// kernels: up to 1024 bins one kernel moves every column through shared memory (the fused partition, which can also read
+// columns in place and carry dictionary codes); above that, a destination per row and a scatter per column.
+//
+// Rows per tile of the partition that runs on ctx for num_buckets buckets, i.e. the tile a column read in place
+// (ZcTile) is laid out for: 8192 when the runs go to peer GPUs (world > 1), else 4096.  0: the unfused partition, which
+// takes neither carried nor in-place columns.
+constexpr int kFusedTileLocal = 4096;  // rows per tile when the partition writes local memory (256 threads x 16)
+constexpr int kFusedTilePeer = 8192;   // ... and when it writes peer GPUs' memory over NVLink (512 threads x 16)
+int partition_tile_rows(hs_ctx* ctx, int num_buckets);
+struct HashedRows {
+  int64_t nrows = 0, ntiles = 0;
+  int num_buckets = 0, owner_mod = 0, nbins = 0;
+  bool to_peers = false;    // the runs go to the owners' memory (move_rows with a peer table)
+  int single_key_type = -1;
+  int nkeys = 0;
+  Buf<KeyColumn> keys;      // device copy of the key descriptors
+  Buf<uint32_t> tile_hist;  // ntiles x nbins; launch_tile_offsets turns the counts into destinations in place
+  Buf<uint16_t> bin_ids;    // every row's bin; not kept by the owner pass (owner_mod > 0), whose partition hashes again
+};
+// K2: hashes the key columns (host descriptors from key_column_of), counts the tile and global histograms
+// (global_hist: nbins entries, zero on entry) and keeps every row's bin.  key_or_and (optional, {0, ~0} on entry):
+// accumulates OR / AND of the sort-encoded values of the last key column.
+void hash_rows(hs_ctx* ctx, const KeyColumn* keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod, bool to_peers,
+               unsigned long long* global_hist, unsigned long long* key_or_and, HashedRows* out);
 // in-place: tile_hist[t][b] <- bucket_base[b] + sum_{t'<t} tile_hist[t'][b]   (bucket_base = exclusive scan of global hist)
 // explicit_base (optional, device, nb entries): start of every bucket's destination instead of the local scan
 void launch_tile_offsets(hs_ctx* ctx, uint32_t* tile_hist, int64_t ntiles, int num_buckets,
                          const unsigned long long* global_hist, unsigned long long* bucket_offsets /* nb+1 or null */,
                          const unsigned long long* explicit_base = nullptr);
-// dest[row] = stable position of the row in bucket-major order
-void launch_partition_dest(hs_ctx* ctx, const uint16_t* bucket, int64_t nrows, int num_buckets,
-                           const uint32_t* tile_offsets, uint32_t* dest);
-// out[dest[i]] = in[i]
-void launch_scatter_column(hs_ctx* ctx, const void* in, void* out, const uint32_t* dest, int64_t nrows, int width);
-// ---- fused partition (hash + stable rank + shared-memory exchange of every column in one kernel) ------------------
-constexpr int kFusedTileLocal = 4096;  // rows per tile when the partition writes local memory (256 threads x 16)
-constexpr int kFusedTilePeer = 8192;   // ... and when it writes peer GPUs' memory over NVLink (512 threads x 16)
-int fused_tile_rows(bool peer_tiles);
-constexpr int kFusedMaxBins = 1024;  // above this the per-warp counters no longer fit next to the exchange buffer
 struct PartColumn {
   const void* in;
   void* out;
@@ -192,33 +201,20 @@ struct PartColumn {
   int32_t pad;
   const ZcTile* tiles = nullptr;  // zero-copy source (in == nullptr), see KeyColumn::tiles
 };
-bool fused_partition_supported(int nbins);
-// bin_ids (optional): receives every row's bin so that launch_partition_rows (same argument) need not hash again
-// key_or_and (optional, {0, ~0} on entry): accumulates OR / AND of the sort-encoded values of the last key column
-// tile histograms M[tile][bin] for fused_tile_rows(peer_tiles)-row tiles (+ global histogram); bin = bucket, or bucket % owner_mod
-void launch_tile_hist(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod,
-                      uint32_t* tile_hist, unsigned long long* global_hist,
-                      unsigned long long* key_or_and = nullptr, int single_key_type = -1, uint16_t* bin_ids = nullptr,
-                      bool peer_tiles = false);
-// single_key_type: HS_TYPE_INT32 / HS_TYPE_INT64 when there is exactly one key column, of that type and without nulls
-// (selects a kernel with the hash inlined for it); -1 otherwise.  See single_key_type_of().
-inline int single_key_type_of(const KeyColumn* h_keys, int nkeys) {
-  return nkeys == 1 && h_keys[0].valid == nullptr && (h_keys[0].type == 0 || h_keys[0].type == 1) ? h_keys[0].type : -1;
-}
-// tile_dst = launch_tile_offsets(tile_hist); moves all columns into bin-major order, stable
-// d_peer_out (optional): [ncols][out_world] peer-mapped output pointers; bucket b is written to GPU b % out_world
-// pack (optional, single GPU only): one more round that reads up to four 16-bit code columns and writes them as ONE
-// 8-byte record per row (slot s in bits [16 s, 16 s + 16)) -- the layout k_dict_pack_all gathers from
+// pack: one more round that reads up to four 16-bit code columns and writes them as ONE 8-byte record per row (slot s in
+// bits [16 s, 16 s + 16)) -- the layout k_dict_pack_all gathers from
 struct CodePackRound {
   const uint16_t* src[4];
   void* out;   // nrows x 8 bytes
   int32_t n;   // code columns in use (0: no such round)
   int32_t pad;
 };
-void launch_partition_rows(hs_ctx* ctx, const KeyColumn* d_keys, int nkeys, int64_t nrows, int num_buckets, int owner_mod,
-                           const uint32_t* tile_dst, const PartColumn* d_cols, int ncols, void* const* d_peer_out = nullptr,
-                           int out_world = 1, int single_key_type = -1, const CodePackRound* pack = nullptr,
-                           const uint16_t* bin_ids = nullptr);
+// K3, after launch_tile_offsets(h.tile_hist): moves the columns (host descriptors, read until the caller's next
+// synchronisation) into bin-major order, stable.  pack (optional): the code records, fused partition only.
+// peer_out (to_peers only): device table of peer-mapped output pointers, one row of ctx->world per column round and then
+// one for the code records; bucket b is written to GPU b % world.
+void move_rows(hs_ctx* ctx, const HashedRows& h, const PartColumn* cols, int ncols, const CodePackRound* pack = nullptr,
+               void* const* peer_out = nullptr);
 // out[i] = sort_encode(in[src ? src[i] : i])  (+ global OR / AND reduction into or_and[0], or_and[1])
 void launch_encode_keys(hs_ctx* ctx, const void* in, int type, const uint32_t* src, int64_t nrows, uint64_t* out,
                         unsigned long long* or_and);

@@ -14,19 +14,12 @@
  * entry points; use one ctx per host thread / per rank.
  *
  * Environment switches (diagnostics and A/B measurements only; results are identical either way):
- *   HS_EXCHANGE=nccl   multi-GPU: NCCL all-to-all instead of the fused partition + NVLink peer stores
  *   HS_NO_CARRY=1      decode dictionary-encoded included columns to values instead of carrying 16-bit codes
  *                      (on several GPUs all ranks must agree)
  *   HS_LSD_SORT=1      sort the first key column with LSD passes over its high bytes + tie fix-up instead of the
  *                      shared-memory local sort (directly, or after one MSD pass)
- *   HS_PART_REHASH=1   partition kernel hashes the keys again instead of reading the stored bucket ids
  *   HS_NO_ZEROCOPY=1   decode aligned PLAIN pages into column arrays instead of reading them in place
- *   HS_PART_BULK=0|1   partition kernel: per-thread stores (0) or cp.async.bulk stores of whole runs (1); default: bulk only for
- *                      runs that leave over NVLink
- *   HS_PEER_TILE=small multi-GPU: the 4096-row partition tile of the single-GPU path instead of the 8192-row one
- *   HS_DEBUG_LOCAL_PEERS=1  multi-GPU: every rank keeps its rows (peer stores go to local memory; wrong results, isolates
- *                      the NVLink share of the exchange time) -- the one switch that changes results
- *   HS_IO_THREADS=n    host threads that read source files / write bucket files (default 16, at most half the cores)
+ *   HS_IO_THREADS=n   host threads that read source files / write bucket files (default 16, at most half the cores)
  *   HS_TIMELINE=1      print the event timeline (H2D / build / D2H begin and end) of every staged or asynchronous call
  */
 #ifndef HS_GPU_H

@@ -46,7 +46,7 @@ def test_golden_vectors_on_gpu(ctx):
     assert h.sum() == 5
 
 
-@pytest.mark.parametrize("nb", [1, 7, 200, 1000, 4096])
+@pytest.mark.parametrize("nb", [1, 7, 200, 1000, 1024, 1025, 4096])
 def test_bucket_ids_match_oracle(ctx, nb):
     rng = np.random.default_rng(nb)
     n = 300_000
@@ -70,13 +70,33 @@ def test_bucket_ids_null_keys(ctx):
     assert np.array_equal(got, O.bucket_ids([k], 200, [valid]))
 
 
+def test_bucket_ids_come_from_the_build_kernel(ctx):
+    """hs_k_bucket_ids runs the hash step of createIndex (k_tile_hist) on both sides of the fused partition's 1024 bins."""
+    rng = np.random.default_rng(4)
+    n = 20_000
+    k64 = rng.integers(-2**63, 2**63 - 1, size=n, dtype=np.int64)
+    k32 = rng.integers(-2**31, 2**31 - 1, size=n, dtype=np.int32)
+    valids = [(rng.random(n) > 0.2).astype(np.uint8), (rng.random(n) > 0.5).astype(np.uint8)]
+    for cols, vs in (([k64], None), ([k32, k64], valids)):
+        for nb in (200, 2048):
+            ctx.profile_enable(True)
+            try:
+                got, _ = ctx.k_bucket_ids(cols, nb, vs)
+                kernels = ctx.profile_report()
+            finally:
+                ctx.profile_enable(False)
+            assert "k_tile_hist" in kernels and "k_bucket_hist" not in kernels, kernels
+            assert np.array_equal(got, O.bucket_ids(cols, nb, vs))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # K3 + K4: partition + segmented sort
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("n,nb,lo,hi", [(1, 200, -5, 5), (100, 3, -5, 5), (4096, 1, 0, 50), (4097, 200, -2**63, 2**63 - 1),
                                          (250_000, 200, -2**63, 2**63 - 1), (250_000, 13, -50, 50),
-                                         (1_000_000, 200, 0, 2**31)])
+                                         (1_000_000, 200, 0, 2**31), (250_000, 1024, -2**63, 2**63 - 1),
+                                         (250_000, 1025, -2**63, 2**63 - 1), (300_000, 4096, 0, 2**31)])
 def test_sort_perm_matches_oracle_exactly(ctx, n, nb, lo, hi):
     rng = np.random.default_rng(n + nb)
     k = rng.integers(lo, hi, size=n, dtype=np.int64)
@@ -127,11 +147,12 @@ def test_sort_perm_nulls_first(ctx):
     k = rng.integers(-100, 100, size=n, dtype=np.int64)
     valid = (rng.random(n) > 0.1).astype(np.uint8)
     k = np.where(valid.astype(bool), k, 0)  # decoded nulls hold 0
-    perm, offs = ctx.k_sort_perm([k], 8, [valid])
-    b = O.bucket_ids([k], 8, [valid])
-    want_perm, want_offs = O.sort_perm([k], 8, b, [valid])
-    assert np.array_equal(offs, want_offs)
-    assert np.array_equal(perm, want_perm)
+    for nb in (8, 2000):  # 2000: the unfused partition scatters the validity bytes as a width-1 column
+        perm, offs = ctx.k_sort_perm([k], nb, [valid])
+        b = O.bucket_ids([k], nb, [valid])
+        want_perm, want_offs = O.sort_perm([k], nb, b, [valid])
+        assert np.array_equal(offs, want_offs)
+        assert np.array_equal(perm, want_perm)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -408,6 +429,49 @@ def test_create_index_with_nulls(ctx, tmp_path):
         m = kvalid & (k >= -10) & (k <= 10)
         assert batch.num_rows == int(m.sum())
         res.free()
+
+
+@pytest.mark.parametrize("nb", [1024, 1025, 4096])
+def test_create_index_on_both_sides_of_the_fused_partition(ctx, tmp_path, nb):
+    """Up to 1024 buckets k_partition_rows moves the rows; above, k_partition_dest + k_scatter at widths 8, 4 and 1."""
+    from hyperspace_b200 import _native
+
+    rng = np.random.default_rng(nb)
+    n = 300_000
+    cols = {"k": rng.integers(-2**63, 2**63 - 1, size=n, dtype=np.int64), "a": rng.integers(-2**40, 2**40, size=n, dtype=np.int64),
+            "d": rng.standard_normal(n), "i": rng.integers(-1000, 1000, size=n, dtype=np.int32),
+            "f": rng.standard_normal(n).astype(np.float32)}
+    ivalid = rng.random(n) > 0.3
+    p = str(tmp_path / "s.parquet")
+    pq.write_table(pa.table({**cols, "i": pa.array(cols["i"], mask=~ivalid)}), p, compression="NONE", use_dictionary=False)
+    ctx.profile_enable(True)
+    try:
+        res, st = ctx.create_index([_native.FileImage(path=p)], ["k"], ["a", "d", "i", "f"], nb, output=_native.HS_OUT_HOST,
+                                   job_uuid="fp")
+        kernels = ctx.profile_report()
+    finally:
+        ctx.profile_enable(False)
+    assert ("k_partition_dest" in kernels) == (nb > 1024) and ("k_partition_rows" in kernels) == (nb <= 1024), kernels
+    assert st["rows_out"] == n
+    perm, offs, order = O.index_rows(cols, ["k"], ["a", "d", "i", "f"], nb)
+    masks = {name: np.ones(n, bool) for name in order}
+    masks["i"] = ivalid
+    total = 0
+    for i, f in enumerate(res.files):
+        assert f.name == O.bucket_file_name(f.bucket, "fp")
+        t = _read_image(res.host_bytes(i))
+        lo, hi = int(offs[f.bucket]), int(offs[f.bucket + 1])
+        assert t.num_rows == hi - lo and t.column_names == order
+        for name in order:
+            arr = t.column(name).combine_chunks()
+            want_valid = masks[name][perm[lo:hi]]
+            assert np.array_equal(np.asarray(arr.is_valid()), want_valid), (name, f.bucket)
+            got = np.asarray(arr.fill_null(0))
+            want = np.where(want_valid, cols[name][perm[lo:hi]], 0).astype(got.dtype)
+            assert np.array_equal(_bits(got), _bits(want)), (name, f.bucket)
+        total += t.num_rows
+    assert total == n
+    res.free()
 
 
 def test_errors_are_loud(ctx, tmp_path):
