@@ -115,7 +115,7 @@ EXPORTED_SYMBOLS = [
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
-    "hs_bucket_join_where",
+    "hs_bucket_join_where", "hs_k_inflate",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -219,6 +219,8 @@ def load_library() -> C.CDLL:
     L.hs_batch_string_offsets.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     L.hs_k_snappy_decompress.restype = C.c_int
     L.hs_k_snappy_decompress.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_int32), *err]
+    L.hs_k_inflate.restype = C.c_int
+    L.hs_k_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
     if L.hs_abi_version() != 1:
         raise HyperspaceGpuError(HS_EINVAL, f"ABI version mismatch: library {L.hs_abi_version()}, binding 1")
     _lib = L
@@ -698,6 +700,13 @@ class Context:
         _check(load_library().hs_k_snappy_decompress(self._h, stream, len(stream), out, uncompressed_len, C.byref(seq), err,
                                                      len(err)), err)
         return out.raw[:uncompressed_len], bool(seq.value)
+
+    def k_inflate(self, stream: bytes, uncompressed_len: int) -> bytes:
+        """The GZIP page decompressor on one page body (one or more gzip members) of `uncompressed_len` bytes."""
+        out = C.create_string_buffer(max(1, uncompressed_len))
+        err = C.create_string_buffer(1024)
+        _check(load_library().hs_k_inflate(self._h, stream, len(stream), out, uncompressed_len, err, len(err)), err)
+        return out.raw[:uncompressed_len]
 
     # ---- read side ----------------------------------------------------------------------------------
     def filter_scan(self, files: Sequence[FileImage], key: str, projected: Sequence[str], lo=None, hi=None, sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (),

@@ -14,6 +14,7 @@
 
 #include "device_utils.cuh"
 #include "engine.h"
+#include "inflate.h"
 #include "spark_types.h"
 
 using namespace hs;
@@ -1629,9 +1630,9 @@ int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out_bu
   return guarded(ctx, err, errlen, [&] {
     Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
     copy_h2d(ctx, d_in.get(), in, n);
-    SnappyBlob blob{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, 0u};
+    PageBlob blob{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, 0u};
     const int64_t blocks = snappy_blocks_of(blob.dst_len, 0);
-    Buf<SnappyBlob> d_blob(ctx, 1);
+    Buf<PageBlob> d_blob(ctx, 1);
     Buf<uint32_t> d_block_in(ctx, (size_t)blocks + 1), d_seq(ctx, 1), d_error(ctx, 1);
     copy_h2d(ctx, d_blob.get(), &blob, sizeof blob);
     fill_bytes(ctx, d_error.get(), 0, 4);
@@ -1643,6 +1644,25 @@ int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out_bu
     if (error) fail(HS_EFORMAT, "corrupt snappy stream (check %u)", error & 0xffffffu);
     if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
     if (sequential) *sequential = (int32_t)seq;
+  });
+}
+
+int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t out_len, char* err, size_t errlen) {
+  if (!ctx || (n && !in) || n > 0xffffffffull || out_len > 0xfffffff0ull || (out_len && !out_buf)) return HS_EINVAL;
+  return guarded(ctx, err, errlen, [&] {
+    Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
+    if (n) copy_h2d(ctx, d_in.get(), in, n);
+    PageBlob blob{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::GZIP};
+    Buf<PageBlob> d_blob(ctx, 1);
+    Buf<uint32_t> d_error(ctx, 1);
+    copy_h2d(ctx, d_blob.get(), &blob, sizeof blob);
+    fill_bytes(ctx, d_error.get(), 0, 4);
+    launch_inflate(ctx, d_blob.get(), 1, d_out.get(), d_error.get());
+    uint32_t error = 0;
+    copy_d2h(ctx, &error, d_error.get(), 4);
+    sync_stream(ctx);
+    if (error) fail(HS_EFORMAT, "corrupt gzip stream: %s (check %u)", gz::inflate_error_text(error & 0xffffffu), error & 0xffffffu);
+    if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
   });
 }
 

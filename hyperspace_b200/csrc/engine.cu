@@ -16,6 +16,7 @@
 
 #include "device_utils.cuh"
 #include "engine.h"
+#include "inflate.h"
 #include "spark_types.h"
 
 namespace hs {
@@ -60,6 +61,7 @@ const char* decode_error_text(uint32_t code) {
     case DERR_STRING_TOO_LONG: return "string / binary value longer than 65535 bytes";
     case DERR_SPARK_RANGE: return "timestamp that Spark 3.1 does not read (an INT96 value before 1900-01-01T00:00:00Z, or millis beyond the int64 micros range)";
     case DERR_DECIMAL_WIDTH: return "decimal value wider than its precision allows";
+    case DERR_GZIP: return "corrupt gzip stream";
   }
   return "unknown decode error";
 }
@@ -396,9 +398,9 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
       if (rg.num_rows == 0) continue;  // writers emit an empty row group for an empty table
       for (int c = 0; c < ncols; c++) {
         const pq::ColumnChunkMeta& cm = rg.columns[idx[c]];
-        if (cm.codec != pq::UNCOMPRESSED && cm.codec != pq::SNAPPY)
-          fail(HS_EUNSUPPORTED, "%s: column '%s' uses compression codec %d; the GPU path reads UNCOMPRESSED and SNAPPY pages", what,
-               columns[c].c_str(), cm.codec);
+        if (cm.codec != pq::UNCOMPRESSED && cm.codec != pq::SNAPPY && cm.codec != pq::GZIP)
+          fail(HS_EUNSUPPORTED, "%s: column '%s' uses compression codec %d; the GPU path reads UNCOMPRESSED, SNAPPY and GZIP pages",
+               what, columns[c].c_str(), cm.codec);
         any_compressed = any_compressed || cm.codec != pq::UNCOMPRESSED;
         if (cm.num_values != rg.num_rows)
           fail(HS_EFORMAT, "%s: column '%s' has %lld values for %lld rows", what, columns[c].c_str(), (long long)cm.num_values,
@@ -488,14 +490,14 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
            decode_error_text(code), detail);
     }
   };
-  // ---- snappy: decompress the compressed page bodies (and dictionary pages) into a scratch buffer, repoint the pages ----
+  // ---- snappy / GZIP: decompress the compressed page bodies (and dictionary pages) into a scratch buffer, repoint the pages ----
   Buf<uint8_t>& d_scratch = set.impl->d_scratch;
   if (any_compressed && n_pages > 0) {
     std::vector<PageDesc> h_pages((size_t)n_pages);
     copy_d2h(ctx, h_pages.data(), d_pages.get(), sizeof(PageDesc) * (size_t)n_pages);
     sync_stream(ctx);
     check_walk();
-    std::vector<SnappyBlob> blobs;
+    std::vector<PageBlob> blobs;
     std::map<const uint8_t*, uint64_t> dict_off;  // stored dictionary page -> scratch offset of its decompressed copy
     uint64_t cursor = 0;
     for (PageDesc& pg : h_pages) {
@@ -504,7 +506,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
         auto it = dict_off.find(pg.dict);
         if (it == dict_off.end()) {
           it = dict_off.emplace(pg.dict, cursor).first;
-          blobs.push_back(SnappyBlob{pg.dict, cursor, (uint32_t)pg.dict_size, (uint32_t)pg.dict_uncompressed_size, 0u, 1u, 0u, 0u});
+          blobs.push_back(PageBlob{pg.dict, cursor, (uint32_t)pg.dict_size, (uint32_t)pg.dict_uncompressed_size, 0u, 1u, 0u,
+                                   (uint32_t)pg.codec});
           cursor += round_up((size_t)pg.dict_uncompressed_size, 16) + 16;
         }
         pg.dict = (const uint8_t*)(uintptr_t)(it->second + 1);  // patched to a pointer below (offset + 1 marks "relocated")
@@ -514,8 +517,8 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
         const uint32_t prefix = pg.page_type == pq::DATA_PAGE_V2 ? (uint32_t)(pg.rep_bytes + std::max(0, pg.def_bytes)) : 0u;
         if (prefix > (uint32_t)pg.size || prefix > (uint32_t)pg.uncompressed_size)
           fail(HS_EFORMAT, "compressed page has level bytes beyond its size");
-        blobs.push_back(SnappyBlob{pg.data, cursor, (uint32_t)pg.size, (uint32_t)pg.uncompressed_size, prefix,
-                                   (uint32_t)(pg.is_compressed ? 1 : 0), 0u, 0u});
+        blobs.push_back(PageBlob{pg.data, cursor, (uint32_t)pg.size, (uint32_t)pg.uncompressed_size, prefix,
+                                 (uint32_t)(pg.is_compressed ? 1 : 0), 0u, (uint32_t)pg.codec});
         pg.data = (const uint8_t*)(uintptr_t)(cursor + 1);
         pg.size = -pg.uncompressed_size;  // negative: data is a scratch offset (+1)
         cursor += round_up((size_t)pg.uncompressed_size, 16) + 16;
@@ -533,21 +536,27 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
         pg.size = pg.uncompressed_size;
       }
     }
-    uint64_t total_blocks = 0;  // 64 KB output blocks, the unit of the decoder's parallelism
+    // each codec's kernels run over its own blobs: the snappy ones first, in page order, then the GZIP ones
+    const size_t n_snappy = (size_t)(std::stable_partition(blobs.begin(), blobs.end(),
+                                                           [](const PageBlob& b) { return b.codec == pq::SNAPPY; }) -
+                                     blobs.begin());
+    uint64_t total_blocks = 0;  // 64 KB output blocks, the unit of the snappy decoder's parallelism
     bool any_verbatim = false;
-    for (SnappyBlob& b : blobs) {
+    for (size_t i = 0; i < n_snappy; i++) {
+      PageBlob& b = blobs[i];
       any_verbatim = any_verbatim || b.prefix != 0 || !b.compressed;
       b.first_block = (uint32_t)total_blocks;
       total_blocks += snappy_blocks_of(b.dst_len, b.prefix);
     }
     if (total_blocks >= 0xffffffffull) fail(HS_EUNSUPPORTED, "more than 256 TB of compressed pages in one call");
-    Buf<SnappyBlob> d_blobs(ctx, std::max<size_t>(1, blobs.size()));
-    Buf<uint32_t> d_block_in(ctx, (size_t)total_blocks + 1), d_sequential(ctx, std::max<size_t>(1, blobs.size()));
-    copy_h2d(ctx, d_blobs.get(), blobs.data(), sizeof(SnappyBlob) * blobs.size());
+    Buf<PageBlob> d_blobs(ctx, std::max<size_t>(1, blobs.size()));
+    Buf<uint32_t> d_block_in(ctx, (size_t)total_blocks + 1), d_sequential(ctx, std::max<size_t>(1, n_snappy));
+    copy_h2d(ctx, d_blobs.get(), blobs.data(), sizeof(PageBlob) * blobs.size());
     copy_h2d(ctx, d_pages.get(), h_pages.data(), sizeof(PageDesc) * (size_t)n_pages);
-    launch_snappy_decompress(ctx, d_blobs.get(), (int64_t)blobs.size(), (int64_t)total_blocks, any_verbatim, d_block_in.get(),
+    launch_snappy_decompress(ctx, d_blobs.get(), (int64_t)n_snappy, (int64_t)total_blocks, any_verbatim, d_block_in.get(),
                              d_sequential.get(),
                              d_scratch.get(), d_flags.get());
+    launch_inflate(ctx, d_blobs.get() + n_snappy, (int64_t)(blobs.size() - n_snappy), d_scratch.get(), d_flags.get());
     sync_stream(ctx);  // host vectors go out of scope
   }
   // ---- strings: the dictionary pages of BYTE_ARRAY columns become tables of references --------------------------------------
@@ -785,6 +794,7 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
                        code == DERR_STRING_TOO_LONG || code == DERR_SPARK_RANGE)
                           ? HS_EUNSUPPORTED
                           : HS_EFORMAT;
+    if (code == DERR_GZIP) fail(ecode, "Parquet decode failed: %s: %s", decode_error_text(code), gz::inflate_error_text(detail));
     if ((code == DERR_SPARK_RANGE || code == DERR_DECIMAL_WIDTH) && detail < (uint32_t)ncols)
       fail(ecode, "Parquet decode failed: column '%s' holds a %s", columns[detail].c_str(), decode_error_text(code));
     fail(ecode, "Parquet decode failed: %s (detail %u)", decode_error_text(code), detail);

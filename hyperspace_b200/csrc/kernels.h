@@ -26,7 +26,7 @@ struct ChunkDesc {          // one per (file, row group, projected column)
   int32_t phys_type;        // pq::PhysType
   int32_t max_def;          // 0 (required) or 1 (optional)
   int32_t file_index;
-  int32_t codec;            // pq::Codec of the chunk (UNCOMPRESSED or SNAPPY)
+  int32_t codec;            // pq::Codec of the chunk (UNCOMPRESSED, SNAPPY or GZIP)
   int32_t conv;             // ValueConv
   int32_t type_length;      // FIXED_LEN_BYTE_ARRAY: bytes per value
   int32_t pad;
@@ -48,7 +48,7 @@ struct PageDesc {           // one per data page
   int32_t uncompressed_size;  // body bytes after decompression (== size for stored pages)
   // compressed chunks only: the chunk's dictionary page as stored, and whether this page / the dictionary is compressed
   int32_t dict_size, dict_uncompressed_size;
-  int32_t is_compressed;      // this page's values are snappy-compressed
+  int32_t is_compressed;      // this page's values are compressed with the chunk's codec
   int32_t codec;
   int32_t chunk;              // index of the column chunk (ChunkDesc) the page belongs to
   int32_t conv;               // ValueConv of the chunk
@@ -93,7 +93,8 @@ enum DecodeError : uint32_t {
   DERR_NONE = 0, DERR_BAD_HEADER = 1, DERR_UNSUPPORTED_ENCODING = 2, DERR_VALUE_COUNT = 3, DERR_COMPRESSED = 4,
   DERR_OVERRUN = 5, DERR_DICT_INDEX = 6, DERR_UNSUPPORTED_TYPE = 7, DERR_SNAPPY = 8, DERR_STRING_TOO_LONG = 9,
   DERR_SPARK_RANGE = 10,    // a timestamp Spark 3.1 refuses to read: INT96 before 1900, MILLIS beyond int64 micros (detail: column)
-  DERR_DECIMAL_WIDTH = 11   // a decimal value wider than its precision's int32 / int64 (detail: column)
+  DERR_DECIMAL_WIDTH = 11,  // a decimal value wider than its precision's int32 / int64 (detail: column)
+  DERR_GZIP = 12            // a GZIP page body fails a check of inflate.h (detail: gz::InflateError)
 };
 // BYTE_ARRAY dictionary pages -> tables of string references (device_utils.cuh: string_ref): one job per dictionary page,
 // walked by one thread (the entries are length-prefixed, so their positions are only found sequentially)
@@ -104,16 +105,17 @@ struct StringDictJob {
 };
 void launch_build_string_dicts(hs_ctx* ctx, const StringDictJob* jobs, int64_t n, uint32_t* d_error);
 
-// ---- snappy (snappy.cu) ---------------------------------------------------------------------------------------------
-struct SnappyBlob {
+// ---- compressed pages: snappy (snappy.cu) and GZIP (inflate.cu) ----------------------------------------------------------
+// one per compressed page (or dictionary page) of a call: where it lies, where its decompressed copy goes
+struct PageBlob {
   const uint8_t* src;   // stored bytes (device)
   uint64_t dst_off;     // offset of the decompressed bytes in the scratch buffer
   uint32_t src_len;
   uint32_t dst_len;     // prefix + decompressed length
   uint32_t prefix;      // leading bytes copied verbatim (v2 level bytes)
-  uint32_t compressed;  // 0: copy, 1: snappy
-  uint32_t first_block; // index of this page's first 64 KB output block in the block table (ascending over the blobs)
-  uint32_t pad;
+  uint32_t compressed;  // 0: copy, 1: compressed with `codec`
+  uint32_t first_block; // snappy: index of this page's first 64 KB output block in the block table (ascending over the blobs)
+  uint32_t codec;       // pq::Codec of the page's chunk: SNAPPY or GZIP
 };
 __host__ __device__ inline uint32_t snappy_blocks_of(uint32_t dst_len, uint32_t prefix) {
   const uint32_t body = dst_len - prefix;
@@ -121,8 +123,12 @@ __host__ __device__ inline uint32_t snappy_blocks_of(uint32_t dst_len, uint32_t 
 }
 // block_in: one uint32 per block (+1), sequential: one uint32 per blob -- scratch of the two launches
 // any_verbatim: some blob has a prefix or is stored uncompressed
-void launch_snappy_decompress(hs_ctx* ctx, const SnappyBlob* blobs, int64_t n, int64_t total_blocks, bool any_verbatim,
+void launch_snappy_decompress(hs_ctx* ctx, const PageBlob* blobs, int64_t n, int64_t total_blocks, bool any_verbatim,
                               uint32_t* block_in, uint32_t* sequential, uint8_t* scratch, uint32_t* d_error);
+
+// GZIP page bodies, one warp per blob: copies what is stored verbatim (prefix, or the whole page when !compressed) and
+// inflates the rest; a failed check sets (DERR_GZIP << 24 | gz::InflateError) in d_error
+void launch_inflate(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch, uint32_t* d_error);
 
 // compression of page bodies: one warp per fragment (<= 65536 bytes) of a page; fragment f of raw bytes [src_off, src_off +
 // len) is written to scratch at dst_off (room for 32 + len + len / 6 bytes), its compressed length to out_len[f]

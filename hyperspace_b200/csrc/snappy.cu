@@ -91,12 +91,12 @@ __device__ __forceinline__ Walk walk_segment(const uint8_t* __restrict__ src, ui
 
 // Pass 1: block_in[first_block + b] = position in the compressed stream (after the v2 prefix) of output block b;
 // sequential[w] = 1 when the page's blocks are not independent (or the stream looks damaged: the decoder reports it).
-__global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_index(const SnappyBlob* __restrict__ blobs, int64_t n,
+__global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_index(const PageBlob* __restrict__ blobs, int64_t n,
                                                                      uint32_t* __restrict__ block_in, uint32_t* __restrict__ sequential) {
   const unsigned lane = threadIdx.x & 31;
   const int64_t w = (int64_t)blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
   if (w >= n) return;
-  const SnappyBlob b = blobs[w];
+  const PageBlob b = blobs[w];
   if (!b.compressed) {
     if (lane == 0) sequential[w] = 0;
     return;
@@ -227,7 +227,7 @@ __device__ __forceinline__ void warp_copy(uint8_t* o, const uint8_t* lit, uint32
 }
 
 // Pass 2: one lane per 64 KB output block (or per page, for a page flagged sequential).
-__global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const SnappyBlob* __restrict__ blobs, int64_t n,
+__global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const PageBlob* __restrict__ blobs, int64_t n,
                                                                       int64_t total_blocks, const uint32_t* __restrict__ block_in,
                                                                       const uint32_t* __restrict__ sequential,
                                                                       uint8_t* __restrict__ scratch, uint32_t* __restrict__ d_error) {
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const Snapp
       const int64_t mid = (lo + hi + 1) >> 1;
       if ((int64_t)blobs[mid].first_block <= blk) lo = mid; else hi = mid - 1;
     }
-    const SnappyBlob b = blobs[lo];
+    const PageBlob b = blobs[lo];
     const uint32_t bi = (uint32_t)(blk - b.first_block);
     const bool seq = b.compressed && sequential[lo] != 0;
     live = b.compressed && !(seq && bi > 0);
@@ -314,11 +314,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const Snapp
 }
 
 // what is stored verbatim: v2 level bytes in front of the values, and pages stored uncompressed inside a compressed chunk
-__global__ void __launch_bounds__(256) k_snappy_levels(const SnappyBlob* __restrict__ blobs, int64_t n, uint8_t* __restrict__ scratch) {
+__global__ void __launch_bounds__(256) k_snappy_levels(const PageBlob* __restrict__ blobs, int64_t n, uint8_t* __restrict__ scratch) {
   const unsigned lane = threadIdx.x & 31;
   const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (w >= n) return;
-  const SnappyBlob b = blobs[w];
+  const PageBlob b = blobs[w];
   const uint32_t bytes = b.compressed ? b.prefix : min(b.src_len, b.dst_len);
   uint8_t* __restrict__ dst = scratch + b.dst_off;
   for (uint32_t j = lane; j < bytes; j += 32) dst[j] = b.src[j];
@@ -326,7 +326,7 @@ __global__ void __launch_bounds__(256) k_snappy_levels(const SnappyBlob* __restr
 
 }  // namespace
 
-void launch_snappy_decompress(hs_ctx* ctx, const SnappyBlob* blobs, int64_t n, int64_t total_blocks, bool any_verbatim,
+void launch_snappy_decompress(hs_ctx* ctx, const PageBlob* blobs, int64_t n, int64_t total_blocks, bool any_verbatim,
                               uint32_t* block_in, uint32_t* sequential, uint8_t* scratch, uint32_t* d_error) {
   if (n == 0) return;
   if (any_verbatim) {

@@ -399,6 +399,10 @@ int hs_k_snappy_compress(hs_ctx* ctx, const void* in, uint64_t n, void* out, uin
  * HS_EFORMAT for a damaged stream.  Kernel-level entry point for the parity tests. */
 int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t out_len, int32_t* sequential, char* err,
                            size_t errlen);
+/* The GZIP page decompressor (k_inflate) on one page body of n bytes -- one or more gzip members -- whose uncompressed
+ * length is out_len.  HS_EFORMAT for a damaged stream; the message names the failed check.  Kernel-level entry point for
+ * the parity tests. */
+int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t out_len, char* err, size_t errlen);
 
 #ifdef __cplusplus
 }
