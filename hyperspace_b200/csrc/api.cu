@@ -1588,36 +1588,18 @@ int hs_k_snappy_compress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf,
                          size_t errlen) {
   if (!ctx || !out_len || (n && !in)) return HS_EINVAL;
   return guarded(ctx, err, errlen, [&] {
-    std::vector<SnappyFragment> frags;
-    uint64_t slot = 0;
-    for (uint64_t o = 0; o < n; o += kSnappyFragment) {
-      const uint32_t len = (uint32_t)std::min<uint64_t>(kSnappyFragment, n - o);
-      frags.push_back(SnappyFragment{o, slot, len, 0});
-      slot += round_up(snappy_max_compressed(len), 16);
-    }
-    Buf<uint8_t> d_in(ctx, std::max<uint64_t>(n, 16) + 16), d_slots(ctx, std::max<uint64_t>(slot, 16));
-    Buf<SnappyFragment> d_frags(ctx, std::max<size_t>(1, frags.size()));
-    Buf<uint32_t> d_len(ctx, std::max<size_t>(1, frags.size()));
-    std::vector<uint32_t> lens(frags.size());
+    Buf<uint8_t> d_in(ctx, std::max<uint64_t>(n, 16) + 16);
     if (n) copy_h2d(ctx, d_in.get(), in, n);
-    copy_h2d(ctx, d_frags.get(), frags.data(), sizeof(SnappyFragment) * frags.size());
-    launch_snappy_compress(ctx, d_frags.get(), (int64_t)frags.size(), d_in.get(), d_slots.get(), d_len.get());
-    copy_d2h(ctx, lens.data(), d_len.get(), 4 * frags.size());
-    sync_stream(ctx);
+    CompressedBodies packed;
+    compress_bodies(ctx, d_in.get(), {{0, n}}, &packed);
     std::vector<uint8_t> stream;
-    for (uint64_t v = n;; v >>= 7) {  // preamble: the uncompressed length
-      if (v >= 0x80) stream.push_back((uint8_t)(v | 0x80));
-      else {
-        stream.push_back((uint8_t)v);
-        break;
-      }
-    }
-    std::vector<uint8_t> piece;
-    for (size_t f = 0; f < frags.size(); f++) {
-      piece.resize(lens[f]);
-      HS_CUDA(cudaMemcpy(piece.data(), d_slots.get() + frags[f].dst_off, lens[f], cudaMemcpyDeviceToHost));
-      stream.insert(stream.end(), piece.begin(), piece.end());
-    }
+    packed.append_preamble(0, stream);
+    std::vector<BlobCopy> pieces;
+    uint64_t end = stream.size();
+    packed.place(0, pieces, &end);
+    stream.resize(end);
+    for (const BlobCopy& pc : pieces)
+      HS_CUDA(cudaMemcpy(stream.data() + pc.dst, packed.slots.get() + pc.src, pc.len, cudaMemcpyDeviceToHost));
     *out_len = stream.size();
     if (stream.size() > cap) fail(HS_ENOMEM, "output buffer too small: %zu bytes needed", stream.size());
     if (out_buf) memcpy(out_buf, stream.data(), stream.size());
@@ -1630,20 +1612,17 @@ int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out_bu
   return guarded(ctx, err, errlen, [&] {
     Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
     copy_h2d(ctx, d_in.get(), in, n);
-    PageBlob blob{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, 0u};
-    const int64_t blocks = snappy_blocks_of(blob.dst_len, 0);
-    Buf<PageBlob> d_blob(ctx, 1);
-    Buf<uint32_t> d_block_in(ctx, (size_t)blocks + 1), d_seq(ctx, 1), d_error(ctx, 1);
-    copy_h2d(ctx, d_blob.get(), &blob, sizeof blob);
+    Buf<uint32_t> d_error(ctx, 1);
     fill_bytes(ctx, d_error.get(), 0, 4);
-    launch_snappy_decompress(ctx, d_blob.get(), 1, blocks, false, d_block_in.get(), d_seq.get(), d_out.get(), d_error.get());
-    uint32_t error = 0, seq = 0;
+    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::SNAPPY}};
+    std::vector<uint32_t> seq;
+    decompress_blobs(ctx, blob, d_out.get(), d_error.get(), &seq);
+    uint32_t error = 0;
     copy_d2h(ctx, &error, d_error.get(), 4);
-    copy_d2h(ctx, &seq, d_seq.get(), 4);
     sync_stream(ctx);
     if (error) fail(HS_EFORMAT, "corrupt snappy stream (check %u)", error & 0xffffffu);
     if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
-    if (sequential) *sequential = (int32_t)seq;
+    if (sequential) *sequential = (int32_t)seq[0];
   });
 }
 
@@ -1652,12 +1631,10 @@ int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_
   return guarded(ctx, err, errlen, [&] {
     Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
     if (n) copy_h2d(ctx, d_in.get(), in, n);
-    PageBlob blob{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::GZIP};
-    Buf<PageBlob> d_blob(ctx, 1);
     Buf<uint32_t> d_error(ctx, 1);
-    copy_h2d(ctx, d_blob.get(), &blob, sizeof blob);
     fill_bytes(ctx, d_error.get(), 0, 4);
-    launch_inflate(ctx, d_blob.get(), 1, d_out.get(), d_error.get());
+    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::GZIP}};
+    decompress_blobs(ctx, blob, d_out.get(), d_error.get());
     uint32_t error = 0;
     copy_d2h(ctx, &error, d_error.get(), 4);
     sync_stream(ctx);

@@ -490,74 +490,13 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
            decode_error_text(code), detail);
     }
   };
-  // ---- snappy / GZIP: decompress the compressed page bodies (and dictionary pages) into a scratch buffer, repoint the pages ----
-  Buf<uint8_t>& d_scratch = set.impl->d_scratch;
+  // ---- compressed pages (and dictionary pages) are decompressed into a scratch buffer and the pages repointed at it ----
   if (any_compressed && n_pages > 0) {
     std::vector<PageDesc> h_pages((size_t)n_pages);
     copy_d2h(ctx, h_pages.data(), d_pages.get(), sizeof(PageDesc) * (size_t)n_pages);
     sync_stream(ctx);
     check_walk();
-    std::vector<PageBlob> blobs;
-    std::map<const uint8_t*, uint64_t> dict_off;  // stored dictionary page -> scratch offset of its decompressed copy
-    uint64_t cursor = 0;
-    for (PageDesc& pg : h_pages) {
-      if (pg.codec == pq::UNCOMPRESSED) continue;
-      if (pg.dict) {  // the dictionary page of a compressed chunk is compressed too
-        auto it = dict_off.find(pg.dict);
-        if (it == dict_off.end()) {
-          it = dict_off.emplace(pg.dict, cursor).first;
-          blobs.push_back(PageBlob{pg.dict, cursor, (uint32_t)pg.dict_size, (uint32_t)pg.dict_uncompressed_size, 0u, 1u, 0u,
-                                   (uint32_t)pg.codec});
-          cursor += round_up((size_t)pg.dict_uncompressed_size, 16) + 16;
-        }
-        pg.dict = (const uint8_t*)(uintptr_t)(it->second + 1);  // patched to a pointer below (offset + 1 marks "relocated")
-        pg.dict_size = -1;
-      }
-      if (pg.is_compressed || pg.size != pg.uncompressed_size) {
-        const uint32_t prefix = pg.page_type == pq::DATA_PAGE_V2 ? (uint32_t)(pg.rep_bytes + std::max(0, pg.def_bytes)) : 0u;
-        if (prefix > (uint32_t)pg.size || prefix > (uint32_t)pg.uncompressed_size)
-          fail(HS_EFORMAT, "compressed page has level bytes beyond its size");
-        blobs.push_back(PageBlob{pg.data, cursor, (uint32_t)pg.size, (uint32_t)pg.uncompressed_size, prefix,
-                                 (uint32_t)(pg.is_compressed ? 1 : 0), 0u, (uint32_t)pg.codec});
-        pg.data = (const uint8_t*)(uintptr_t)(cursor + 1);
-        pg.size = -pg.uncompressed_size;  // negative: data is a scratch offset (+1)
-        cursor += round_up((size_t)pg.uncompressed_size, 16) + 16;
-      }
-    }
-    d_scratch.alloc(ctx, std::max<uint64_t>(cursor, 16) + 16);  // decoders may read one aligned word past a page
-    for (PageDesc& pg : h_pages) {
-      if (pg.codec == pq::UNCOMPRESSED) continue;
-      if (pg.dict_size == -1) {
-        pg.dict = d_scratch.get() + ((uintptr_t)pg.dict - 1);
-        pg.dict_size = pg.dict_uncompressed_size;
-      }
-      if (pg.size < 0) {
-        pg.data = d_scratch.get() + ((uintptr_t)pg.data - 1);
-        pg.size = pg.uncompressed_size;
-      }
-    }
-    // each codec's kernels run over its own blobs: the snappy ones first, in page order, then the GZIP ones
-    const size_t n_snappy = (size_t)(std::stable_partition(blobs.begin(), blobs.end(),
-                                                           [](const PageBlob& b) { return b.codec == pq::SNAPPY; }) -
-                                     blobs.begin());
-    uint64_t total_blocks = 0;  // 64 KB output blocks, the unit of the snappy decoder's parallelism
-    bool any_verbatim = false;
-    for (size_t i = 0; i < n_snappy; i++) {
-      PageBlob& b = blobs[i];
-      any_verbatim = any_verbatim || b.prefix != 0 || !b.compressed;
-      b.first_block = (uint32_t)total_blocks;
-      total_blocks += snappy_blocks_of(b.dst_len, b.prefix);
-    }
-    if (total_blocks >= 0xffffffffull) fail(HS_EUNSUPPORTED, "more than 256 TB of compressed pages in one call");
-    Buf<PageBlob> d_blobs(ctx, std::max<size_t>(1, blobs.size()));
-    Buf<uint32_t> d_block_in(ctx, (size_t)total_blocks + 1), d_sequential(ctx, std::max<size_t>(1, n_snappy));
-    copy_h2d(ctx, d_blobs.get(), blobs.data(), sizeof(PageBlob) * blobs.size());
-    copy_h2d(ctx, d_pages.get(), h_pages.data(), sizeof(PageDesc) * (size_t)n_pages);
-    launch_snappy_decompress(ctx, d_blobs.get(), (int64_t)n_snappy, (int64_t)total_blocks, any_verbatim, d_block_in.get(),
-                             d_sequential.get(),
-                             d_scratch.get(), d_flags.get());
-    launch_inflate(ctx, d_blobs.get() + n_snappy, (int64_t)(blobs.size() - n_snappy), d_scratch.get(), d_flags.get());
-    sync_stream(ctx);  // host vectors go out of scope
+    decompress_pages(ctx, h_pages, d_pages.get(), &set.impl->d_scratch, d_flags.get());
   }
   // ---- strings: the dictionary pages of BYTE_ARRAY columns become tables of references --------------------------------------
   Buf<uint64_t> d_string_dicts;
@@ -1008,6 +947,8 @@ struct PagePlan {
   uint64_t hdr_off;   // arena offset of the page header
   uint32_t hdr_len;   // Thrift header bytes
   uint32_t body_len;  // page bytes behind the header
+  int32_t page_type;  // what the header says: pq::PageType, the number of values and their pq::Encoding
+  int32_t num_values, encoding;
 };
 struct FilePlan {
   int seg = 0;
@@ -1015,6 +956,34 @@ struct FilePlan {
   std::vector<pq::OutRowGroup> rgs;
   std::vector<std::pair<size_t, size_t>> chunk_pages;  // per (row group, column): first page, page count
 };
+// Appends the end of a file to `skeleton`: the footer, its length and the magic.  `at` is the arena offset the footer goes
+// to and seg_begin the sorted position of the file's first row: the min / max placeholders of the sorted key in the footer
+// become one StatPatch per row group.
+void append_file_end(const std::vector<pq::SchemaColumn>& schema, const std::vector<pq::OutRowGroup>& rgs, int64_t rows,
+                     const std::string& schema_json, uint64_t seg_begin, uint64_t at, std::vector<uint8_t>& skeleton,
+                     std::vector<StatPatch>& patches) {
+  std::vector<pq::StatSlot> slots;
+  std::vector<uint8_t> footer = pq::write_footer(schema, rgs, rows, schema_json, &slots);
+  for (const pq::StatSlot& sl : slots) {
+    StatPatch sp;
+    int64_t row0 = 0;
+    for (int g = 0; g < sl.row_group; g++) row0 += rgs[g].num_rows;
+    sp.first_pos = seg_begin + (uint64_t)row0;
+    sp.last_pos = sp.first_pos + (uint64_t)rgs[sl.row_group].num_rows - 1;
+    for (int j = 0; j < 2; j++) {
+      sp.min_off[j] = at + sl.min_off[j];
+      sp.max_off[j] = at + sl.max_off[j];
+    }
+    sp.width = sl.width;
+    sp.pad = 0;
+    patches.push_back(sp);
+  }
+  skeleton.insert(skeleton.end(), footer.begin(), footer.end());
+  const uint32_t flen = (uint32_t)footer.size();
+  const uint8_t* lp = (const uint8_t*)&flen;
+  skeleton.insert(skeleton.end(), lp, lp + 4);
+  skeleton.insert(skeleton.end(), {'P', 'A', 'R', '1'});
+}
 
 }  // namespace
 
@@ -1313,7 +1282,8 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
           copies.push_back(ByteCopy{cursor, (uint32_t)dicts[c].skel_off, (uint32_t)dicts[c].skel_len});
           if (compress) {
             const uint32_t hl = header_len_at(dicts[c].skel_off);
-            page_plans.push_back(PagePlan{cursor, hl, (uint32_t)(dicts[c].skel_len - hl)});
+            page_plans.push_back(PagePlan{cursor, hl, (uint32_t)(dicts[c].skel_len - hl), pq::DICTIONARY_PAGE,
+                                          (int32_t)dicts[c].ndict, pq::ENC_PLAIN_DICTIONARY});
           }
           cursor += dicts[c].skel_len;
           ch.data_page_offset = (int64_t)(cursor - file_off);
@@ -1380,7 +1350,8 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
           }
           if (compress) {
             const uint32_t hl = header_len_at(b);
-            page_plans.push_back(PagePlan{page_begin, hl, (uint32_t)(cursor - page_begin - hl)});
+            page_plans.push_back(PagePlan{page_begin, hl, (uint32_t)(cursor - page_begin - hl), pq::DATA_PAGE, (int32_t)np,
+                                          dicts[c].use ? pq::ENC_PLAIN_DICTIONARY : pq::ENC_PLAIN});
           }
         }
         ch.total_size = (int64_t)(cursor - chunk_begin);
@@ -1399,28 +1370,8 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
     }
     {
       const size_t b = skeleton.size();
-      std::vector<pq::StatSlot> slots;
-      std::vector<uint8_t> footer = pq::write_footer(schema, rgs, n, schema_json, &slots);
-      for (const pq::StatSlot& sl : slots) {
-        StatPatch sp;
-        int64_t row0 = 0;
-        for (int g = 0; g < sl.row_group; g++) row0 += rgs[g].num_rows;
-        sp.first_pos = req.seg_offsets[s] + (uint64_t)row0;
-        sp.last_pos = sp.first_pos + (uint64_t)rgs[sl.row_group].num_rows - 1;
-        for (int j = 0; j < 2; j++) {
-          sp.min_off[j] = cursor + sl.min_off[j];
-          sp.max_off[j] = cursor + sl.max_off[j];
-        }
-        sp.width = sl.width;
-        sp.pad = 0;
-        stat_patches.push_back(sp);
-      }
+      append_file_end(schema, rgs, n, schema_json, req.seg_offsets[s], cursor, skeleton, stat_patches);
       if (compress) file_plans.back().rgs = rgs;
-      skeleton.insert(skeleton.end(), footer.begin(), footer.end());
-      uint32_t flen = (uint32_t)footer.size();
-      const uint8_t* lp = (const uint8_t*)&flen;
-      skeleton.insert(skeleton.end(), lp, lp + 4);
-      skeleton.insert(skeleton.end(), {'P', 'A', 'R', '1'});
       emit(cursor, b);
       cursor += skeleton.size() - b;
     }
@@ -1468,7 +1419,6 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
   const std::vector<ColDict>& dicts = L.dicts;
   const std::vector<int>& carried_cols = L.carried_cols;
   const std::vector<StatPatch>& stat_patches = L.stat_patches;
-  const std::vector<uint8_t>& skeleton = L.skeleton;
   const std::vector<ByteCopy>& copies = L.copies;
   const bool compress = L.compress;
   const std::vector<PagePlan>& page_plans = L.page_plans;
@@ -1563,31 +1513,13 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
   }
   // ---- SNAPPY: the pages just written are compressed and the files laid out again ------------------------------------------
   // Compressed sizes are data: the files cannot be laid out before the pages exist.  So the uncompressed images above serve
-  // as the compressor's input; every page body is cut into 64 KB fragments that compress in parallel into worst-case sized
-  // slots; their lengths come back to the host, which lays the files out again (new page headers, new footers, the codec in
-  // every chunk) and a copy kernel moves the fragments into place.
+  // as the compressor's input; the compressed sizes of the page bodies come back to the host, which lays the files out
+  // again (new page headers, new footers, the codec in every chunk) and a copy kernel moves the compressed pieces into place.
   if (compress && !page_plans.empty()) {
-    std::vector<SnappyFragment> frags;
-    std::vector<size_t> page_first_frag(page_plans.size() + 1, 0);
-    uint64_t slot_cursor = 0;
-    for (size_t i = 0; i < page_plans.size(); i++) {
-      page_first_frag[i] = frags.size();
-      const PagePlan& pp = page_plans[i];
-      for (uint32_t o = 0; o < pp.body_len; o += kSnappyFragment) {
-        const uint32_t len = std::min<uint32_t>(kSnappyFragment, pp.body_len - o);
-        frags.push_back(SnappyFragment{pp.hdr_off + pp.hdr_len + o, slot_cursor, len, 0});
-        slot_cursor += round_up(snappy_max_compressed(len), 16);
-      }
-    }
-    page_first_frag[page_plans.size()] = frags.size();
-    Buf<uint8_t> d_slots(ctx, std::max<uint64_t>(slot_cursor, 16));
-    Buf<SnappyFragment> d_frags(ctx, std::max<size_t>(1, frags.size()));
-    Buf<uint32_t> d_flen(ctx, std::max<size_t>(1, frags.size()));
-    std::vector<uint32_t> flen(frags.size());
-    copy_h2d(ctx, d_frags.get(), frags.data(), sizeof(SnappyFragment) * frags.size());
-    launch_snappy_compress(ctx, d_frags.get(), (int64_t)frags.size(), out->arena.get(), d_slots.get(), d_flen.get());
-    copy_d2h(ctx, flen.data(), d_flen.get(), 4 * frags.size());
-    sync_stream(ctx);
+    std::vector<std::pair<uint64_t, uint64_t>> bodies;
+    for (const PagePlan& pp : page_plans) bodies.emplace_back(pp.hdr_off + pp.hdr_len, pp.body_len);
+    CompressedBodies packed;
+    compress_bodies(ctx, out->arena.get(), bodies, &packed);
     // second layout
     std::vector<uint8_t> skel2;
     std::vector<ByteCopy> copies2;
@@ -1598,10 +1530,6 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
       copies2.push_back(ByteCopy{cur2, (uint32_t)skel_begin, (uint32_t)(skel2.size() - skel_begin)});
       cur2 += skel2.size() - skel_begin;
     };
-    // header fields by destination offset
-    std::map<uint64_t, size_t> skel_at;  // arena offset -> skeleton position of the bytes copied there
-    for (const ByteCopy& bc : copies) skel_at[bc.dst] = bc.src;
-    size_t page_i = 0;
     std::vector<OutFile> files2;
     for (size_t fi = 0; fi < file_plans.size(); fi++) {
       FilePlan& fp = file_plans[fi];
@@ -1621,58 +1549,23 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
           const uint64_t chunk_begin = cur2;
           int64_t uncomp = 0;
           bool first_data = true;
-          for (size_t pi = range.first; pi < range.first + range.second; pi++, page_i++) {
+          for (size_t pi = range.first; pi < range.first + range.second; pi++) {
             const PagePlan& pp = page_plans[pi];
-            // parse the first layout's header of this page
-            auto it = skel_at.find(pp.hdr_off);
-            if (it == skel_at.end()) fail(HS_EINVAL, "internal: page header not found in the layout");
-            thrift::Reader r(skeleton.data() + it->second, skeleton.data() + it->second + pp.hdr_len);
-            int32_t ptype = -1, nvals = 0, enc = 0;
-            int16_t fid = 0;
-            for (;;) {
-              const uint8_t t = r.field(fid);
-              if (r.bad || t == thrift::T_STOP) break;
-              if (fid == 1) ptype = (int32_t)r.zigzag();
-              else if (fid == 5 || fid == 7) {
-                int16_t f2 = 0;
-                for (;;) {
-                  const uint8_t t2 = r.field(f2);
-                  if (r.bad || t2 == thrift::T_STOP) break;
-                  if (f2 == 1) nvals = (int32_t)r.zigzag();
-                  else if (f2 == 2) enc = (int32_t)r.zigzag();
-                  else r.skip(t2);
-                }
-              } else r.skip(t);
-            }
-            // compressed body = varint(uncompressed length) + the fragments' element streams
-            uint8_t pre[5];
-            int pl = 0;
-            for (uint32_t v = pp.body_len;; v >>= 7) {
-              if (v >= 0x80) pre[pl++] = (uint8_t)(v | 0x80);
-              else {
-                pre[pl++] = (uint8_t)v;
-                break;
-              }
-            }
-            uint64_t comp = (uint64_t)pl;
-            for (size_t f = page_first_frag[pi]; f < page_first_frag[pi + 1]; f++) comp += flen[f];
+            const uint64_t comp = packed.size(pi);
             if (comp >= (1ull << 31)) fail(HS_EUNSUPPORTED, "a compressed page exceeds 2 GiB");
             const size_t b0 = skel2.size();
-            if (ptype == pq::DICTIONARY_PAGE) {
+            if (pp.page_type == pq::DICTIONARY_PAGE) {
               ch.dictionary_page_offset = (int64_t)(cur2 - file_off);
-              pq::write_dict_page_header(skel2, (int32_t)pp.body_len, nvals, (int32_t)comp);
+              pq::write_dict_page_header(skel2, (int32_t)pp.body_len, pp.num_values, (int32_t)comp);
             } else {
               if (first_data) ch.data_page_offset = (int64_t)(cur2 - file_off);
               first_data = false;
-              pq::write_data_page_header(skel2, (int32_t)pp.body_len, nvals, enc, (int32_t)comp);
+              pq::write_data_page_header(skel2, (int32_t)pp.body_len, pp.num_values, pp.encoding, (int32_t)comp);
             }
             uncomp += (int64_t)(skel2.size() - b0) + pp.body_len;
-            skel2.insert(skel2.end(), pre, pre + pl);
+            packed.append_preamble(pi, skel2);
             emit2(b0);
-            for (size_t f = page_first_frag[pi]; f < page_first_frag[pi + 1]; f++) {
-              blobs.push_back(BlobCopy{frags[f].dst_off, cur2, flen[f], 0});
-              cur2 += flen[f];
-            }
+            packed.place(pi, blobs, &cur2);
           }
           ch.total_size = (int64_t)(cur2 - chunk_begin);
           ch.total_uncompressed = uncomp;
@@ -1685,27 +1578,7 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
       }
       {
         const size_t b0 = skel2.size();
-        std::vector<pq::StatSlot> slots;
-        std::vector<uint8_t> footer = pq::write_footer(schema, fp.rgs, fp.rows, schema_json, &slots);
-        for (const pq::StatSlot& sl : slots) {
-          StatPatch sp;
-          int64_t row0 = 0;
-          for (int g = 0; g < sl.row_group; g++) row0 += fp.rgs[g].num_rows;
-          sp.first_pos = req.seg_offsets[fp.seg] + (uint64_t)row0;
-          sp.last_pos = sp.first_pos + (uint64_t)fp.rgs[sl.row_group].num_rows - 1;
-          for (int j = 0; j < 2; j++) {
-            sp.min_off[j] = cur2 + sl.min_off[j];
-            sp.max_off[j] = cur2 + sl.max_off[j];
-          }
-          sp.width = sl.width;
-          sp.pad = 0;
-          patches2.push_back(sp);
-        }
-        skel2.insert(skel2.end(), footer.begin(), footer.end());
-        const uint32_t flen32 = (uint32_t)footer.size();
-        const uint8_t* lp = (const uint8_t*)&flen32;
-        skel2.insert(skel2.end(), lp, lp + 4);
-        skel2.insert(skel2.end(), {'P', 'A', 'R', '1'});
+        append_file_end(schema, fp.rgs, fp.rows, schema_json, req.seg_offsets[fp.seg], cur2, skel2, patches2);
         emit2(b0);
       }
       OutFile of = out->files[fi];
@@ -1722,7 +1595,7 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
     copy_h2d(ctx, d_copies2.get(), copies2.data(), copies2.size() * sizeof(ByteCopy));
     copy_h2d(ctx, d_blobs.get(), blobs.data(), blobs.size() * sizeof(BlobCopy));
     launch_scatter_bytes(ctx, d_copies2.get(), (int64_t)copies2.size(), d_skel2.get(), arena2.get());
-    launch_copy_blobs(ctx, d_blobs.get(), (int64_t)blobs.size(), d_slots.get(), arena2.get());
+    launch_copy_blobs(ctx, d_blobs.get(), (int64_t)blobs.size(), packed.slots.get(), arena2.get());
     if (!patches2.empty()) {
       Buf<StatPatch> d_sp(ctx, patches2.size());
       copy_h2d(ctx, d_sp.get(), patches2.data(), sizeof(StatPatch) * patches2.size());

@@ -18,7 +18,7 @@
 // The decoder never reads past a page's compressed bytes (the bit reader shifts in zeros there and reports truncation).
 #include "device_utils.cuh"
 #include "inflate.h"
-#include "kernels.h"
+#include "page_codec_kernels.h"
 
 namespace hs {
 

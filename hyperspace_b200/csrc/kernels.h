@@ -105,7 +105,11 @@ struct StringDictJob {
 };
 void launch_build_string_dicts(hs_ctx* ctx, const StringDictJob* jobs, int64_t n, uint32_t* d_error);
 
-// ---- compressed pages: snappy (snappy.cu) and GZIP (inflate.cu) ----------------------------------------------------------
+// ---- compressed pages (page_codec.cu; the kernels of each codec: snappy.cu, inflate.cu) --------------------------------
+// Decompresses every compressed data page and dictionary page of `pages` (host copy of d_pages) into *scratch, repoints
+// the descriptors at the decompressed bytes and uploads them to d_pages.  A dictionary page shared by several data pages
+// is decompressed once.  A failed check sets d_error (DERR_SNAPPY / DERR_GZIP).  Synchronises the stream once.
+void decompress_pages(hs_ctx* ctx, std::vector<PageDesc>& pages, PageDesc* d_pages, Buf<uint8_t>* scratch, uint32_t* d_error);
 // one per compressed page (or dictionary page) of a call: where it lies, where its decompressed copy goes
 struct PageBlob {
   const uint8_t* src;   // stored bytes (device)
@@ -114,32 +118,14 @@ struct PageBlob {
   uint32_t dst_len;     // prefix + decompressed length
   uint32_t prefix;      // leading bytes copied verbatim (v2 level bytes)
   uint32_t compressed;  // 0: copy, 1: compressed with `codec`
-  uint32_t first_block; // snappy: index of this page's first 64 KB output block in the block table (ascending over the blobs)
+  uint32_t first_block; // filled by decompress_blobs (snappy: the page's first 64 KB output block in the block table)
   uint32_t codec;       // pq::Codec of the page's chunk: SNAPPY or GZIP
 };
-__host__ __device__ inline uint32_t snappy_blocks_of(uint32_t dst_len, uint32_t prefix) {
-  const uint32_t body = dst_len - prefix;
-  return body == 0 ? 1u : (body + 65535u) / 65536u;
-}
-// block_in: one uint32 per block (+1), sequential: one uint32 per blob -- scratch of the two launches
-// any_verbatim: some blob has a prefix or is stored uncompressed
-void launch_snappy_decompress(hs_ctx* ctx, const PageBlob* blobs, int64_t n, int64_t total_blocks, bool any_verbatim,
-                              uint32_t* block_in, uint32_t* sequential, uint8_t* scratch, uint32_t* d_error);
-
-// GZIP page bodies, one warp per blob: copies what is stored verbatim (prefix, or the whole page when !compressed) and
-// inflates the rest; a failed check sets (DERR_GZIP << 24 | gz::InflateError) in d_error
-void launch_inflate(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch, uint32_t* d_error);
-
-// compression of page bodies: one warp per fragment (<= 65536 bytes) of a page; fragment f of raw bytes [src_off, src_off +
-// len) is written to scratch at dst_off (room for 32 + len + len / 6 bytes), its compressed length to out_len[f]
-struct SnappyFragment {
-  uint64_t src_off, dst_off;
-  uint32_t len, pad;
-};
-constexpr uint32_t kSnappyFragment = 65536;
-inline uint64_t snappy_max_compressed(uint64_t len) { return 32 + len + len / 6; }
-void launch_snappy_compress(hs_ctx* ctx, const SnappyFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
-                            uint32_t* out_len);
+// Decompresses the blobs into `scratch`: chooses and launches the kernels of each codec (the blobs are reordered by
+// codec).  sequential (optional, host): per blob in its new order, 1 where a snappy stream was decoded front to back.
+// Synchronises the stream once.
+void decompress_blobs(hs_ctx* ctx, std::vector<PageBlob>& blobs, uint8_t* scratch, uint32_t* d_error,
+                      std::vector<uint32_t>* sequential = nullptr);
 
 // Walks the page headers of every chunk.  mode 0: page_counts[chunk] = number of data pages.
 // mode 1: fills pages[page_offsets[chunk] ...].
@@ -387,6 +373,22 @@ struct BlobCopy {
   uint32_t len, pad;
 };
 void launch_copy_blobs(hs_ctx* ctx, const BlobCopy* blobs, int64_t n, const uint8_t* src_base, uint8_t* dst_base);
+// Page bodies compressed with SNAPPY (page_codec.cu).  A body's compressed form is its preamble, which the host writes,
+// followed by its pieces, which lie in `slots` on the device.
+struct CompressedBodies {
+  Buf<uint8_t> slots;
+  std::vector<uint64_t> raw_len;     // per body: uncompressed bytes
+  std::vector<size_t> first_piece;   // per body (+1): its pieces
+  std::vector<BlobCopy> pieces;      // src: offset in slots, len: compressed bytes
+  uint64_t size(size_t body) const;  // compressed bytes of the body: preamble + pieces
+  void append_preamble(size_t body, std::vector<uint8_t>& out) const;
+  // appends the body's pieces to `copies` with consecutive destinations from *dst on; advances *dst
+  void place(size_t body, std::vector<BlobCopy>& copies, uint64_t* dst) const;
+};
+// Compresses the bodies (offset, length) of `raw` (device), each on its own.  Synchronises the stream once: the
+// compressed sizes are data.
+void compress_bodies(hs_ctx* ctx, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
+                     CompressedBodies* out);
 // Synthetic table generator: rows [first_row, first_row+n) of column `col` (0..4) of table T (SURVEY.md section 8d)
 void launch_synth_column(hs_ctx* ctx, int col, int64_t first_row, int64_t n, void* out);
 

@@ -1,0 +1,142 @@
+// page_codec.cu -- page compression behind one entry point each way: decompress_pages for the readers (under it
+// decompress_blobs, which the kernel tests reach too) and compress_bodies for the encoder.  The callers say which bytes
+// are compressed and where the result goes; what a codec's kernels need besides that -- how the work is cut up, their
+// scratch tables, which of them run -- is decided here.  The kernels are in snappy.cu (SNAPPY, both ways) and inflate.cu
+// (GZIP).
+#include <algorithm>
+#include <map>
+#include <set>
+
+#include "page_codec_kernels.h"
+#include "parquet_meta.h"
+
+namespace hs {
+
+void decompress_blobs(hs_ctx* ctx, std::vector<PageBlob>& blobs, uint8_t* scratch, uint32_t* d_error,
+                      std::vector<uint32_t>* sequential) {
+  // each codec's kernels run over its own blobs: the snappy ones first, in page order, then the GZIP ones
+  const size_t n_snappy = (size_t)(std::stable_partition(blobs.begin(), blobs.end(),
+                                                         [](const PageBlob& b) { return b.codec == pq::SNAPPY; }) -
+                                   blobs.begin());
+  uint64_t total_blocks = 0;  // 64 KB output blocks, the unit of the snappy decoder's parallelism
+  bool any_verbatim = false;
+  for (size_t i = 0; i < n_snappy; i++) {
+    PageBlob& b = blobs[i];
+    any_verbatim = any_verbatim || b.prefix != 0 || !b.compressed;
+    b.first_block = (uint32_t)total_blocks;
+    total_blocks += snappy_blocks_of(b.dst_len, b.prefix);
+  }
+  if (total_blocks >= 0xffffffffull) fail(HS_EUNSUPPORTED, "more than 256 TB of compressed pages in one call");
+  Buf<PageBlob> d_blobs(ctx, std::max<size_t>(1, blobs.size()));
+  Buf<uint32_t> d_block_in(ctx, (size_t)total_blocks + 1), d_sequential(ctx, std::max<size_t>(1, n_snappy));
+  copy_h2d(ctx, d_blobs.get(), blobs.data(), sizeof(PageBlob) * blobs.size());
+  launch_snappy_decompress(ctx, d_blobs.get(), (int64_t)n_snappy, (int64_t)total_blocks, any_verbatim, d_block_in.get(),
+                           d_sequential.get(), scratch, d_error);
+  launch_inflate(ctx, d_blobs.get() + n_snappy, (int64_t)(blobs.size() - n_snappy), scratch, d_error);
+  if (sequential) {
+    sequential->assign(blobs.size(), 0u);
+    copy_d2h(ctx, sequential->data(), d_sequential.get(), sizeof(uint32_t) * n_snappy);
+  }
+  sync_stream(ctx);  // the blobs (and whatever else the caller uploaded from host vectors) may go out of scope
+}
+
+void decompress_pages(hs_ctx* ctx, std::vector<PageDesc>& pages, PageDesc* d_pages, Buf<uint8_t>* scratch, uint32_t* d_error) {
+  // a page is decompressed (or, stored inside a compressed chunk, copied) when its stored bytes are not its decoded bytes
+  auto relocated = [](const PageDesc& pg) { return pg.is_compressed || pg.size != pg.uncompressed_size; };
+  auto level_bytes = [](const PageDesc& pg) {  // v2: the levels in front of the values are stored verbatim
+    return pg.page_type == pq::DATA_PAGE_V2 ? (uint32_t)(pg.rep_bytes + std::max(0, pg.def_bytes)) : 0u;
+  };
+  auto room = [](int32_t bytes) { return (uint64_t)round_up((size_t)bytes, 16) + 16; };
+  // every size is in the descriptors: the scratch bytes first, then real pointers.  The dictionary page of a compressed
+  // chunk is compressed too, and all data pages of the chunk name the same one.
+  std::set<const uint8_t*> dicts_seen;
+  uint64_t total = 0;
+  for (const PageDesc& pg : pages) {
+    if (pg.codec == pq::UNCOMPRESSED) continue;
+    if (pg.dict && dicts_seen.insert(pg.dict).second) total += room(pg.dict_uncompressed_size);
+    if (!relocated(pg)) continue;
+    if (level_bytes(pg) > (uint32_t)pg.size || level_bytes(pg) > (uint32_t)pg.uncompressed_size)
+      fail(HS_EFORMAT, "compressed page has level bytes beyond its size");
+    total += room(pg.uncompressed_size);
+  }
+  scratch->alloc(ctx, std::max<uint64_t>(total, 16) + 16);  // decoders may read one aligned word past a page
+  std::vector<PageBlob> blobs;
+  std::map<const uint8_t*, uint64_t> dict_off;  // stored dictionary page -> scratch offset of its decompressed copy
+  uint64_t cursor = 0;
+  for (PageDesc& pg : pages) {
+    if (pg.codec == pq::UNCOMPRESSED) continue;
+    if (pg.dict) {
+      auto it = dict_off.find(pg.dict);
+      if (it == dict_off.end()) {
+        it = dict_off.emplace(pg.dict, cursor).first;
+        blobs.push_back(PageBlob{pg.dict, cursor, (uint32_t)pg.dict_size, (uint32_t)pg.dict_uncompressed_size, 0u, 1u, 0u,
+                                 (uint32_t)pg.codec});
+        cursor += room(pg.dict_uncompressed_size);
+      }
+      pg.dict = scratch->get() + it->second;
+      pg.dict_size = pg.dict_uncompressed_size;
+    }
+    if (relocated(pg)) {
+      blobs.push_back(PageBlob{pg.data, cursor, (uint32_t)pg.size, (uint32_t)pg.uncompressed_size, level_bytes(pg),
+                               (uint32_t)(pg.is_compressed ? 1 : 0), 0u, (uint32_t)pg.codec});
+      pg.data = scratch->get() + cursor;
+      pg.size = pg.uncompressed_size;
+      cursor += room(pg.uncompressed_size);
+    }
+  }
+  copy_h2d(ctx, d_pages, pages.data(), sizeof(PageDesc) * pages.size());
+  decompress_blobs(ctx, blobs, scratch->get(), d_error);
+}
+
+void compress_bodies(hs_ctx* ctx, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
+                     CompressedBodies* out) {
+  // A body is cut into 64 KB fragments that compress in parallel, each into a slot of worst-case size.
+  std::vector<SnappyFragment> frags;
+  out->raw_len.clear();
+  out->first_piece.clear();
+  uint64_t slot_cursor = 0;
+  for (const auto& body : bodies) {
+    out->raw_len.push_back(body.second);
+    out->first_piece.push_back(frags.size());
+    for (uint64_t o = 0; o < body.second; o += kSnappyFragment) {
+      const uint32_t len = (uint32_t)std::min<uint64_t>(kSnappyFragment, body.second - o);
+      frags.push_back(SnappyFragment{body.first + o, slot_cursor, len, 0});
+      slot_cursor += round_up(snappy_max_compressed(len), 16);
+    }
+  }
+  out->first_piece.push_back(frags.size());
+  out->slots.alloc(ctx, std::max<uint64_t>(slot_cursor, 16));
+  Buf<SnappyFragment> d_frags(ctx, std::max<size_t>(1, frags.size()));
+  Buf<uint32_t> d_flen(ctx, std::max<size_t>(1, frags.size()));
+  std::vector<uint32_t> flen(frags.size());
+  copy_h2d(ctx, d_frags.get(), frags.data(), sizeof(SnappyFragment) * frags.size());
+  launch_snappy_compress(ctx, d_frags.get(), (int64_t)frags.size(), raw, out->slots.get(), d_flen.get());
+  copy_d2h(ctx, flen.data(), d_flen.get(), 4 * frags.size());
+  sync_stream(ctx);
+  out->pieces.resize(frags.size());
+  for (size_t f = 0; f < frags.size(); f++) out->pieces[f] = BlobCopy{frags[f].dst_off, 0, flen[f], 0};
+}
+
+// snappy's preamble: the uncompressed length, as the varint Thrift writes too
+void CompressedBodies::append_preamble(size_t body, std::vector<uint8_t>& out) const {
+  thrift::Writer w;
+  w.varint(raw_len[body]);
+  out.insert(out.end(), w.buf.begin(), w.buf.end());
+}
+
+uint64_t CompressedBodies::size(size_t body) const {
+  std::vector<uint8_t> preamble;
+  append_preamble(body, preamble);
+  uint64_t bytes = preamble.size();
+  for (size_t f = first_piece[body]; f < first_piece[body + 1]; f++) bytes += pieces[f].len;
+  return bytes;
+}
+
+void CompressedBodies::place(size_t body, std::vector<BlobCopy>& copies, uint64_t* dst) const {
+  for (size_t f = first_piece[body]; f < first_piece[body + 1]; f++) {
+    copies.push_back(BlobCopy{pieces[f].src, *dst, pieces[f].len, 0});
+    *dst += pieces[f].len;
+  }
+}
+
+}  // namespace hs

@@ -29,7 +29,7 @@
 #include <climits>
 
 #include "device_utils.cuh"
-#include "kernels.h"
+#include "page_codec_kernels.h"
 
 namespace hs {
 

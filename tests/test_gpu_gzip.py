@@ -180,6 +180,31 @@ def test_mixed_codecs_in_one_call(ctx):
     assert e.value.code == N.HS_EUNSUPPORTED and "'v2'" in str(e.value) and "codec 6" in str(e.value)
 
 
+def test_each_codec_kernel_runs_once_over_mixed_sources(ctx):
+    n = 60_000
+    rng = np.random.default_rng(11)
+    t = pa.table({"k": rng.integers(0, 1 << 40, n, dtype=np.int64),
+                  "v": pa.array(rng.integers(0, 1000, n, dtype=np.int64), mask=rng.random(n) < 0.2)})
+    parts = [t.slice(0, 20_000), t.slice(20_000, 20_000), t.slice(40_000)]
+    # v2 pages keep their (here non-empty) definition levels uncompressed in front of the values: the snappy decoder
+    # copies them with a kernel of its own, which runs only when some page needs it.  PLAIN values, so that the pages
+    # shrink and pyarrow does store them compressed.
+    v2 = _image(parts[0], compression="snappy", data_page_version="2.0", use_dictionary=False)
+    v1 = _image(parts[0], compression="snappy", use_dictionary=False)
+    rest = [_image(parts[1], compression="gzip"), _image(parts[2], compression="none")]
+    plain, _, _ = _build(ctx, [_image(p, compression="none") for p in parts], "k", ["v"])
+    a, _, kern = _build(ctx, [v2] + rest, "k", ["v"], profile=True)
+    assert a == plain
+    assert {k: kern[k]["launches"] for k in kern if k.startswith("k_snappy") or k == "k_inflate"} == \
+        {"k_snappy_levels": 1, "k_snappy_index": 1, "k_snappy_blocks": 1, "k_inflate": 1}
+    b, _, kern = _build(ctx, [v1] + rest, "k", ["v"], profile=True)
+    assert b == plain
+    assert {k: kern[k]["launches"] for k in kern if k.startswith("k_snappy") or k == "k_inflate"} == \
+        {"k_snappy_index": 1, "k_snappy_blocks": 1, "k_inflate": 1}
+    _, _, kern = _build(ctx, rest, "k", ["v"], profile=True)
+    assert [k for k in kern if k.startswith("k_snappy")] == [] and kern["k_inflate"]["launches"] == 1
+
+
 def test_corrupt_gzip_page_is_a_format_error(ctx):
     from hyperspace_b200 import _native as N
 
