@@ -81,6 +81,12 @@ class PredicateSpec(C.Structure):
                 ("lo_bytes", C.c_char_p), ("hi_bytes", C.c_char_p), ("lo_len", C.c_uint32), ("hi_len", C.c_uint32)]
 
 
+class PredicateAnySpec(C.Structure):
+    _fields_ = [("column", C.c_char_p), ("literal_type", C.c_int32), ("scale", C.c_int32), ("n_values", C.c_int64),
+                ("values_i", C.c_void_p), ("values_f", C.c_void_p), ("values_bytes", C.c_void_p), ("values_offsets", C.c_void_p),
+                ("ranges", C.POINTER(PredicateSpec)), ("n_ranges", C.c_int32), ("reserved", C.c_int32)]
+
+
 class JoinSpec(C.Structure):
     _fields_ = [("left_files", C.POINTER(SourceFile)), ("n_left", C.c_int32),
                 ("right_files", C.POINTER(SourceFile)), ("n_right", C.c_int32),
@@ -115,7 +121,7 @@ EXPORTED_SYMBOLS = [
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
-    "hs_bucket_join_where", "hs_k_inflate",
+    "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -165,6 +171,15 @@ def load_library() -> C.CDLL:
     L.hs_filter_scan_where.restype = C.c_int
     L.hs_filter_scan_where.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32, C.POINTER(C.c_void_p),
                                        C.POINTER(Stats), *err]
+    L.hs_filter_scan_any.restype = C.c_int
+    L.hs_filter_scan_any.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32,
+                                     C.POINTER(PredicateAnySpec), C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p),
+                                     C.POINTER(Stats), *err]
+    L.hs_bucket_join_any.restype = C.c_int
+    L.hs_bucket_join_any.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
+                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                     C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join.restype = C.c_int
     L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join_where.restype = C.c_int
@@ -340,6 +355,99 @@ def _predicate_array(predicates: Sequence[tuple]):
             else:
                 setattr(p, side + "_f", float(v))
     return preds, len(split)
+
+
+def any_values(values) -> Tuple[int, int, object]:
+    """The listed values of an IN term as (HS_TYPE_* literal type, decimal scale, values): an int64 or float64 numpy array,
+    or a list of bytes for strings.  None is dropped.  Spark casts the list to its widest type: a float among numbers
+    makes every value a double; a Decimal among ints makes every value a decimal, all brought to the largest scale
+    exactly; datetimes are timestamps' micros (longs).  Numpy int / float arrays pass without a Python object per value.
+    Raises ValueError for strings mixed with numbers and for booleans or other values."""
+    if isinstance(values, np.ndarray) and values.dtype.kind in "iu":
+        return HS_TYPE_INT64, 0, np.ascontiguousarray(values, dtype=np.int64)
+    if isinstance(values, np.ndarray) and values.dtype.kind == "f":
+        return HS_TYPE_DOUBLE, 0, np.ascontiguousarray(values, dtype=np.float64)
+    if isinstance(values, np.ndarray) and values.dtype.kind == "b":
+        raise ValueError("a boolean list cannot be compared")
+    vals = [v for v in (values.tolist() if isinstance(values, np.ndarray) else values) if v is not None]
+    kinds = set()
+    for v in vals:
+        if isinstance(v, (bool, np.bool_)):
+            raise ValueError("a boolean literal cannot be listed in IN")
+        if isinstance(v, (str, bytes, bytearray, np.str_, np.bytes_)):
+            kinds.add("s")
+        elif isinstance(v, (float, np.floating)):
+            kinds.add("f")
+        elif isinstance(v, decimal.Decimal):
+            kinds.add("d")
+        elif isinstance(v, (int, np.integer, datetime.datetime)):
+            kinds.add("i")
+        else:
+            raise ValueError(f"unsupported literal {v!r} in IN")
+    if "s" in kinds and len(kinds) > 1:
+        raise ValueError("an IN list cannot mix string and numeric values")
+    if "s" in kinds:
+        return HS_TYPE_STRING, 0, [v.encode("utf-8") if isinstance(v, str) else bytes(v) for v in vals]
+    ints = [timestamp_micros(v) if isinstance(v, datetime.datetime) else v for v in vals]
+    if "f" in kinds:
+        return HS_TYPE_DOUBLE, 0, np.array([float(v) for v in ints], dtype=np.float64)
+    if "d" in kinds:
+        scale = max(decimal_unscaled(v)[1] for v in ints if isinstance(v, decimal.Decimal))
+        out = []
+        for v in ints:
+            unscaled, sc = decimal_unscaled(v) if isinstance(v, decimal.Decimal) else (int(v), 0)
+            unscaled *= 10 ** (scale - sc)
+            if not -2**63 <= unscaled < 2**63:
+                raise ValueError(f"decimal literal {v} has more than 18 significant digits at scale {scale}")
+            out.append(unscaled)
+        return HS_TYPE_DECIMAL, scale, np.array(out, dtype=np.int64)
+    for v in ints:
+        if not -2**63 <= int(v) < 2**63:
+            raise ValueError(f"integer literal {v} does not fit in a long")
+    return HS_TYPE_INT64, 0, np.array([int(v) for v in ints], dtype=np.int64)
+
+
+def _one_literal_type(lo, hi):
+    """The bounds of one range of a disjunction as literals of one type: decimals (and an int beside a decimal) at the
+    larger of their scales, exactly; other mixes are left for _predicate_array to refuse."""
+    if lo is None or hi is None or not ({type(lo), type(hi)} & {decimal.Decimal}):
+        return lo, hi
+    if any(isinstance(v, (float, np.floating)) for v in (lo, hi)):
+        return lo, hi
+    lo, hi = decimal.Decimal(lo), decimal.Decimal(hi)
+    scale = max(decimal_unscaled(lo)[1], decimal_unscaled(hi)[1])
+    q = decimal.Decimal(1).scaleb(-scale)
+    return lo.quantize(q), hi.quantize(q)
+
+
+def _any_array(terms: Sequence[tuple]):
+    """``(column, values, ranges)`` terms -> (hs_predicate_any array, count, buffers to keep alive).  values go through
+    any_values; ranges are ``(lo, lo_strict, hi, hi_strict)`` tuples with _predicate_array's literal typing."""
+    keep = []
+    arr = (PredicateAnySpec * max(1, len(terms)))()
+    for a, (column, values, ranges) in zip(arr, terms):
+        a.column = column.encode()
+        lt, scale, vals = any_values(values)
+        a.literal_type, a.scale, a.n_values = lt, scale, len(vals)
+        if lt == HS_TYPE_STRING:
+            offs = np.zeros(len(vals) + 1, dtype=np.uint64)
+            offs[1:] = np.cumsum([len(v) for v in vals], dtype=np.uint64) if vals else []
+            blob = np.frombuffer(b"".join(vals) or b"\0", dtype=np.uint8)
+            keep += [offs, blob]
+            a.values_bytes, a.values_offsets = blob.ctypes.data, offs.ctypes.data
+        else:
+            keep.append(vals)
+            if lt == HS_TYPE_DOUBLE:
+                a.values_f = vals.ctypes.data
+            else:
+                a.values_i = vals.ctypes.data
+        ranges = [(lo, ls, hi, hs) for (lo, hi), (_, ls, _, hs) in ((_one_literal_type(r[0], r[2]), r) for r in ranges)]
+        rp, nr = _predicate_array([(column, lo, ls, hi, hs) for lo, ls, hi, hs in ranges])
+        if nr != len(ranges):
+            raise ValueError("a range of an OR must have bounds of one literal type")
+        keep.append(rp)
+        a.ranges, a.n_ranges = rp, nr
+    return arr, len(terms), keep
 
 
 def _source_array(files: Sequence[FileImage]):
@@ -756,6 +864,34 @@ class Context:
         _check(L.hs_filter_scan_where(self._h, C.byref(spec), preds, n_preds, C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
+    def filter_scan_any(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
+                        terms: Sequence[tuple], sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (),
+                        file_buckets: Optional[Sequence[int]] = None, num_buckets: int = 0, output: int = HS_OUT_HOST
+                        ) -> Tuple[Batch, Dict[str, float]]:
+        """hs_filter_scan_any: filter_scan_where's predicates AND-ed with disjunction terms ``(column, values, ranges)``:
+        the row's value equals one of `values` (see any_values) or lies in one of `ranges` (``(lo, lo_strict, hi,
+        hi_strict)``).  file_buckets / num_buckets: the bucket of every file of an index bucketed on `key` alone, for
+        skipping the files a point lookup cannot hit."""
+        L = load_library()
+        src, keep = _source_array(files)
+        pc = _cstr_array(projected)
+        spec = ScanSpec()
+        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
+        spec.key_column = key.encode() if key else None
+        spec.projected_columns, spec.n_projected = pc, len(projected)
+        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
+        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
+        spec.output = output
+        preds, n_preds = _predicate_array(predicates)
+        anys, n_anys, keep_any = _any_array(terms)
+        fb = np.ascontiguousarray(file_buckets if file_buckets is not None else [0], dtype=np.int32)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_filter_scan_any(self._h, C.byref(spec), preds, n_preds, anys, n_anys,
+                                    fb.ctypes.data if file_buckets is not None else None, num_buckets if file_buckets is not None else 0,
+                                    C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
     def _join_spec(self, left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns, right_columns,
                    output):
         ls, k1 = _source_array(left)
@@ -805,6 +941,28 @@ class Context:
         err = C.create_string_buffer(1024)
         _check(L.hs_bucket_join_where(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, rp, nrp, C.byref(res), C.byref(st),
                                       err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
+    def bucket_join_any(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                        right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                        left_columns: Sequence[str], right_columns: Sequence[str], left_predicates: Sequence[tuple] = (),
+                        right_predicates: Sequence[tuple] = (), left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (),
+                        output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_any: bucket_join_where with filter_scan_any's disjunction terms on either side."""
+        L = load_library()
+        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
+                                     right_columns, output)
+        lk, rk = _cstr_array(left_keys), _cstr_array(right_keys)
+        if len(left_keys) != len(right_keys):
+            raise ValueError("left_keys and right_keys must pair up")
+        lp, nlp = _predicate_array(left_predicates)
+        rp, nrp = _predicate_array(right_predicates)
+        la, nla, k1 = _any_array(left_terms)
+        ra, nra, k2 = _any_array(right_terms)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_bucket_join_any(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, rp, nrp, ra, nra, C.byref(res),
+                                    C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------

@@ -844,16 +844,6 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
   b->nrows = n_out;
 }
 
-__global__ void k_ranges_to_indices(const int64_t* __restrict__ bounds, const uint64_t* __restrict__ seg_offsets,
-                                    const uint64_t* __restrict__ out_offsets, int nseg, uint32_t* __restrict__ out_idx) {
-  // one CTA per segment
-  const int s = blockIdx.x;
-  if (s >= nseg) return;
-  const int64_t first = bounds[2 * s], last = bounds[2 * s + 1];
-  const uint64_t base = seg_offsets[s], o = out_offsets[s];
-  for (int64_t i = first + threadIdx.x; i < last; i += blockDim.x) out_idx[o + (i - first)] = (uint32_t)(base + i);
-}
-
 }  // extern "C"
 
 // ---- predicates: Spark 3.1's binary-comparison coercion, decided once on the host ---------------------------------------
@@ -1037,12 +1027,242 @@ static PredRange intersect_ranges(int type, const std::vector<ResolvedPredicate>
   return r;
 }
 
+// ---- disjunctions on one column (hs_predicate_any) ------------------------------------------------------------------
+// A term becomes a sorted list of disjoint ranges of the column (SetRange, on the host), every value and range resolved by
+// resolve_predicate.  Numeric ranges are inclusive sort_encode values with both bounds present (an open side is the end
+// of the encoded domain); string ranges are bytes with their strictness, a missing bound open.
+struct SetRange {
+  bool has_lo = false, has_hi = false, lo_strict = false, hi_strict = false;
+  uint64_t lo = 0, hi = 0;
+  std::string lo_b, hi_b;
+};
+using RangeSet = std::vector<SetRange>;
+
+static int set_bound_cmp(bool str, uint64_t a, const std::string& as, uint64_t b, const std::string& bs) {
+  if (str) return host_string_compare((const uint8_t*)as.data(), (uint32_t)as.size(), (const uint8_t*)bs.data(), (uint32_t)bs.size());
+  return a < b ? -1 : (a > b ? 1 : 0);
+}
+static bool set_range_empty(bool str, const SetRange& r) {
+  if (!r.has_lo || !r.has_hi) return false;
+  const int c = set_bound_cmp(str, r.lo, r.lo_b, r.hi, r.hi_b);
+  return c > 0 || (c == 0 && (r.lo_strict || r.hi_strict));
+}
+static bool lo_before(bool str, const SetRange& a, const SetRange& b) {  // a starts below b
+  if (!a.has_lo || !b.has_lo) return !a.has_lo && b.has_lo;
+  const int c = set_bound_cmp(str, a.lo, a.lo_b, b.lo, b.lo_b);
+  return c < 0 || (c == 0 && !a.lo_strict && b.lo_strict);
+}
+static bool hi_before(bool str, const SetRange& a, const SetRange& b) {  // a ends below b
+  if (!a.has_hi || !b.has_hi) return a.has_hi && !b.has_hi;
+  const int c = set_bound_cmp(str, a.hi, a.hi_b, b.hi, b.hi_b);
+  return c < 0 || (c == 0 && a.hi_strict && !b.hi_strict);
+}
+static void take_lo(SetRange* r, const SetRange& from) { r->has_lo = from.has_lo, r->lo = from.lo, r->lo_b = from.lo_b, r->lo_strict = from.lo_strict; }
+static void take_hi(SetRange* r, const SetRange& from) { r->has_hi = from.has_hi, r->hi = from.hi, r->hi_b = from.hi_b, r->hi_strict = from.hi_strict; }
+
+// sorts, drops empty ranges and merges overlapping and adjacent ones
+static void normalise_set(bool str, RangeSet* rs) {
+  rs->erase(std::remove_if(rs->begin(), rs->end(), [&](const SetRange& r) { return set_range_empty(str, r); }), rs->end());
+  std::sort(rs->begin(), rs->end(), [&](const SetRange& a, const SetRange& b) { return lo_before(str, a, b); });
+  RangeSet out;
+  for (SetRange& r : *rs) {
+    bool joins = false;
+    if (!out.empty()) {
+      const SetRange& cur = out.back();
+      if (!cur.has_hi || !r.has_lo) joins = true;
+      else if (!str) joins = r.lo <= cur.hi || r.lo - 1 == cur.hi;  // r.lo > cur.hi >= 0 in the second test
+      else {
+        const int c = set_bound_cmp(true, r.lo, r.lo_b, cur.hi, cur.hi_b);
+        joins = c < 0 || (c == 0 && !(r.lo_strict && cur.hi_strict));
+      }
+    }
+    if (!joins) out.push_back(std::move(r));
+    else if (hi_before(str, out.back(), r)) take_hi(&out.back(), r);
+  }
+  *rs = std::move(out);
+}
+
+static RangeSet intersect_sets(bool str, const RangeSet& a, const RangeSet& b) {
+  RangeSet out;
+  size_t i = 0, j = 0;
+  while (i < a.size() && j < b.size()) {
+    SetRange r;
+    take_lo(&r, lo_before(str, a[i], b[j]) ? b[j] : a[i]);
+    const bool a_first = hi_before(str, a[i], b[j]);
+    take_hi(&r, a_first ? a[i] : b[j]);
+    if (!set_range_empty(str, r)) out.push_back(std::move(r));
+    if (a_first) i++;
+    else j++;
+  }
+  return out;
+}
+
+static uint64_t encoded_max(int type) { return type == HS_TYPE_INT32 || type == HS_TYPE_FLOAT ? 0xffffffffull : ~0ull; }
+
+// a resolved range (resolve_predicate / intersect_ranges) as a set of at most one range; string bounds from the host bytes
+static SetRange set_range_of(int type, const PredRange& r, const uint8_t* lo_host, uint32_t lo_len, const uint8_t* hi_host,
+                             uint32_t hi_len) {
+  SetRange s;
+  if (type == HS_TYPE_STRING) {
+    s.has_lo = r.has_lo, s.has_hi = r.has_hi, s.lo_strict = r.lo_strict, s.hi_strict = r.hi_strict;
+    if (r.has_lo && lo_len) s.lo_b.assign((const char*)lo_host, lo_len);
+    if (r.has_hi && hi_len) s.hi_b.assign((const char*)hi_host, hi_len);
+    return s;
+  }
+  s.has_lo = s.has_hi = true;
+  s.lo = r.has_lo ? r.lo : 0;
+  s.hi = r.has_hi ? r.hi : encoded_max(type);
+  return s;
+}
+
+// Every value and range of the term on column c, as one sorted disjoint set; values that match nothing (int_col IN (2.5))
+// are dropped.  The refusals are resolve_predicate's, for the list's literal type and for every range.
+static RangeSet resolve_any(hs_ctx* ctx, const hs_predicate_any& a, const DevColumn& c) {
+  const bool str = c.type == HS_TYPE_STRING;
+  std::vector<Buf<uint8_t>> scratch;
+  ResolvedPredicate rp;
+  RangeSet out;
+  hs_predicate p;
+  memset(&p, 0, sizeof p);
+  p.column = a.column;
+  p.literal_type = a.literal_type;
+  p.scale = a.scale;
+  p.has_lo = p.has_hi = 1;
+  const bool lit_long = a.literal_type == HS_TYPE_INT64 || a.literal_type == HS_TYPE_DECIMAL;
+  const int col_scale = is_decimal(c.schema) ? c.schema.scale : 0, lit_scale = a.literal_type == HS_TYPE_DECIMAL ? a.scale : 0;
+  if (a.n_values > 0) resolve_predicate(ctx, p, c, &scratch, &rp);  // the list's refusals, once
+  out.reserve((size_t)a.n_values + a.n_ranges);
+  for (int64_t k = 0; k < a.n_values; k++) {
+    SetRange s;
+    if (str) {
+      const uint64_t b = a.values_offsets[k], e = a.values_offsets[k + 1];
+      s.has_lo = s.has_hi = true;
+      s.lo_b.assign((const char*)a.values_bytes + b, e - b);
+      s.hi_b = s.lo_b;
+      out.push_back(std::move(s));
+      continue;
+    }
+    // an integer column against an integer literal at its own scale equals at most one value: the literal's own encoding,
+    // confirmed by the comparison; everything else goes through the binary searches of resolve_predicate
+    if (lit_long && col_scale == lit_scale && (c.type == HS_TYPE_INT64 || (c.type == HS_TYPE_INT32 && a.values_i[k] == (int32_t)a.values_i[k]))) {
+      const uint64_t e = c.type == HS_TYPE_INT32 ? (uint64_t)((uint32_t)(int32_t)a.values_i[k] ^ 0x80000000u)
+                                                 : (uint64_t)a.values_i[k] ^ 0x8000000000000000ull;
+      if (compare_encoded(c.type, e, a.literal_type, a.values_i[k], 0.0, col_scale, lit_scale) == 0) {
+        s.has_lo = s.has_hi = true;
+        s.lo = s.hi = e;
+        out.push_back(std::move(s));
+        continue;
+      }
+    }
+    if (lit_long) p.lo_i = p.hi_i = a.values_i[k];
+    else p.lo_f = p.hi_f = a.values_f[k];
+    out.push_back(set_range_of(c.type, resolve_predicate(ctx, p, c, &scratch, &rp), nullptr, 0, nullptr, 0));
+  }
+  for (int32_t r = 0; r < a.n_ranges; r++) {
+    hs_predicate q = a.ranges[r];
+    q.column = a.column;
+    const PredRange pr = resolve_predicate(ctx, q, c, &scratch, &rp);
+    out.push_back(set_range_of(c.type, pr, rp.lo_host, rp.lo_len, rp.hi_host, rp.hi_len));
+  }
+  normalise_set(str, &out);
+  return out;
+}
+
+// the device form of a set: PredRanges of the column's type (string bounds reference one device copy of their bytes,
+// kept in `holder`)
+static void upload_set(hs_ctx* ctx, int type, const RangeSet& s, Buf<PredRange>* d_set, std::vector<Buf<uint8_t>>* holder) {
+  std::vector<PredRange> h(std::max<size_t>(1, s.size()));
+  uint8_t* bytes = nullptr;
+  std::vector<uint8_t> hb;
+  if (type == HS_TYPE_STRING) {
+    for (const SetRange& r : s) hb.insert(hb.end(), r.lo_b.begin(), r.lo_b.end()), hb.insert(hb.end(), r.hi_b.begin(), r.hi_b.end());
+    holder->emplace_back(ctx, hb.size() + 16);
+    bytes = holder->back().get();
+    if (!hb.empty()) copy_h2d(ctx, bytes, hb.data(), hb.size());
+  }
+  uint64_t off = 0;
+  for (size_t i = 0; i < s.size(); i++) {
+    const SetRange& r = s[i];
+    PredRange& d = h[i];
+    d = PredRange{};
+    d.type = type;
+    d.has_lo = r.has_lo, d.has_hi = r.has_hi, d.lo_strict = r.lo_strict, d.hi_strict = r.hi_strict;
+    if (type == HS_TYPE_STRING) {
+      d.lo = string_ref(bytes + off, (uint32_t)r.lo_b.size());
+      off += r.lo_b.size();
+      d.hi = string_ref(bytes + off, (uint32_t)r.hi_b.size());
+      off += r.hi_b.size();
+    } else {
+      d.lo = r.lo, d.hi = r.hi;
+    }
+  }
+  d_set->alloc(ctx, h.size());
+  copy_h2d(ctx, d_set->get(), h.data(), sizeof(PredRange) * h.size());
+  sync_stream(ctx);
+}
+
+static bool set_is_points(bool str, const RangeSet& s) {
+  for (const SetRange& r : s) {
+    if (!r.has_lo || !r.has_hi) return false;
+    if (str ? (r.lo_b != r.hi_b || r.lo_strict || r.hi_strict) : r.lo != r.hi) return false;
+  }
+  return true;
+}
+
+// the bucket of every point of a key set, by the hash the build used (hash_rows over a column of the key's storage type
+// and schema: key_column_of gives a decimal(p <= 9) the hashLong kind)
+static std::vector<int> point_buckets(hs_ctx* ctx, const DevColumn& key, const RangeSet& pts, int num_buckets) {
+  const int64_t n = (int64_t)pts.size();
+  std::vector<int> out(n);
+  if (n == 0) return out;
+  DevColumn c;
+  c.name = key.name;
+  c.type = key.type;
+  c.width = key.width;
+  c.schema = key.schema;
+  c.data.alloc(ctx, (size_t)n * c.width + 16);
+  std::vector<Buf<uint8_t>> holder;
+  Buf<PredRange> d_set;
+  std::vector<uint8_t> raw((size_t)n * c.width);
+  if (key.type == HS_TYPE_STRING) {  // the references of the uploaded lower bounds
+    upload_set(ctx, key.type, pts, &d_set, &holder);
+    std::vector<PredRange> h(n);
+    copy_d2h(ctx, h.data(), d_set.get(), sizeof(PredRange) * n);
+    sync_stream(ctx);
+    for (int64_t i = 0; i < n; i++) memcpy(raw.data() + 8 * i, &h[i].lo, 8);
+  } else {
+    for (int64_t i = 0; i < n; i++) {
+      if (key.width == 4) {
+        const uint32_t v = (uint32_t)pts[i].lo ^ 0x80000000u;
+        memcpy(raw.data() + 4 * i, &v, 4);
+      } else {
+        const uint64_t v = pts[i].lo ^ 0x8000000000000000ull;
+        memcpy(raw.data() + 8 * i, &v, 8);
+      }
+    }
+  }
+  copy_h2d(ctx, c.data.get(), raw.data(), raw.size());
+  const KeyColumn kc = key_column_of(c);
+  Buf<unsigned long long> ghist(ctx, num_buckets);
+  fill_bytes(ctx, ghist.get(), 0, 8 * num_buckets);
+  HashedRows hashed;
+  hash_rows(ctx, &kc, 1, n, num_buckets, 0, false, ghist.get(), nullptr, &hashed);
+  std::vector<uint16_t> hb(n);
+  copy_d2h(ctx, hb.data(), hashed.bin_ids.get(), 2 * n);
+  sync_stream(ctx);
+  for (int64_t i = 0; i < n; i++) out[i] = hb[i];
+  return out;
+}
+
 // The one filter scan: the sorted path binary-searches the key column's windows and decodes the other columns only inside
 // them, then evaluates the predicates on other columns over the window rows; the unsorted path (source files, Hybrid
 // Scan's appended files, the lineage NOT-IN) evaluates every predicate over all rows.
 // legacy (hs_filter_scan): predicates may have no bound (the row's key must then not be null, as that call always did),
 // literal types follow the column, and floating-point keys are refused (the call's bounds are int64).
+// anys: disjunction terms.  On the key column they turn the key's one window per file into one window per range of the
+// key's set; elsewhere they are set-form residual predicates.  file_buckets (optional): see hs_filter_scan_any.
 static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int n_preds, bool legacy,
+                            const hs_predicate_any* anys, int n_anys, const int32_t* file_buckets, int num_buckets,
                             hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   *out = nullptr;
   hs_stats st;
@@ -1067,11 +1287,65 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     if (try_sorted) col_of(spec->key_column);
     std::vector<int> proj_idx;
     for (int i = 0; i < spec->n_projected; i++) proj_idx.push_back(col_of(spec->projected_columns[i]));
-    std::vector<int> pred_col(n_preds);
+    std::vector<int> pred_col(n_preds), any_col(n_anys);
     for (int i = 0; i < n_preds; i++) pred_col[i] = col_of(preds[i].column);
+    for (int i = 0; i < n_anys; i++) any_col[i] = col_of(anys[i].column);
     const int lineage_col = spec->n_deleted_file_ids > 0 ? col_of("_data_file_id") : -1;
+    std::vector<Buf<uint8_t>> bound_bytes;
+    std::vector<ResolvedPredicate> rps(n_preds);
+    // The key's set (when a term is on the key, or for pruning): the predicates on the key and every term on it,
+    // intersected.  Without a term on the key its one range per file is intersect_ranges' result, as without terms.
+    auto on_key_name = [&](const char* column) { return spec->key_column && strcmp(column, spec->key_column) == 0; };
+    bool key_terms = false;
+    for (int i = 0; i < n_anys; i++) key_terms = key_terms || on_key_name(anys[i].column);
+    auto key_set_of = [&](const DevColumn& kc) {
+      const bool str = kc.type == HS_TYPE_STRING;
+      SetRange all;  // every value: an open string range, the whole encoded domain
+      if (!str) all.has_lo = all.has_hi = true, all.hi = encoded_max(kc.type);
+      RangeSet s{all};
+      for (int i = 0; i < n_preds; i++)
+        if (on_key_name(preds[i].column)) {
+          ResolvedPredicate rp;
+          const PredRange r = resolve_predicate(ctx, preds[i], kc, &bound_bytes, &rp);
+          s = intersect_sets(str, s, RangeSet{set_range_of(kc.type, r, rp.lo_host, rp.lo_len, rp.hi_host, rp.hi_len)});
+        }
+      for (int i = 0; i < n_anys; i++)
+        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, resolve_any(ctx, anys[i], kc));
+      return s;
+    };
+    // Bucket pruning: a key whose windows are points lives in the files of the points' buckets only
+    const hs_source_file* files = spec->files;
+    int n_files = spec->n_files;
+    std::vector<hs_source_file> kept;
+    std::vector<int> kept_bucket, point_bucket;
+    RangeSet key_set;
+    bool have_key_set = false;
+    if (file_buckets && num_buckets > 0 && spec->key_column && n_files > 0) {
+      for (int f = 0; f < n_files; f++)
+        if (file_buckets[f] < 0 || file_buckets[f] >= num_buckets) fail(HS_EINVAL, "bucket id %d out of range", file_buckets[f]);
+      const DevColumn kc = source_column_type(ctx, files[0], spec->key_column);
+      const bool hashable = kc.type == HS_TYPE_INT32 || kc.type == HS_TYPE_INT64 || kc.type == HS_TYPE_STRING;
+      bool keyed = key_terms;
+      for (int i = 0; i < n_preds; i++) keyed = keyed || on_key_name(preds[i].column);
+      if (hashable && keyed) {
+        key_set = key_set_of(kc);
+        have_key_set = true;
+        if (set_is_points(kc.type == HS_TYPE_STRING, key_set)) {
+          point_bucket = point_buckets(ctx, kc, key_set, num_buckets);
+          std::vector<char> hit(num_buckets, 0);
+          for (int b : point_bucket) hit[b] = 1;
+          for (int f = 0; f < n_files; f++)
+            if (hit[file_buckets[f]]) kept.push_back(files[f]), kept_bucket.push_back(file_buckets[f]);
+          // no file can hold a row: the first one is opened to give the result its columns, and searched for nothing
+          if (kept.empty()) kept.push_back(files[0]), kept_bucket.push_back(-1);
+          files = kept.data();
+          n_files = (int)kept.size();
+        }
+      }
+    }
+    const bool pruned = !kept.empty();
     SourceSet src;
-    open_sources(ctx, spec->files, spec->n_files, &src, &st);
+    open_sources(ctx, files, n_files, &src, &st);
     Table t;
     // phase 1 (sorted path): only the key column; the other columns are decoded after the binary search, restricted to
     // the pages that hold rows inside the windows
@@ -1080,18 +1354,28 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     if (legacy && try_sorted && t.cols[0].type != HS_TYPE_STRING && t.cols[0].type != HS_TYPE_INT64 && t.cols[0].type != HS_TYPE_INT32)
       fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
     const int64_t n = t.nrows;
-    std::vector<Buf<uint8_t>> bound_bytes;
-    std::vector<ResolvedPredicate> rps(n_preds);
     auto resolve = [&](int i) {
       rps[i].col = pred_col[i];
       rps[i].r = resolve_predicate(ctx, preds[i], t.cols[pred_col[i]], &bound_bytes, &rps[i]);
     };
+    std::vector<Buf<PredRange>> any_sets(n_anys);
     auto residual_set = [&](bool skip_key) {
       PredSet ps;
       for (int i = 0; i < n_preds; i++) {
         if (skip_key && pred_col[i] == 0) continue;
         const DevColumn& c = t.cols[rps[i].col];
         ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, rps[i].r};
+      }
+      for (int i = 0; i < n_anys; i++) {
+        if (skip_key && any_col[i] == 0) continue;
+        const DevColumn& c = t.cols[any_col[i]];
+        const RangeSet s = resolve_any(ctx, anys[i], c);
+        upload_set(ctx, c.type, s, &any_sets[i], &bound_bytes);
+        PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
+        d.r.type = c.type;
+        d.set = any_sets[i].get();
+        d.n_set = (int64_t)s.size();
+        ps.p[ps.n++] = d;
       }
       return ps;
     };
@@ -1106,53 +1390,99 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       t = std::move(full);
     }
     if (sorted) {
-      // K7: two binary searches per file, on the intersection of the predicates on the key
+      // K7: two binary searches per (file, range of the key): the intersection of the predicates on the key, or the
+      // disjoint ranges of the key's set
       const int ktype = t.cols[0].type;
       if (ktype < HS_TYPE_INT32 || ktype > HS_TYPE_STRING || ktype == HS_TYPE_BOOL)
         fail(HS_EUNSUPPORTED, "filter scan: the sorted key column '%s' must be int32 / int64 / float / double / string", cols[0].c_str());
-      std::vector<ResolvedPredicate> on_key;
+      int on_key = 0;
       for (int i = 0; i < n_preds; i++)
-        if (pred_col[i] == 0) {
-          resolve(i);
-          on_key.push_back(rps[i]);
-        }
-      const PredRange key_range = intersect_ranges(ktype, on_key);
-      const int nseg = spec->n_files;
+        if (pred_col[i] == 0) resolve(i), on_key++;
+      for (int i = 0; i < n_anys; i++) on_key += any_col[i] == 0;
+      const int nseg = n_files;
       std::vector<uint64_t> seg(nseg + 1);
       for (int f = 0; f <= nseg; f++) seg[f] = (uint64_t)t.file_row_begin[f];
       Buf<uint64_t> d_seg(ctx, nseg + 1);
-      Buf<int64_t> d_bounds(ctx, 2 * std::max(1, nseg));
       copy_h2d(ctx, d_seg.get(), seg.data(), 8 * (nseg + 1));
-      launch_range_bounds(ctx, t.cols[0].data.get(), key_range, d_seg.get(), nseg, d_bounds.get());
-      std::vector<int64_t> bounds(2 * std::max(1, nseg));
-      copy_d2h(ctx, bounds.data(), d_bounds.get(), 16 * nseg);
+      Buf<PredRange> d_ranges;
+      std::vector<uint2> work;
+      if (key_terms || pruned) {
+        if (!have_key_set) key_set = key_set_of(t.cols[0]);
+        upload_set(ctx, ktype, key_set, &d_ranges, &bound_bytes);
+        work.reserve((size_t)nseg * (pruned ? 1 : key_set.size()));
+        for (int f = 0; f < nseg; f++)
+          for (size_t r = 0; r < key_set.size(); r++)
+            if (!pruned || point_bucket[r] == kept_bucket[f]) work.push_back(make_uint2((unsigned)f, (unsigned)r));
+      } else {
+        std::vector<ResolvedPredicate> on_key_preds;
+        for (int i = 0; i < n_preds; i++)
+          if (pred_col[i] == 0) on_key_preds.push_back(rps[i]);
+        const PredRange key_range = intersect_ranges(ktype, on_key_preds);
+        d_ranges.alloc(ctx, 1);
+        copy_h2d(ctx, d_ranges.get(), &key_range, sizeof key_range);
+        for (int f = 0; f < nseg; f++) work.push_back(make_uint2((unsigned)f, 0u));
+      }
+      const int64_t nwork = (int64_t)work.size();
+      Buf<uint2> d_work(ctx, std::max<int64_t>(1, nwork));
+      Buf<int64_t> d_bounds(ctx, 2 * std::max<int64_t>(1, nwork));
+      if (nwork) copy_h2d(ctx, d_work.get(), work.data(), sizeof(uint2) * nwork);
+      launch_range_bounds(ctx, t.cols[0].data.get(), ktype, d_ranges.get(), d_seg.get(), d_work.get(), nwork, d_bounds.get());
+      std::vector<int64_t> bounds(2 * std::max<int64_t>(1, nwork));
+      if (nwork) copy_d2h(ctx, bounds.data(), d_bounds.get(), 16 * nwork);
       sync_stream(ctx);
-      std::vector<uint64_t> oo(nseg + 1, 0);
-      for (int f = 0; f < nseg; f++) oo[f + 1] = oo[f] + (uint64_t)(bounds[2 * f + 1] - bounds[2 * f]);
-      if (cols.size() > 1) {  // phase 2: decode the other columns, only the pages inside each file's [first, last)
-        std::vector<std::pair<int64_t, int64_t>> windows(nseg);
-        for (int f = 0; f < nseg; f++) windows[f] = {bounds[2 * f], bounds[2 * f + 1]};
+      // The windows, file by file and ascending inside a file (the ranges are), touching ones merged.  The pages to decode
+      // keep the empty windows too: an empty window still decodes the page it falls inside, as the one-range scan always
+      // has (so a nullable column keeps its validity array when no row qualifies); the candidate rows need only the
+      // non-empty ones.
+      FileWindows fw;
+      fw.offsets.assign(nseg + 1, 0);
+      std::vector<int64_t> win;         // non-empty windows: [lo, hi) global rows
+      std::vector<uint64_t> oo(1, 0);   // output offset of every non-empty window
+      int prev_f = -1, prev_win_f = -1;
+      for (int64_t w = 0; w < nwork; w++) {
+        const int f = (int)work[w].x;
+        const int64_t first = bounds[2 * w], last = bounds[2 * w + 1];
+        if (prev_f == f && fw.windows.back().second >= first) {
+          fw.windows.back().second = std::max(fw.windows.back().second, last);
+        } else {
+          fw.windows.push_back({first, last});
+          fw.offsets[f + 1]++;
+        }
+        prev_f = f;
+        if (last <= first) continue;
+        if (prev_win_f == f && win.back() == (int64_t)seg[f] + first) {
+          win.back() = (int64_t)seg[f] + last;
+        } else {
+          win.push_back((int64_t)seg[f] + first);
+          win.push_back((int64_t)seg[f] + last);
+          oo.push_back(oo.back());
+        }
+        prev_win_f = f;
+        oo.back() += (uint64_t)(last - first);
+      }
+      for (int f = 0; f < nseg; f++) fw.offsets[f + 1] += fw.offsets[f];
+      const int64_t nwin = (int64_t)win.size() / 2;
+      if (cols.size() > 1) {  // phase 2: decode the other columns, only the pages inside the windows
         std::vector<std::string> rest(cols.begin() + 1, cols.end());
         Table others;
-        decode_sources(ctx, src, rest, &windows, &others, &st);
+        decode_sources(ctx, src, rest, &fw, &others, &st);
         for (auto& c : others.cols) t.cols.push_back(std::move(c));
       }
-      const int64_t n_cand = (int64_t)oo[nseg];
-      Buf<uint64_t> d_oo(ctx, nseg + 1);
-      copy_h2d(ctx, d_oo.get(), oo.data(), 8 * (nseg + 1));
+      const int64_t n_cand = (int64_t)oo.back();
+      Buf<int64_t> d_win(ctx, std::max<size_t>(2, win.size()));
+      Buf<uint64_t> d_oo(ctx, oo.size());
+      if (nwin) copy_h2d(ctx, d_win.get(), win.data(), 8 * win.size());
+      copy_h2d(ctx, d_oo.get(), oo.data(), 8 * oo.size());
       idx.alloc(ctx, std::max<int64_t>(1, n_cand));
-      if (nseg) {
-        k_ranges_to_indices<<<nseg, 256, 0, ctx->stream>>>(d_bounds.get(), d_seg.get(), d_oo.get(), nseg, idx.get());
-        HS_LAUNCH_CHECK(ctx);
-      }
+      if (nseg) launch_windows_to_indices(ctx, d_win.get(), d_oo.get(), nwin, n_cand, idx.get());
       n_out = n_cand;
-      if ((int)on_key.size() < n_preds) {
+      if (on_key < n_preds + n_anys) {
         // residual: the predicates on other columns, over the window rows, compacted through the candidate list
         for (int i = 0; i < n_preds; i++)
           if (pred_col[i] != 0) resolve(i);
-        Buf<uint32_t> kept;
-        n_out = select_rows(ctx, residual_set(true), idx.get(), n_cand, nullptr, nullptr, 0, &kept);
-        idx = std::move(kept);
+        Buf<uint32_t> kept_rows;
+        n_out = select_rows(ctx, residual_set(true), idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
+        idx = std::move(kept_rows);
       }
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
@@ -1202,6 +1532,52 @@ static int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_
   return HS_OK;
 }
 
+// The same for the disjunction terms beside n_preds predicates: their counts, arrays, offsets and string lengths.
+static int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_stats* stats, char* err, size_t errlen) {
+  char msg[256];
+  auto refuse = [&](int code) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "%s", msg);
+    return code;
+  };
+  if (n_anys < 0 || (n_anys > 0 && !anys)) return snprintf(msg, sizeof msg, "filter scan: bad term array"), refuse(HS_EINVAL);
+  if (n_preds + n_anys > kMaxPredicates)
+    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
+  for (int i = 0; i < n_anys; i++) {
+    const hs_predicate_any& a = anys[i];
+    if (!a.column) return snprintf(msg, sizeof msg, "filter scan: term without a column"), refuse(HS_EINVAL);
+    const char* c = a.column;
+    if (a.n_values < 0 || a.n_ranges < 0 || (a.n_ranges > 0 && !a.ranges))
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has a bad value or range array", c), refuse(HS_EINVAL);
+    if (a.n_values + a.n_ranges > (1ll << 24))
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than 2^24 values and ranges", c), refuse(HS_EUNSUPPORTED);
+    if (a.literal_type != HS_TYPE_INT64 && a.literal_type != HS_TYPE_DOUBLE && a.literal_type != HS_TYPE_STRING &&
+        a.literal_type != HS_TYPE_DECIMAL)
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has an unknown literal type", c), refuse(HS_EINVAL);
+    if (a.n_values > 0) {
+      const bool missing = a.literal_type == HS_TYPE_STRING ? (!a.values_offsets || (!a.values_bytes && a.values_offsets[a.n_values] != a.values_offsets[0]))
+                                                            : (a.literal_type == HS_TYPE_DOUBLE ? !a.values_f : !a.values_i);
+      if (missing) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has no value array", c), refuse(HS_EINVAL);
+      if (a.literal_type == HS_TYPE_STRING)
+        for (int64_t k = 0; k < a.n_values; k++) {
+          if (a.values_offsets[k + 1] < a.values_offsets[k])
+            return snprintf(msg, sizeof msg, "filter scan: term on '%s' has descending value offsets", c), refuse(HS_EINVAL);
+          if (a.values_offsets[k + 1] - a.values_offsets[k] > kMaxStringLen)
+            return snprintf(msg, sizeof msg, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c), refuse(HS_EUNSUPPORTED);
+        }
+    }
+    for (int r = 0; r < a.n_ranges; r++) {
+      if (a.ranges[r].column && strcmp(a.ranges[r].column, c) != 0)
+        return snprintf(msg, sizeof msg, "filter scan: a range of the term on '%s' names another column", c), refuse(HS_EINVAL);
+      hs_predicate q = a.ranges[r];
+      q.column = c;
+      const int rc = check_predicates(&q, 1, false, stats, err, errlen);
+      if (rc != HS_OK) return rc;
+    }
+  }
+  return HS_OK;
+}
+
 extern "C" {
 
 int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
@@ -1221,7 +1597,7 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
   p.lo_i = spec->lo, p.hi_i = spec->hi;
   p.lo_bytes = spec->lo_bytes, p.hi_bytes = spec->hi_bytes;
   p.lo_len = spec->lo_len, p.hi_len = spec->hi_len;
-  return filter_scan_core(ctx, spec, &p, 1, true, out, stats, err, errlen);
+  return filter_scan_core(ctx, spec, &p, 1, true, nullptr, 0, nullptr, 0, out, stats, err, errlen);
 }
 
 int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
@@ -1230,7 +1606,25 @@ int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predica
   *out = nullptr;
   const int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
   if (rc != HS_OK) return rc;
-  return filter_scan_core(ctx, spec, preds, n_preds, false, out, stats, err, errlen);
+  return filter_scan_core(ctx, spec, preds, n_preds, false, nullptr, 0, nullptr, 0, out, stats, err, errlen);
+}
+
+int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                       const hs_predicate_any* anys, int32_t n_anys, const int32_t* file_buckets, int32_t num_buckets,
+                       hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds) || num_buckets < 0 || (num_buckets > 0 && !file_buckets))
+    return HS_EINVAL;
+  *out = nullptr;
+  int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
+  if (rc == HS_OK) rc = check_anys(anys, n_anys, n_preds, stats, err, errlen);
+  if (rc != HS_OK) return rc;
+  if (num_buckets > kMaxBuckets) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "numBuckets must be in 1..%d", kMaxBuckets);
+    return HS_EUNSUPPORTED;
+  }
+  return filter_scan_core(ctx, spec, preds, n_preds, false, anys, n_anys, num_buckets > 0 ? file_buckets : nullptr, num_buckets,
+                          out, stats, err, errlen);
 }
 
 }  // extern "C"
@@ -1319,7 +1713,9 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, int
 // probes on the key columns where they lie: the decoded columns, or their gather through the side's permutation.
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                             int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
-                            int n_right_preds, bool legacy, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+                            int n_right_preds, const hs_predicate_any* left_anys, int n_left_anys,
+                            const hs_predicate_any* right_anys, int n_right_anys, bool legacy, hs_batch** out, hs_stats* stats,
+                            char* err, size_t errlen) {
   hs_stats st;
   memset(&st, 0, sizeof st);
   std::unique_ptr<hs_batch> res(new hs_batch());
@@ -1330,9 +1726,10 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.start();
     const int nb = spec->num_buckets;
     if (nb < 1) fail(HS_EINVAL, "num_buckets must be positive");
-    // columns to decode: the keys first, then the projection, then the predicate columns
+    // columns to decode: the keys first, then the projection, then the predicate and term columns
     auto side_columns = [&](const char* const* keys, const char* const* proj, int n_proj, const hs_predicate* preds, int n_preds,
-                            std::vector<int>* proj_idx, std::vector<int>* pred_idx) {
+                            const hs_predicate_any* anys, int n_anys, std::vector<int>* proj_idx, std::vector<int>* pred_idx,
+                            std::vector<int>* any_idx) {
       std::vector<std::string> cols;
       for (int k = 0; k < n_keys; k++) {
         if (!keys[k]) fail(HS_EINVAL, "bucket join: missing key column");
@@ -1347,11 +1744,14 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       };
       for (int i = 0; i < n_proj; i++) proj_idx->push_back(col_of(proj[i]));
       for (int i = 0; i < n_preds; i++) pred_idx->push_back(col_of(preds[i].column));
+      for (int i = 0; i < n_anys; i++) any_idx->push_back(col_of(anys[i].column));
       return cols;
     };
-    std::vector<int> lproj, rproj, lpred, rpred;
-    const std::vector<std::string> lcols = side_columns(left_keys, spec->left_columns, spec->n_left_columns, left_preds, n_left_preds, &lproj, &lpred);
-    const std::vector<std::string> rcols = side_columns(right_keys, spec->right_columns, spec->n_right_columns, right_preds, n_right_preds, &rproj, &rpred);
+    std::vector<int> lproj, rproj, lpred, rpred, lany, rany;
+    const std::vector<std::string> lcols = side_columns(left_keys, spec->left_columns, spec->n_left_columns, left_preds, n_left_preds,
+                                                        left_anys, n_left_anys, &lproj, &lpred, &lany);
+    const std::vector<std::string> rcols = side_columns(right_keys, spec->right_columns, spec->n_right_columns, right_preds, n_right_preds,
+                                                        right_anys, n_right_anys, &rproj, &rpred, &rany);
     JoinSide L, R;
     prepare_join_side(ctx, &L, spec->left_files, spec->n_left, spec->left_buckets, nb, lcols, n_keys, legacy, &st);
     prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, n_keys, legacy, &st);
@@ -1370,7 +1770,9 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
     // side selection: IS NOT NULL on the nullable key columns, then the side's predicates
     std::vector<Buf<uint8_t>> bound_bytes;
-    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx) {
+    std::vector<Buf<PredRange>> any_sets;
+    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, const hs_predicate_any* anys,
+                          const std::vector<int>& any_idx) {
       PredSet ps;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
@@ -1386,9 +1788,21 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
         const PredRange r = resolve_predicate(ctx, preds[i], c, &bound_bytes, &rp);
         ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, r};
       }
+      for (size_t i = 0; i < any_idx.size(); i++) {
+        const DevColumn& c = s.t.cols[any_idx[i]];
+        const RangeSet set = resolve_any(ctx, anys[i], c);
+        any_sets.emplace_back();
+        upload_set(ctx, c.type, set, &any_sets.back(), &bound_bytes);
+        PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
+        d.r.type = c.type;
+        d.set = any_sets.back().get();
+        d.n_set = (int64_t)set.size();
+        ps.p[ps.n++] = d;
+      }
       return ps;
     };
-    const PredSet lps = side_preds(L, left_preds, lpred), rps = side_preds(R, right_preds, rpred);
+    any_sets.reserve(n_left_anys + n_right_anys);
+    const PredSet lps = side_preds(L, left_preds, lpred, left_anys, lany), rps = side_preds(R, right_preds, rpred, right_anys, rany);
     StageTimer t_sel(ctx);
     t_sel.start();
     select_join_side(ctx, &L, lps, nb);
@@ -1449,7 +1863,8 @@ extern "C" {
 int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out) return HS_EINVAL;
   *out = nullptr;
-  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, true, out, stats, err, errlen);
+  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, true, out,
+                          stats, err, errlen);
 }
 
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
@@ -1470,8 +1885,34 @@ int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* cons
   int rc = check_predicates(left_preds, n_left_preds, false, stats, err, errlen);
   if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
   if (rc != HS_OK) return rc;
-  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, false,
-                          out, stats, err, errlen);
+  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, nullptr, 0,
+                          nullptr, 0, false, out, stats, err, errlen);
+}
+
+int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
+                       int32_t n_left_anys, const hs_predicate* right_preds, int32_t n_right_preds,
+                       const hs_predicate_any* right_anys, int32_t n_right_anys, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen) {
+  if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
+      (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
+    return HS_EINVAL;
+  *out = nullptr;
+  auto refuse = [&](int code, const char* msg) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "%s", msg);
+    return code;
+  };
+  if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
+  if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
+  if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
+  int rc = check_predicates(left_preds, n_left_preds, false, stats, err, errlen);
+  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
+  if (rc == HS_OK) rc = check_anys(left_anys, n_left_anys, n_left_preds, stats, err, errlen);
+  if (rc == HS_OK) rc = check_anys(right_anys, n_right_anys, n_right_preds, stats, err, errlen);
+  if (rc != HS_OK) return rc;
+  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, left_anys,
+                          n_left_anys, right_anys, n_right_anys, false, out, stats, err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

@@ -350,9 +350,49 @@ struct DecodeCache {
 };
 static void free_decode_cache(void* p) { delete static_cast<DecodeCache*>(p); }
 
-void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>& columns,
-                    const std::vector<std::pair<int64_t, int64_t>>* file_windows, Table* out, hs_stats* stats,
-                    const CarryOptions* carry) {
+DevColumn source_column_type(hs_ctx* ctx, const hs_source_file& sf, const std::string& name) {
+  const std::string what = sf.path ? sf.path : "source file";
+  uint64_t size = sf.size;
+  std::vector<uint8_t> tail(8), footer;
+  auto read_at = [&](uint64_t off, uint8_t* dst, uint64_t n) {
+    if (sf.data && sf.on_device) HS_CUDA(cudaMemcpy(dst, (const uint8_t*)sf.data + off, n, cudaMemcpyDeviceToHost));
+    else if (sf.data) memcpy(dst, (const uint8_t*)sf.data + off, n);
+    else {
+      int fd = open(sf.path, O_RDONLY);
+      if (fd < 0) fail(HS_EIO, "cannot open %s", sf.path);
+      const ssize_t r = pread(fd, dst, n, (off_t)off);
+      close(fd);
+      if (r != (ssize_t)n) fail(HS_EIO, "short read on %s", sf.path);
+    }
+  };
+  if (!sf.data) {
+    if (!sf.path) fail(HS_EINVAL, "source file without path or data");
+    struct stat stt;
+    if (stat(sf.path, &stt) != 0) fail(HS_EIO, "cannot stat %s", sf.path);
+    size = (uint64_t)stt.st_size;
+  }
+  if (size < 12) fail(HS_EFORMAT, "%s: not a Parquet file", what.c_str());
+  read_at(size - 8, tail.data(), 8);
+  uint32_t flen;
+  memcpy(&flen, tail.data(), 4);
+  if (memcmp(tail.data() + 4, "PAR1", 4) != 0 || (uint64_t)flen + 12 > size) fail(HS_EFORMAT, "%s: not a Parquet file", what.c_str());
+  footer.resize(flen);
+  read_at(size - 8 - flen, footer.data(), flen);
+  const pq::FileMeta fm = pq::parse_footer_bytes(footer.data(), flen, what.c_str());
+  const int idx = find_column(fm, name);
+  if (idx < 0) fail(HS_EINVAL, "%s: column '%s' not found", what.c_str(), name.c_str());
+  const SourceType st = source_type_of(fm.columns[idx], what.c_str());
+  DevColumn dc;
+  dc.name = name;
+  dc.type = st.type;
+  dc.width = type_width(st.type);
+  dc.schema = st.schema;
+  dc.schema.name = name;
+  return dc;
+}
+
+void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>& columns, const FileWindows* file_windows,
+                    Table* out, hs_stats* stats, const CarryOptions* carry) {
   StageTimer t_plan(ctx), t_dec(ctx);
   const int n_files = set.n_files;
   std::vector<FileImage>& imgs = set.impl->imgs;
@@ -709,20 +749,25 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
   alloc_destinations();
   copy_h2d(ctx, d_cols.get(), h_cols.data(), sizeof(ColumnOut) * ncols);
   // ---- decode -----------------------------------------------------------------------------------------
-  // optional per-file row windows (file-relative -> global): pages that do not intersect their file's window are skipped
-  Buf<int64_t> d_window;
+  // optional per-file row windows (file-relative -> global): pages that intersect none of their file's windows are skipped
+  Buf<int64_t> d_window, d_window_offsets;
   if (file_windows) {
-    std::vector<int64_t> w(2 * (size_t)n_files);
-    for (int f = 0; f < n_files; f++) {
-      w[2 * f] = out->file_row_begin[f] + (*file_windows)[f].first;
-      w[2 * f + 1] = out->file_row_begin[f] + (*file_windows)[f].second;
-    }
+    const FileWindows& fw = *file_windows;
+    std::vector<int64_t> w(2 * std::max<size_t>(1, fw.windows.size()));
+    for (int f = 0; f < n_files; f++)
+      for (int64_t i = fw.offsets[f]; i < fw.offsets[f + 1]; i++) {
+        w[2 * i] = out->file_row_begin[f] + fw.windows[i].first;
+        w[2 * i + 1] = out->file_row_begin[f] + fw.windows[i].second;
+      }
     d_window.alloc(ctx, w.size());
+    d_window_offsets.alloc(ctx, n_files + 1);
     copy_h2d(ctx, d_window.get(), w.data(), 8 * w.size());
+    copy_h2d(ctx, d_window_offsets.get(), fw.offsets.data(), 8 * ((size_t)n_files + 1));
     sync_stream(ctx);
   }
   launch_decode_pages(ctx, d_pages.get(), n_pages, d_cols.get(), d_flags.get() + 1, file_windows ? d_window.get() : nullptr,
-                      d_flags.get(), std::find(col_converted.begin(), col_converted.end(), true) != col_converted.end());
+                      d_window_offsets.get(), d_flags.get(),
+                      std::find(col_converted.begin(), col_converted.end(), true) != col_converted.end());
   std::vector<uint32_t> flags(1 + ncols);
   copy_d2h(ctx, flags.data(), d_flags.get(), sizeof(uint32_t) * (1 + ncols));
   t_dec.stop();

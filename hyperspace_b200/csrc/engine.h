@@ -141,10 +141,17 @@ struct SourceSet {
   SourceSet& operator=(const SourceSet&) = delete;
 };
 void open_sources(hs_ctx* ctx, const hs_source_file* files, int n_files, SourceSet* set, hs_stats* stats);
-// file_windows (optional): per file, the half-open range of file-relative rows that must be decoded
-void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>& columns,
-                    const std::vector<std::pair<int64_t, int64_t>>* file_windows, Table* out, hs_stats* stats,
-                    const CarryOptions* carry = nullptr);
+// The rows of each file that must be decoded: windows[offsets[f] .. offsets[f+1]) are file f's half-open ranges of
+// file-relative rows, ascending and disjoint (offsets: n_files + 1 entries).
+struct FileWindows {
+  std::vector<int64_t> offsets;
+  std::vector<std::pair<int64_t, int64_t>> windows;
+};
+// file_windows (optional): only the pages that intersect one of their file's windows are decoded
+void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>& columns, const FileWindows* file_windows,
+                    Table* out, hs_stats* stats, const CarryOptions* carry = nullptr);
+// type, width and schema of column `name` as decode_sources would decode it, read from the footer of `file` alone
+DevColumn source_column_type(hs_ctx* ctx, const hs_source_file& file, const std::string& name);
 
 // K2-K4 on a decoded table whose first nkeys columns are the indexed columns.
 // defer_settle: the sort may be left queued (sort_rows' may_defer) -- the caller must call settle_sort() after its next

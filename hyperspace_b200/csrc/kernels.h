@@ -131,11 +131,13 @@ void decompress_blobs(hs_ctx* ctx, std::vector<PageBlob>& blobs, uint8_t* scratc
 // mode 1: fills pages[page_offsets[chunk] ...].
 void launch_walk_pages(hs_ctx* ctx, const ChunkDesc* chunks, int n_chunks, int32_t* page_counts,
                        const int64_t* page_offsets, PageDesc* pages, uint32_t* d_error, int mode);
-// Decodes all pages into the column arrays.  row_window (optional, device, 2 x int64 per file: [lo, hi) global rows)
-// restricts decoding to pages that intersect the window of their file.  any_converted: some page has a ValueConv (those
-// are decoded by k_decode_converted_pages, launched right after k_decode_pages).
+// Decodes all pages into the column arrays.  windows (optional, device): [lo, hi) global rows, ascending and disjoint
+// within a file; the windows of file f are windows[window_offsets[f] .. window_offsets[f+1]) (pairs).  A page is decoded
+// only when it intersects one of its file's windows.  any_converted: some page has a ValueConv (those are decoded by
+// k_decode_converted_pages, launched right after k_decode_pages).
 void launch_decode_pages(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, const ColumnOut* cols,
-                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error, bool any_converted);
+                         uint32_t* col_has_nulls, const int64_t* windows, const int64_t* window_offsets, uint32_t* d_error,
+                         bool any_converted);
 
 // ---- hash / partition (hash_partition.cu) ---------------------------------------------------------------------------
 struct KeyColumn {
@@ -408,15 +410,24 @@ struct PredDesc {
   const void* data;      // column values (string references for strings)
   const uint8_t* valid;  // nullptr: no nulls; a null never satisfies a predicate
   PredRange r;           // neither bound: the row only has to be non-null (a join side's key columns)
+  // set form (a disjunction on the column): when set is not nullptr the value must lie in one of the n_set ranges at set
+  // (device; ascending and disjoint, of type r.type), and r's bounds are not used
+  const PredRange* set = nullptr;
+  int64_t n_set = 0;
 };
 struct PredSet {
   PredDesc p[kMaxPredicates + kMaxJoinKeys];  // a join side: its predicates plus one IS NOT NULL per nullable key column
   int n = 0;
 };
-// per sorted segment s (ascending on `keys`): bounds[2s] = first row inside r, bounds[2s+1] = first row above r
-// (segment-relative)
-void launch_range_bounds(hs_ctx* ctx, const void* keys, const PredRange& r, const uint64_t* seg_offsets, int nseg,
-                         int64_t* bounds);
+// The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
+// work[w] = {s, r} with r indexing `ranges` (device); bounds[2w] = first row of s inside ranges[r], bounds[2w+1] = first
+// row above it (segment-relative).  All ranges are of type ranges_type.
+void launch_range_bounds(hs_ctx* ctx, const void* keys, int ranges_type, const PredRange* ranges, const uint64_t* seg_offsets,
+                         const uint2* work, int64_t nwork, int64_t* bounds);
+// the candidate rows of sorted windows: out_idx[o] = win[2w] + (o - out_offsets[w]) for out_offsets[w] <= o <
+// out_offsets[w+1] (win: [lo, hi) global rows, out_offsets: nwin + 1 entries).  One thread per output row.
+void launch_windows_to_indices(hs_ctx* ctx, const int64_t* win, const uint64_t* out_offsets, int64_t nwin, int64_t n_out,
+                               uint32_t* out_idx);
 // mask[i] = every predicate of `preds` holds for row cand[i] (row i when cand is nullptr)
 void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, uint32_t* mask);
 // The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its

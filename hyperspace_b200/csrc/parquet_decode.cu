@@ -908,18 +908,29 @@ __global__ void k_build_string_dicts(const StringDictJob* __restrict__ jobs, int
   }
 }
 
+// a page lies outside every window of its file (launch_decode_pages): one binary search for the first window ending after
+// the page's first row
+__device__ __forceinline__ bool page_outside_windows(const PageDesc& pg, const int64_t* __restrict__ windows,
+                                                     const int64_t* __restrict__ window_offsets) {
+  int64_t lo = window_offsets[pg.file_index], hi = window_offsets[pg.file_index + 1];
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (windows[2 * mid + 1] <= pg.first_row) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo == window_offsets[pg.file_index + 1] || windows[2 * lo] >= pg.first_row + pg.num_values;
+}
+
 __global__ void __launch_bounds__(kDecodeThreads) k_decode_pages(const PageDesc* __restrict__ pages,
                                                                  const ColumnOut* __restrict__ cols,
                                                                  uint32_t* col_has_nulls,
-                                                                 const int64_t* __restrict__ row_window,
+                                                                 const int64_t* __restrict__ windows,
+                                                                 const int64_t* __restrict__ window_offsets,
                                                                  uint32_t* d_error) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   DecodeShared& sm = *reinterpret_cast<DecodeShared*>(smem_raw);
   const PageDesc pg = pages[blockIdx.x];
-  if (row_window) {
-    const int64_t lo = row_window[2 * pg.file_index], hi = row_window[2 * pg.file_index + 1];
-    if (pg.first_row + pg.num_values <= lo || pg.first_row >= hi) return;
-  }
+  if (windows && page_outside_windows(pg, windows, window_offsets)) return;
   const ColumnOut co = cols[pg.col];
   if (co.skip || pg.conv != CONV_NONE) return;  // zero-copy column: read in place by the partition; converted: below
   switch (pg.phys_type) {
@@ -944,16 +955,14 @@ __global__ void __launch_bounds__(kDecodeThreads) k_decode_pages(const PageDesc*
 __global__ void __launch_bounds__(kDecodeThreads) k_decode_converted_pages(const PageDesc* __restrict__ pages,
                                                                            const ColumnOut* __restrict__ cols,
                                                                            uint32_t* col_has_nulls,
-                                                                           const int64_t* __restrict__ row_window,
+                                                                           const int64_t* __restrict__ windows,
+                                                                           const int64_t* __restrict__ window_offsets,
                                                                            uint32_t* d_error) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   DecodeShared& sm = *reinterpret_cast<DecodeShared*>(smem_raw);
   const PageDesc pg = pages[blockIdx.x];
   if (pg.conv == CONV_NONE) return;
-  if (row_window) {
-    const int64_t lo = row_window[2 * pg.file_index], hi = row_window[2 * pg.file_index + 1];
-    if (pg.first_row + pg.num_values <= lo || pg.first_row >= hi) return;
-  }
+  if (windows && page_outside_windows(pg, windows, window_offsets)) return;
   const ColumnOut co = cols[pg.col];
   // the column's width, whatever the stored type
   if (co.width == 8) decode_page<8, true>(pg, co, col_has_nulls + pg.col, d_error, sm);
@@ -995,7 +1004,8 @@ void launch_fill_zc_tiles(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, Z
 }
 
 void launch_decode_pages(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, const ColumnOut* cols,
-                         uint32_t* col_has_nulls, const int64_t* row_window, uint32_t* d_error, bool any_converted) {
+                         uint32_t* col_has_nulls, const int64_t* windows, const int64_t* window_offsets, uint32_t* d_error,
+                         bool any_converted) {
   if (n_pages == 0) return;
   static DeviceOnce attr_set_once;
   bool& attr_set = attr_set_once(ctx->device);
@@ -1007,13 +1017,14 @@ void launch_decode_pages(hs_ctx* ctx, const PageDesc* pages, int64_t n_pages, co
   {
     KernelScope _ks(ctx, "k_decode_pages");
     k_decode_pages<<<(unsigned)n_pages, kDecodeThreads, sizeof(DecodeShared), ctx->stream>>>(pages, cols, col_has_nulls,
-                                                                                             row_window, d_error);
+                                                                                             windows, window_offsets, d_error);
     HS_LAUNCH_CHECK(ctx);
   }
   if (any_converted) {
     KernelScope _ks(ctx, "k_decode_converted_pages");
     k_decode_converted_pages<<<(unsigned)n_pages, kDecodeThreads, sizeof(DecodeShared), ctx->stream>>>(pages, cols, col_has_nulls,
-                                                                                                       row_window, d_error);
+                                                                                                       windows, window_offsets,
+                                                                                                       d_error);
     HS_LAUNCH_CHECK(ctx);
   }
 }

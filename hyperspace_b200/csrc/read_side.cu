@@ -43,19 +43,39 @@ __device__ __forceinline__ int64_t first_at_least(const void* col, int64_t b, in
   return lo;
 }
 
-// K7 window search, one thread per sorted file: bounds[2s] = first row inside the range, bounds[2s+1] = first row above it.
-// Numeric bounds are inclusive (strictness is folded in on the host); string bounds carry their strictness.
+// K7 window search, one thread per (sorted file, range) work item: bounds[2w] = first row inside the range, bounds[2w+1] =
+// first row above it.  Numeric bounds are inclusive (strictness is folded in on the host); string bounds carry their
+// strictness.
 template <int KT>
-__global__ void k_range_bounds(const void* __restrict__ keys, PredRange r, const uint64_t* __restrict__ seg_offsets, int nseg,
+__global__ void k_range_bounds(const void* __restrict__ keys, const PredRange* __restrict__ ranges,
+                               const uint64_t* __restrict__ seg_offsets, const uint2* __restrict__ work, int64_t nwork,
                                int64_t* __restrict__ bounds) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= nseg) return;
-  const int64_t b = (int64_t)seg_offsets[s], n = (int64_t)seg_offsets[s + 1] - b;
+  const int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= nwork) return;
+  const uint2 sr = work[w];
+  const PredRange r = ranges[sr.y];
+  const int64_t b = (int64_t)seg_offsets[sr.x], n = (int64_t)seg_offsets[sr.x + 1] - b;
   int64_t first = r.has_lo ? first_at_least<KT>(keys, b, n, r.lo, r.lo_strict ? 1 : 0) : 0;
   int64_t last = r.has_hi ? first_at_least<KT>(keys, b, n, r.hi, r.hi_strict ? 0 : 1) : n;
   if (last < first) last = first;
-  bounds[2 * s] = first;
-  bounds[2 * s + 1] = last;
+  bounds[2 * w] = first;
+  bounds[2 * w + 1] = last;
+}
+
+// one thread per output row: the window holding output position o is found by binary search over the windows' output
+// offsets, so millions of windows of 0-2 rows cost no more than a few long ones
+__global__ void k_ranges_to_indices(const int64_t* __restrict__ win, const uint64_t* __restrict__ out_offsets, int64_t nwin,
+                                    int64_t n_out, uint32_t* __restrict__ out_idx) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; o < n_out; o += stride) {
+    int64_t lo = 0, hi = nwin - 1;  // last window with out_offsets[w] <= o
+    while (lo < hi) {
+      const int64_t mid = hi - ((hi - lo) >> 1);
+      if (out_offsets[mid] <= (uint64_t)o) lo = mid;
+      else hi = mid - 1;
+    }
+    out_idx[o] = (uint32_t)(win[2 * lo] + (o - (int64_t)out_offsets[lo]));
+  }
 }
 
 template <int KT>
@@ -63,6 +83,20 @@ __device__ __forceinline__ bool in_range(const void* col, int64_t i, const PredR
   if (r.has_lo && cmp_bound<KT>(col, i, r.lo) < (r.lo_strict ? 1 : 0)) return false;
   if (r.has_hi && cmp_bound<KT>(col, i, r.hi) > (r.hi_strict ? -1 : 0)) return false;
   return true;
+}
+
+// the predicate on row i: its range, or (set form) one binary search for the first range of the set not below the value
+template <int KT>
+__device__ __forceinline__ bool holds(const PredDesc& d, int64_t i) {
+  if (!d.set) return in_range<KT>(d.data, i, d.r);
+  int64_t lo = 0, hi = d.n_set;
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    const PredRange& r = d.set[mid];
+    if (r.has_hi && cmp_bound<KT>(d.data, i, r.hi) > (r.hi_strict ? -1 : 0)) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < d.n_set && in_range<KT>(d.data, i, d.set[lo]);
 }
 
 // The residual conjunction, one thread per candidate row: mask[i] = every predicate holds for row cand[i] (row i without a
@@ -80,11 +114,11 @@ __global__ void k_predicate_mask(const __grid_constant__ PredSet ps, const uint3
         continue;
       }
       switch (d.r.type) {
-        case HS_TYPE_INT32: ok = in_range<HS_TYPE_INT32>(d.data, row, d.r); break;
-        case HS_TYPE_INT64: ok = in_range<HS_TYPE_INT64>(d.data, row, d.r); break;
-        case HS_TYPE_FLOAT: ok = in_range<HS_TYPE_FLOAT>(d.data, row, d.r); break;
-        case HS_TYPE_DOUBLE: ok = in_range<HS_TYPE_DOUBLE>(d.data, row, d.r); break;
-        default: ok = in_range<HS_TYPE_STRING>(d.data, row, d.r); break;
+        case HS_TYPE_INT32: ok = holds<HS_TYPE_INT32>(d, row); break;
+        case HS_TYPE_INT64: ok = holds<HS_TYPE_INT64>(d, row); break;
+        case HS_TYPE_FLOAT: ok = holds<HS_TYPE_FLOAT>(d, row); break;
+        case HS_TYPE_DOUBLE: ok = holds<HS_TYPE_DOUBLE>(d, row); break;
+        default: ok = holds<HS_TYPE_STRING>(d, row); break;
       }
     }
     mask[i] = ok ? 1u : 0u;
@@ -323,19 +357,25 @@ void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid
   HS_LAUNCH_CHECK(ctx);
 }
 
-void launch_range_bounds(hs_ctx* ctx, const void* keys, const PredRange& r, const uint64_t* seg_offsets, int nseg,
-                         int64_t* bounds) {
+void launch_range_bounds(hs_ctx* ctx, const void* keys, int ranges_type, const PredRange* ranges, const uint64_t* seg_offsets,
+                         const uint2* work, int64_t nwork, int64_t* bounds) {
   KernelScope _ks(ctx, "k_range_bounds");
-  if (nseg == 0) return;
-  const int grid = (nseg + 127) / 128;
-  switch (r.type) {
-    case HS_TYPE_INT32: k_range_bounds<HS_TYPE_INT32><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
-    case HS_TYPE_INT64: k_range_bounds<HS_TYPE_INT64><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
-    case HS_TYPE_FLOAT: k_range_bounds<HS_TYPE_FLOAT><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
-    case HS_TYPE_DOUBLE: k_range_bounds<HS_TYPE_DOUBLE><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
-    case HS_TYPE_STRING: k_range_bounds<HS_TYPE_STRING><<<grid, 128, 0, ctx->stream>>>(keys, r, seg_offsets, nseg, bounds); break;
-    default: fail(HS_EUNSUPPORTED, "range search over a column of type %d", r.type);
+  if (nwork == 0) return;
+  const unsigned grid = (unsigned)ceil_div(nwork, 128);
+  switch (ranges_type) {
+    case HS_TYPE_INT32: k_range_bounds<HS_TYPE_INT32><<<grid, 128, 0, ctx->stream>>>(keys, ranges, seg_offsets, work, nwork, bounds); break;
+    case HS_TYPE_INT64: k_range_bounds<HS_TYPE_INT64><<<grid, 128, 0, ctx->stream>>>(keys, ranges, seg_offsets, work, nwork, bounds); break;
+    case HS_TYPE_FLOAT: k_range_bounds<HS_TYPE_FLOAT><<<grid, 128, 0, ctx->stream>>>(keys, ranges, seg_offsets, work, nwork, bounds); break;
+    case HS_TYPE_DOUBLE: k_range_bounds<HS_TYPE_DOUBLE><<<grid, 128, 0, ctx->stream>>>(keys, ranges, seg_offsets, work, nwork, bounds); break;
+    case HS_TYPE_STRING: k_range_bounds<HS_TYPE_STRING><<<grid, 128, 0, ctx->stream>>>(keys, ranges, seg_offsets, work, nwork, bounds); break;
+    default: fail(HS_EUNSUPPORTED, "range search over a column of type %d", ranges_type);
   }
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_windows_to_indices(hs_ctx* ctx, const int64_t* win, const uint64_t* out_offsets, int64_t nwin, int64_t n_out,
+                               uint32_t* out_idx) {
+  k_ranges_to_indices<<<grid_for(ctx, n_out, 256, 16), 256, 0, ctx->stream>>>(win, out_offsets, nwin, n_out, out_idx);
   HS_LAUNCH_CHECK(ctx);
 }
 

@@ -184,26 +184,39 @@ def _host_column(d: np.ndarray) -> np.ndarray:
         return d.copy()
 
 
+def _terms_text(pred) -> str:
+    """The disjunction terms of a filter for explain(), long lists cut short: `k IN (1, 2, 3, ... 997 more)`."""
+    anys = pred.disjunctions() if pred else []
+    return "".join(f", where=({a})" for a in anys)
+
+
 class ScanExec:
-    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- always hs_filter_scan_where
-    with the filter's comparisons as its predicates."""
+    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_where with
+    the filter's comparisons as its predicates, or hs_filter_scan_any when the filter has disjunction terms (isin, |)."""
 
     def __init__(self, session, lin: Linear, cand: Optional[Candidate]):
         self.session, self.lin, self.cand = session, lin, cand
 
     def describe(self) -> str:
         if self.cand is None:
-            return f"GpuSourceScan(files={len(self.lin.relation.files)}, predicate={self.lin.predicate})"
+            return f"GpuSourceScan(files={len(self.lin.relation.files)}, predicate={self.lin.predicate}{_terms_text(self.lin.predicate)})"
         e = self.cand.entry
         extra = ""
         if self.cand.appended or self.cand.deleted_ids:
             extra = f", hybridScan(appended={len(self.cand.appended)}, deletedIds={self.cand.deleted_ids})"
-        return f"GpuIndexScan(Hyperspace(Type: CI, Name: {e.name}, LogVersion: {e.id}), files={len(e.index_files)}{extra})"
+        return (f"GpuIndexScan(Hyperspace(Type: CI, Name: {e.name}, LogVersion: {e.id}), files={len(e.index_files)}{extra}"
+                f"{_terms_text(self.lin.predicate)})")
 
-    def _scan(self, files, key, out_cols, sorted_on_key, deleted_ids=()):
+    def _scan(self, files, key, out_cols, sorted_on_key, deleted_ids=(), buckets=None, num_buckets=0):
         preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
-        batch, _ = self.session.gpu.filter_scan_where(files, key, out_cols, preds, sorted_on_key=sorted_on_key,
-                                                      deleted_file_ids=list(deleted_ids))
+        terms = [a.as_native() for a in self.lin.predicate.disjunctions()] if self.lin.predicate else []
+        if terms:  # file_buckets only where the files are bucketed on the key alone
+            batch, _ = self.session.gpu.filter_scan_any(files, key, out_cols, preds, terms, sorted_on_key=sorted_on_key,
+                                                        deleted_file_ids=list(deleted_ids), file_buckets=buckets,
+                                                        num_buckets=num_buckets)
+        else:
+            batch, _ = self.session.gpu.filter_scan_where(files, key, out_cols, preds, sorted_on_key=sorted_on_key,
+                                                          deleted_file_ids=list(deleted_ids))
         types = dict(self.lin.relation.schema)
         out = {n: spark_values(_host_column(d), types.get(n)) for n, d, _ in batch.columns}
         batch.free()
@@ -218,10 +231,14 @@ class ScanExec:
         pred_cols = self.lin.predicate.columns if self.lin.predicate else []
         key = next((c for c in pred_cols if c.lower() == first.lower()), first)
         parts = []
+        # a point lookup on the key of a single-column index reads only the files of the points' buckets
+        terms = self.lin.predicate.disjunctions() if self.lin.predicate else []
+        buckets = [bucket_id_of(f) for f in e.index_files] if terms and len(e.indexedColumns) == 1 else None
+        nb = e.numBuckets if buckets is not None else 0
         if self.cand.deleted_ids:  # NOT (_data_file_id IN deleted): CoveringIndexRuleUtils.scala:244-253
-            parts.append(self._scan(_file_images(e.index_files), key, out_cols, False, self.cand.deleted_ids))
+            parts.append(self._scan(_file_images(e.index_files), key, out_cols, False, self.cand.deleted_ids, buckets, nb))
         else:  # index files are sorted on the first indexed column: binary search when the filter bounds it
-            parts.append(self._scan(_file_images(e.index_files), key, out_cols, key in pred_cols))
+            parts.append(self._scan(_file_images(e.index_files), key, out_cols, key in pred_cols, (), buckets, nb))
         if self.cand.appended:     # appended source files are scanned raw and unioned: CoveringIndexRuleUtils.scala:191-212
             parts.append(self._scan(_file_images([f[0] for f in self.cand.appended]), None, out_cols, False))
         return _concat(parts, out_cols)
@@ -245,8 +262,8 @@ class BucketJoinExec:
             return f"Hyperspace(Type: CI, Name: {c.entry.name}, LogVersion: {c.entry.id})"
 
         keys = ", ".join(f"{l} = {r}" for l, r in (self.keys or self.condition or []))
-        filters = "".join(f", {n}Filter={lin.predicate.conjuncts()}" for n, lin in (("left", self.left), ("right", self.right))
-                          if lin.predicate)
+        filters = "".join(f", {n}Filter={lin.predicate.conjuncts()}{_terms_text(lin.predicate)}"
+                          for n, lin in (("left", self.left), ("right", self.right)) if lin.predicate)
         return f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, keys=[{keys}]{filters}, exchange=none)"
 
     def _side(self, lin: Linear, cand: Optional[Candidate], keys: List[str], nb: int):
@@ -283,8 +300,13 @@ class BucketJoinExec:
         try:
             lp = self.left.predicate.conjuncts() if self.left.predicate else []
             rp = self.right.predicate.conjuncts() if self.right.predicate else []
-            batch, _ = self.session.gpu.bucket_join_where(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                          lp, rp)
+            lt_, rt_ = ([a.as_native() for a in lin.predicate.disjunctions()] if lin.predicate else [] for lin in (self.left, self.right))
+            if lt_ or rt_:
+                batch, _ = self.session.gpu.bucket_join_any(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                            lp, rp, lt_, rt_)
+            else:
+                batch, _ = self.session.gpu.bucket_join_where(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                              lp, rp)
         finally:
             for t in lt + rt:
                 t.free()

@@ -96,12 +96,44 @@ _TERM_SIDES = {">=": ((False,), ()), ">": ((True,), ()), "<=": ((), (False,)), "
 
 
 @dataclass
+class AnyTerm:
+    """A disjunction on one column (Spark's In / InSet, or an Or of comparisons on that column): the value equals one of
+    ``values`` (a list, or a numpy array) or lies in one of ``ranges``, each ``(lo, lo_strict, hi, hi_strict)`` with None
+    for an open side."""
+    column: str
+    values: object = field(default_factory=list)
+    ranges: List[Tuple[object, bool, object, bool]] = field(default_factory=list)
+
+    def __str__(self) -> str:
+        vals = self.values.tolist() if isinstance(self.values, np.ndarray) else list(self.values)
+        shown = ", ".join(repr(v) for v in vals[:3]) + (f", ... {len(vals) - 3} more" if len(vals) > 3 else "")
+        parts = [f"{self.column} IN ({shown})"] if vals or not self.ranges else []
+        for lo, ls, hi, hs in self.ranges:
+            side = [f"{self.column} {'>' if ls else '>='} {lo!r}"] if lo is not None else []
+            side += [f"{self.column} {'<' if hs else '<='} {hi!r}"] if hi is not None else []
+            parts.append(" AND ".join(side))
+        return " OR ".join(f"({p})" if " AND " in p and len(parts) > 1 else p for p in parts)
+
+    def as_native(self) -> Tuple[str, object, List[tuple]]:
+        """(column, values, ranges) for Context.filter_scan_any / bucket_join_any."""
+        return self.column, self.values, list(self.ranges)
+
+
+def _merge_values(a, b):
+    if isinstance(a, np.ndarray) and isinstance(b, np.ndarray) and a.dtype.kind == b.dtype.kind:
+        return np.concatenate([a, b])
+    return (a.tolist() if isinstance(a, np.ndarray) else list(a)) + (b.tolist() if isinstance(b, np.ndarray) else list(b))
+
+
+@dataclass
 class Predicate:
     """Conjunction of comparisons with literals.  ``bounds`` is the inclusive integer (or byte-string) range per column, which
     the plan layer uses to pick an index; ``terms`` are the comparisons as written -- (column, operator, literal) with the
-    operator one of >=, >, <=, <, == -- which the engine evaluates with Spark's type coercion."""
+    operator one of >=, >, <=, <, == -- which the engine evaluates with Spark's type coercion.  ``anys`` are AND-ed
+    disjunctions on one column each (``isin`` and ``|``)."""
     bounds: Dict[str, Tuple[Optional[int], Optional[int]]]
     terms: List[Tuple[str, str, object]] = field(default_factory=list)
+    anys: List[AnyTerm] = field(default_factory=list, repr=False)  # explain() shows them by their SQL form
 
     def __and__(self, other: "Predicate") -> "Predicate":
         out = dict(self.bounds)
@@ -111,7 +143,44 @@ class Predicate:
                 lo = l0 if lo is None else (lo if l0 is None else max(lo, l0))
                 hi = h0 if hi is None else (hi if h0 is None else min(hi, h0))
             out[c] = (lo, hi)
-        return Predicate(out, self._as_terms() + other._as_terms())
+        return Predicate(out, self._as_terms() + other._as_terms(), self.anys + other.anys)
+
+    def __or__(self, other: "Predicate") -> "Predicate":
+        """An Or of branches on one and the same column, each a comparison, a conjunction of comparisons that is one range
+        (at most one lower and one upper bound), or an isin / Or on that column; anything else raises."""
+        c = self._single_column()
+        if other._single_column().lower() != c.lower():
+            raise LE.HyperspaceException(f"an OR across columns ({c}, {other._single_column()}) is not handled by the GPU path")
+        merged = AnyTerm(c)
+        for branch in (self, other):
+            if branch.anys:
+                merged.values = _merge_values(merged.values, branch.anys[0].values)
+                merged.ranges += branch.anys[0].ranges
+            else:
+                merged.ranges.append(branch._one_range())
+        return Predicate({}, [], [merged])
+
+    def _single_column(self) -> str:
+        cols = {c.lower(): c for c in self.columns}
+        if len(cols) != 1 or len(self.anys) > 1 or (self.anys and self._as_terms()):
+            raise LE.HyperspaceException("an OR branch must compare one column, the same one in every branch")
+        return next(iter(cols.values()))
+
+    def _one_range(self) -> Tuple[object, bool, object, bool]:
+        lo = hi = None
+        lo_s = hi_s = False
+        for c, v_lo, ls, v_hi, hs in self.conjuncts():
+            if (v_lo is not None and lo is not None) or (v_hi is not None and hi is not None):
+                raise LE.HyperspaceException("an OR branch must be one range: at most one lower and one upper bound")
+            if v_lo is not None:
+                lo, lo_s = v_lo, ls
+            if v_hi is not None:
+                hi, hi_s = v_hi, hs
+        return lo, lo_s, hi, hi_s
+
+    def disjunctions(self) -> List[AnyTerm]:
+        """The AND-ed disjunction terms (isin, |), which conjuncts() does not list."""
+        return list(self.anys)
 
     def _as_terms(self) -> List[Tuple[str, str, object]]:
         """The comparisons; a Predicate built from bounds alone states them as inclusive bounds, so that a conjunction with
@@ -128,7 +197,7 @@ class Predicate:
 
     @property
     def columns(self) -> List[str]:
-        return list(self.bounds)
+        return list(self.bounds) + [a.column for a in self.anys if a.column not in self.bounds]
 
     def conjuncts(self) -> List[Tuple[str, object, bool, object, bool]]:
         """The comparisons as (column, lo, lo_strict, hi, hi_strict) ranges for Context.filter_scan_where (a Predicate
@@ -198,6 +267,20 @@ class Column:
         if not math.isfinite(n) or n != math.floor(n):
             return Predicate({self.name: (1, 0)}, [(self.name, "==", v)])  # an integer never equals a fraction: empty range
         return Predicate({self.name: (int(n), int(n))}, [(self.name, "==", v)])
+
+    def isin(self, *values) -> Predicate:
+        """PySpark's Column.isin: varargs, or one list / tuple / set / numpy array.  None is dropped (it never makes a row
+        qualify); ints, floats, Decimals, datetimes, str and bytes are accepted, and the list is cast as Spark casts it
+        (a float makes every value a double, Decimals share one scale).  Strings mixed with numbers raise."""
+        from ._native import any_values
+
+        vals = values[0] if len(values) == 1 and isinstance(values[0], (list, tuple, set, frozenset, np.ndarray)) else values
+        vals = vals if isinstance(vals, np.ndarray) else [v for v in vals if v is not None]
+        try:
+            any_values(vals)
+        except ValueError as e:
+            raise LE.HyperspaceException(f"isin on '{self.name}': {e}") from None
+        return Predicate({}, [], [AnyTerm(self.name, vals)])
 
     def between(self, lo, hi):
         terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
@@ -342,7 +425,8 @@ class DataFrame:
 
     def filter(self, predicate: Predicate) -> "DataFrame":
         resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
-                             [(self._resolve(c), op, v) for c, op, v in predicate.terms])
+                             [(self._resolve(c), op, v) for c, op, v in predicate.terms],
+                             [AnyTerm(self._resolve(a.column), a.values, list(a.ranges)) for a in predicate.anys])
         return DataFrame(self.session, FilterNode(self.plan, resolved))
 
     where = filter

@@ -281,6 +281,44 @@ typedef struct {
 int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
                          hs_stats* stats, char* err, size_t errlen);
 
+/* A disjunction on one column -- Spark's In / InSet, and an Or whose branches all compare the same column: the row
+ * qualifies when its value equals one of the n_values listed values or lies inside one of the n_ranges ranges.  Every `=`
+ * and every range is evaluated as the hs_predicate of the same literal would be (the wider type decides, decimals compare
+ * exactly, NaN equals NaN, -0.0 equals 0.0): this is Spark's In, which compares with the type's ordering (Spark 3.1's InSet,
+ * used above 10 values, treats NaN and -0.0 differently in its interpreted and generated forms; this follows In).  A null
+ * row never qualifies; a NULL inside the list never makes a row qualify, so the caller drops it.  n_values == 0 with no
+ * ranges selects nothing.  The values are columnar, by literal_type: HS_TYPE_INT64 / HS_TYPE_DECIMAL (unscaled, with
+ * `scale`) in values_i, HS_TYPE_DOUBLE in values_f, HS_TYPE_STRING as values_bytes[values_offsets[k] ..
+ * values_offsets[k+1]) (n_values + 1 ascending offsets, each value at most 65535 bytes).  ranges[r].column is NULL or
+ * `column`.  At most 2^24 values plus ranges per term (HS_EUNSUPPORTED above); string values on a numeric column, numeric
+ * values on a string column, double values on decimal and timestamp columns: HS_EUNSUPPORTED.  A NULL array with a nonzero
+ * count, or descending offsets: HS_EINVAL. */
+typedef struct {
+  const char* column;
+  int32_t literal_type;        /* of the listed values: HS_TYPE_INT64 / HS_TYPE_DOUBLE / HS_TYPE_STRING / HS_TYPE_DECIMAL */
+  int32_t scale;               /* HS_TYPE_DECIMAL */
+  int64_t n_values;
+  const int64_t* values_i;     /* INT64, DECIMAL (unscaled) */
+  const double* values_f;      /* DOUBLE */
+  const void* values_bytes;    /* STRING: value k = values_bytes[values_offsets[k] .. values_offsets[k+1]) */
+  const uint64_t* values_offsets;
+  const hs_predicate* ranges;  /* hs_predicate semantics; column NULL or == column */
+  int32_t n_ranges;
+  int32_t reserved;
+} hs_predicate_any;
+
+/* hs_filter_scan_where with disjunction terms AND-ed to the predicates (n_preds + n_anys <= 16).  On sorted files a term on
+ * key_column becomes many windows per file, one per disjoint range of its values; terms on other columns (and every term
+ * on unsorted files) are evaluated per row.  file_buckets / num_buckets (optional: NULL / 0) give each file's bucket and
+ * assert that the files are bucketed on key_column alone (Spark's bucket hash, as hs_create_index writes them): when the
+ * key's windows are points only (listed values, ranges with lo == hi, equalities in preds) and the key is int32, int64,
+ * string, timestamp or decimal, only the files of the points' buckets are opened, each point is searched only in the files
+ * of its own bucket, and stats count only those files.  The rows are the same, in the same order (file, then row), as
+ * without file_buckets.  Without terms and buckets this is hs_filter_scan_where. */
+int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                       const hs_predicate_any* anys, int32_t n_anys, const int32_t* file_buckets, int32_t num_buckets,
+                       hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
 typedef struct {
   const hs_source_file* left_files;  /* index files of the left side, any order; bucket id parsed from the name */
   int32_t n_left;
@@ -321,6 +359,14 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                          int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate* right_preds,
                          int32_t n_right_preds, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
+/* hs_bucket_join_where with hs_predicate_any terms AND-ed to each side's predicates (n_preds + n_anys <= 16 per side),
+ * evaluated per row in the side selection.  No bucket pruning on join sides. */
+int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
+                       int32_t n_left_anys, const hs_predicate* right_preds, int32_t n_right_preds,
+                       const hs_predicate_any* right_anys, int32_t n_right_anys, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen);
 
 int64_t hs_batch_num_rows(const hs_batch* b);
 int32_t hs_batch_on_device(const hs_batch* b); /* != 0: the column pointers are device pointers (output = HS_OUT_DEVICE) */
