@@ -121,7 +121,7 @@ EXPORTED_SYMBOLS = [
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
-    "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any",
+    "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -236,6 +236,8 @@ def load_library() -> C.CDLL:
     L.hs_k_snappy_decompress.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_int32), *err]
     L.hs_k_inflate.restype = C.c_int
     L.hs_k_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
+    L.hs_k_lz4.restype = C.c_int
+    L.hs_k_lz4.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
     if L.hs_abi_version() != 1:
         raise HyperspaceGpuError(HS_EINVAL, f"ABI version mismatch: library {L.hs_abi_version()}, binding 1")
     _lib = L
@@ -814,6 +816,14 @@ class Context:
         out = C.create_string_buffer(max(1, uncompressed_len))
         err = C.create_string_buffer(1024)
         _check(load_library().hs_k_inflate(self._h, stream, len(stream), out, uncompressed_len, err, len(err)), err)
+        return out.raw[:uncompressed_len]
+
+    def k_lz4(self, stream: bytes, uncompressed_len: int, codec: int = 7) -> bytes:
+        """The LZ4 page decompressor on one page body of `uncompressed_len` bytes: codec 7 (LZ4_RAW, one block) or 5 (LZ4:
+        Hadoop-framed blocks, or one raw block)."""
+        out = C.create_string_buffer(max(1, uncompressed_len))
+        err = C.create_string_buffer(1024)
+        _check(load_library().hs_k_lz4(self._h, codec, stream, len(stream), out, uncompressed_len, err, len(err)), err)
         return out.raw[:uncompressed_len]
 
     # ---- read side ----------------------------------------------------------------------------------

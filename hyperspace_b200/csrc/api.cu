@@ -15,6 +15,7 @@
 #include "device_utils.cuh"
 #include "engine.h"
 #include "inflate.h"
+#include "lz4_block.h"
 #include "spark_types.h"
 
 using namespace hs;
@@ -2080,6 +2081,25 @@ int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_
     copy_d2h(ctx, &error, d_error.get(), 4);
     sync_stream(ctx);
     if (error) fail(HS_EFORMAT, "corrupt gzip stream: %s (check %u)", gz::inflate_error_text(error & 0xffffffu), error & 0xffffffu);
+    if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
+  });
+}
+
+int hs_k_lz4(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out_buf, uint64_t out_len, char* err, size_t errlen) {
+  if (!ctx || (codec != pq::LZ4 && codec != pq::LZ4_RAW) || (n && !in) || n > 0xffffffffull || out_len > 0xfffffff0ull ||
+      (out_len && !out_buf))
+    return HS_EINVAL;
+  return guarded(ctx, err, errlen, [&] {
+    Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
+    if (n) copy_h2d(ctx, d_in.get(), in, n);
+    Buf<uint32_t> d_error(ctx, 1);
+    fill_bytes(ctx, d_error.get(), 0, 4);
+    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)codec}};
+    decompress_blobs(ctx, blob, d_out.get(), d_error.get());
+    uint32_t error = 0;
+    copy_d2h(ctx, &error, d_error.get(), 4);
+    sync_stream(ctx);
+    if (error) fail(HS_EFORMAT, "corrupt lz4 block: %s (check %u)", lz4::lz4_error_text(error & 0xffffffu), error & 0xffffffu);
     if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
   });
 }

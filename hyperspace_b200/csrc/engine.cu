@@ -17,6 +17,7 @@
 #include "device_utils.cuh"
 #include "engine.h"
 #include "inflate.h"
+#include "lz4_block.h"
 #include "spark_types.h"
 
 namespace hs {
@@ -62,6 +63,7 @@ const char* decode_error_text(uint32_t code) {
     case DERR_SPARK_RANGE: return "timestamp that Spark 3.1 does not read (an INT96 value before 1900-01-01T00:00:00Z, or millis beyond the int64 micros range)";
     case DERR_DECIMAL_WIDTH: return "decimal value wider than its precision allows";
     case DERR_GZIP: return "corrupt gzip stream";
+    case DERR_LZ4: return "corrupt lz4 block";
   }
   return "unknown decode error";
 }
@@ -438,8 +440,10 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
       if (rg.num_rows == 0) continue;  // writers emit an empty row group for an empty table
       for (int c = 0; c < ncols; c++) {
         const pq::ColumnChunkMeta& cm = rg.columns[idx[c]];
-        if (cm.codec != pq::UNCOMPRESSED && cm.codec != pq::SNAPPY && cm.codec != pq::GZIP)
-          fail(HS_EUNSUPPORTED, "%s: column '%s' uses compression codec %d; the GPU path reads UNCOMPRESSED, SNAPPY and GZIP pages",
+        if (cm.codec != pq::UNCOMPRESSED && cm.codec != pq::SNAPPY && cm.codec != pq::GZIP && cm.codec != pq::LZ4 &&
+            cm.codec != pq::LZ4_RAW)
+          fail(HS_EUNSUPPORTED,
+               "%s: column '%s' uses compression codec %d; the GPU path reads UNCOMPRESSED, SNAPPY, GZIP, LZ4 and LZ4_RAW pages",
                what, columns[c].c_str(), cm.codec);
         any_compressed = any_compressed || cm.codec != pq::UNCOMPRESSED;
         if (cm.num_values != rg.num_rows)
@@ -779,6 +783,7 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
                           ? HS_EUNSUPPORTED
                           : HS_EFORMAT;
     if (code == DERR_GZIP) fail(ecode, "Parquet decode failed: %s: %s", decode_error_text(code), gz::inflate_error_text(detail));
+    if (code == DERR_LZ4) fail(ecode, "Parquet decode failed: %s: %s", decode_error_text(code), lz4::lz4_error_text(detail));
     if ((code == DERR_SPARK_RANGE || code == DERR_DECIMAL_WIDTH) && detail < (uint32_t)ncols)
       fail(ecode, "Parquet decode failed: column '%s' holds a %s", columns[detail].c_str(), decode_error_text(code));
     fail(ecode, "Parquet decode failed: %s (detail %u)", decode_error_text(code), detail);

@@ -26,7 +26,7 @@ struct ChunkDesc {          // one per (file, row group, projected column)
   int32_t phys_type;        // pq::PhysType
   int32_t max_def;          // 0 (required) or 1 (optional)
   int32_t file_index;
-  int32_t codec;            // pq::Codec of the chunk (UNCOMPRESSED, SNAPPY or GZIP)
+  int32_t codec;            // pq::Codec of the chunk (UNCOMPRESSED, SNAPPY, GZIP, LZ4 or LZ4_RAW)
   int32_t conv;             // ValueConv
   int32_t type_length;      // FIXED_LEN_BYTE_ARRAY: bytes per value
   int32_t pad;
@@ -94,7 +94,8 @@ enum DecodeError : uint32_t {
   DERR_OVERRUN = 5, DERR_DICT_INDEX = 6, DERR_UNSUPPORTED_TYPE = 7, DERR_SNAPPY = 8, DERR_STRING_TOO_LONG = 9,
   DERR_SPARK_RANGE = 10,    // a timestamp Spark 3.1 refuses to read: INT96 before 1900, MILLIS beyond int64 micros (detail: column)
   DERR_DECIMAL_WIDTH = 11,  // a decimal value wider than its precision's int32 / int64 (detail: column)
-  DERR_GZIP = 12            // a GZIP page body fails a check of inflate.h (detail: gz::InflateError)
+  DERR_GZIP = 12,           // a GZIP page body fails a check of inflate.h (detail: gz::InflateError)
+  DERR_LZ4 = 13             // an LZ4 / LZ4_RAW page body fails a check of lz4_block.h (detail: lz4::Lz4Error)
 };
 // BYTE_ARRAY dictionary pages -> tables of string references (device_utils.cuh: string_ref): one job per dictionary page,
 // walked by one thread (the entries are length-prefixed, so their positions are only found sequentially)
@@ -105,10 +106,10 @@ struct StringDictJob {
 };
 void launch_build_string_dicts(hs_ctx* ctx, const StringDictJob* jobs, int64_t n, uint32_t* d_error);
 
-// ---- compressed pages (page_codec.cu; the kernels of each codec: snappy.cu, inflate.cu) --------------------------------
+// ---- compressed pages (page_codec.cu; the kernels of each codec: snappy.cu, inflate.cu, lz4.cu) -----------------------
 // Decompresses every compressed data page and dictionary page of `pages` (host copy of d_pages) into *scratch, repoints
 // the descriptors at the decompressed bytes and uploads them to d_pages.  A dictionary page shared by several data pages
-// is decompressed once.  A failed check sets d_error (DERR_SNAPPY / DERR_GZIP).  Synchronises the stream once.
+// is decompressed once.  A failed check sets d_error (DERR_SNAPPY / DERR_GZIP / DERR_LZ4).  Synchronises the stream once.
 void decompress_pages(hs_ctx* ctx, std::vector<PageDesc>& pages, PageDesc* d_pages, Buf<uint8_t>* scratch, uint32_t* d_error);
 // one per compressed page (or dictionary page) of a call: where it lies, where its decompressed copy goes
 struct PageBlob {
@@ -119,7 +120,7 @@ struct PageBlob {
   uint32_t prefix;      // leading bytes copied verbatim (v2 level bytes)
   uint32_t compressed;  // 0: copy, 1: compressed with `codec`
   uint32_t first_block; // filled by decompress_blobs (snappy: the page's first 64 KB output block in the block table)
-  uint32_t codec;       // pq::Codec of the page's chunk: SNAPPY or GZIP
+  uint32_t codec;       // pq::Codec of the page's chunk: SNAPPY, GZIP, LZ4 or LZ4_RAW
 };
 // Decompresses the blobs into `scratch`: chooses and launches the kernels of each codec (the blobs are reordered by
 // codec).  sequential (optional, host): per blob in its new order, 1 where a snappy stream was decoded front to back.

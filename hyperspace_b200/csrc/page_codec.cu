@@ -1,8 +1,8 @@
 // page_codec.cu -- page compression behind one entry point each way: decompress_pages for the readers (under it
 // decompress_blobs, which the kernel tests reach too) and compress_bodies for the encoder.  The callers say which bytes
 // are compressed and where the result goes; what a codec's kernels need besides that -- how the work is cut up, their
-// scratch tables, which of them run -- is decided here.  The kernels are in snappy.cu (SNAPPY, both ways) and inflate.cu
-// (GZIP).
+// scratch tables, which of them run -- is decided here.  The kernels are in snappy.cu (SNAPPY, both ways), inflate.cu
+// (GZIP) and lz4.cu (LZ4 and LZ4_RAW).
 #include <algorithm>
 #include <map>
 #include <set>
@@ -14,10 +14,14 @@ namespace hs {
 
 void decompress_blobs(hs_ctx* ctx, std::vector<PageBlob>& blobs, uint8_t* scratch, uint32_t* d_error,
                       std::vector<uint32_t>* sequential) {
-  // each codec's kernels run over its own blobs: the snappy ones first, in page order, then the GZIP ones
+  // each codec's kernels run over its own blobs: the snappy ones first, in page order, then the GZIP ones, then the LZ4
+  // ones of both framings
   const size_t n_snappy = (size_t)(std::stable_partition(blobs.begin(), blobs.end(),
                                                          [](const PageBlob& b) { return b.codec == pq::SNAPPY; }) -
                                    blobs.begin());
+  const size_t n_gzip = (size_t)(std::stable_partition(blobs.begin() + n_snappy, blobs.end(),
+                                                       [](const PageBlob& b) { return b.codec == pq::GZIP; }) -
+                                 blobs.begin()) - n_snappy;
   uint64_t total_blocks = 0;  // 64 KB output blocks, the unit of the snappy decoder's parallelism
   bool any_verbatim = false;
   for (size_t i = 0; i < n_snappy; i++) {
@@ -32,7 +36,8 @@ void decompress_blobs(hs_ctx* ctx, std::vector<PageBlob>& blobs, uint8_t* scratc
   copy_h2d(ctx, d_blobs.get(), blobs.data(), sizeof(PageBlob) * blobs.size());
   launch_snappy_decompress(ctx, d_blobs.get(), (int64_t)n_snappy, (int64_t)total_blocks, any_verbatim, d_block_in.get(),
                            d_sequential.get(), scratch, d_error);
-  launch_inflate(ctx, d_blobs.get() + n_snappy, (int64_t)(blobs.size() - n_snappy), scratch, d_error);
+  launch_inflate(ctx, d_blobs.get() + n_snappy, (int64_t)n_gzip, scratch, d_error);
+  launch_lz4(ctx, d_blobs.get() + n_snappy + n_gzip, (int64_t)(blobs.size() - n_snappy - n_gzip), scratch, d_error);
   if (sequential) {
     sequential->assign(blobs.size(), 0u);
     copy_d2h(ctx, sequential->data(), d_sequential.get(), sizeof(uint32_t) * n_snappy);

@@ -1,5 +1,5 @@
-// page_codec_kernels.h -- what page_codec.cu and the codec kernel files (snappy.cu, inflate.cu) share.  Private to those
-// three translation units: everyone else goes through decompress_pages / decompress_blobs / compress_bodies (kernels.h).
+// page_codec_kernels.h -- what page_codec.cu and the codec kernel files (snappy.cu, inflate.cu, lz4.cu) share.  Private to
+// those four translation units: everyone else goes through decompress_pages / decompress_blobs / compress_bodies (kernels.h).
 #pragma once
 #include "kernels.h"
 
@@ -19,6 +19,10 @@ void launch_snappy_decompress(hs_ctx* ctx, const PageBlob* blobs, int64_t n, int
 // GZIP page bodies, one warp per blob: copies what is stored verbatim (prefix, or the whole page when !compressed) and
 // inflates the rest; a failed check sets (DERR_GZIP << 24 | gz::InflateError) in d_error
 void launch_inflate(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch, uint32_t* d_error);
+
+// LZ4 (codec 5, Hadoop-framed) and LZ4_RAW (codec 7) page bodies, one warp per blob: copies what is stored verbatim and
+// decodes the rest; a failed check sets (DERR_LZ4 << 24 | lz4::Lz4Error) in d_error
+void launch_lz4(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch, uint32_t* d_error);
 
 // compression of page bodies: one warp per fragment (<= 65536 bytes) of a page; fragment f of raw bytes [src_off, src_off +
 // len) is written to scratch at dst_off (room for 32 + len + len / 6 bytes), its compressed length to out_len[f]

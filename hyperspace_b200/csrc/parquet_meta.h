@@ -17,7 +17,7 @@ namespace pq {
 enum PhysType : int32_t { BOOLEAN = 0, INT32 = 1, INT64 = 2, INT96 = 3, FLOAT = 4, DOUBLE = 5, BYTE_ARRAY = 6, FIXED_LEN_BYTE_ARRAY = 7 };
 enum Repetition : int32_t { REQUIRED = 0, OPTIONAL = 1, REPEATED = 2 };
 enum Encoding : int32_t { ENC_PLAIN = 0, ENC_PLAIN_DICTIONARY = 2, ENC_RLE = 3, ENC_BIT_PACKED = 4, ENC_RLE_DICTIONARY = 8 };
-enum Codec : int32_t { UNCOMPRESSED = 0, SNAPPY = 1, GZIP = 2 };
+enum Codec : int32_t { UNCOMPRESSED = 0, SNAPPY = 1, GZIP = 2, LZ4 = 5, LZ4_RAW = 7 };
 enum PageType : int32_t { DATA_PAGE = 0, INDEX_PAGE = 1, DICTIONARY_PAGE = 2, DATA_PAGE_V2 = 3 };
 
 struct SchemaColumn {

@@ -449,6 +449,10 @@ int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out, u
  * length is out_len.  HS_EFORMAT for a damaged stream; the message names the failed check.  Kernel-level entry point for
  * the parity tests. */
 int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t out_len, char* err, size_t errlen);
+/* The LZ4 page decompressor (k_lz4) on one page body of n bytes whose uncompressed length is out_len: codec 7 (LZ4_RAW,
+ * one block) or 5 (LZ4: Hadoop-framed blocks, or one raw block); any other codec is HS_EINVAL.  HS_EFORMAT for a damaged
+ * body; the message names the failed check.  Kernel-level entry point for the parity tests. */
+int hs_k_lz4(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out, uint64_t out_len, char* err, size_t errlen);
 
 #ifdef __cplusplus
 }
