@@ -24,7 +24,7 @@ HS_TYPE_INT32, HS_TYPE_INT64, HS_TYPE_FLOAT, HS_TYPE_DOUBLE, HS_TYPE_BOOL, HS_TY
 HS_TYPE_DECIMAL = 6  # predicate literals only: unscaled value in lo_i / hi_i, scale in `scale`
 HS_SAVE_OVERWRITE, HS_SAVE_APPEND = 0, 1
 HS_OUT_FILES, HS_OUT_HOST, HS_OUT_DEVICE = 0, 1, 2
-HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY = 0, 1
+HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
                HS_TYPE_BOOL: np.uint8}
@@ -121,7 +121,7 @@ EXPORTED_SYMBOLS = [
     "hs_stage_sources", "hs_staged_num_files", "hs_staged_file", "hs_staged_wait", "hs_staged_free",
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
-    "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4",
+    "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -238,6 +238,8 @@ def load_library() -> C.CDLL:
     L.hs_k_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
     L.hs_k_lz4.restype = C.c_int
     L.hs_k_lz4.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
+    L.hs_k_compress.restype = C.c_int
+    L.hs_k_compress.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), *err]
     if L.hs_abi_version() != 1:
         raise HyperspaceGpuError(HS_EINVAL, f"ABI version mismatch: library {L.hs_abi_version()}, binding 1")
     _lib = L
@@ -825,6 +827,16 @@ class Context:
         err = C.create_string_buffer(1024)
         _check(load_library().hs_k_lz4(self._h, codec, stream, len(stream), out, uncompressed_len, err, len(err)), err)
         return out.raw[:uncompressed_len]
+
+    def k_compress(self, data: bytes, codec: int) -> bytes:
+        """The index page compressor on one page body: HS_CODEC_GZIP (one gzip member) or HS_CODEC_LZ4 (Hadoop-framed
+        blocks, one group per 64 KB)."""
+        cap = 64 + len(data) + len(data) // 64 + 64 * (len(data) // 65536 + 1)
+        out = C.create_string_buffer(cap)
+        n = C.c_uint64(0)
+        err = C.create_string_buffer(1024)
+        _check(load_library().hs_k_compress(self._h, codec, data, len(data), out, cap, C.byref(n), err, len(err)), err)
+        return out.raw[:n.value]
 
     # ---- read side ----------------------------------------------------------------------------------
     def filter_scan(self, files: Sequence[FileImage], key: str, projected: Sequence[str], lo=None, hi=None, sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (),

@@ -55,6 +55,23 @@ int guarded(hs_ctx* ctx, char* err, size_t errlen, F&& f) {
   }
 }
 
+// hs_index_spec.compression -> the codec of the index pages: those Spark 3.1 writes and this engine reads back
+int output_codec(int32_t compression) {
+  switch (compression) {
+    case HS_CODEC_UNCOMPRESSED: return pq::UNCOMPRESSED;
+    case HS_CODEC_SNAPPY: return pq::SNAPPY;
+    case HS_CODEC_GZIP: return pq::GZIP;
+    case HS_CODEC_LZ4: return pq::LZ4;
+    default:
+      fail(HS_EUNSUPPORTED, "compression codec %d; the GPU path writes UNCOMPRESSED (0), SNAPPY (1), GZIP (2) and LZ4 (5) pages",
+           compression);
+  }
+}
+// the file-name extension of parquet-mr's CompressionCodecName
+const char* codec_extension(int codec) {
+  return codec == pq::SNAPPY ? ".snappy" : codec == pq::GZIP ? ".gz" : codec == pq::LZ4 ? ".lz4" : "";
+}
+
 void write_file_atomic(const std::string& dir, const std::string& name, const uint8_t* data, uint64_t size) {
   const std::string tmp = dir + "/." + name + ".tmp";
   const std::string fin = dir + "/" + name;
@@ -609,16 +626,14 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
       req.rows_per_page = spec->rows_per_page;
       req.rows_per_row_group = spec->rows_per_row_group;
       req.use_dictionary = spec->disable_dictionary == 0;
-      if (spec->compression != HS_CODEC_UNCOMPRESSED && spec->compression != HS_CODEC_SNAPPY)
-        fail(HS_EUNSUPPORTED, "compression codec %d; the GPU path writes UNCOMPRESSED and SNAPPY pages", spec->compression);
-      req.codec = spec->compression == HS_CODEC_SNAPPY ? pq::SNAPPY : pq::UNCOMPRESSED;
+      req.codec = output_codec(spec->compression);
       const std::string uuid = spec->job_uuid ? spec->job_uuid : make_uuid();
       req.seg_names.resize(spec->num_buckets);
       for (int b = 0; b < spec->num_buckets; b++) {
         // Spark FileFormatWriter: part-<task>-<jobUUID>_<bucket>.c000<codec ext>.parquet ; bucket id parsed back by
         // BucketingUtils.getBucketId (relied on by actions/OptimizeAction.scala:110)
         char nm[160];
-        snprintf(nm, sizeof nm, "part-%05d-%s_%05d.c000%s.parquet", b, uuid.c_str(), b, req.codec == pq::SNAPPY ? ".snappy" : "");
+        snprintf(nm, sizeof nm, "part-%05d-%s_%05d.c000%s.parquet", b, uuid.c_str(), b, codec_extension(req.codec));
         req.seg_names[b] = nm;
       }
       // The files are laid out before the sort when their layout does not depend on the sorted order: a local sort of a
@@ -2026,14 +2041,15 @@ int hs_synth_table(hs_ctx* ctx, int64_t first_row, int64_t nrows, int32_t ncols,
                            err, errlen);
 }
 
-int hs_k_snappy_compress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t cap, uint64_t* out_len, char* err,
-                         size_t errlen) {
-  if (!ctx || !out_len || (n && !in)) return HS_EINVAL;
+namespace {
+// one page body through compress_bodies, as the encoder compresses it: preamble, pieces, trailer
+int compress_one_body(hs_ctx* ctx, int codec, const void* in, uint64_t n, void* out_buf, uint64_t cap, uint64_t* out_len,
+                      char* err, size_t errlen) {
   return guarded(ctx, err, errlen, [&] {
     Buf<uint8_t> d_in(ctx, std::max<uint64_t>(n, 16) + 16);
     if (n) copy_h2d(ctx, d_in.get(), in, n);
     CompressedBodies packed;
-    compress_bodies(ctx, d_in.get(), {{0, n}}, &packed);
+    compress_bodies(ctx, codec, d_in.get(), {{0, n}}, &packed);
     std::vector<uint8_t> stream;
     packed.append_preamble(0, stream);
     std::vector<BlobCopy> pieces;
@@ -2042,10 +2058,24 @@ int hs_k_snappy_compress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf,
     stream.resize(end);
     for (const BlobCopy& pc : pieces)
       HS_CUDA(cudaMemcpy(stream.data() + pc.dst, packed.slots.get() + pc.src, pc.len, cudaMemcpyDeviceToHost));
+    packed.append_trailer(0, stream);
     *out_len = stream.size();
     if (stream.size() > cap) fail(HS_ENOMEM, "output buffer too small: %zu bytes needed", stream.size());
     if (out_buf) memcpy(out_buf, stream.data(), stream.size());
   });
+}
+}  // namespace
+
+int hs_k_snappy_compress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t cap, uint64_t* out_len, char* err,
+                         size_t errlen) {
+  if (!ctx || !out_len || (n && !in)) return HS_EINVAL;
+  return compress_one_body(ctx, pq::SNAPPY, in, n, out_buf, cap, out_len, err, errlen);
+}
+
+int hs_k_compress(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out_buf, uint64_t cap, uint64_t* out_len,
+                  char* err, size_t errlen) {
+  if (!ctx || !out_len || (n && !in) || (codec != HS_CODEC_GZIP && codec != HS_CODEC_LZ4)) return HS_EINVAL;
+  return compress_one_body(ctx, codec, in, n, out_buf, cap, out_len, err, errlen);
 }
 
 int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t out_len, int32_t* sequential,

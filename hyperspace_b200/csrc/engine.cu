@@ -1259,7 +1259,7 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
   std::vector<StatPatch>& stat_patches = L.stat_patches;
   std::vector<uint8_t>& skeleton = L.skeleton;
   std::vector<ByteCopy>& copies = L.copies;
-  L.compress = req.codec == pq::SNAPPY;
+  L.compress = req.codec != pq::UNCOMPRESSED;
   const bool compress = L.compress;
   std::vector<PagePlan>& page_plans = L.page_plans;
   std::vector<FilePlan>& file_plans = L.file_plans;
@@ -1561,7 +1561,7 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
                              kDictCapacity, rec.get(), d_page_begin.get(), P, out->arena.get());
     }
   }
-  // ---- SNAPPY: the pages just written are compressed and the files laid out again ------------------------------------------
+  // ---- SNAPPY, GZIP, LZ4: the pages just written are compressed and the files laid out again -----------------------------
   // Compressed sizes are data: the files cannot be laid out before the pages exist.  So the uncompressed images above serve
   // as the compressor's input; the compressed sizes of the page bodies come back to the host, which lays the files out
   // again (new page headers, new footers, the codec in every chunk) and a copy kernel moves the compressed pieces into place.
@@ -1569,7 +1569,7 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
     std::vector<std::pair<uint64_t, uint64_t>> bodies;
     for (const PagePlan& pp : page_plans) bodies.emplace_back(pp.hdr_off + pp.hdr_len, pp.body_len);
     CompressedBodies packed;
-    compress_bodies(ctx, out->arena.get(), bodies, &packed);
+    compress_bodies(ctx, req.codec, out->arena.get(), bodies, &packed);
     // second layout
     std::vector<uint8_t> skel2;
     std::vector<ByteCopy> copies2;
@@ -1616,10 +1616,13 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
             packed.append_preamble(pi, skel2);
             emit2(b0);
             packed.place(pi, blobs, &cur2);
+            const size_t t0 = skel2.size();
+            packed.append_trailer(pi, skel2);
+            if (skel2.size() > t0) emit2(t0);
           }
           ch.total_size = (int64_t)(cur2 - chunk_begin);
           ch.total_uncompressed = uncomp;
-          ch.codec = pq::SNAPPY;
+          ch.codec = req.codec;
           rg_comp += ch.total_size;
           rg_uncomp += uncomp;
         }

@@ -174,7 +174,7 @@ struct EncodeRequest {
   int64_t rows_per_row_group = 0;
   std::vector<int64_t> seg_rows_per_row_group;  // optional per-segment override
   bool use_dictionary = true;                   // dictionary-encode columns whose distinct values fit (like parquet-mr)
-  int codec = 0;                                // pq::Codec of the written pages: UNCOMPRESSED or SNAPPY (Spark's default)
+  int codec = 0;                                // pq::Codec of the written pages: UNCOMPRESSED, SNAPPY, GZIP or LZ4
   DictProbe* probe = nullptr;                   // optional: first-stage dictionary probes already launched (consumed)
 };
 struct EncodedFiles {
@@ -187,7 +187,7 @@ void encode_segments(hs_ctx* ctx, const EncodeRequest& req, EncodedFiles* out, h
 // key into its pages.  layout_segments: the dictionary decisions, the host page plan and skeleton, the arena (out->arena,
 // out->files) and the upload of the page tables; it needs the bucket sizes and req.plan, and the sorted rows (req.d_perm)
 // only for a table where layout_needs_sorted_rows() holds (nullable or string columns: their page sizes depend on the
-// order).  write_segments: the kernels that fill the pages, footer statistics and SNAPPY; key_pages_written: the sort
+// order).  write_segments: the kernels that fill the pages, footer statistics and the page codec; key_pages_written: the sort
 // has stored column 0 already (to key_page_dest()).
 struct EncodeLayout {
   struct Impl;  // engine.cu

@@ -376,21 +376,25 @@ struct BlobCopy {
   uint32_t len, pad;
 };
 void launch_copy_blobs(hs_ctx* ctx, const BlobCopy* blobs, int64_t n, const uint8_t* src_base, uint8_t* dst_base);
-// Page bodies compressed with SNAPPY (page_codec.cu).  A body's compressed form is its preamble, which the host writes,
-// followed by its pieces, which lie in `slots` on the device.
+// Page bodies compressed with a page codec (page_codec.cu): SNAPPY, GZIP or LZ4 (Hadoop-framed).  A body's compressed form
+// is its preamble and its trailer, which the host writes (snappy's length varint; the gzip member's header, and its final
+// block, CRC-32 and ISIZE), around its pieces, which lie in `slots` on the device.
 struct CompressedBodies {
+  int codec = 0;                     // pq::Codec
   Buf<uint8_t> slots;
   std::vector<uint64_t> raw_len;     // per body: uncompressed bytes
+  std::vector<uint32_t> crc;         // GZIP, per body: CRC-32 of the uncompressed bytes
   std::vector<size_t> first_piece;   // per body (+1): its pieces
   std::vector<BlobCopy> pieces;      // src: offset in slots, len: compressed bytes
-  uint64_t size(size_t body) const;  // compressed bytes of the body: preamble + pieces
+  uint64_t size(size_t body) const;  // compressed bytes of the body: preamble + pieces + trailer
   void append_preamble(size_t body, std::vector<uint8_t>& out) const;
+  void append_trailer(size_t body, std::vector<uint8_t>& out) const;
   // appends the body's pieces to `copies` with consecutive destinations from *dst on; advances *dst
   void place(size_t body, std::vector<BlobCopy>& copies, uint64_t* dst) const;
 };
-// Compresses the bodies (offset, length) of `raw` (device), each on its own.  Synchronises the stream once: the
-// compressed sizes are data.
-void compress_bodies(hs_ctx* ctx, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
+// Compresses the bodies (offset, length) of `raw` (device), each on its own, with `codec` (pq::SNAPPY, GZIP or LZ4).
+// Synchronises the stream once: the compressed sizes are data.
+void compress_bodies(hs_ctx* ctx, int codec, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
                      CompressedBodies* out);
 // Synthetic table generator: rows [first_row, first_row+n) of column `col` (0..4) of table T (SURVEY.md section 8d)
 void launch_synth_column(hs_ctx* ctx, int col, int64_t first_row, int64_t n, void* out);

@@ -18,6 +18,7 @@
 // each chunk; a body that fails as groups is decoded again as one raw block, over whatever the attempt wrote.
 #include "device_utils.cuh"
 #include "lz4_block.h"
+#include "lz77.cuh"
 #include "page_codec_kernels.h"
 
 namespace hs {
@@ -150,6 +151,70 @@ void launch_lz4(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch,
   if (n == 0) return;
   KernelScope _ks(ctx, "k_lz4");
   k_lz4<<<(unsigned)ceil_div(n, kWarpsPerCta), kWarpsPerCta * 32, 0, ctx->stream>>>(blobs, n, scratch, d_error);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+}  // namespace hs
+
+// =====================================================================================================================
+// LZ4 compression of index pages (Spark 2.4-3.1's spark.sql.parquet.compression.codec=lz4: codec 5, Hadoop's Lz4Codec
+// framing), one warp per 64 KB fragment of a page body, four warps per CTA.  A fragment is parsed by lz77_parse (lz77.cuh)
+// under LZ4's end-of-block rules and becomes one block in a Hadoop group of one chunk -- what Arrow's Lz4HadoopCodec
+// requires, and far below the 256 KB buffer of Hadoop's BlockDecompressorStream.  A page body is its fragments' groups
+// back to back.
+// =====================================================================================================================
+namespace hs {
+namespace {
+
+constexpr int kCompWarps = 4;
+
+struct Lz4Emitter {
+  const uint8_t* __restrict__ in;
+  uint8_t* __restrict__ out;  // the block
+  uint32_t op;
+  unsigned lane;
+
+  __device__ __forceinline__ void literals(uint32_t from, uint32_t to) {
+    for (uint32_t j = lane; j < to - from; j += 32) out[op + j] = in[from + j];
+    op += to - from;
+  }
+  __device__ __forceinline__ void sequence(uint32_t lit, uint32_t q, uint32_t offset, uint32_t mlen) {
+    op = lz4::put_sequence_head(out, op, q - lit, mlen, lane == 0);
+    literals(lit, q);
+    op = lz4::put_match(out, op, offset, mlen, lane == 0);
+  }
+  __device__ __forceinline__ void finish(uint32_t lit, uint32_t len) {
+    op = lz4::put_sequence_head(out, op, len - lit, 0, lane == 0);
+    literals(lit, len);
+  }
+};
+
+__global__ void __launch_bounds__(kCompWarps * 32) k_lz4_compress(const PageFragment* __restrict__ frags, int64_t n,
+                                                                   const uint8_t* __restrict__ raw, uint8_t* __restrict__ scratch,
+                                                                   uint32_t* __restrict__ out_len) {
+  __shared__ uint32_t s_table[kCompWarps][kLz77Table];
+  const unsigned lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int64_t f = (int64_t)blockIdx.x * kCompWarps + wib;
+  if (f >= n) return;
+  const PageFragment fr = frags[f];
+  uint8_t* group = scratch + fr.dst_off;
+  Lz4Emitter emit{raw + fr.src_off, group + lz4::kHadoopGroupHeader, 0u, lane};
+  lz77_parse(raw + fr.src_off, fr.len, s_table[wib], lane,
+             Lz77Limits{0xffffu, 0xffffffffu, lz4::kMatchStartMargin, lz4::kLastLiterals}, emit);
+  if (lane == 0) {
+    lz4::put_be32(group, fr.len);
+    lz4::put_be32(group + 4, emit.op);
+    out_len[f] = lz4::kHadoopGroupHeader + emit.op;
+  }
+}
+
+}  // namespace
+
+void launch_lz4_compress(hs_ctx* ctx, const PageFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
+                         uint32_t* out_len) {
+  KernelScope _ks(ctx, "k_lz4_compress");
+  if (n == 0) return;
+  k_lz4_compress<<<(unsigned)ceil_div(n, kCompWarps), kCompWarps * 32, 0, ctx->stream>>>(frags, n, raw, scratch, out_len);
   HS_LAUNCH_CHECK(ctx);
 }
 

@@ -151,6 +151,49 @@ HS_HD uint32_t hadoop_next(const uint8_t* src, uint32_t n, uint32_t out, uint32_
   return HADOOP_CHUNK;
 }
 
+// ---- encoding (lz4.cu's compressor, and the host build of the tests) ---------------------------------------------------------
+// A block the compressor writes keeps the end-of-block rules without the decoder's short-sequence exceptions: no match
+// starts in the last kMatchStartMargin bytes of the block, and the last kLastLiterals bytes are literals of the final
+// sequence.
+constexpr uint32_t kMatchStartMargin = 12, kLastLiterals = 5;
+constexpr uint32_t kHadoopGroupHeader = 8;  // a group of one chunk: [BE u32 raw length][BE u32 compressed length][block]
+
+// the largest block of len bytes: literals only, one token and len / 255 + 1 length bytes
+HS_HD uint64_t block_bound(uint64_t len) { return len + len / 255 + 16; }
+
+HS_HD void put_be32(uint8_t* p, uint32_t v) {
+  p[0] = (uint8_t)(v >> 24);
+  p[1] = (uint8_t)(v >> 16);
+  p[2] = (uint8_t)(v >> 8);
+  p[3] = (uint8_t)v;
+}
+// 15 in a nibble, then bytes of 255 and the rest: the length fields of literals and matches
+HS_HD uint32_t put_length_bytes(uint8_t* out, uint32_t op, uint32_t v, bool write) {
+  for (; v >= 255; v -= 255) {
+    if (write) out[op] = 255;
+    op++;
+  }
+  if (write) out[op] = (uint8_t)v;
+  return op + 1;
+}
+// The token and literal-length bytes at out[op] of a sequence of lit_len literals and a match of match_len >= 4 bytes
+// (0: the block's last sequence, literals only).  Returns where its literals go.  Only the lane with `write` stores.
+HS_HD uint32_t put_sequence_head(uint8_t* out, uint32_t op, uint32_t lit_len, uint32_t match_len, bool write) {
+  const uint32_t ml = match_len ? match_len - 4 : 0;
+  if (write) out[op] = (uint8_t)((lit_len < 15 ? lit_len : 15) << 4 | (ml < 15 ? ml : 15));
+  op++;
+  return lit_len >= 15 ? put_length_bytes(out, op, lit_len - 15, write) : op;
+}
+// The offset and match-length bytes after the sequence's literals, at out[op]; returns the position after them.
+HS_HD uint32_t put_match(uint8_t* out, uint32_t op, uint32_t offset, uint32_t match_len, bool write) {
+  if (write) {
+    out[op] = (uint8_t)offset;
+    out[op + 1] = (uint8_t)(offset >> 8);
+  }
+  op += 2;
+  return match_len - 4 >= 15 ? put_length_bytes(out, op, match_len - 4 - 15, write) : op;
+}
+
 // ---- serial decoding (the host build of the tests) -------------------------------------------------------------------------
 // The block src[ip, n) into dst from `out` (its start) with capacity cap; out ends past the block's output.
 inline uint32_t decode_block_serial(const uint8_t* src, uint32_t ip, uint32_t n, uint8_t* dst, uint32_t& out, uint32_t cap) {

@@ -2,11 +2,13 @@
 // decompress_blobs, which the kernel tests reach too) and compress_bodies for the encoder.  The callers say which bytes
 // are compressed and where the result goes; what a codec's kernels need besides that -- how the work is cut up, their
 // scratch tables, which of them run -- is decided here.  The kernels are in snappy.cu (SNAPPY, both ways), inflate.cu
-// (GZIP) and lz4.cu (LZ4 and LZ4_RAW).
+// (GZIP, reading), deflate.cu (GZIP, writing) and lz4.cu (LZ4 and LZ4_RAW reading, LZ4 writing).
 #include <algorithm>
 #include <map>
 #include <set>
 
+#include "deflate.h"
+#include "lz4_block.h"
 #include "page_codec_kernels.h"
 #include "parquet_meta.h"
 
@@ -93,46 +95,86 @@ void decompress_pages(hs_ctx* ctx, std::vector<PageDesc>& pages, PageDesc* d_pag
   decompress_blobs(ctx, blobs, scratch->get(), d_error);
 }
 
-void compress_bodies(hs_ctx* ctx, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
+void compress_bodies(hs_ctx* ctx, int codec, const uint8_t* raw, const std::vector<std::pair<uint64_t, uint64_t>>& bodies,
                      CompressedBodies* out) {
-  // A body is cut into 64 KB fragments that compress in parallel, each into a slot of worst-case size.
-  std::vector<SnappyFragment> frags;
+  if (codec != pq::SNAPPY && codec != pq::GZIP && codec != pq::LZ4) fail(HS_EINVAL, "internal: no compressor for codec %d", codec);
+  // A body is cut into 64 KB fragments that compress in parallel, each into a slot of its codec's worst-case size.
+  auto slot_bytes = [codec](uint32_t len) -> uint64_t {
+    const uint64_t bound = codec == pq::SNAPPY ? snappy_max_compressed(len)
+                           : codec == pq::GZIP ? gz::deflate_fragment_bound(len) + 4
+                                               : lz4::kHadoopGroupHeader + lz4::block_bound(len);
+    return round_up(bound, 16);
+  };
+  std::vector<PageFragment> frags;
+  out->codec = codec;
   out->raw_len.clear();
   out->first_piece.clear();
   uint64_t slot_cursor = 0;
   for (const auto& body : bodies) {
     out->raw_len.push_back(body.second);
     out->first_piece.push_back(frags.size());
-    for (uint64_t o = 0; o < body.second; o += kSnappyFragment) {
-      const uint32_t len = (uint32_t)std::min<uint64_t>(kSnappyFragment, body.second - o);
-      frags.push_back(SnappyFragment{body.first + o, slot_cursor, len, 0});
-      slot_cursor += round_up(snappy_max_compressed(len), 16);
+    for (uint64_t o = 0; o < body.second; o += kCompressFragment) {
+      const uint32_t len = (uint32_t)std::min<uint64_t>(kCompressFragment, body.second - o);
+      frags.push_back(PageFragment{body.first + o, slot_cursor, len, 0});
+      slot_cursor += slot_bytes(len);
     }
   }
   out->first_piece.push_back(frags.size());
   out->slots.alloc(ctx, std::max<uint64_t>(slot_cursor, 16));
-  Buf<SnappyFragment> d_frags(ctx, std::max<size_t>(1, frags.size()));
-  Buf<uint32_t> d_flen(ctx, std::max<size_t>(1, frags.size()));
-  std::vector<uint32_t> flen(frags.size());
-  copy_h2d(ctx, d_frags.get(), frags.data(), sizeof(SnappyFragment) * frags.size());
-  launch_snappy_compress(ctx, d_frags.get(), (int64_t)frags.size(), raw, out->slots.get(), d_flen.get());
+  Buf<PageFragment> d_frags(ctx, std::max<size_t>(1, frags.size()));
+  Buf<uint32_t> d_flen(ctx, std::max<size_t>(1, frags.size())), d_fcrc(ctx, std::max<size_t>(1, frags.size()));
+  std::vector<uint32_t> flen(frags.size()), fcrc(frags.size());
+  copy_h2d(ctx, d_frags.get(), frags.data(), sizeof(PageFragment) * frags.size());
+  if (codec == pq::SNAPPY) {
+    launch_snappy_compress(ctx, d_frags.get(), (int64_t)frags.size(), raw, out->slots.get(), d_flen.get());
+  } else if (codec == pq::GZIP) {
+    launch_deflate_compress(ctx, d_frags.get(), (int64_t)frags.size(), raw, out->slots.get(), d_flen.get(), d_fcrc.get());
+    copy_d2h(ctx, fcrc.data(), d_fcrc.get(), 4 * frags.size());
+  } else {
+    launch_lz4_compress(ctx, d_frags.get(), (int64_t)frags.size(), raw, out->slots.get(), d_flen.get());
+  }
   copy_d2h(ctx, flen.data(), d_flen.get(), 4 * frags.size());
   sync_stream(ctx);
   out->pieces.resize(frags.size());
   for (size_t f = 0; f < frags.size(); f++) out->pieces[f] = BlobCopy{frags[f].dst_off, 0, flen[f], 0};
+  out->crc.assign(bodies.size(), 0u);
+  if (codec == pq::GZIP) {
+    // the member's CRC-32 from its fragments': each is shifted past the bytes after it (gz::crc32_piece's combination)
+    for (size_t b = 0; b < bodies.size(); b++) {
+      uint32_t x = 0;
+      for (size_t f = out->first_piece[b]; f < out->first_piece[b + 1]; f++) {
+        const uint64_t after = bodies[b].first + bodies[b].second - frags[f].src_off - frags[f].len;
+        x ^= gz::crc32_multmodp(gz::crc32_x8n(after), fcrc[f]);
+      }
+      out->crc[b] = x;
+    }
+  }
 }
 
-// snappy's preamble: the uncompressed length, as the varint Thrift writes too
+// snappy's preamble is the uncompressed length, as the varint Thrift writes too; the gzip member's is its header
 void CompressedBodies::append_preamble(size_t body, std::vector<uint8_t>& out) const {
-  thrift::Writer w;
-  w.varint(raw_len[body]);
-  out.insert(out.end(), w.buf.begin(), w.buf.end());
+  if (codec == pq::SNAPPY) {
+    thrift::Writer w;
+    w.varint(raw_len[body]);
+    out.insert(out.end(), w.buf.begin(), w.buf.end());
+  } else if (codec == pq::GZIP) {
+    out.insert(out.end(), std::begin(gz::kGzipHeader), std::end(gz::kGzipHeader));
+  }
+}
+
+// the gzip member's final block, CRC-32 and ISIZE
+void CompressedBodies::append_trailer(size_t body, std::vector<uint8_t>& out) const {
+  if (codec != pq::GZIP) return;
+  uint8_t t[10];
+  gz::gzip_trailer(crc[body], raw_len[body], t);
+  out.insert(out.end(), t, t + sizeof t);
 }
 
 uint64_t CompressedBodies::size(size_t body) const {
-  std::vector<uint8_t> preamble;
-  append_preamble(body, preamble);
-  uint64_t bytes = preamble.size();
+  std::vector<uint8_t> ends;
+  append_preamble(body, ends);
+  append_trailer(body, ends);
+  uint64_t bytes = ends.size();
   for (size_t f = first_piece[body]; f < first_piece[body + 1]; f++) bytes += pieces[f].len;
   return bytes;
 }

@@ -24,15 +24,23 @@ void launch_inflate(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scra
 // decodes the rest; a failed check sets (DERR_LZ4 << 24 | lz4::Lz4Error) in d_error
 void launch_lz4(hs_ctx* ctx, const PageBlob* blobs, int64_t n, uint8_t* scratch, uint32_t* d_error);
 
-// compression of page bodies: one warp per fragment (<= 65536 bytes) of a page; fragment f of raw bytes [src_off, src_off +
-// len) is written to scratch at dst_off (room for 32 + len + len / 6 bytes), its compressed length to out_len[f]
-struct SnappyFragment {
+// Compression of page bodies: one warp per fragment (<= 65536 bytes) of a page; fragment f of raw bytes [src_off, src_off +
+// len) is written to scratch at dst_off (room for the codec's bound below), its compressed length to out_len[f].
+struct PageFragment {
   uint64_t src_off, dst_off;
   uint32_t len, pad;
 };
-constexpr uint32_t kSnappyFragment = 65536;
+constexpr uint32_t kCompressFragment = 65536;
+// SNAPPY: the fragment's element stream (the body's varint preamble is the host's)
 inline uint64_t snappy_max_compressed(uint64_t len) { return 32 + len + len / 6; }
-void launch_snappy_compress(hs_ctx* ctx, const SnappyFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
+void launch_snappy_compress(hs_ctx* ctx, const PageFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
                             uint32_t* out_len);
+// GZIP: the fragment's DEFLATE blocks, ending in a sync flush (room: gz::deflate_fragment_bound + 4, as the last word is
+// stored whole), and out_crc[f], its CRC-32 without pre- and post-inversion (the member around it is the host's)
+void launch_deflate_compress(hs_ctx* ctx, const PageFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
+                             uint32_t* out_len, uint32_t* out_crc);
+// LZ4: the fragment as one block in a Hadoop group of one chunk (room: lz4::kHadoopGroupHeader + lz4::block_bound)
+void launch_lz4_compress(hs_ctx* ctx, const PageFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
+                         uint32_t* out_len);
 
 }  // namespace hs

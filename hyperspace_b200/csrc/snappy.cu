@@ -29,6 +29,7 @@
 #include <climits>
 
 #include "device_utils.cuh"
+#include "lz77.cuh"
 #include "page_codec_kernels.h"
 
 namespace hs {
@@ -354,23 +355,13 @@ void launch_snappy_decompress(hs_ctx* ctx, const PageBlob* blobs, int64_t n, int
 // (index/DataFrameWriterExtensions.scala:59-66 goes through DataFrameWriter; file names ...c000.snappy.parquet,
 // T/index/VacuumOutdatedActionTest.scala:67).  A page's compressed body is the varint of its uncompressed length followed by
 // the element streams of its fragments, which are compressed independently (back-references never leave a fragment, as in
-// snappy's own 64 KB blocks) and therefore in parallel.
-//
-// Per fragment: the 32 lanes probe 32 consecutive positions at a time against a 2048-entry hash table of earlier positions
-// (4-byte hashes); the first lane whose candidate matches wins, the literal before it is flushed, the match is extended 32
-// bytes per ballot and emitted as copies with 2-byte offsets.  Windows without a match make the stride grow (snappy's own
-// heuristic), so incompressible data costs little more than the literal copy.  The table takes atomicMax updates: the
-// output is the same on every run.
+// snappy's own 64 KB blocks) and therefore in parallel.  The fragment is parsed by lz77_parse (lz77.cuh); its sequences
+// become a literal element and copies with 2-byte offsets.
 // =====================================================================================================================
 namespace hs {
 namespace {
 
 constexpr int kCompWarps = 4;
-constexpr uint32_t kCompTable = 2048;
-
-__device__ __forceinline__ uint32_t load32_any(const uint8_t* p) {
-  return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
-}
 
 // literal [from, to) of `in` -> out; returns the new output position (all lanes take part)
 __device__ __forceinline__ uint32_t emit_literal(const uint8_t* __restrict__ in, uint32_t from, uint32_t to, uint8_t* __restrict__ out,
@@ -399,58 +390,14 @@ __device__ __forceinline__ uint32_t emit_literal(const uint8_t* __restrict__ in,
   return op + hdr + len;
 }
 
-__global__ void __launch_bounds__(kCompWarps * 32) k_snappy_compress(const SnappyFragment* __restrict__ frags, int64_t n,
-                                                                      const uint8_t* __restrict__ raw, uint8_t* __restrict__ scratch,
-                                                                      uint32_t* __restrict__ out_len) {
-  __shared__ uint32_t s_table[kCompWarps][kCompTable];
-  const unsigned lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int64_t f = (int64_t)blockIdx.x * kCompWarps + wib;
-  if (f >= n) return;
-  const SnappyFragment fr = frags[f];
-  const uint8_t* in = raw + fr.src_off;
-  uint8_t* out = scratch + fr.dst_off;
-  const uint32_t len = fr.len;
-  uint32_t* table = s_table[wib];
-  for (uint32_t i = lane; i < kCompTable; i += 32) table[i] = 0;
-  __syncwarp();
-  uint32_t ip = 0, lit = 0, op = 0, misses = 0;
-  while (ip + 4 <= len) {
-    const uint32_t pos = ip + lane;
-    const bool can = pos + 4 <= len;
-    uint32_t w = 0, h = 0, cand = 0;
-    if (can) {
-      w = load32_any(in + pos);
-      h = (w * 0x1e35a7bdu) >> 21;  // 11 bits
-      cand = table[h];
-    }
-    __syncwarp();
-    const bool match = can && cand < pos && load32_any(in + cand) == w;
-    const unsigned m = __ballot_sync(0xffffffffu, match);
-    // only positions up to the match enter the table: the scan resumes right behind the match, and an entry that points
-    // past the scan position can never be a candidate (it would shadow the useful, earlier one)
-    const int fl = m ? __ffs(m) - 1 : 31;
-    if (can && (int)lane <= fl) atomicMax(&table[h], pos);
-    __syncwarp();
-    if (m == 0) {
-      misses++;
-      ip += 32u << min(misses >> 2, 4u);
-      continue;
-    }
-    misses = 0;
-    const uint32_t q = ip + fl;
-    const uint32_t c = __shfl_sync(0xffffffffu, cand, fl);
+struct SnappyEmitter {
+  const uint8_t* __restrict__ in;
+  uint8_t* __restrict__ out;
+  uint32_t op;
+  unsigned lane;
+
+  __device__ __forceinline__ void sequence(uint32_t lit, uint32_t q, uint32_t offset, uint32_t mlen) {
     op = emit_literal(in, lit, q, out, op, lane);
-    // extend the match 32 bytes at a time
-    uint32_t mlen = 4;
-    for (;;) {
-      const uint32_t a = q + mlen + lane;
-      const bool eq = a < len && in[a] == in[c + mlen + lane];
-      const unsigned e = __ballot_sync(0xffffffffu, eq);
-      const uint32_t run = e == 0xffffffffu ? 32u : (uint32_t)(__ffs(~e) - 1);
-      mlen += run;
-      if (run < 32) break;
-    }
-    const uint32_t offset = q - c;
     if (mlen <= 11 && offset < 2048) {  // short match nearby: the 2-byte copy element (4..11 bytes, 11-bit offset)
       if (lane == 0) {
         out[op] = (uint8_t)(1u | ((mlen - 4) << 2) | ((offset >> 8) << 5));
@@ -471,17 +418,27 @@ __global__ void __launch_bounds__(kCompWarps * 32) k_snappy_compress(const Snapp
       }
       op += 3 * ((mlen + 63) / 64);
     }
-    ip = q + mlen;
-    lit = ip;
-    __syncwarp();
   }
-  op = emit_literal(in, lit, len, out, op, lane);
-  if (lane == 0) out_len[f] = op;
+  __device__ __forceinline__ void finish(uint32_t lit, uint32_t len) { op = emit_literal(in, lit, len, out, op, lane); }
+};
+
+__global__ void __launch_bounds__(kCompWarps * 32) k_snappy_compress(const PageFragment* __restrict__ frags, int64_t n,
+                                                                      const uint8_t* __restrict__ raw, uint8_t* __restrict__ scratch,
+                                                                      uint32_t* __restrict__ out_len) {
+  __shared__ uint32_t s_table[kCompWarps][kLz77Table];
+  const unsigned lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int64_t f = (int64_t)blockIdx.x * kCompWarps + wib;
+  if (f >= n) return;
+  const PageFragment fr = frags[f];
+  SnappyEmitter emit{raw + fr.src_off, scratch + fr.dst_off, 0u, lane};
+  // every offset of a fragment fits the 2-byte copy, and a copy may end anywhere
+  lz77_parse(raw + fr.src_off, fr.len, s_table[wib], lane, Lz77Limits{0xffffu, 0xffffffffu, 4u, 0u}, emit);
+  if (lane == 0) out_len[f] = emit.op;
 }
 
 }  // namespace
 
-void launch_snappy_compress(hs_ctx* ctx, const SnappyFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
+void launch_snappy_compress(hs_ctx* ctx, const PageFragment* frags, int64_t n, const uint8_t* raw, uint8_t* scratch,
                             uint32_t* out_len) {
   KernelScope _ks(ctx, "k_snappy_compress");
   if (n == 0) return;

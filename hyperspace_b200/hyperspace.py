@@ -85,6 +85,12 @@ class _DataAction(_Action):
         self.version_id = 0 if latest is None else latest + 1
         self.index_data_path = data_manager.get_path(self.version_id)
         self.tracker = LE.FileIdTracker()
+        self.codec = 0
+
+    def _resolve_codec(self) -> None:
+        """The page codec of the files this action writes (spark.sql.parquet.compression.codec); raises for one the
+        engine does not write, before any log entry exists."""
+        self.codec = self.session.conf.parquet_compression_codec
 
     def _build_entry(self, name, indexed, included, num_buckets, lineage: bool, rel: RelationNode, content: LE.Content,
                      properties: Optional[Dict[str, str]] = None, update: Optional[LE.Update] = None) -> LE.IndexLogEntry:
@@ -114,7 +120,8 @@ class _DataAction(_Action):
         images = [_native.FileImage(path=LE.from_uri(u), file_id=(id_of(u, s, m) if id_of else -1)) for u, s, m in files]
         res, _ = self.session.gpu.create_index(images, list(indexed), [c for c in included if not (lineage and c == LE.DATA_FILE_NAME_ID)],
                                                num_buckets, out_dir=out_dir, output=_native.HS_OUT_FILES, save_mode=save_mode,
-                                               lineage=lineage, deleted_file_ids=list(deleted_ids), job_uuid=str(uuid.uuid4()))
+                                               lineage=lineage, deleted_file_ids=list(deleted_ids), job_uuid=str(uuid.uuid4()),
+                                               compression=self.codec)
         res.free()
 
 
@@ -128,6 +135,7 @@ class CreateAction(_DataAction):
         self.lineage = session.conf.lineage_enabled
 
     def validate(self) -> None:  # CreateAction.scala:50-81
+        self._resolve_codec()
         if not isinstance(self.df.plan, RelationNode):
             raise HyperspaceException("Only creating index over HDFS file based scan nodes is supported. "
                                       "Source plan must be a bare relation (spark.read.parquet).")
@@ -194,6 +202,7 @@ class RefreshAction(_RefreshBase):
 
     def validate(self) -> None:
         super().validate()
+        self._resolve_codec()
         if not self.appended and not self.deleted:
             raise NoChangesException("Refresh full aborted as no source data changed.")
 
@@ -214,6 +223,7 @@ class RefreshIncrementalAction(_RefreshBase):
 
     def validate(self) -> None:
         super().validate()
+        self._resolve_codec()
         if not self.appended and not self.deleted:
             raise NoChangesException("Refresh incremental aborted as no source data change found.")
         if self.deleted and not self.lineage:
@@ -285,6 +295,7 @@ class OptimizeAction(_DataAction):
         self.to_ignore = [f for f in infos if f.name not in keep]
 
     def validate(self) -> None:
+        self._resolve_codec()
         if self.mode.lower() not in (OPTIMIZE_MODE_QUICK, OPTIMIZE_MODE_FULL):
             raise HyperspaceException(f"Unsupported optimize mode '{self.mode}' found.")
         if self.prev.state != States.ACTIVE:

@@ -41,6 +41,9 @@ INDEX_HYBRID_SCAN_DELETED_RATIO_THRESHOLD = "spark.hyperspace.index.hybridscan.m
 OPTIMIZE_FILE_SIZE_THRESHOLD = "spark.hyperspace.index.optimize.fileSizeThreshold"
 OPTIMIZE_FILE_SIZE_THRESHOLD_DEFAULT = 256 * 1024 * 1024
 HYPERSPACE_ENABLED = "spark.hyperspace.enabled"  # session flag toggled by enableHyperspace()/disableHyperspace()
+PARQUET_COMPRESSION_CODEC = "spark.sql.parquet.compression.codec"
+# the codecs of spark.sql.parquet.compression.codec that index files are written with -> Parquet's codec ids (HS_CODEC_*)
+PARQUET_OUTPUT_CODECS = {"none": 0, "uncompressed": 0, "snappy": 1, "gzip": 2, "lz4": 5}
 
 
 class RuntimeConf:
@@ -81,6 +84,19 @@ class RuntimeConf:
     @property
     def hybrid_scan_deleted_ratio(self) -> float:
         return float(self._v.get(INDEX_HYBRID_SCAN_DELETED_RATIO_THRESHOLD, 0.2))
+
+    @property
+    def parquet_compression_codec(self) -> int:
+        """The codec of the index files' pages (HS_CODEC_*), from spark.sql.parquet.compression.codec, case-insensitive as
+        Spark's ParquetOptions reads it.  Unset: UNCOMPRESSED.  A codec the engine does not write raises."""
+        name = self._v.get(PARQUET_COMPRESSION_CODEC)
+        if name is None:
+            return 0
+        codec = PARQUET_OUTPUT_CODECS.get(str(name).lower())
+        if codec is None:
+            raise LE.HyperspaceException(f"Index files cannot be written with {PARQUET_COMPRESSION_CODEC}={name}: "
+                                         f"the codecs written are {', '.join(PARQUET_OUTPUT_CODECS)}.")
+        return codec
 
     @property
     def optimize_file_size_threshold(self) -> int:

@@ -123,6 +123,8 @@ typedef struct {
 
 #define HS_CODEC_UNCOMPRESSED 0
 #define HS_CODEC_SNAPPY 1
+#define HS_CODEC_GZIP 2 /* one gzip member per page */
+#define HS_CODEC_LZ4 5  /* Hadoop's Lz4Codec framing, as Spark 2.4-3.1 write it */
 
 #define HS_OUT_FILES 0  /* write <out_dir>/part-<bbbbb>-<uuid>_<bbbbb>.c000.parquet (the reference's effect) */
 #define HS_OUT_HOST 1   /* keep the bucket file images in pinned host memory owned by the result handle */
@@ -149,8 +151,10 @@ typedef struct {
   int32_t n_deleted_file_ids;
   int32_t disable_dictionary; /* 0 (default): dictionary-encode columns whose distinct values fit a dictionary page, as
                                  parquet-mr does; != 0: PLAIN only */
-  int32_t compression;        /* HS_CODEC_*: codec of the index pages.  HS_CODEC_SNAPPY is what Spark writes by default
-                                 (files are then named ...c000.snappy.parquet, T/index/VacuumOutdatedActionTest.scala:67) */
+  int32_t compression;        /* HS_CODEC_*: codec of the index pages, spark.sql.parquet.compression.codec.  HS_CODEC_SNAPPY is
+                                 what Spark writes by default (files are then named ...c000.snappy.parquet,
+                                 T/index/VacuumOutdatedActionTest.scala:67); GZIP and LZ4 files end in .c000.gz.parquet and
+                                 .c000.lz4.parquet.  Other codecs are HS_EUNSUPPORTED. */
   int32_t reserved;
 } hs_index_spec;
 
@@ -453,6 +457,11 @@ int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t ou
  * one block) or 5 (LZ4: Hadoop-framed blocks, or one raw block); any other codec is HS_EINVAL.  HS_EFORMAT for a damaged
  * body; the message names the failed check.  Kernel-level entry point for the parity tests. */
 int hs_k_lz4(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out, uint64_t out_len, char* err, size_t errlen);
+/* The page compressor of index builds on one page body of n bytes, through the same path as the encoder: codec HS_CODEC_GZIP
+ * (one gzip member) or HS_CODEC_LZ4 (Hadoop-framed blocks, one per 64 KB); any other codec is HS_EINVAL.  *out_len is the
+ * compressed size; HS_ENOMEM when it exceeds cap.  Kernel-level entry point for the parity tests. */
+int hs_k_compress(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out, uint64_t cap, uint64_t* out_len, char* err,
+                  size_t errlen);
 
 #ifdef __cplusplus
 }
