@@ -864,26 +864,32 @@ class Context:
         _check(L.hs_filter_scan(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
+    @staticmethod
+    def _scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output):
+        """The hs_scan_spec of filter_scan_where / filter_scan_any, and the arrays it points into."""
+        src, src_keep = _source_array(files)
+        pc = _cstr_array(projected)
+        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
+        spec = ScanSpec()
+        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
+        spec.key_column = key.encode() if key else None
+        spec.projected_columns, spec.n_projected = pc, len(projected)
+        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
+        spec.output = output
+        return spec, (src, src_keep, pc, dl)
+
     def filter_scan_where(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
                           sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (), output: int = HS_OUT_HOST
                           ) -> Tuple[Batch, Dict[str, float]]:
         """hs_filter_scan_where: rows where every predicate holds.  A predicate is ``(column, lo, lo_strict, hi, hi_strict)``
         with None for a missing bound; the literal type follows the Python value (int -> long, float -> double, str / bytes
         -> string) and the engine applies Spark's comparison coercion."""
-        L = load_library()
-        src, keep = _source_array(files)
-        pc = _cstr_array(projected)
-        spec = ScanSpec()
-        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
-        spec.key_column = key.encode() if key else None
-        spec.projected_columns, spec.n_projected = pc, len(projected)
-        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
-        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
-        spec.output = output
+        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
         preds, n_preds = _predicate_array(predicates)
         res, st = C.c_void_p(), Stats()
         err = C.create_string_buffer(1024)
-        _check(L.hs_filter_scan_where(self._h, C.byref(spec), preds, n_preds, C.byref(res), C.byref(st), err, len(err)), err)
+        _check(load_library().hs_filter_scan_where(self._h, C.byref(spec), preds, n_preds, C.byref(res), C.byref(st), err, len(err)),
+               err)
         return Batch(res.value, self), st.as_dict()
 
     def filter_scan_any(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
@@ -895,15 +901,7 @@ class Context:
         hi_strict)``).  file_buckets / num_buckets: the bucket of every file of an index bucketed on `key` alone, for
         skipping the files a point lookup cannot hit."""
         L = load_library()
-        src, keep = _source_array(files)
-        pc = _cstr_array(projected)
-        spec = ScanSpec()
-        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
-        spec.key_column = key.encode() if key else None
-        spec.projected_columns, spec.n_projected = pc, len(projected)
-        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
-        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
-        spec.output = output
+        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
         preds, n_preds = _predicate_array(predicates)
         anys, n_anys, keep_any = _any_array(terms)
         fb = np.ascontiguousarray(file_buckets if file_buckets is not None else [0], dtype=np.int32)
@@ -943,6 +941,17 @@ class Context:
         _check(L.hs_bucket_join(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
+    def _join_where_args(self, left, left_buckets, right, right_buckets, num_buckets, left_keys, right_keys, left_columns,
+                         right_columns, left_predicates, right_predicates, output):
+        """What bucket_join_where and bucket_join_any pass alike: the spec (and the arrays it points into), the key name
+        arrays, and each side's predicate array with its count."""
+        if len(left_keys) != len(right_keys):
+            raise ValueError("left_keys and right_keys must pair up")
+        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
+                                     right_columns, output)
+        return (spec, keep, _cstr_array(left_keys), _cstr_array(right_keys), _predicate_array(left_predicates),
+                _predicate_array(right_predicates))
+
     def bucket_join_where(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
                           right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
                           left_columns: Sequence[str], right_columns: Sequence[str], left_predicates: Sequence[tuple] = (),
@@ -951,18 +960,13 @@ class Context:
         columns), keeping on each side only the rows where every predicate of that side holds.  Predicates are
         filter_scan_where's ``(column, lo, lo_strict, hi, hi_strict)`` tuples.  Rows with a null key join nothing.  The
         side selection's time is in ``ms_exchange``."""
-        L = load_library()
-        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
-                                     right_columns, output)
-        lk, rk = _cstr_array(left_keys), _cstr_array(right_keys)
-        if len(left_keys) != len(right_keys):
-            raise ValueError("left_keys and right_keys must pair up")
-        lp, nlp = _predicate_array(left_predicates)
-        rp, nrp = _predicate_array(right_predicates)
+        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
+                                                                          left_keys, right_keys, left_columns, right_columns,
+                                                                          left_predicates, right_predicates, output)
         res, st = C.c_void_p(), Stats()
         err = C.create_string_buffer(1024)
-        _check(L.hs_bucket_join_where(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, rp, nrp, C.byref(res), C.byref(st),
-                                      err, len(err)), err)
+        _check(load_library().hs_bucket_join_where(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, rp, nrp, C.byref(res),
+                                                   C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     def bucket_join_any(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
@@ -972,13 +976,9 @@ class Context:
                         output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
         """hs_bucket_join_any: bucket_join_where with filter_scan_any's disjunction terms on either side."""
         L = load_library()
-        spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
-                                     right_columns, output)
-        lk, rk = _cstr_array(left_keys), _cstr_array(right_keys)
-        if len(left_keys) != len(right_keys):
-            raise ValueError("left_keys and right_keys must pair up")
-        lp, nlp = _predicate_array(left_predicates)
-        rp, nrp = _predicate_array(right_predicates)
+        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
+                                                                          left_keys, right_keys, left_columns, right_columns,
+                                                                          left_predicates, right_predicates, output)
         la, nla, k1 = _any_array(left_terms)
         ra, nra, k2 = _any_array(right_terms)
         res, st = C.c_void_p(), Stats()

@@ -16,7 +16,7 @@
 #include "engine.h"
 #include "inflate.h"
 #include "lz4_block.h"
-#include "spark_types.h"
+#include "predicates.h"
 
 using namespace hs;
 
@@ -862,339 +862,31 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
 
 }  // extern "C"
 
-// ---- predicates: Spark 3.1's binary-comparison coercion, decided once on the host ---------------------------------------
-// Every predicate becomes a PredRange (kernels.h): numeric columns get an inclusive range of sort_encode values, found by
-// binary search over the encoded domain with the comparison Spark would evaluate -- in the wider of the column's and the
-// literal's types (int < long < float < double), with SQLOrderingUtil's order (NaN == NaN, NaN above +inf, -0.0 == 0.0).
-// Every cast on the way (int/long -> double, float -> double, long -> float) is monotone, so the rows satisfying a bound
-// are one end of the encoded order, and rounding casts (long -> double beyond 2^53) are followed exactly.
+// ---- predicates: resolved on the host (predicates.h), uploaded here -------------------------------------------------
 
-template <typename F>
-static int spark_compare(F a, F b) {  // SQLOrderingUtil.compareDoubles / compareFloats
-  const bool na = a != a, nb = b != b;
-  if (na || nb) return na == nb ? 0 : (na ? 1 : -1);
-  return a < b ? -1 : (a > b ? 1 : 0);
-}
-
-// the column value whose sort_encode is e, compared with the literal (lit_i when lit_type is HS_TYPE_INT64 or
-// HS_TYPE_DECIMAL, else lit_f).  Integer columns and integer / decimal literals compare as decimals of their scales
-// (col_scale: the column's, 0 unless it is a decimal; lit_scale: the literal's, 0 for HS_TYPE_INT64).
-static int compare_encoded(int col_type, uint64_t e, int lit_type, int64_t lit_i, double lit_f, int col_scale, int lit_scale) {
-  const bool lit_long = lit_type == HS_TYPE_INT64 || lit_type == HS_TYPE_DECIMAL;
-  switch (col_type) {
-    case HS_TYPE_INT32:
-    case HS_TYPE_INT64: {
-      const int64_t v = col_type == HS_TYPE_INT32 ? (int64_t)(int32_t)((uint32_t)e ^ 0x80000000u) : (int64_t)(e ^ 0x8000000000000000ull);
-      if (lit_long) return compare_scaled(v, col_scale, lit_i, lit_scale);
-      return spark_compare((double)v, lit_f);
-    }
-    case HS_TYPE_FLOAT: {
-      const uint32_t u = (uint32_t)e, bits = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-      float f;
-      memcpy(&f, &bits, 4);
-      return lit_long ? spark_compare(f, (float)lit_i) : spark_compare((double)f, lit_f);
-    }
-    default: {
-      const uint64_t bits = (e & 0x8000000000000000ull) ? (e & 0x7fffffffffffffffull) : ~e;
-      double d;
-      memcpy(&d, &bits, 8);
-      return spark_compare(d, lit_long ? (double)lit_i : lit_f);
-    }
-  }
-}
-
-// encoded values of a column type, lowest to highest (floating point: -inf .. the NaNs above +inf)
-static void encoded_domain(int col_type, uint64_t* lo, uint64_t* hi) {
-  switch (col_type) {
-    case HS_TYPE_INT32: *lo = 0, *hi = 0xffffffffull; return;
-    case HS_TYPE_INT64: *lo = 0, *hi = ~0ull; return;
-    case HS_TYPE_FLOAT: *lo = 0x007fffffull, *hi = 0xffffffffull; return;   // ~bits(-inf)
-    default: *lo = 0x000fffffffffffffull, *hi = ~0ull; return;             // ~bits(-inf)
-  }
-}
-
-struct ResolvedPredicate {
-  int col = -1;  // index into the scan's decoded columns
-  PredRange r{};
-  const uint8_t* lo_host = nullptr;  // string bounds, for intersecting them on the host
-  const uint8_t* hi_host = nullptr;
-  uint32_t lo_len = 0, hi_len = 0;
+// Device memory that uploaded descriptors point into: string bound bytes and set-form range arrays, with the host
+// arrays their copies read from (a large copy reads its source until the stream is synchronised).  Kept until the
+// kernels that read them have run.
+struct PredUploads {
+  std::vector<Buf<uint8_t>> bytes;
+  std::vector<Buf<PredRange>> sets;
+  std::vector<std::vector<uint8_t>> staged_bytes;
+  std::vector<std::vector<PredRange>> staged_sets;
 };
 
-// p.literal_type < 0 (hs_filter_scan): the literal type follows the column -- int64 bounds on an integer column, bytes on a
-// string column.  The bytes of string bounds are copied to `holder` (device).
-static PredRange resolve_predicate(hs_ctx* ctx, const hs_predicate& p, const DevColumn& c, std::vector<Buf<uint8_t>>* holder,
-                                   ResolvedPredicate* rp) {
-  const bool str_col = c.type == HS_TYPE_STRING;
-  int lit = p.literal_type;
-  if (lit < 0) {
-    if (!str_col && c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64) fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
-    lit = str_col ? HS_TYPE_STRING : HS_TYPE_INT64;
-  }
-  if (c.type == HS_TYPE_BOOL) fail(HS_EUNSUPPORTED, "filter scan: predicates on the boolean column '%s' are not handled", c.name.c_str());
-  if (c.type < HS_TYPE_INT32 || c.type > HS_TYPE_STRING) fail(HS_EUNSUPPORTED, "filter scan: column '%s' has an unhandled type", c.name.c_str());
-  if (str_col != (lit == HS_TYPE_STRING))
-    fail(HS_EUNSUPPORTED, "filter scan: a %s literal cannot be compared with the %s column '%s'", lit == HS_TYPE_STRING ? "string" : "numeric",
-         str_col ? "string" : "numeric", c.name.c_str());
-  // Spark compares these in double: the caller keeps the conjunct in a Filter of its own
-  const bool dec_col = is_decimal(c.schema), ts_col = is_timestamp(c.schema);
-  if (lit == HS_TYPE_DOUBLE && (dec_col || ts_col))
-    fail(HS_EUNSUPPORTED, "filter scan: a double literal cannot be compared with the %s column '%s'", dec_col ? "decimal" : "timestamp",
-         c.name.c_str());
-  if (lit == HS_TYPE_DECIMAL && (ts_col || (c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64)))
-    fail(HS_EUNSUPPORTED, "filter scan: a decimal literal cannot be compared with the %s column '%s'",
-         ts_col ? "timestamp" : (c.type == HS_TYPE_STRING ? "string" : "floating-point"), c.name.c_str());
-  if (lit == HS_TYPE_DECIMAL && (p.scale < 0 || p.scale > 38))
-    fail(HS_EINVAL, "filter scan: decimal literal on '%s' has scale %d", c.name.c_str(), p.scale);
-  const int col_scale = dec_col ? c.schema.scale : 0, lit_scale = lit == HS_TYPE_DECIMAL ? p.scale : 0;
-  PredRange r{};
-  r.type = c.type;
-  r.has_lo = p.has_lo != 0;
-  r.has_hi = p.has_hi != 0;
-  if (str_col) {
-    if ((p.has_lo && p.lo_len && !p.lo_bytes) || (p.has_hi && p.hi_len && !p.hi_bytes))
-      fail(HS_EINVAL, "filter scan: string column '%s' needs lo_bytes / hi_bytes", c.name.c_str());
-    if (p.lo_len > kMaxStringLen || p.hi_len > kMaxStringLen) fail(HS_EUNSUPPORTED, "string bound longer than 65535 bytes");
-    const uint32_t ll = p.has_lo ? p.lo_len : 0, hl = p.has_hi ? p.hi_len : 0;
-    holder->emplace_back(ctx, (size_t)ll + hl + 16);
-    uint8_t* d = holder->back().get();
-    if (ll) copy_h2d(ctx, d, p.lo_bytes, ll);
-    if (hl) copy_h2d(ctx, d + ll, p.hi_bytes, hl);
-    r.lo = string_ref(d, ll);
-    r.hi = string_ref(d + ll, hl);
-    r.lo_strict = r.has_lo && p.lo_strict;
-    r.hi_strict = r.has_hi && p.hi_strict;
-    rp->lo_host = (const uint8_t*)p.lo_bytes, rp->lo_len = ll;
-    rp->hi_host = (const uint8_t*)p.hi_bytes, rp->hi_len = hl;
-    return r;
-  }
-  uint64_t emin, emax;
-  encoded_domain(c.type, &emin, &emax);
-  auto cmp = [&](uint64_t e, bool hi_side) {
-    return compare_encoded(c.type, e, lit, hi_side ? p.hi_i : p.lo_i, hi_side ? p.hi_f : p.lo_f, col_scale, lit_scale);
-  };
-  bool empty = false;
-  if (r.has_lo) {  // smallest e with value >= lo (> lo when strict)
-    const int t = p.lo_strict ? 1 : 0;
-    if (cmp(emax, false) < t) {
-      empty = true;
-    } else {
-      uint64_t a = emin, b = emax;
-      while (a < b) {
-        const uint64_t mid = a + ((b - a) >> 1);
-        if (cmp(mid, false) >= t) b = mid;
-        else a = mid + 1;
-      }
-      r.lo = a;
-    }
-  }
-  if (r.has_hi) {  // largest e with value <= hi (< hi when strict)
-    const int t = p.hi_strict ? -1 : 0;
-    if (cmp(emin, true) > t) {
-      empty = true;
-    } else {
-      uint64_t a = emin, b = emax;
-      while (a < b) {
-        const uint64_t mid = b - ((b - a) >> 1);
-        if (cmp(mid, true) <= t) a = mid;
-        else b = mid - 1;
-      }
-      r.hi = a;
-    }
-  }
-  if (empty) r.has_lo = r.has_hi = 1, r.lo = 1, r.hi = 0;
-  return r;
-}
-
-static int host_string_compare(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
-  const int c = memcmp(a, b, std::min(la, lb));
-  if (c) return c < 0 ? -1 : 1;
-  return la == lb ? 0 : (la < lb ? -1 : 1);
-}
-
-// the conjunction of predicates on one column as one range (the window search takes one range per file)
-static PredRange intersect_ranges(int type, const std::vector<ResolvedPredicate>& ps) {
-  PredRange r{};
-  r.type = type;
-  const uint8_t *lo_b = nullptr, *hi_b = nullptr;
-  uint32_t lo_l = 0, hi_l = 0;
-  for (const ResolvedPredicate& p : ps) {
-    if (p.r.has_lo) {
-      bool take = !r.has_lo;
-      if (!take && type == HS_TYPE_STRING) {
-        const int c = host_string_compare(p.lo_host, p.lo_len, lo_b, lo_l);
-        take = c > 0 || (c == 0 && p.r.lo_strict);
-      } else if (!take) {
-        take = p.r.lo > r.lo;
-      }
-      if (take) r.has_lo = 1, r.lo = p.r.lo, r.lo_strict = p.r.lo_strict, lo_b = p.lo_host, lo_l = p.lo_len;
-    }
-    if (p.r.has_hi) {
-      bool take = !r.has_hi;
-      if (!take && type == HS_TYPE_STRING) {
-        const int c = host_string_compare(p.hi_host, p.hi_len, hi_b, hi_l);
-        take = c < 0 || (c == 0 && p.r.hi_strict);
-      } else if (!take) {
-        take = p.r.hi < r.hi;
-      }
-      if (take) r.has_hi = 1, r.hi = p.r.hi, r.hi_strict = p.r.hi_strict, hi_b = p.hi_host, hi_l = p.hi_len;
-    }
-  }
-  return r;
-}
-
-// ---- disjunctions on one column (hs_predicate_any) ------------------------------------------------------------------
-// A term becomes a sorted list of disjoint ranges of the column (SetRange, on the host), every value and range resolved by
-// resolve_predicate.  Numeric ranges are inclusive sort_encode values with both bounds present (an open side is the end
-// of the encoded domain); string ranges are bytes with their strictness, a missing bound open.
-struct SetRange {
-  bool has_lo = false, has_hi = false, lo_strict = false, hi_strict = false;
-  uint64_t lo = 0, hi = 0;
-  std::string lo_b, hi_b;
-};
-using RangeSet = std::vector<SetRange>;
-
-static int set_bound_cmp(bool str, uint64_t a, const std::string& as, uint64_t b, const std::string& bs) {
-  if (str) return host_string_compare((const uint8_t*)as.data(), (uint32_t)as.size(), (const uint8_t*)bs.data(), (uint32_t)bs.size());
-  return a < b ? -1 : (a > b ? 1 : 0);
-}
-static bool set_range_empty(bool str, const SetRange& r) {
-  if (!r.has_lo || !r.has_hi) return false;
-  const int c = set_bound_cmp(str, r.lo, r.lo_b, r.hi, r.hi_b);
-  return c > 0 || (c == 0 && (r.lo_strict || r.hi_strict));
-}
-static bool lo_before(bool str, const SetRange& a, const SetRange& b) {  // a starts below b
-  if (!a.has_lo || !b.has_lo) return !a.has_lo && b.has_lo;
-  const int c = set_bound_cmp(str, a.lo, a.lo_b, b.lo, b.lo_b);
-  return c < 0 || (c == 0 && !a.lo_strict && b.lo_strict);
-}
-static bool hi_before(bool str, const SetRange& a, const SetRange& b) {  // a ends below b
-  if (!a.has_hi || !b.has_hi) return a.has_hi && !b.has_hi;
-  const int c = set_bound_cmp(str, a.hi, a.hi_b, b.hi, b.hi_b);
-  return c < 0 || (c == 0 && a.hi_strict && !b.hi_strict);
-}
-static void take_lo(SetRange* r, const SetRange& from) { r->has_lo = from.has_lo, r->lo = from.lo, r->lo_b = from.lo_b, r->lo_strict = from.lo_strict; }
-static void take_hi(SetRange* r, const SetRange& from) { r->has_hi = from.has_hi, r->hi = from.hi, r->hi_b = from.hi_b, r->hi_strict = from.hi_strict; }
-
-// sorts, drops empty ranges and merges overlapping and adjacent ones
-static void normalise_set(bool str, RangeSet* rs) {
-  rs->erase(std::remove_if(rs->begin(), rs->end(), [&](const SetRange& r) { return set_range_empty(str, r); }), rs->end());
-  std::sort(rs->begin(), rs->end(), [&](const SetRange& a, const SetRange& b) { return lo_before(str, a, b); });
-  RangeSet out;
-  for (SetRange& r : *rs) {
-    bool joins = false;
-    if (!out.empty()) {
-      const SetRange& cur = out.back();
-      if (!cur.has_hi || !r.has_lo) joins = true;
-      else if (!str) joins = r.lo <= cur.hi || r.lo - 1 == cur.hi;  // r.lo > cur.hi >= 0 in the second test
-      else {
-        const int c = set_bound_cmp(true, r.lo, r.lo_b, cur.hi, cur.hi_b);
-        joins = c < 0 || (c == 0 && !(r.lo_strict && cur.hi_strict));
-      }
-    }
-    if (!joins) out.push_back(std::move(r));
-    else if (hi_before(str, out.back(), r)) take_hi(&out.back(), r);
-  }
-  *rs = std::move(out);
-}
-
-static RangeSet intersect_sets(bool str, const RangeSet& a, const RangeSet& b) {
-  RangeSet out;
-  size_t i = 0, j = 0;
-  while (i < a.size() && j < b.size()) {
-    SetRange r;
-    take_lo(&r, lo_before(str, a[i], b[j]) ? b[j] : a[i]);
-    const bool a_first = hi_before(str, a[i], b[j]);
-    take_hi(&r, a_first ? a[i] : b[j]);
-    if (!set_range_empty(str, r)) out.push_back(std::move(r));
-    if (a_first) i++;
-    else j++;
-  }
-  return out;
-}
-
-static uint64_t encoded_max(int type) { return type == HS_TYPE_INT32 || type == HS_TYPE_FLOAT ? 0xffffffffull : ~0ull; }
-
-// a resolved range (resolve_predicate / intersect_ranges) as a set of at most one range; string bounds from the host bytes
-static SetRange set_range_of(int type, const PredRange& r, const uint8_t* lo_host, uint32_t lo_len, const uint8_t* hi_host,
-                             uint32_t hi_len) {
-  SetRange s;
-  if (type == HS_TYPE_STRING) {
-    s.has_lo = r.has_lo, s.has_hi = r.has_hi, s.lo_strict = r.lo_strict, s.hi_strict = r.hi_strict;
-    if (r.has_lo && lo_len) s.lo_b.assign((const char*)lo_host, lo_len);
-    if (r.has_hi && hi_len) s.hi_b.assign((const char*)hi_host, hi_len);
-    return s;
-  }
-  s.has_lo = s.has_hi = true;
-  s.lo = r.has_lo ? r.lo : 0;
-  s.hi = r.has_hi ? r.hi : encoded_max(type);
-  return s;
-}
-
-// Every value and range of the term on column c, as one sorted disjoint set; values that match nothing (int_col IN (2.5))
-// are dropped.  The refusals are resolve_predicate's, for the list's literal type and for every range.
-static RangeSet resolve_any(hs_ctx* ctx, const hs_predicate_any& a, const DevColumn& c) {
-  const bool str = c.type == HS_TYPE_STRING;
-  std::vector<Buf<uint8_t>> scratch;
-  ResolvedPredicate rp;
-  RangeSet out;
-  hs_predicate p;
-  memset(&p, 0, sizeof p);
-  p.column = a.column;
-  p.literal_type = a.literal_type;
-  p.scale = a.scale;
-  p.has_lo = p.has_hi = 1;
-  const bool lit_long = a.literal_type == HS_TYPE_INT64 || a.literal_type == HS_TYPE_DECIMAL;
-  const int col_scale = is_decimal(c.schema) ? c.schema.scale : 0, lit_scale = a.literal_type == HS_TYPE_DECIMAL ? a.scale : 0;
-  if (a.n_values > 0) resolve_predicate(ctx, p, c, &scratch, &rp);  // the list's refusals, once
-  out.reserve((size_t)a.n_values + a.n_ranges);
-  for (int64_t k = 0; k < a.n_values; k++) {
-    SetRange s;
-    if (str) {
-      const uint64_t b = a.values_offsets[k], e = a.values_offsets[k + 1];
-      s.has_lo = s.has_hi = true;
-      s.lo_b.assign((const char*)a.values_bytes + b, e - b);
-      s.hi_b = s.lo_b;
-      out.push_back(std::move(s));
-      continue;
-    }
-    // an integer column against an integer literal at its own scale equals at most one value: the literal's own encoding,
-    // confirmed by the comparison; everything else goes through the binary searches of resolve_predicate
-    if (lit_long && col_scale == lit_scale && (c.type == HS_TYPE_INT64 || (c.type == HS_TYPE_INT32 && a.values_i[k] == (int32_t)a.values_i[k]))) {
-      const uint64_t e = c.type == HS_TYPE_INT32 ? (uint64_t)((uint32_t)(int32_t)a.values_i[k] ^ 0x80000000u)
-                                                 : (uint64_t)a.values_i[k] ^ 0x8000000000000000ull;
-      if (compare_encoded(c.type, e, a.literal_type, a.values_i[k], 0.0, col_scale, lit_scale) == 0) {
-        s.has_lo = s.has_hi = true;
-        s.lo = s.hi = e;
-        out.push_back(std::move(s));
-        continue;
-      }
-    }
-    if (lit_long) p.lo_i = p.hi_i = a.values_i[k];
-    else p.lo_f = p.hi_f = a.values_f[k];
-    out.push_back(set_range_of(c.type, resolve_predicate(ctx, p, c, &scratch, &rp), nullptr, 0, nullptr, 0));
-  }
-  for (int32_t r = 0; r < a.n_ranges; r++) {
-    hs_predicate q = a.ranges[r];
-    q.column = a.column;
-    const PredRange pr = resolve_predicate(ctx, q, c, &scratch, &rp);
-    out.push_back(set_range_of(c.type, pr, rp.lo_host, rp.lo_len, rp.hi_host, rp.hi_len));
-  }
-  normalise_set(str, &out);
-  return out;
-}
-
-// the device form of a set: PredRanges of the column's type (string bounds reference one device copy of their bytes,
-// kept in `holder`)
-static void upload_set(hs_ctx* ctx, int type, const RangeSet& s, Buf<PredRange>* d_set, std::vector<Buf<uint8_t>>* holder) {
+// The PredRanges of a set on a column of type `type`: the one place string bounds go to the device (one copy of their
+// bytes, referenced by the ranges).  Returns them; as_array: uploads them instead, to up->sets.back(), for the set form
+// and the window search.
+static std::vector<PredRange> upload_set(hs_ctx* ctx, int type, const RangeSet& s, PredUploads* up, bool as_array) {
   std::vector<PredRange> h(std::max<size_t>(1, s.size()));
   uint8_t* bytes = nullptr;
-  std::vector<uint8_t> hb;
   if (type == HS_TYPE_STRING) {
+    std::vector<uint8_t> hb;
     for (const SetRange& r : s) hb.insert(hb.end(), r.lo_b.begin(), r.lo_b.end()), hb.insert(hb.end(), r.hi_b.begin(), r.hi_b.end());
-    holder->emplace_back(ctx, hb.size() + 16);
-    bytes = holder->back().get();
+    up->bytes.emplace_back(ctx, hb.size() + 16);
+    bytes = up->bytes.back().get();
     if (!hb.empty()) copy_h2d(ctx, bytes, hb.data(), hb.size());
+    up->staged_bytes.push_back(std::move(hb));
   }
   uint64_t off = 0;
   for (size_t i = 0; i < s.size(); i++) {
@@ -1212,17 +904,45 @@ static void upload_set(hs_ctx* ctx, int type, const RangeSet& s, Buf<PredRange>*
       d.lo = r.lo, d.hi = r.hi;
     }
   }
-  d_set->alloc(ctx, h.size());
-  copy_h2d(ctx, d_set->get(), h.data(), sizeof(PredRange) * h.size());
-  sync_stream(ctx);
+  if (!as_array) return h;
+  up->sets.emplace_back(ctx, h.size());
+  copy_h2d(ctx, up->sets.back().get(), h.data(), sizeof(PredRange) * h.size());
+  up->staged_sets.push_back(std::move(h));
+  return {};
 }
 
-static bool set_is_points(bool str, const RangeSet& s) {
-  for (const SetRange& r : s) {
-    if (!r.has_lo || !r.has_hi) return false;
-    if (str ? (r.lo_b != r.hi_b || r.lo_strict || r.hi_strict) : r.lo != r.hi) return false;
+static PredColumn pred_column(const DevColumn& c) { return PredColumn{c.type, c.schema, c.name}; }
+
+// Appends to ps the descriptors of the predicates and terms on the columns of t (pred_col[i], any_col[i]), skipping
+// those on column skip_col: a predicate in scalar form, a term in set form.
+static void add_predicates(hs_ctx* ctx, const Table& t, const hs_predicate* preds, const std::vector<int>& pred_col,
+                           const hs_predicate_any* anys, const std::vector<int>& any_col, int skip_col, PredSet* ps,
+                           PredUploads* up) {
+  for (size_t i = 0; i < pred_col.size(); i++) {
+    if (pred_col[i] == skip_col) continue;
+    const DevColumn& c = t.cols[pred_col[i]];
+    const RangeSet one{resolve_range(preds[i], pred_column(c))};
+    ps->p[ps->n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, upload_set(ctx, c.type, one, up, false)[0]};
   }
-  return true;
+  for (size_t i = 0; i < any_col.size(); i++) {
+    if (any_col[i] == skip_col) continue;
+    const DevColumn& c = t.cols[any_col[i]];
+    const RangeSet s = resolve_term(anys[i], pred_column(c));
+    upload_set(ctx, c.type, s, up, true);
+    PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
+    d.r.type = c.type;
+    d.set = up->sets.back().get();
+    d.n_set = (int64_t)s.size();
+    ps->p[ps->n++] = d;
+  }
+}
+
+// the index of column nm in cols, appended when it is not there yet
+static int column_index(std::vector<std::string>* cols, const std::string& nm) {
+  auto it = std::find(cols->begin(), cols->end(), nm);
+  if (it != cols->end()) return (int)(it - cols->begin());
+  cols->push_back(nm);
+  return (int)cols->size() - 1;
 }
 
 // the bucket of every point of a key set, by the hash the build used (hash_rows over a column of the key's storage type
@@ -1237,15 +957,19 @@ static std::vector<int> point_buckets(hs_ctx* ctx, const DevColumn& key, const R
   c.width = key.width;
   c.schema = key.schema;
   c.data.alloc(ctx, (size_t)n * c.width + 16);
-  std::vector<Buf<uint8_t>> holder;
-  Buf<PredRange> d_set;
+  Buf<uint8_t> bytes;
   std::vector<uint8_t> raw((size_t)n * c.width);
-  if (key.type == HS_TYPE_STRING) {  // the references of the uploaded lower bounds
-    upload_set(ctx, key.type, pts, &d_set, &holder);
-    std::vector<PredRange> h(n);
-    copy_d2h(ctx, h.data(), d_set.get(), sizeof(PredRange) * n);
-    sync_stream(ctx);
-    for (int64_t i = 0; i < n; i++) memcpy(raw.data() + 8 * i, &h[i].lo, 8);
+  if (key.type == HS_TYPE_STRING) {  // references into one device copy of the points' bytes
+    std::vector<uint8_t> hb;
+    for (const SetRange& r : pts) hb.insert(hb.end(), r.lo_b.begin(), r.lo_b.end());
+    bytes.alloc(ctx, hb.size() + 16);
+    if (!hb.empty()) copy_h2d(ctx, bytes.get(), hb.data(), hb.size());
+    uint64_t off = 0;
+    for (int64_t i = 0; i < n; i++) {
+      const uint64_t ref = string_ref(bytes.get() + off, (uint32_t)pts[i].lo_b.size());
+      memcpy(raw.data() + 8 * i, &ref, 8);
+      off += pts[i].lo_b.size();
+    }
   } else {
     for (int64_t i = 0; i < n; i++) {
       if (key.width == 4) {
@@ -1294,39 +1018,26 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     // columns to decode: the key first (sorted path), then the projection, the predicate columns, and lineage when
     // deletes must be filtered
     std::vector<std::string> cols;
-    auto col_of = [&](const std::string& nm) {
-      auto it = std::find(cols.begin(), cols.end(), nm);
-      if (it != cols.end()) return (int)(it - cols.begin());
-      cols.push_back(nm);
-      return (int)cols.size() - 1;
-    };
-    if (try_sorted) col_of(spec->key_column);
+    if (try_sorted) column_index(&cols, spec->key_column);
     std::vector<int> proj_idx;
-    for (int i = 0; i < spec->n_projected; i++) proj_idx.push_back(col_of(spec->projected_columns[i]));
+    for (int i = 0; i < spec->n_projected; i++) proj_idx.push_back(column_index(&cols, spec->projected_columns[i]));
     std::vector<int> pred_col(n_preds), any_col(n_anys);
-    for (int i = 0; i < n_preds; i++) pred_col[i] = col_of(preds[i].column);
-    for (int i = 0; i < n_anys; i++) any_col[i] = col_of(anys[i].column);
-    const int lineage_col = spec->n_deleted_file_ids > 0 ? col_of("_data_file_id") : -1;
-    std::vector<Buf<uint8_t>> bound_bytes;
-    std::vector<ResolvedPredicate> rps(n_preds);
+    for (int i = 0; i < n_preds; i++) pred_col[i] = column_index(&cols, preds[i].column);
+    for (int i = 0; i < n_anys; i++) any_col[i] = column_index(&cols, anys[i].column);
+    const int lineage_col = spec->n_deleted_file_ids > 0 ? column_index(&cols, "_data_file_id") : -1;
+    PredUploads uploads;
     // The key's set (when a term is on the key, or for pruning): the predicates on the key and every term on it,
-    // intersected.  Without a term on the key its one range per file is intersect_ranges' result, as without terms.
+    // intersected.
     auto on_key_name = [&](const char* column) { return spec->key_column && strcmp(column, spec->key_column) == 0; };
     bool key_terms = false;
     for (int i = 0; i < n_anys; i++) key_terms = key_terms || on_key_name(anys[i].column);
     auto key_set_of = [&](const DevColumn& kc) {
       const bool str = kc.type == HS_TYPE_STRING;
-      SetRange all;  // every value: an open string range, the whole encoded domain
-      if (!str) all.has_lo = all.has_hi = true, all.hi = encoded_max(kc.type);
-      RangeSet s{all};
+      RangeSet s{SetRange{}};  // every value
       for (int i = 0; i < n_preds; i++)
-        if (on_key_name(preds[i].column)) {
-          ResolvedPredicate rp;
-          const PredRange r = resolve_predicate(ctx, preds[i], kc, &bound_bytes, &rp);
-          s = intersect_sets(str, s, RangeSet{set_range_of(kc.type, r, rp.lo_host, rp.lo_len, rp.hi_host, rp.hi_len)});
-        }
+        if (on_key_name(preds[i].column)) s = intersect_sets(str, s, RangeSet{resolve_range(preds[i], pred_column(kc))});
       for (int i = 0; i < n_anys; i++)
-        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, resolve_any(ctx, anys[i], kc));
+        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, resolve_term(anys[i], pred_column(kc)));
       return s;
     };
     // Bucket pruning: a key whose windows are points lives in the files of the points' buckets only
@@ -1370,31 +1081,6 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     if (legacy && try_sorted && t.cols[0].type != HS_TYPE_STRING && t.cols[0].type != HS_TYPE_INT64 && t.cols[0].type != HS_TYPE_INT32)
       fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
     const int64_t n = t.nrows;
-    auto resolve = [&](int i) {
-      rps[i].col = pred_col[i];
-      rps[i].r = resolve_predicate(ctx, preds[i], t.cols[pred_col[i]], &bound_bytes, &rps[i]);
-    };
-    std::vector<Buf<PredRange>> any_sets(n_anys);
-    auto residual_set = [&](bool skip_key) {
-      PredSet ps;
-      for (int i = 0; i < n_preds; i++) {
-        if (skip_key && pred_col[i] == 0) continue;
-        const DevColumn& c = t.cols[rps[i].col];
-        ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, rps[i].r};
-      }
-      for (int i = 0; i < n_anys; i++) {
-        if (skip_key && any_col[i] == 0) continue;
-        const DevColumn& c = t.cols[any_col[i]];
-        const RangeSet s = resolve_any(ctx, anys[i], c);
-        upload_set(ctx, c.type, s, &any_sets[i], &bound_bytes);
-        PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
-        d.r.type = c.type;
-        d.set = any_sets[i].get();
-        d.n_set = (int64_t)s.size();
-        ps.p[ps.n++] = d;
-      }
-      return ps;
-    };
     StageTimer t_scan(ctx);
     t_scan.start();
     Buf<uint32_t> idx;
@@ -1406,43 +1092,41 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       t = std::move(full);
     }
     if (sorted) {
-      // K7: two binary searches per (file, range of the key): the intersection of the predicates on the key, or the
-      // disjoint ranges of the key's set
+      // K7: two binary searches per (file, range of the key)
       const int ktype = t.cols[0].type;
       if (ktype < HS_TYPE_INT32 || ktype > HS_TYPE_STRING || ktype == HS_TYPE_BOOL)
         fail(HS_EUNSUPPORTED, "filter scan: the sorted key column '%s' must be int32 / int64 / float / double / string", cols[0].c_str());
       int on_key = 0;
-      for (int i = 0; i < n_preds; i++)
-        if (pred_col[i] == 0) resolve(i), on_key++;
+      for (int i = 0; i < n_preds; i++) on_key += pred_col[i] == 0;
       for (int i = 0; i < n_anys; i++) on_key += any_col[i] == 0;
       const int nseg = n_files;
       std::vector<uint64_t> seg(nseg + 1);
       for (int f = 0; f <= nseg; f++) seg[f] = (uint64_t)t.file_row_begin[f];
       Buf<uint64_t> d_seg(ctx, nseg + 1);
       copy_h2d(ctx, d_seg.get(), seg.data(), 8 * (nseg + 1));
-      Buf<PredRange> d_ranges;
-      std::vector<uint2> work;
-      if (key_terms || pruned) {
-        if (!have_key_set) key_set = key_set_of(t.cols[0]);
-        upload_set(ctx, ktype, key_set, &d_ranges, &bound_bytes);
-        work.reserve((size_t)nseg * (pruned ? 1 : key_set.size()));
-        for (int f = 0; f < nseg; f++)
-          for (size_t r = 0; r < key_set.size(); r++)
-            if (!pruned || point_bucket[r] == kept_bucket[f]) work.push_back(make_uint2((unsigned)f, (unsigned)r));
-      } else {
-        std::vector<ResolvedPredicate> on_key_preds;
+      // The key's ranges: its set when a term is on the key or the files are pruned; otherwise the intersection of the
+      // predicates on the key, one range kept even when it is empty, so that every file still decodes the page its
+      // empty window falls on (below)
+      if (!(key_terms || pruned)) {
+        SetRange r;
         for (int i = 0; i < n_preds; i++)
-          if (pred_col[i] == 0) on_key_preds.push_back(rps[i]);
-        const PredRange key_range = intersect_ranges(ktype, on_key_preds);
-        d_ranges.alloc(ctx, 1);
-        copy_h2d(ctx, d_ranges.get(), &key_range, sizeof key_range);
-        for (int f = 0; f < nseg; f++) work.push_back(make_uint2((unsigned)f, 0u));
+          if (pred_col[i] == 0) r = intersect_range(ktype == HS_TYPE_STRING, r, resolve_range(preds[i], pred_column(t.cols[0])));
+        key_set = RangeSet{r};
+      } else if (!have_key_set) {
+        key_set = key_set_of(t.cols[0]);
       }
+      upload_set(ctx, ktype, key_set, &uploads, true);
+      const PredRange* d_ranges = uploads.sets.back().get();
+      std::vector<uint2> work;
+      work.reserve((size_t)nseg * (pruned ? 1 : key_set.size()));
+      for (int f = 0; f < nseg; f++)
+        for (size_t r = 0; r < key_set.size(); r++)
+          if (!pruned || point_bucket[r] == kept_bucket[f]) work.push_back(make_uint2((unsigned)f, (unsigned)r));
       const int64_t nwork = (int64_t)work.size();
       Buf<uint2> d_work(ctx, std::max<int64_t>(1, nwork));
       Buf<int64_t> d_bounds(ctx, 2 * std::max<int64_t>(1, nwork));
       if (nwork) copy_h2d(ctx, d_work.get(), work.data(), sizeof(uint2) * nwork);
-      launch_range_bounds(ctx, t.cols[0].data.get(), ktype, d_ranges.get(), d_seg.get(), d_work.get(), nwork, d_bounds.get());
+      launch_range_bounds(ctx, t.cols[0].data.get(), ktype, d_ranges, d_seg.get(), d_work.get(), nwork, d_bounds.get());
       std::vector<int64_t> bounds(2 * std::max<int64_t>(1, nwork));
       if (nwork) copy_d2h(ctx, bounds.data(), d_bounds.get(), 16 * nwork);
       sync_stream(ctx);
@@ -1494,17 +1178,18 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       n_out = n_cand;
       if (on_key < n_preds + n_anys) {
         // residual: the predicates on other columns, over the window rows, compacted through the candidate list
-        for (int i = 0; i < n_preds; i++)
-          if (pred_col[i] != 0) resolve(i);
+        PredSet residual;
+        add_predicates(ctx, t, preds, pred_col, anys, any_col, 0, &residual, &uploads);
         Buf<uint32_t> kept_rows;
-        n_out = select_rows(ctx, residual_set(true), idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
+        n_out = select_rows(ctx, residual, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
         idx = std::move(kept_rows);
       }
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
-      for (int i = 0; i < n_preds; i++) resolve(i);
+      PredSet ps;
+      add_predicates(ctx, t, preds, pred_col, anys, any_col, -1, &ps, &uploads);
       const int64_t* file_ids = lineage_col >= 0 ? (const int64_t*)t.cols[lineage_col].data.get() : nullptr;
-      n_out = select_rows(ctx, residual_set(false), nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
+      n_out = select_rows(ctx, ps, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
     }
     sync_stream(ctx);
     t_scan.stop();
@@ -1523,75 +1208,6 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
   if (stats) *stats = st;
   if (rc == HS_OK) *out = res.release();
   return rc;
-}
-
-// The refusals of a predicate list that need no data (hs_filter_scan_where, hs_bucket_join_where): HS_OK or the code,
-// with stats zeroed and the message in err.  bounds_in_spec: hs_filter_scan_where was also given the bounds of
-// hs_filter_scan.
-static int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_in_spec, hs_stats* stats, char* err,
-                            size_t errlen) {
-  auto refuse = [&](int code, const char* msg, const char* what) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, msg, what);
-    return code;
-  };
-  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
-  if (bounds_in_spec) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
-  for (int i = 0; i < n_preds; i++) {
-    const hs_predicate& p = preds[i];
-    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
-    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
-    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING &&
-        p.literal_type != HS_TYPE_DECIMAL)
-      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
-  }
-  return HS_OK;
-}
-
-// The same for the disjunction terms beside n_preds predicates: their counts, arrays, offsets and string lengths.
-static int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_stats* stats, char* err, size_t errlen) {
-  char msg[256];
-  auto refuse = [&](int code) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "%s", msg);
-    return code;
-  };
-  if (n_anys < 0 || (n_anys > 0 && !anys)) return snprintf(msg, sizeof msg, "filter scan: bad term array"), refuse(HS_EINVAL);
-  if (n_preds + n_anys > kMaxPredicates)
-    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
-  for (int i = 0; i < n_anys; i++) {
-    const hs_predicate_any& a = anys[i];
-    if (!a.column) return snprintf(msg, sizeof msg, "filter scan: term without a column"), refuse(HS_EINVAL);
-    const char* c = a.column;
-    if (a.n_values < 0 || a.n_ranges < 0 || (a.n_ranges > 0 && !a.ranges))
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has a bad value or range array", c), refuse(HS_EINVAL);
-    if (a.n_values + a.n_ranges > (1ll << 24))
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than 2^24 values and ranges", c), refuse(HS_EUNSUPPORTED);
-    if (a.literal_type != HS_TYPE_INT64 && a.literal_type != HS_TYPE_DOUBLE && a.literal_type != HS_TYPE_STRING &&
-        a.literal_type != HS_TYPE_DECIMAL)
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has an unknown literal type", c), refuse(HS_EINVAL);
-    if (a.n_values > 0) {
-      const bool missing = a.literal_type == HS_TYPE_STRING ? (!a.values_offsets || (!a.values_bytes && a.values_offsets[a.n_values] != a.values_offsets[0]))
-                                                            : (a.literal_type == HS_TYPE_DOUBLE ? !a.values_f : !a.values_i);
-      if (missing) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has no value array", c), refuse(HS_EINVAL);
-      if (a.literal_type == HS_TYPE_STRING)
-        for (int64_t k = 0; k < a.n_values; k++) {
-          if (a.values_offsets[k + 1] < a.values_offsets[k])
-            return snprintf(msg, sizeof msg, "filter scan: term on '%s' has descending value offsets", c), refuse(HS_EINVAL);
-          if (a.values_offsets[k + 1] - a.values_offsets[k] > kMaxStringLen)
-            return snprintf(msg, sizeof msg, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c), refuse(HS_EUNSUPPORTED);
-        }
-    }
-    for (int r = 0; r < a.n_ranges; r++) {
-      if (a.ranges[r].column && strcmp(a.ranges[r].column, c) != 0)
-        return snprintf(msg, sizeof msg, "filter scan: a range of the term on '%s' names another column", c), refuse(HS_EINVAL);
-      hs_predicate q = a.ranges[r];
-      q.column = c;
-      const int rc = check_predicates(&q, 1, false, stats, err, errlen);
-      if (rc != HS_OK) return rc;
-    }
-  }
-  return HS_OK;
 }
 
 extern "C" {
@@ -1618,11 +1234,7 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
 
 int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
                          hs_stats* stats, char* err, size_t errlen) {
-  if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds)) return HS_EINVAL;
-  *out = nullptr;
-  const int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
-  if (rc != HS_OK) return rc;
-  return filter_scan_core(ctx, spec, preds, n_preds, false, nullptr, 0, nullptr, 0, out, stats, err, errlen);
+  return hs_filter_scan_any(ctx, spec, preds, n_preds, nullptr, 0, nullptr, 0, out, stats, err, errlen);
 }
 
 int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
@@ -1752,15 +1364,9 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
         if (std::find(cols.begin(), cols.end(), keys[k]) != cols.end()) fail(HS_EINVAL, "bucket join: key column '%s' given twice", keys[k]);
         cols.push_back(keys[k]);
       }
-      auto col_of = [&](const std::string& nm) {
-        auto it = std::find(cols.begin(), cols.end(), nm);
-        if (it != cols.end()) return (int)(it - cols.begin());
-        cols.push_back(nm);
-        return (int)cols.size() - 1;
-      };
-      for (int i = 0; i < n_proj; i++) proj_idx->push_back(col_of(proj[i]));
-      for (int i = 0; i < n_preds; i++) pred_idx->push_back(col_of(preds[i].column));
-      for (int i = 0; i < n_anys; i++) any_idx->push_back(col_of(anys[i].column));
+      for (int i = 0; i < n_proj; i++) proj_idx->push_back(column_index(&cols, proj[i]));
+      for (int i = 0; i < n_preds; i++) pred_idx->push_back(column_index(&cols, preds[i].column));
+      for (int i = 0; i < n_anys; i++) any_idx->push_back(column_index(&cols, anys[i].column));
       return cols;
     };
     std::vector<int> lproj, rproj, lpred, rpred, lany, rany;
@@ -1785,8 +1391,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       }
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
     // side selection: IS NOT NULL on the nullable key columns, then the side's predicates
-    std::vector<Buf<uint8_t>> bound_bytes;
-    std::vector<Buf<PredRange>> any_sets;
+    PredUploads uploads;
     auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, const hs_predicate_any* anys,
                           const std::vector<int>& any_idx) {
       PredSet ps;
@@ -1798,26 +1403,9 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
           ps.p[ps.n++] = d;
         }
       }
-      for (size_t i = 0; i < pred_idx.size(); i++) {
-        const DevColumn& c = s.t.cols[pred_idx[i]];
-        ResolvedPredicate rp;
-        const PredRange r = resolve_predicate(ctx, preds[i], c, &bound_bytes, &rp);
-        ps.p[ps.n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, r};
-      }
-      for (size_t i = 0; i < any_idx.size(); i++) {
-        const DevColumn& c = s.t.cols[any_idx[i]];
-        const RangeSet set = resolve_any(ctx, anys[i], c);
-        any_sets.emplace_back();
-        upload_set(ctx, c.type, set, &any_sets.back(), &bound_bytes);
-        PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
-        d.r.type = c.type;
-        d.set = any_sets.back().get();
-        d.n_set = (int64_t)set.size();
-        ps.p[ps.n++] = d;
-      }
+      add_predicates(ctx, s.t, preds, pred_idx, anys, any_idx, -1, &ps, &uploads);
       return ps;
     };
-    any_sets.reserve(n_left_anys + n_right_anys);
     const PredSet lps = side_preds(L, left_preds, lpred, left_anys, lany), rps = side_preds(R, right_preds, rpred, right_anys, rany);
     StageTimer t_sel(ctx);
     t_sel.start();
@@ -1886,23 +1474,8 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                          int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate* right_preds,
                          int32_t n_right_preds, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
-  if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
-      (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
-    return HS_EINVAL;
-  *out = nullptr;
-  auto refuse = [&](int code, const char* msg) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "%s", msg);
-    return code;
-  };
-  if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
-  if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
-  if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
-  int rc = check_predicates(left_preds, n_left_preds, false, stats, err, errlen);
-  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
-  if (rc != HS_OK) return rc;
-  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, nullptr, 0,
-                          nullptr, 0, false, out, stats, err, errlen);
+  return hs_bucket_join_any(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, nullptr, 0, right_preds, n_right_preds,
+                            nullptr, 0, out, stats, err, errlen);
 }
 
 int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,

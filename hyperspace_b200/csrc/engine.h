@@ -8,6 +8,7 @@
 #include "hs_common.h"
 #include "kernels.h"
 #include "parquet_meta.h"
+#include "spark_types.h"
 
 namespace hs {
 
@@ -41,12 +42,6 @@ struct DevColumn {
 };
 
 constexpr int kMaxCarried = 4;  // codes per record
-
-// Spark types that ride on an int32 / int64 column (DevColumn::schema holds the leaf the index file declares)
-inline bool is_decimal(const pq::SchemaColumn& s) { return s.converted_type == pq::CT_DECIMAL; }
-inline bool is_timestamp(const pq::SchemaColumn& s) {
-  return s.type == pq::INT64 && (s.converted_type == pq::CT_TIMESTAMP_MICROS || s.converted_type == pq::CT_TIMESTAMP_MILLIS);
-}
 
 // The hash and partition kernels' view of a key column.  The one place that decides how a key value is hashed: Spark
 // hashes a decimal(p <= 9) -- an int32 here -- as hashLong of the sign-extended unscaled value.

@@ -1,0 +1,358 @@
+// predicates.h -- filter predicates resolved on the host, with Spark 3.1's binary-comparison coercion: every predicate
+// (hs_predicate) and disjunction term (hs_predicate_any) on a column becomes ranges of the column's values (SetRange),
+// which api.cu uploads as the kernels' PredRanges.  Host code only: no CUDA call; tests/native/predicates.cu runs it.
+//
+// Numeric columns get inclusive ranges of sort_encode values, found by binary search over the encoded domain with the
+// comparison Spark would evaluate -- in the wider of the column's and the literal's types (int < long < float < double),
+// with SQLOrderingUtil's order (NaN == NaN, NaN above +inf, -0.0 == 0.0).  Every cast on the way (int/long -> double,
+// float -> double, long -> float) is monotone, so the rows satisfying a bound are one end of the encoded order, and
+// rounding casts (long -> double beyond 2^53) are followed exactly.  String columns keep the bounds' bytes and strictness.
+#pragma once
+#include <algorithm>
+#include <cstdint>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "device_utils.cuh"
+#include "spark_types.h"
+
+namespace hs {
+
+// A column as the predicates see it: HS storage type, the leaf the index file declares (decimal scale, timestamp), name.
+struct PredColumn {
+  int type;
+  const pq::SchemaColumn& schema;
+  const std::string& name;
+};
+
+template <typename F>
+inline int spark_compare(F a, F b) {  // SQLOrderingUtil.compareDoubles / compareFloats
+  const bool na = a != a, nb = b != b;
+  if (na || nb) return na == nb ? 0 : (na ? 1 : -1);
+  return a < b ? -1 : (a > b ? 1 : 0);
+}
+
+// the column value whose sort_encode is e, compared with the literal (lit_i when lit_type is HS_TYPE_INT64 or
+// HS_TYPE_DECIMAL, else lit_f).  Integer columns and integer / decimal literals compare as decimals of their scales
+// (col_scale: the column's, 0 unless it is a decimal; lit_scale: the literal's, 0 for HS_TYPE_INT64).
+inline int compare_encoded(int col_type, uint64_t e, int lit_type, int64_t lit_i, double lit_f, int col_scale, int lit_scale) {
+  const bool lit_long = lit_type == HS_TYPE_INT64 || lit_type == HS_TYPE_DECIMAL;
+  switch (col_type) {
+    case HS_TYPE_INT32:
+    case HS_TYPE_INT64: {
+      const int64_t v = col_type == HS_TYPE_INT32 ? (int64_t)(int32_t)((uint32_t)e ^ 0x80000000u) : (int64_t)(e ^ 0x8000000000000000ull);
+      if (lit_long) return compare_scaled(v, col_scale, lit_i, lit_scale);
+      return spark_compare((double)v, lit_f);
+    }
+    case HS_TYPE_FLOAT: {
+      const uint32_t u = (uint32_t)e, bits = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+      float f;
+      memcpy(&f, &bits, 4);
+      return lit_long ? spark_compare(f, (float)lit_i) : spark_compare((double)f, lit_f);
+    }
+    default: {
+      const uint64_t bits = (e & 0x8000000000000000ull) ? (e & 0x7fffffffffffffffull) : ~e;
+      double d;
+      memcpy(&d, &bits, 8);
+      return spark_compare(d, lit_long ? (double)lit_i : lit_f);
+    }
+  }
+}
+
+// encoded values of a column type, lowest to highest (floating point: -inf .. the NaNs above +inf)
+inline void encoded_domain(int col_type, uint64_t* lo, uint64_t* hi) {
+  switch (col_type) {
+    case HS_TYPE_INT32: *lo = 0, *hi = 0xffffffffull; return;
+    case HS_TYPE_INT64: *lo = 0, *hi = ~0ull; return;
+    case HS_TYPE_FLOAT: *lo = 0x007fffffull, *hi = 0xffffffffull; return;   // ~bits(-inf)
+    default: *lo = 0x000fffffffffffffull, *hi = ~0ull; return;             // ~bits(-inf)
+  }
+}
+
+// One range of a column's values.  Numeric: inclusive sort_encode bounds (the strictness is resolved into them; lo > hi
+// is empty); strings: the bounds' bytes with their strictness.  A missing bound is open.
+struct SetRange {
+  bool has_lo = false, has_hi = false, lo_strict = false, hi_strict = false;
+  uint64_t lo = 0, hi = 0;
+  std::string lo_b, hi_b;
+};
+// a term's ranges; normalised (normalise_set): sorted, disjoint, none empty
+using RangeSet = std::vector<SetRange>;
+
+// One predicate on column c as one range, possibly empty (numeric: lo = 1, hi = 0).  p.literal_type < 0 (hs_filter_scan):
+// the literal type follows the column -- int64 bounds on an integer column, bytes on a string column.
+inline SetRange resolve_range(const hs_predicate& p, const PredColumn& c) {
+  const bool str_col = c.type == HS_TYPE_STRING;
+  int lit = p.literal_type;
+  if (lit < 0) {
+    if (!str_col && c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64) fail(HS_EUNSUPPORTED, "filter scan: key column must be int32 / int64 / string");
+    lit = str_col ? HS_TYPE_STRING : HS_TYPE_INT64;
+  }
+  if (c.type == HS_TYPE_BOOL) fail(HS_EUNSUPPORTED, "filter scan: predicates on the boolean column '%s' are not handled", c.name.c_str());
+  if (c.type < HS_TYPE_INT32 || c.type > HS_TYPE_STRING) fail(HS_EUNSUPPORTED, "filter scan: column '%s' has an unhandled type", c.name.c_str());
+  if (str_col != (lit == HS_TYPE_STRING))
+    fail(HS_EUNSUPPORTED, "filter scan: a %s literal cannot be compared with the %s column '%s'", lit == HS_TYPE_STRING ? "string" : "numeric",
+         str_col ? "string" : "numeric", c.name.c_str());
+  // Spark compares these in double: the caller keeps the conjunct in a Filter of its own
+  const bool dec_col = is_decimal(c.schema), ts_col = is_timestamp(c.schema);
+  if (lit == HS_TYPE_DOUBLE && (dec_col || ts_col))
+    fail(HS_EUNSUPPORTED, "filter scan: a double literal cannot be compared with the %s column '%s'", dec_col ? "decimal" : "timestamp",
+         c.name.c_str());
+  if (lit == HS_TYPE_DECIMAL && (ts_col || (c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64)))
+    fail(HS_EUNSUPPORTED, "filter scan: a decimal literal cannot be compared with the %s column '%s'",
+         ts_col ? "timestamp" : (c.type == HS_TYPE_STRING ? "string" : "floating-point"), c.name.c_str());
+  if (lit == HS_TYPE_DECIMAL && (p.scale < 0 || p.scale > 38))
+    fail(HS_EINVAL, "filter scan: decimal literal on '%s' has scale %d", c.name.c_str(), p.scale);
+  const int col_scale = dec_col ? c.schema.scale : 0, lit_scale = lit == HS_TYPE_DECIMAL ? p.scale : 0;
+  SetRange r;
+  r.has_lo = p.has_lo != 0;
+  r.has_hi = p.has_hi != 0;
+  if (str_col) {
+    if ((p.has_lo && p.lo_len && !p.lo_bytes) || (p.has_hi && p.hi_len && !p.hi_bytes))
+      fail(HS_EINVAL, "filter scan: string column '%s' needs lo_bytes / hi_bytes", c.name.c_str());
+    if (p.lo_len > kMaxStringLen || p.hi_len > kMaxStringLen) fail(HS_EUNSUPPORTED, "string bound longer than 65535 bytes");
+    if (r.has_lo && p.lo_len) r.lo_b.assign((const char*)p.lo_bytes, p.lo_len);
+    if (r.has_hi && p.hi_len) r.hi_b.assign((const char*)p.hi_bytes, p.hi_len);
+    r.lo_strict = r.has_lo && p.lo_strict;
+    r.hi_strict = r.has_hi && p.hi_strict;
+    return r;
+  }
+  uint64_t emin, emax;
+  encoded_domain(c.type, &emin, &emax);
+  auto cmp = [&](uint64_t e, bool hi_side) {
+    return compare_encoded(c.type, e, lit, hi_side ? p.hi_i : p.lo_i, hi_side ? p.hi_f : p.lo_f, col_scale, lit_scale);
+  };
+  bool empty = false;
+  if (r.has_lo) {  // smallest e with value >= lo (> lo when strict)
+    const int t = p.lo_strict ? 1 : 0;
+    if (cmp(emax, false) < t) {
+      empty = true;
+    } else {
+      uint64_t a = emin, b = emax;
+      while (a < b) {
+        const uint64_t mid = a + ((b - a) >> 1);
+        if (cmp(mid, false) >= t) b = mid;
+        else a = mid + 1;
+      }
+      r.lo = a;
+    }
+  }
+  if (r.has_hi) {  // largest e with value <= hi (< hi when strict)
+    const int t = p.hi_strict ? -1 : 0;
+    if (cmp(emin, true) > t) {
+      empty = true;
+    } else {
+      uint64_t a = emin, b = emax;
+      while (a < b) {
+        const uint64_t mid = b - ((b - a) >> 1);
+        if (cmp(mid, true) <= t) a = mid;
+        else b = mid - 1;
+      }
+      r.hi = a;
+    }
+  }
+  if (empty) r.has_lo = r.has_hi = true, r.lo = 1, r.hi = 0;
+  return r;
+}
+
+inline int host_string_compare(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  const int c = memcmp(a, b, std::min(la, lb));
+  if (c) return c < 0 ? -1 : 1;
+  return la == lb ? 0 : (la < lb ? -1 : 1);
+}
+inline int set_bound_cmp(bool str, uint64_t a, const std::string& as, uint64_t b, const std::string& bs) {
+  if (str) return host_string_compare((const uint8_t*)as.data(), (uint32_t)as.size(), (const uint8_t*)bs.data(), (uint32_t)bs.size());
+  return a < b ? -1 : (a > b ? 1 : 0);
+}
+inline bool set_range_empty(bool str, const SetRange& r) {
+  if (!r.has_lo || !r.has_hi) return false;
+  const int c = set_bound_cmp(str, r.lo, r.lo_b, r.hi, r.hi_b);
+  return c > 0 || (c == 0 && (r.lo_strict || r.hi_strict));
+}
+inline bool lo_before(bool str, const SetRange& a, const SetRange& b) {  // a starts below b
+  if (!a.has_lo || !b.has_lo) return !a.has_lo && b.has_lo;
+  const int c = set_bound_cmp(str, a.lo, a.lo_b, b.lo, b.lo_b);
+  return c < 0 || (c == 0 && !a.lo_strict && b.lo_strict);
+}
+inline bool hi_before(bool str, const SetRange& a, const SetRange& b) {  // a ends below b
+  if (!a.has_hi || !b.has_hi) return a.has_hi && !b.has_hi;
+  const int c = set_bound_cmp(str, a.hi, a.hi_b, b.hi, b.hi_b);
+  return c < 0 || (c == 0 && a.hi_strict && !b.hi_strict);
+}
+
+// the values in both a and b: the later lower bound and the earlier upper bound; the result may be empty
+inline SetRange intersect_range(bool str, const SetRange& a, const SetRange& b) {
+  const SetRange& lo = lo_before(str, a, b) ? b : a;
+  const SetRange& hi = hi_before(str, a, b) ? a : b;
+  SetRange r;
+  r.has_lo = lo.has_lo, r.lo = lo.lo, r.lo_b = lo.lo_b, r.lo_strict = lo.lo_strict;
+  r.has_hi = hi.has_hi, r.hi = hi.hi, r.hi_b = hi.hi_b, r.hi_strict = hi.hi_strict;
+  return r;
+}
+
+// sorts, drops empty ranges and merges overlapping and adjacent ones
+inline void normalise_set(bool str, RangeSet* rs) {
+  rs->erase(std::remove_if(rs->begin(), rs->end(), [&](const SetRange& r) { return set_range_empty(str, r); }), rs->end());
+  std::sort(rs->begin(), rs->end(), [&](const SetRange& a, const SetRange& b) { return lo_before(str, a, b); });
+  RangeSet out;
+  for (SetRange& r : *rs) {
+    bool joins = false;
+    if (!out.empty()) {
+      const SetRange& cur = out.back();
+      if (!cur.has_hi || !r.has_lo) joins = true;
+      else if (!str) joins = r.lo <= cur.hi || r.lo - 1 == cur.hi;  // r.lo > cur.hi >= 0 in the second test
+      else {
+        const int c = set_bound_cmp(true, r.lo, r.lo_b, cur.hi, cur.hi_b);
+        joins = c < 0 || (c == 0 && !(r.lo_strict && cur.hi_strict));
+      }
+    }
+    if (!joins) {
+      out.push_back(std::move(r));
+    } else if (hi_before(str, out.back(), r)) {
+      SetRange& cur = out.back();
+      cur.has_hi = r.has_hi, cur.hi = r.hi, cur.hi_b = std::move(r.hi_b), cur.hi_strict = r.hi_strict;
+    }
+  }
+  *rs = std::move(out);
+}
+
+// the values in both normalised sets, normalised
+inline RangeSet intersect_sets(bool str, const RangeSet& a, const RangeSet& b) {
+  RangeSet out;
+  size_t i = 0, j = 0;
+  while (i < a.size() && j < b.size()) {
+    SetRange r = intersect_range(str, a[i], b[j]);
+    if (!set_range_empty(str, r)) out.push_back(std::move(r));
+    if (hi_before(str, a[i], b[j])) i++;
+    else j++;
+  }
+  return out;
+}
+
+// Every value and range of the term on column c, as one normalised set; values that match nothing (int_col IN (2.5))
+// are dropped.  The refusals are resolve_range's, for the list's literal type and for every range.
+inline RangeSet resolve_term(const hs_predicate_any& a, const PredColumn& c) {
+  const bool str = c.type == HS_TYPE_STRING;
+  RangeSet out;
+  hs_predicate p;
+  memset(&p, 0, sizeof p);
+  p.column = a.column;
+  p.literal_type = a.literal_type;
+  p.scale = a.scale;
+  p.has_lo = p.has_hi = 1;
+  const bool lit_long = a.literal_type == HS_TYPE_INT64 || a.literal_type == HS_TYPE_DECIMAL;
+  const int col_scale = is_decimal(c.schema) ? c.schema.scale : 0, lit_scale = a.literal_type == HS_TYPE_DECIMAL ? a.scale : 0;
+  if (a.n_values > 0) resolve_range(p, c);  // the list's refusals, once
+  out.reserve((size_t)a.n_values + a.n_ranges);
+  for (int64_t k = 0; k < a.n_values; k++) {
+    SetRange s;
+    if (str) {
+      const uint64_t b = a.values_offsets[k], e = a.values_offsets[k + 1];
+      s.has_lo = s.has_hi = true;
+      s.lo_b.assign((const char*)a.values_bytes + b, e - b);
+      s.hi_b = s.lo_b;
+      out.push_back(std::move(s));
+      continue;
+    }
+    // an integer column against an integer literal at its own scale equals at most one value: the literal's own encoding,
+    // confirmed by the comparison; everything else goes through the binary searches of resolve_range
+    if (lit_long && col_scale == lit_scale && (c.type == HS_TYPE_INT64 || (c.type == HS_TYPE_INT32 && a.values_i[k] == (int32_t)a.values_i[k]))) {
+      const uint64_t e = c.type == HS_TYPE_INT32 ? (uint64_t)((uint32_t)(int32_t)a.values_i[k] ^ 0x80000000u)
+                                                 : (uint64_t)a.values_i[k] ^ 0x8000000000000000ull;
+      if (compare_encoded(c.type, e, a.literal_type, a.values_i[k], 0.0, col_scale, lit_scale) == 0) {
+        s.has_lo = s.has_hi = true;
+        s.lo = s.hi = e;
+        out.push_back(std::move(s));
+        continue;
+      }
+    }
+    if (lit_long) p.lo_i = p.hi_i = a.values_i[k];
+    else p.lo_f = p.hi_f = a.values_f[k];
+    out.push_back(resolve_range(p, c));
+  }
+  for (int32_t r = 0; r < a.n_ranges; r++) {
+    hs_predicate q = a.ranges[r];
+    q.column = a.column;
+    out.push_back(resolve_range(q, c));
+  }
+  normalise_set(str, &out);
+  return out;
+}
+
+inline bool set_is_points(bool str, const RangeSet& s) {
+  for (const SetRange& r : s) {
+    if (!r.has_lo || !r.has_hi) return false;
+    if (str ? (r.lo_b != r.hi_b || r.lo_strict || r.hi_strict) : r.lo != r.hi) return false;
+  }
+  return true;
+}
+
+// The refusals of a predicate list that need no data: HS_OK or the code, with stats zeroed and the message in err.
+// bounds_in_spec: hs_filter_scan_where was also given the bounds of hs_filter_scan.
+inline int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_in_spec, hs_stats* stats, char* err, size_t errlen) {
+  auto refuse = [&](int code, const char* msg, const char* what) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, msg, what);
+    return code;
+  };
+  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
+  if (bounds_in_spec) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
+  for (int i = 0; i < n_preds; i++) {
+    const hs_predicate& p = preds[i];
+    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
+    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
+    if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING &&
+        p.literal_type != HS_TYPE_DECIMAL)
+      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
+  }
+  return HS_OK;
+}
+
+// The same for the disjunction terms beside n_preds predicates: their counts, arrays, offsets and string lengths.
+inline int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_stats* stats, char* err, size_t errlen) {
+  char msg[256];
+  auto refuse = [&](int code) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "%s", msg);
+    return code;
+  };
+  if (n_anys < 0 || (n_anys > 0 && !anys)) return snprintf(msg, sizeof msg, "filter scan: bad term array"), refuse(HS_EINVAL);
+  if (n_preds + n_anys > kMaxPredicates)
+    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
+  for (int i = 0; i < n_anys; i++) {
+    const hs_predicate_any& a = anys[i];
+    if (!a.column) return snprintf(msg, sizeof msg, "filter scan: term without a column"), refuse(HS_EINVAL);
+    const char* c = a.column;
+    if (a.n_values < 0 || a.n_ranges < 0 || (a.n_ranges > 0 && !a.ranges))
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has a bad value or range array", c), refuse(HS_EINVAL);
+    if (a.n_values + a.n_ranges > (1ll << 24))
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than 2^24 values and ranges", c), refuse(HS_EUNSUPPORTED);
+    if (a.literal_type != HS_TYPE_INT64 && a.literal_type != HS_TYPE_DOUBLE && a.literal_type != HS_TYPE_STRING &&
+        a.literal_type != HS_TYPE_DECIMAL)
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has an unknown literal type", c), refuse(HS_EINVAL);
+    if (a.n_values > 0) {
+      const bool missing = a.literal_type == HS_TYPE_STRING ? (!a.values_offsets || (!a.values_bytes && a.values_offsets[a.n_values] != a.values_offsets[0]))
+                                                            : (a.literal_type == HS_TYPE_DOUBLE ? !a.values_f : !a.values_i);
+      if (missing) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has no value array", c), refuse(HS_EINVAL);
+      if (a.literal_type == HS_TYPE_STRING)
+        for (int64_t k = 0; k < a.n_values; k++) {
+          if (a.values_offsets[k + 1] < a.values_offsets[k])
+            return snprintf(msg, sizeof msg, "filter scan: term on '%s' has descending value offsets", c), refuse(HS_EINVAL);
+          if (a.values_offsets[k + 1] - a.values_offsets[k] > kMaxStringLen)
+            return snprintf(msg, sizeof msg, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c), refuse(HS_EUNSUPPORTED);
+        }
+    }
+    for (int r = 0; r < a.n_ranges; r++) {
+      if (a.ranges[r].column && strcmp(a.ranges[r].column, c) != 0)
+        return snprintf(msg, sizeof msg, "filter scan: a range of the term on '%s' names another column", c), refuse(HS_EINVAL);
+      hs_predicate q = a.ranges[r];
+      q.column = c;
+      const int rc = check_predicates(&q, 1, false, stats, err, errlen);
+      if (rc != HS_OK) return rc;
+    }
+  }
+  return HS_OK;
+}
+
+}  // namespace hs

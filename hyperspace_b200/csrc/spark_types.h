@@ -10,6 +10,12 @@
 
 namespace hs {
 
+// Spark types that ride on an int32 / int64 column (DevColumn::schema holds the leaf the index file declares)
+inline bool is_decimal(const pq::SchemaColumn& s) { return s.converted_type == pq::CT_DECIMAL; }
+inline bool is_timestamp(const pq::SchemaColumn& s) {
+  return s.type == pq::INT64 && (s.converted_type == pq::CT_TIMESTAMP_MICROS || s.converted_type == pq::CT_TIMESTAMP_MILLIS);
+}
+
 // A source column as the engine keeps it: its HS storage type, how the decoder converts the stored values (ValueConv), and
 // the Parquet leaf the index file declares for it.  Spark 3.1's TimestampType (INT96, INT64 TIMESTAMP_MILLIS / MICROS)
 // becomes int64 micros, written as INT64 TIMESTAMP_MICROS; DecimalType(p <= 18) (INT32, INT64 or FIXED_LEN_BYTE_ARRAY)

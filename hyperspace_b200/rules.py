@@ -7,7 +7,7 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan_where (K1 + K7) and hs_bucket_join_where (K1 + K8).
+Physical execution is the C ABI: hs_filter_scan_any (K1 + K7) and hs_bucket_join_any (K1 + K8).
 """
 from __future__ import annotations
 
@@ -191,8 +191,8 @@ def _terms_text(pred) -> str:
 
 
 class ScanExec:
-    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_where with
-    the filter's comparisons as its predicates, or hs_filter_scan_any when the filter has disjunction terms (isin, |)."""
+    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_any with
+    the filter's comparisons as its predicates and its disjunctions (isin, |) as its terms."""
 
     def __init__(self, session, lin: Linear, cand: Optional[Candidate]):
         self.session, self.lin, self.cand = session, lin, cand
@@ -210,13 +210,9 @@ class ScanExec:
     def _scan(self, files, key, out_cols, sorted_on_key, deleted_ids=(), buckets=None, num_buckets=0):
         preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
         terms = [a.as_native() for a in self.lin.predicate.disjunctions()] if self.lin.predicate else []
-        if terms:  # file_buckets only where the files are bucketed on the key alone
-            batch, _ = self.session.gpu.filter_scan_any(files, key, out_cols, preds, terms, sorted_on_key=sorted_on_key,
-                                                        deleted_file_ids=list(deleted_ids), file_buckets=buckets,
-                                                        num_buckets=num_buckets)
-        else:
-            batch, _ = self.session.gpu.filter_scan_where(files, key, out_cols, preds, sorted_on_key=sorted_on_key,
-                                                          deleted_file_ids=list(deleted_ids))
+        # file_buckets only where the files are bucketed on the key alone
+        batch, _ = self.session.gpu.filter_scan_any(files, key, out_cols, preds, terms, sorted_on_key=sorted_on_key,
+                                                    deleted_file_ids=list(deleted_ids), file_buckets=buckets, num_buckets=num_buckets)
         types = dict(self.lin.relation.schema)
         out = {n: spark_values(_host_column(d), types.get(n)) for n, d, _ in batch.columns}
         batch.free()
@@ -301,12 +297,8 @@ class BucketJoinExec:
             lp = self.left.predicate.conjuncts() if self.left.predicate else []
             rp = self.right.predicate.conjuncts() if self.right.predicate else []
             lt_, rt_ = ([a.as_native() for a in lin.predicate.disjunctions()] if lin.predicate else [] for lin in (self.left, self.right))
-            if lt_ or rt_:
-                batch, _ = self.session.gpu.bucket_join_any(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                            lp, rp, lt_, rt_)
-            else:
-                batch, _ = self.session.gpu.bucket_join_where(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                              lp, rp)
+            batch, _ = self.session.gpu.bucket_join_any(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                        lp, rp, lt_, rt_)
         finally:
             for t in lt + rt:
                 t.free()
