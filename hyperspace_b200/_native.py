@@ -24,6 +24,9 @@ HS_TYPE_INT32, HS_TYPE_INT64, HS_TYPE_FLOAT, HS_TYPE_DOUBLE, HS_TYPE_BOOL, HS_TY
 HS_TYPE_DECIMAL = 6  # predicate literals only: unscaled value in lo_i / hi_i, scale in `scale`
 HS_SAVE_OVERWRITE, HS_SAVE_APPEND = 0, 1
 HS_OUT_FILES, HS_OUT_HOST, HS_OUT_DEVICE = 0, 1, 2
+# hs_predicate_any.flags
+HS_TERM_NOT, HS_TERM_NULL_TRUE, HS_TERM_NULL_FALSE = 1, 2, 4
+HS_TERM_STARTS_WITH, HS_TERM_ENDS_WITH, HS_TERM_CONTAINS, HS_TERM_LIKE = 8, 16, 32, 64
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -84,7 +87,7 @@ class PredicateSpec(C.Structure):
 class PredicateAnySpec(C.Structure):
     _fields_ = [("column", C.c_char_p), ("literal_type", C.c_int32), ("scale", C.c_int32), ("n_values", C.c_int64),
                 ("values_i", C.c_void_p), ("values_f", C.c_void_p), ("values_bytes", C.c_void_p), ("values_offsets", C.c_void_p),
-                ("ranges", C.POINTER(PredicateSpec)), ("n_ranges", C.c_int32), ("reserved", C.c_int32)]
+                ("ranges", C.POINTER(PredicateSpec)), ("n_ranges", C.c_int32), ("flags", C.c_int32)]
 
 
 class JoinSpec(C.Structure):
@@ -425,12 +428,14 @@ def _one_literal_type(lo, hi):
 
 
 def _any_array(terms: Sequence[tuple]):
-    """``(column, values, ranges)`` terms -> (hs_predicate_any array, count, buffers to keep alive).  values go through
-    any_values; ranges are ``(lo, lo_strict, hi, hi_strict)`` tuples with _predicate_array's literal typing."""
+    """``(column, values, ranges)`` or ``(column, values, ranges, flags)`` terms -> (hs_predicate_any array, count, buffers
+    to keep alive).  values go through any_values; ranges are ``(lo, lo_strict, hi, hi_strict)`` tuples with
+    _predicate_array's literal typing; flags are HS_TERM_* (a pattern term lists its pattern as its one value)."""
     keep = []
     arr = (PredicateAnySpec * max(1, len(terms)))()
-    for a, (column, values, ranges) in zip(arr, terms):
+    for a, (column, values, ranges, *flags) in zip(arr, terms):
         a.column = column.encode()
+        a.flags = flags[0] if flags else 0
         lt, scale, vals = any_values(values)
         a.literal_type, a.scale, a.n_values = lt, scale, len(vals)
         if lt == HS_TYPE_STRING:
@@ -898,7 +903,7 @@ class Context:
                         ) -> Tuple[Batch, Dict[str, float]]:
         """hs_filter_scan_any: filter_scan_where's predicates AND-ed with disjunction terms ``(column, values, ranges)``:
         the row's value equals one of `values` (see any_values) or lies in one of `ranges` (``(lo, lo_strict, hi,
-        hi_strict)``).  file_buckets / num_buckets: the bucket of every file of an index bucketed on `key` alone, for
+        hi_strict)``).  A fourth element gives the term's HS_TERM_* flags: NOT, a null outcome, or a string pattern.  file_buckets / num_buckets: the bucket of every file of an index bucketed on `key` alone, for
         skipping the files a point lookup cannot hit."""
         L = load_library()
         spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)

@@ -168,7 +168,7 @@ void drop_deleted_rows(hs_ctx* ctx, Table& t, const int64_t* deleted, int ndelet
   if (lc < 0) fail(HS_EINVAL, "deleted_file_ids given but the source has no _data_file_id column (index built without lineage)");
   if (t.nrows == 0) return;
   Buf<uint32_t> idx;
-  const int64_t kept = select_rows(ctx, PredSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
+  const int64_t kept = select_rows(ctx, PredSet{}, PatternSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
   gather_table(ctx, t, idx.get(), kept);
 }
 
@@ -374,24 +374,32 @@ int hs_profile_report(hs_ctx* ctx, char* out, size_t outlen) {
   if (!ctx || !out || !outlen) return HS_EINVAL;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  std::map<std::string, std::pair<int, double>> acc;
+  struct Acc {
+    int launches = 0;
+    double ms = 0;
+    int64_t items = 0;
+  };
+  std::map<std::string, Acc> acc;
   for (auto& k : ctx->kevents) {
     float ms = 0;
     if (cudaEventElapsedTime(&ms, k.a, k.b) != cudaSuccess) {
       cudaGetLastError();
       continue;
     }
-    auto& e = acc[k.name];
-    e.first++;
-    e.second += ms;
+    Acc& e = acc[k.name];
+    e.launches++;
+    e.ms += ms;
+    e.items += k.items;
   }
   std::string s = "{";
   bool first = true;
   for (auto& kv : acc) {
     char buf[256];
-    snprintf(buf, sizeof buf, "%s\"%s\": {\"launches\": %d, \"ms\": %.6f}", first ? "" : ", ", kv.first.c_str(), kv.second.first,
-             kv.second.second);
+    snprintf(buf, sizeof buf, "%s\"%s\": {\"launches\": %d, \"ms\": %.6f", first ? "" : ", ", kv.first.c_str(), kv.second.launches,
+             kv.second.ms);
     s += buf;
+    if (kv.second.items) s += ", \"items\": " + std::to_string(kv.second.items);
+    s += "}";
     first = false;
   }
   s += "}";
@@ -870,6 +878,9 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
 struct PredUploads {
   std::vector<Buf<uint8_t>> bytes;
   std::vector<Buf<PredRange>> sets;
+  std::vector<Buf<uint16_t>> items;
+  std::vector<Buf<int32_t>> fails;
+  std::vector<Buf<PatSeg>> segs;
   std::vector<std::vector<uint8_t>> staged_bytes;
   std::vector<std::vector<PredRange>> staged_sets;
 };
@@ -913,11 +924,43 @@ static std::vector<PredRange> upload_set(hs_ctx* ctx, int type, const RangeSet& 
 
 static PredColumn pred_column(const DevColumn& c) { return PredColumn{c.type, c.schema, c.name}; }
 
+// Every term's resolution (predicates.h: resolve_any), computed once per side of a call: the key's windows and the
+// residual share it.  A term resolves against its own column, which is the same column before and after decoding.
+struct TermResolutions {
+  const hs_predicate_any* anys;
+  std::vector<std::unique_ptr<ResolvedTerm>> r;
+  TermResolutions(const hs_predicate_any* a, int n) : anys(a), r(n) {}
+  const ResolvedTerm& operator()(int i, const DevColumn& c) {
+    if (!r[i]) r[i].reset(new ResolvedTerm(resolve_any(anys[i], pred_column(c))));
+    return *r[i];
+  }
+};
+
+// The compiled pattern of term a on the string column c, uploaded for k_pattern_mask.  cp lives in the term's resolution,
+// which outlasts the copies that read it.
+static PatternDesc upload_pattern(hs_ctx* ctx, const DevColumn& c, const hs_predicate_any& a, const CompiledPattern& cp, PredUploads* up) {
+  up->items.emplace_back(ctx, std::max<size_t>(1, cp.items.size()));
+  up->fails.emplace_back(ctx, std::max<size_t>(1, cp.fail.size()));
+  up->segs.emplace_back(ctx, cp.segs.size());
+  if (!cp.items.empty()) {
+    copy_h2d(ctx, up->items.back().get(), cp.items.data(), 2 * cp.items.size());
+    copy_h2d(ctx, up->fails.back().get(), cp.fail.data(), 4 * cp.fail.size());
+  }
+  copy_h2d(ctx, up->segs.back().get(), cp.segs.data(), sizeof(PatSeg) * cp.segs.size());
+  PatternDesc d{};
+  d.refs = (const uint64_t*)c.data.get(), d.valid = c.has_nulls ? c.valid.get() : nullptr;
+  d.items = up->items.back().get(), d.fail = up->fails.back().get(), d.segs = up->segs.back().get();
+  d.nseg = (int32_t)cp.segs.size(), d.whole = cp.whole, d.negate = (a.flags & HS_TERM_NOT) != 0;
+  d.null_true = term_null_selects(a.flags);
+  return d;
+}
+
 // Appends to ps the descriptors of the predicates and terms on the columns of t (pred_col[i], any_col[i]), skipping
-// those on column skip_col: a predicate in scalar form, a term in set form.
+// those on column skip_col that its windows already decide: a predicate in scalar form, a term in set form, and to pats
+// a pattern term that is not a prefix (on skip_col too: the windows only bound its values).
 static void add_predicates(hs_ctx* ctx, const Table& t, const hs_predicate* preds, const std::vector<int>& pred_col,
-                           const hs_predicate_any* anys, const std::vector<int>& any_col, int skip_col, PredSet* ps,
-                           PredUploads* up) {
+                           TermResolutions& terms, const std::vector<int>& any_col, int skip_col, PredSet* ps,
+                           PatternSet* pats, PredUploads* up) {
   for (size_t i = 0; i < pred_col.size(); i++) {
     if (pred_col[i] == skip_col) continue;
     const DevColumn& c = t.cols[pred_col[i]];
@@ -925,14 +968,20 @@ static void add_predicates(hs_ctx* ctx, const Table& t, const hs_predicate* pred
     ps->p[ps->n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, upload_set(ctx, c.type, one, up, false)[0]};
   }
   for (size_t i = 0; i < any_col.size(); i++) {
-    if (any_col[i] == skip_col) continue;
     const DevColumn& c = t.cols[any_col[i]];
-    const RangeSet s = resolve_term(anys[i], pred_column(c));
+    const ResolvedTerm& rt = terms((int)i, c);
+    const RangeSet& s = rt.set;
+    if (!rt.exact) {
+      pats->p[pats->n++] = upload_pattern(ctx, c, terms.anys[i], rt.pattern, up);
+      continue;
+    }
+    if (any_col[i] == skip_col) continue;
     upload_set(ctx, c.type, s, up, true);
     PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
     d.r.type = c.type;
     d.set = up->sets.back().get();
     d.n_set = (int64_t)s.size();
+    d.null_true = term_null_selects(terms.anys[i].flags);
     ps->p[ps->n++] = d;
   }
 }
@@ -1026,18 +1075,23 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     for (int i = 0; i < n_anys; i++) any_col[i] = column_index(&cols, anys[i].column);
     const int lineage_col = spec->n_deleted_file_ids > 0 ? column_index(&cols, "_data_file_id") : -1;
     PredUploads uploads;
+    TermResolutions terms(anys, n_anys);
     // The key's set (when a term is on the key, or for pruning): the predicates on the key and every term on it,
     // intersected.
     auto on_key_name = [&](const char* column) { return spec->key_column && strcmp(column, spec->key_column) == 0; };
-    bool key_terms = false;
-    for (int i = 0; i < n_anys; i++) key_terms = key_terms || on_key_name(anys[i].column);
+    // a term that selects null keys (IS NULL, NOT (k <=> v)) finds them in the null key's bucket: no pruning then
+    bool key_terms = false, key_nulls = false;
+    for (int i = 0; i < n_anys; i++) {
+      key_terms = key_terms || on_key_name(anys[i].column);
+      key_nulls = key_nulls || (on_key_name(anys[i].column) && term_null_selects(anys[i].flags));
+    }
     auto key_set_of = [&](const DevColumn& kc) {
       const bool str = kc.type == HS_TYPE_STRING;
       RangeSet s{SetRange{}};  // every value
       for (int i = 0; i < n_preds; i++)
         if (on_key_name(preds[i].column)) s = intersect_sets(str, s, RangeSet{resolve_range(preds[i], pred_column(kc))});
       for (int i = 0; i < n_anys; i++)
-        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, resolve_term(anys[i], pred_column(kc)));
+        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, terms(i, kc).set);
       return s;
     };
     // Bucket pruning: a key whose windows are points lives in the files of the points' buckets only
@@ -1054,7 +1108,7 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       const bool hashable = kc.type == HS_TYPE_INT32 || kc.type == HS_TYPE_INT64 || kc.type == HS_TYPE_STRING;
       bool keyed = key_terms;
       for (int i = 0; i < n_preds; i++) keyed = keyed || on_key_name(preds[i].column);
-      if (hashable && keyed) {
+      if (hashable && keyed && !key_nulls) {
         key_set = key_set_of(kc);
         have_key_set = true;
         if (set_is_points(kc.type == HS_TYPE_STRING, key_set)) {
@@ -1096,9 +1150,9 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       const int ktype = t.cols[0].type;
       if (ktype < HS_TYPE_INT32 || ktype > HS_TYPE_STRING || ktype == HS_TYPE_BOOL)
         fail(HS_EUNSUPPORTED, "filter scan: the sorted key column '%s' must be int32 / int64 / float / double / string", cols[0].c_str());
-      int on_key = 0;
+      int on_key = 0;  // the predicates and terms the windows decide (a pattern that is not a prefix stays residual)
       for (int i = 0; i < n_preds; i++) on_key += pred_col[i] == 0;
-      for (int i = 0; i < n_anys; i++) on_key += any_col[i] == 0;
+      for (int i = 0; i < n_anys; i++) on_key += any_col[i] == 0 && terms(i, t.cols[0]).exact;
       const int nseg = n_files;
       std::vector<uint64_t> seg(nseg + 1);
       for (int f = 0; f <= nseg; f++) seg[f] = (uint64_t)t.file_row_begin[f];
@@ -1179,17 +1233,19 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       if (on_key < n_preds + n_anys) {
         // residual: the predicates on other columns, over the window rows, compacted through the candidate list
         PredSet residual;
-        add_predicates(ctx, t, preds, pred_col, anys, any_col, 0, &residual, &uploads);
+        PatternSet pats;
+        add_predicates(ctx, t, preds, pred_col, terms, any_col, 0, &residual, &pats, &uploads);
         Buf<uint32_t> kept_rows;
-        n_out = select_rows(ctx, residual, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
+        n_out = select_rows(ctx, residual, pats, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
         idx = std::move(kept_rows);
       }
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
       PredSet ps;
-      add_predicates(ctx, t, preds, pred_col, anys, any_col, -1, &ps, &uploads);
+      PatternSet pats;
+      add_predicates(ctx, t, preds, pred_col, terms, any_col, -1, &ps, &pats, &uploads);
       const int64_t* file_ids = lineage_col >= 0 ? (const int64_t*)t.cols[lineage_col].data.get() : nullptr;
-      n_out = select_rows(ctx, ps, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
+      n_out = select_rows(ctx, ps, pats, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
     }
     sync_stream(ctx);
     t_scan.stop();
@@ -1321,11 +1377,11 @@ static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file*
 
 // Side selection: keeps the rows whose key columns are all non-null and where every predicate of the side holds.  The
 // predicates run over the sorted positions as their candidate list, so the compacted rows stay in sorted order and a
-// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps is empty.
-static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, int nb) {
-  if (ps.n == 0) return;
+// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps and pats are empty.
+static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, const PatternSet& pats, int nb) {
+  if (ps.n == 0 && pats.n == 0) return;
   Buf<uint64_t> offs;
-  side->n = select_rows(ctx, ps, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
+  side->n = select_rows(ctx, ps, pats, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
   side->perm = side->kept.get();
   std::vector<uint32_t> bounds(nb + 1);
   for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
@@ -1392,8 +1448,9 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
     // side selection: IS NOT NULL on the nullable key columns, then the side's predicates
     PredUploads uploads;
-    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, const hs_predicate_any* anys,
-                          const std::vector<int>& any_idx) {
+    TermResolutions lterms(left_anys, n_left_anys), rterms(right_anys, n_right_anys);  // outlive the copies of their patterns
+    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, TermResolutions& terms,
+                          const std::vector<int>& any_idx, PatternSet* pats) {
       PredSet ps;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
@@ -1403,14 +1460,15 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
           ps.p[ps.n++] = d;
         }
       }
-      add_predicates(ctx, s.t, preds, pred_idx, anys, any_idx, -1, &ps, &uploads);
+      add_predicates(ctx, s.t, preds, pred_idx, terms, any_idx, -1, &ps, pats, &uploads);
       return ps;
     };
-    const PredSet lps = side_preds(L, left_preds, lpred, left_anys, lany), rps = side_preds(R, right_preds, rpred, right_anys, rany);
+    PatternSet lpats, rpats;
+    const PredSet lps = side_preds(L, left_preds, lpred, lterms, lany, &lpats), rps = side_preds(R, right_preds, rpred, rterms, rany, &rpats);
     StageTimer t_sel(ctx);
     t_sel.start();
-    select_join_side(ctx, &L, lps, nb);
-    select_join_side(ctx, &R, rps, nb);
+    select_join_side(ctx, &L, lps, lpats, nb);
+    select_join_side(ctx, &R, rps, rpats, nb);
     t_sel.stop();
     // the key columns in (selected) sorted order
     std::vector<Buf<uint8_t>> key_bufs;
@@ -1452,7 +1510,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
-    if (lps.n || rps.n) st.ms_exchange += t_sel.ms();
+    if (lps.n || rps.n || lpats.n || rpats.n) st.ms_exchange += t_sel.ms();
     st.rows_out = (int64_t)total_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;

@@ -144,6 +144,7 @@ struct hs_ctx {
   struct KEvent {
     const char* name;
     cudaEvent_t a, b;
+    int64_t items;  // work items of the launch, for kernels that report them (0: none)
   };
   std::vector<KEvent> kevents;
   std::vector<cudaEvent_t> event_pool;
@@ -262,7 +263,8 @@ struct DeviceOnce {
 struct KernelScope {
   hs_ctx* ctx;
   size_t idx = (size_t)-1;
-  KernelScope(hs_ctx* c, const char* name) : ctx(c) {
+  // items: the launch's work items, reported by hs_profile_report when nonzero
+  KernelScope(hs_ctx* c, const char* name, int64_t items = 0) : ctx(c) {
     if (!c->profile) return;
     auto take = [&]() {
       cudaEvent_t e;
@@ -274,7 +276,7 @@ struct KernelScope {
       }
       return e;
     };
-    hs_ctx::KEvent ke{name, take(), take()};
+    hs_ctx::KEvent ke{name, take(), take(), items};
     cudaEventRecord(ke.a, c->stream);
     idx = c->kevents.size();
     c->kevents.push_back(ke);

@@ -3,6 +3,7 @@
 #include <functional>
 
 #include "hs_common.h"
+#include "string_match.h"
 
 namespace hs {
 
@@ -413,15 +414,31 @@ struct PredRange {
 };
 struct PredDesc {
   const void* data;      // column values (string references for strings)
-  const uint8_t* valid;  // nullptr: no nulls; a null never satisfies a predicate
+  const uint8_t* valid;  // nullptr: no nulls; a null row qualifies only when null_true is set
   PredRange r;           // neither bound: the row only has to be non-null (a join side's key columns)
   // set form (a disjunction on the column): when set is not nullptr the value must lie in one of the n_set ranges at set
   // (device; ascending and disjoint, of type r.type), and r's bounds are not used
   const PredRange* set = nullptr;
   int64_t n_set = 0;
+  int32_t null_true = 0;  // a null row makes the predicate true (IS NULL, NOT (c <=> v)): predicates.h term_null_selects
 };
 struct PredSet {
   PredDesc p[kMaxPredicates + kMaxJoinKeys];  // a join side: its predicates plus one IS NOT NULL per nullable key column
+  int n = 0;
+};
+// A string pattern term the ranges cannot express (EndsWith, Contains, a LIKE that is not a prefix), compiled on the host
+// (predicates.h: compile_pattern) for pattern_matches (string_match.h): items and segs are device copies.  A non-null row
+// qualifies when the match, inverted under negate, holds; a null row when null_true is set.
+struct PatternDesc {
+  const uint64_t* refs;  // string references of the column
+  const uint8_t* valid;  // nullptr: no nulls
+  const uint16_t* items;
+  const int32_t* fail;
+  const PatSeg* segs;
+  int32_t nseg, whole, negate, null_true;
+};
+struct PatternSet {
+  PatternDesc p[kMaxPredicates];
   int n = 0;
 };
 // The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
@@ -435,6 +452,9 @@ void launch_windows_to_indices(hs_ctx* ctx, const int64_t* win, const uint64_t* 
                                uint32_t* out_idx);
 // mask[i] = every predicate of `preds` holds for row cand[i] (row i when cand is nullptr)
 void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, uint32_t* mask);
+// mask[i] = 0 where a pattern of `pats` does not hold for row cand[i] (row i when cand is nullptr); launches nothing when
+// pats is empty
+void launch_pattern_mask(hs_ctx* ctx, const PatternSet& pats, const uint32_t* cand, int64_t n, uint32_t* mask);
 // The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its
 // type's width (type[k]: HS_TYPE_INT32 / HS_TYPE_INT64, or HS_TYPE_STRING for string references).  The tuples compare
 // column by column, integers as signed values, strings in byte order.
@@ -458,10 +478,11 @@ void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* val
 void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                          const uint64_t* offsets, uint8_t* out);
 // Row selection over n candidates (cand[i], or row i when cand is nullptr): keeps those where every predicate of `preds`
-// holds and, when ndeleted > 0, whose file_ids[i] is not in the host array `deleted`.  The kept candidates go to *kept in
-// their order; returns how many there are (after a stream synchronisation).  offsets, when given, receives the exclusive
-// scan of the keep mask (n+1 entries): offsets[i] is the number of kept candidates before i.
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, const int64_t* file_ids,
-                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets = nullptr);
+// and every pattern of `pats` holds and, when ndeleted > 0, whose file_ids[i] is not in the host array `deleted`.  The kept
+// candidates go to *kept in their order; returns how many there are (after a stream synchronisation).  offsets, when given,
+// receives the exclusive scan of the keep mask (n+1 entries): offsets[i] is the number of kept candidates before i.
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const uint32_t* cand, int64_t n,
+                    const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
+                    Buf<uint64_t>* offsets = nullptr);
 
 }  // namespace hs

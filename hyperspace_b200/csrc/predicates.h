@@ -7,6 +7,9 @@
 // with SQLOrderingUtil's order (NaN == NaN, NaN above +inf, -0.0 == 0.0).  Every cast on the way (int/long -> double,
 // float -> double, long -> float) is monotone, so the rows satisfying a bound are one end of the encoded order, and
 // rounding casts (long -> double beyond 2^53) are followed exactly.  String columns keep the bounds' bytes and strictness.
+// A term's flags (HS_TERM_*) add NOT -- the complement of the set over the column's domain --, a null outcome, and string
+// patterns: a prefix is one range; other patterns are compiled for the matcher of string_match.h, their literal prefix
+// bounding the values they can match.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -16,6 +19,7 @@
 
 #include "device_utils.cuh"
 #include "spark_types.h"
+#include "string_match.h"
 
 namespace hs {
 
@@ -288,6 +292,185 @@ inline bool set_is_points(bool str, const RangeSet& s) {
   return true;
 }
 
+// ---- NOT, null tests and string patterns (hs_predicate_any.flags) -------------------------------------------------------
+
+constexpr int kTermPatterns = HS_TERM_STARTS_WITH | HS_TERM_ENDS_WITH | HS_TERM_CONTAINS | HS_TERM_LIKE;
+constexpr int kTermFlags = HS_TERM_NOT | HS_TERM_NULL_TRUE | HS_TERM_NULL_FALSE | kTermPatterns;
+constexpr uint16_t kAnyRun = 257;  // LIKE's `%` in a parsed pattern (string_match.h: kAnyChar is `_`)
+
+// Whether a null row qualifies under the term: only when the term is true there -- NULL_TRUE, or NULL_FALSE under NOT
+// (NOT keeps unknown unknown).
+inline bool term_null_selects(int flags) {
+  return (flags & HS_TERM_NOT) ? (flags & HS_TERM_NULL_FALSE) != 0 : (flags & HS_TERM_NULL_TRUE) != 0;
+}
+
+// The values of a column of type col_type outside the normalised set s, normalised.  Numeric: the gaps of the encoded
+// domain (encoded_domain); strings: the gaps between the bounds, each bound's strictness flipped, from "" up.
+inline RangeSet complement_set(int col_type, const RangeSet& s) {
+  RangeSet out;
+  if (col_type == HS_TYPE_STRING) {
+    SetRange gap;
+    gap.has_lo = true;  // from "" inclusive: every value
+    for (const SetRange& r : s) {
+      if (r.has_lo) {
+        SetRange g = gap;
+        g.has_hi = true, g.hi_b = r.lo_b, g.hi_strict = !r.lo_strict;
+        if (!set_range_empty(true, g)) out.push_back(std::move(g));
+      }
+      if (!r.has_hi) return out;
+      gap = SetRange{};
+      gap.has_lo = true, gap.lo_b = r.hi_b, gap.lo_strict = !r.hi_strict;
+    }
+    out.push_back(std::move(gap));
+    return out;
+  }
+  uint64_t emin, emax;
+  encoded_domain(col_type, &emin, &emax);
+  auto push = [&](uint64_t lo, uint64_t hi) {
+    SetRange g;
+    g.has_lo = g.has_hi = true, g.lo = lo, g.hi = hi;
+    out.push_back(g);
+  };
+  uint64_t next = emin;  // the lowest value not yet covered by s or a gap
+  for (const SetRange& r : s) {
+    const uint64_t lo = r.has_lo ? r.lo : emin, hi = r.has_hi ? r.hi : emax;
+    if (lo > next) push(next, lo - 1);
+    if (hi >= emax) return out;
+    next = std::max(next, hi + 1);
+  }
+  push(next, emax);
+  return out;
+}
+
+// The strings that start with p: [p, succ(p)), succ(p) being p without its trailing 0xff bytes and the last byte left
+// incremented; open above when nothing is left (p empty or all 0xff).
+inline SetRange prefix_range(const std::string& p) {
+  SetRange r;
+  r.has_lo = true, r.lo_b = p;
+  std::string hi = p;
+  while (!hi.empty() && (uint8_t)hi.back() == 0xff) hi.pop_back();
+  if (!hi.empty()) {
+    hi.back() = (char)((uint8_t)hi.back() + 1);
+    r.has_hi = r.hi_strict = true, r.hi_b = std::move(hi);
+  }
+  return r;
+}
+
+// A LIKE pattern with the escape character '\' as items: literal bytes, kAnyChar (`_`) and kAnyRun (`%`).  Spark's
+// refusals (StringUtils.escapeLikeRegex): HS_EINVAL.
+inline std::vector<uint16_t> parse_like(const std::string& pat) {
+  std::vector<uint16_t> out;
+  out.reserve(pat.size());
+  for (size_t i = 0; i < pat.size(); i++) {
+    const uint8_t ch = (uint8_t)pat[i];
+    if (ch == '\\') {
+      if (i + 1 == pat.size()) fail(HS_EINVAL, "the pattern '%s' is invalid, it is not allowed to end with the escape character", pat.c_str());
+      const uint8_t nx = (uint8_t)pat[++i];
+      if (nx != '_' && nx != '%' && nx != '\\') {
+        const std::string c = pat.substr(i, utf8_char_len(nx));
+        fail(HS_EINVAL, "the pattern '%s' is invalid, the escape character is not allowed to precede '%s'", pat.c_str(), c.c_str());
+      }
+      out.push_back(nx);
+    } else {
+      out.push_back(ch == '_' ? kAnyChar : (ch == '%' ? kAnyRun : ch));
+    }
+  }
+  return out;
+}
+
+// A pattern term compiled for pattern_matches (string_match.h), and what the host can say of it without a matcher.
+struct CompiledPattern {
+  std::vector<uint16_t> items;  // literal bytes and kAnyChar
+  std::vector<int32_t> fail;    // per item: the KMP failure function of its segment (string_match.h: find_literal)
+  std::vector<PatSeg> segs;     // the runs between `%`s
+  bool whole = false;           // no `%`: the one segment spans the value
+  std::string prefix;           // the literal bytes before the first wildcard
+  bool prefix_only = false;     // no wildcard but `%` after the prefix: the pattern is a prefix range, or an equality when whole
+};
+
+// kind: one of HS_TERM_STARTS_WITH / ENDS_WITH / CONTAINS / LIKE
+inline CompiledPattern compile_pattern(int kind, const std::string& pat) {
+  std::vector<uint16_t> seq;
+  if (kind == HS_TERM_LIKE) {
+    seq = parse_like(pat);
+  } else {
+    if (kind != HS_TERM_STARTS_WITH) seq.push_back(kAnyRun);
+    for (unsigned char ch : pat) seq.push_back(ch);
+    if (kind != HS_TERM_ENDS_WITH) seq.push_back(kAnyRun);
+  }
+  CompiledPattern cp;
+  size_t k = 0;
+  while (k < seq.size() && seq[k] < kAnyChar) cp.prefix.push_back((char)seq[k++]);
+  cp.prefix_only = std::all_of(seq.begin() + k, seq.end(), [](uint16_t it) { return it == kAnyRun; });
+  PatSeg cur{0, 0, 0};
+  for (uint16_t it : seq) {
+    if (it == kAnyRun) {
+      cp.segs.push_back(cur);
+      cur = PatSeg{(uint32_t)cp.items.size(), 0, 0};
+      continue;
+    }
+    cp.items.push_back(it);
+    cur.len++;
+    cur.any_char |= it == kAnyChar;
+  }
+  cp.segs.push_back(cur);
+  cp.whole = cp.segs.size() == 1;
+  // fail[off + j]: the longest proper prefix of the segment's first j + 1 items that is also their suffix
+  cp.fail.assign(cp.items.size(), 0);
+  for (const PatSeg& g : cp.segs) {
+    const uint16_t* it = cp.items.data() + g.off;
+    int32_t* f = cp.fail.data() + g.off;
+    for (uint32_t j = 1, k = 0; j < g.len; j++) {
+      while (k > 0 && it[j] != it[k]) k = f[k - 1];
+      if (it[j] == it[k]) k++;
+      f[j] = (int32_t)k;
+    }
+  }
+  return cp;
+}
+
+// the pattern of a pattern term (check_anys has checked its shape)
+inline std::string term_pattern(const hs_predicate_any& a) {
+  const uint64_t b = a.values_offsets[0], e = a.values_offsets[1];
+  return e > b ? std::string((const char*)a.values_bytes + b, e - b) : std::string();
+}
+
+// A term resolved once for both uses: the key's windows and the residual.
+struct ResolvedTerm {
+  // the values of non-null rows for which the term is true, normalised: resolve_term's set, a pattern's prefix range (an
+  // equality for a LIKE without wildcards), complemented under NOT
+  RangeSet set;
+  // false for a pattern that is not a prefix: `set` then only bounds the values it can match (its literal prefix; every
+  // value under NOT), and `pattern` is what the matcher runs
+  bool exact = true;
+  CompiledPattern pattern;
+};
+
+// Patterns on other than string columns, and any flag on a boolean column: HS_EUNSUPPORTED.
+inline ResolvedTerm resolve_any(const hs_predicate_any& a, const PredColumn& c) {
+  ResolvedTerm rt;
+  if (const int kind = a.flags & kTermPatterns) {
+    if (c.type != HS_TYPE_STRING)
+      fail(HS_EUNSUPPORTED, "filter scan: a string pattern cannot be applied to the %s column '%s'", c.type == HS_TYPE_BOOL ? "boolean" : "numeric",
+           c.name.c_str());
+    rt.pattern = compile_pattern(kind, term_pattern(a));
+    const CompiledPattern& cp = rt.pattern;
+    if (cp.prefix_only && cp.whole) {
+      SetRange r;
+      r.has_lo = r.has_hi = true, r.lo_b = r.hi_b = cp.prefix;
+      rt.set.push_back(std::move(r));
+    } else {
+      rt.set.push_back(prefix_range(cp.prefix));
+    }
+    rt.exact = cp.prefix_only;
+  } else {
+    if (a.flags && c.type == HS_TYPE_BOOL) fail(HS_EUNSUPPORTED, "filter scan: predicates on the boolean column '%s' are not handled", c.name.c_str());
+    rt.set = resolve_term(a, c);
+  }
+  if (a.flags & HS_TERM_NOT) rt.set = rt.exact ? complement_set(c.type, rt.set) : RangeSet{SetRange{}};
+  return rt;
+}
+
 // The refusals of a predicate list that need no data: HS_OK or the code, with stats zeroed and the message in err.
 // bounds_in_spec: hs_filter_scan_where was also given the bounds of hs_filter_scan.
 inline int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_in_spec, hs_stats* stats, char* err, size_t errlen) {
@@ -331,6 +514,13 @@ inline int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_
     if (a.literal_type != HS_TYPE_INT64 && a.literal_type != HS_TYPE_DOUBLE && a.literal_type != HS_TYPE_STRING &&
         a.literal_type != HS_TYPE_DECIMAL)
       return snprintf(msg, sizeof msg, "filter scan: term on '%s' has an unknown literal type", c), refuse(HS_EINVAL);
+    const int kind = a.flags & kTermPatterns;
+    if (a.flags & ~kTermFlags) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has unknown flags 0x%x", c, a.flags), refuse(HS_EINVAL);
+    if ((a.flags & HS_TERM_NULL_TRUE) && (a.flags & HS_TERM_NULL_FALSE))
+      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has two null outcomes", c), refuse(HS_EINVAL);
+    if (kind & (kind - 1)) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than one pattern kind", c), refuse(HS_EINVAL);
+    if (kind && (a.literal_type != HS_TYPE_STRING || a.n_values != 1 || a.n_ranges != 0))
+      return snprintf(msg, sizeof msg, "filter scan: the pattern term on '%s' needs one string value and no ranges", c), refuse(HS_EINVAL);
     if (a.n_values > 0) {
       const bool missing = a.literal_type == HS_TYPE_STRING ? (!a.values_offsets || (!a.values_bytes && a.values_offsets[a.n_values] != a.values_offsets[0]))
                                                             : (a.literal_type == HS_TYPE_DOUBLE ? !a.values_f : !a.values_i);
@@ -342,6 +532,13 @@ inline int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_
           if (a.values_offsets[k + 1] - a.values_offsets[k] > kMaxStringLen)
             return snprintf(msg, sizeof msg, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c), refuse(HS_EUNSUPPORTED);
         }
+    }
+    if (kind == HS_TERM_LIKE) {
+      try {
+        parse_like(term_pattern(a));
+      } catch (const Error& e) {
+        return snprintf(msg, sizeof msg, "%s", e.what()), refuse(e.code);
+      }
     }
     for (int r = 0; r < a.n_ranges; r++) {
       if (a.ranges[r].column && strcmp(a.ranges[r].column, c) != 0)

@@ -109,8 +109,8 @@ __global__ void k_predicate_mask(const __grid_constant__ PredSet ps, const uint3
     bool ok = true;
     for (int p = 0; p < ps.n && ok; p++) {
       const PredDesc& d = ps.p[p];
-      if (d.valid && !d.valid[row]) {  // a null never satisfies a comparison
-        ok = false;
+      if (d.valid && !d.valid[row]) {  // a null satisfies no comparison; a null test or NOT (c <=> v) says so in null_true
+        ok = d.null_true != 0;
         continue;
       }
       switch (d.r.type) {
@@ -122,6 +122,30 @@ __global__ void k_predicate_mask(const __grid_constant__ PredSet ps, const uint3
       }
     }
     mask[i] = ok ? 1u : 0u;
+  }
+}
+
+// The pattern terms, one thread per candidate row: clears mask[i] where one of them does not hold for row cand[i] (row i
+// without a candidate list).  A thread matches its row's whole value; rows already dropped by k_predicate_mask are skipped.
+// Measured (DESIGN.md section 6), the string scans are bound by the key decode, not by this kernel, on short values; on
+// 1 KB values a warp per value would coalesce the loads that a thread per row does not.
+__global__ void k_pattern_mask(const __grid_constant__ PatternSet ps, const uint32_t* __restrict__ cand, int64_t n,
+                               uint32_t* __restrict__ mask) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (!mask[i]) continue;
+    const int64_t row = cand ? (int64_t)cand[i] : i;
+    bool ok = true;
+    for (int p = 0; p < ps.n && ok; p++) {
+      const PatternDesc& d = ps.p[p];
+      if (d.valid && !d.valid[row]) {
+        ok = d.null_true != 0;
+        continue;
+      }
+      const uint64_t ref = d.refs[row];
+      ok = pattern_matches(ref_ptr(ref), ref_len(ref), d.items, d.fail, d.segs, d.nseg, d.whole != 0) != (d.negate != 0);
+    }
+    if (!ok) mask[i] = 0;
   }
 }
 
@@ -359,7 +383,7 @@ void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid
 
 void launch_range_bounds(hs_ctx* ctx, const void* keys, int ranges_type, const PredRange* ranges, const uint64_t* seg_offsets,
                          const uint2* work, int64_t nwork, int64_t* bounds) {
-  KernelScope _ks(ctx, "k_range_bounds");
+  KernelScope _ks(ctx, "k_range_bounds", nwork);
   if (nwork == 0) return;
   const unsigned grid = (unsigned)ceil_div(nwork, 128);
   switch (ranges_type) {
@@ -383,6 +407,14 @@ void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* ca
   KernelScope _ks(ctx, "k_predicate_mask");
   if (n == 0) return;
   k_predicate_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(preds, cand, n, mask);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_pattern_mask(hs_ctx* ctx, const PatternSet& pats, const uint32_t* cand, int64_t n, uint32_t* mask) {
+  if (pats.n == 0) return;
+  KernelScope _ks(ctx, "k_pattern_mask");
+  if (n == 0) return;
+  k_pattern_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(pats, cand, n, mask);
   HS_LAUNCH_CHECK(ctx);
 }
 
@@ -417,13 +449,14 @@ void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t
   }
 }
 
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const uint32_t* cand, int64_t n, const int64_t* file_ids,
-                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets) {
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const uint32_t* cand, int64_t n,
+                    const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets) {
   Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
   Buf<uint64_t> own_offsets;
   if (!offsets) offsets = &own_offsets;
   offsets->alloc(ctx, n + 1);
   launch_predicate_mask(ctx, preds, cand, n, mask.get());
+  launch_pattern_mask(ctx, pats, cand, n, mask.get());
   Buf<int64_t> d_deleted;
   if (n > 0 && ndeleted > 0) {
     d_deleted.alloc(ctx, ndeleted);

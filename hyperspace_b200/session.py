@@ -18,6 +18,7 @@ files the native call reads -- the same decision FilterIndexRule / JoinIndexRule
 """
 from __future__ import annotations
 
+import dataclasses
 import datetime
 import decimal
 import math
@@ -111,28 +112,72 @@ class RuntimeConf:
 _TERM_SIDES = {">=": ((False,), ()), ">": ((True,), ()), "<=": ((), (False,)), "<": ((), (True,)), "==": ((False,), (False,))}
 
 
+# string patterns of a term -> (explain() form, hs_predicate_any flag)
+_PATTERNS = {"startswith": ("StartsWith", 8), "endswith": ("EndsWith", 16), "contains": ("Contains", 32), "like": ("LIKE", 64)}
+_TERM_NOT, _TERM_NULL_TRUE, _TERM_NULL_FALSE = 1, 2, 4  # hs_predicate_any.flags (include/hs_gpu.h)
+
+
 @dataclass
 class AnyTerm:
     """A disjunction on one column (Spark's In / InSet, or an Or of comparisons on that column): the value equals one of
     ``values`` (a list, or a numpy array) or lies in one of ``ranges``, each ``(lo, lo_strict, hi, hi_strict)`` with None
-    for an open side."""
+    for an open side.  In three-valued logic: ``null`` is what a null row gives (True: IsNull; False: EqualNullSafe; None:
+    unknown); ``null_in_list``: the isin list held a None, so a value outside the list gives unknown rather than false;
+    ``pattern``: a string pattern (startswith / endswith / contains / like) whose one value is the pattern; ``negated``:
+    Not of all that."""
     column: str
     values: object = field(default_factory=list)
     ranges: List[Tuple[object, bool, object, bool]] = field(default_factory=list)
+    null: Optional[bool] = None
+    negated: bool = False
+    pattern: Optional[str] = None
+    null_in_list: bool = False
 
-    def __str__(self) -> str:
+    def _inner(self) -> str:
+        c = self.column
+        if self.pattern:
+            name = _PATTERNS[self.pattern][0]
+            return f"{c} LIKE {self.values[0]!r}" if self.pattern == "like" else f"{name}({c}, {self.values[0]!r})"
         vals = self.values.tolist() if isinstance(self.values, np.ndarray) else list(self.values)
-        shown = ", ".join(repr(v) for v in vals[:3]) + (f", ... {len(vals) - 3} more" if len(vals) > 3 else "")
-        parts = [f"{self.column} IN ({shown})"] if vals or not self.ranges else []
+        if not vals and not self.ranges and self.null is True:
+            return f"{c} IS NULL"
+        if self.null is False:
+            parts = [f"{c} <=> {v!r}" for v in vals[:3]] + ([f"... {len(vals) - 3} more"] if len(vals) > 3 else [])
+        else:
+            shown = ", ".join(repr(v) for v in vals[:3]) + (f", ... {len(vals) - 3} more" if len(vals) > 3 else "")
+            parts = [f"{c} IN ({shown})"] if vals or not self.ranges else []
         for lo, ls, hi, hs in self.ranges:
-            side = [f"{self.column} {'>' if ls else '>='} {lo!r}"] if lo is not None else []
-            side += [f"{self.column} {'<' if hs else '<='} {hi!r}"] if hi is not None else []
+            side = [f"{c} {'>' if ls else '>='} {lo!r}"] if lo is not None else []
+            side += [f"{c} {'<' if hs else '<='} {hi!r}"] if hi is not None else []
             parts.append(" AND ".join(side))
+        if self.null is True:
+            parts.append(f"{c} IS NULL")
         return " OR ".join(f"({p})" if " AND " in p and len(parts) > 1 else p for p in parts)
 
-    def as_native(self) -> Tuple[str, object, List[tuple]]:
-        """(column, values, ranges) for Context.filter_scan_any / bucket_join_any."""
-        return self.column, self.values, list(self.ranges)
+    def __str__(self) -> str:
+        if not self.negated:
+            return self._inner()
+        if not self.pattern and self.null is True and not len(self.values) and not self.ranges:
+            return f"{self.column} IS NOT NULL"
+        return f"NOT ({self._inner()})"
+
+    def as_native(self) -> tuple:
+        """(column, values, ranges), with the HS_TERM_* flags as a fourth element when there are any, for
+        Context.filter_scan_any / bucket_join_any."""
+        if self.negated and self.null_in_list:  # NOT (k IN (..., NULL)): false or unknown on every row
+            return self.column, [], []
+        flags = (_TERM_NOT if self.negated else 0) | (_PATTERNS[self.pattern][1] if self.pattern else 0)
+        flags |= {True: _TERM_NULL_TRUE, False: _TERM_NULL_FALSE, None: 0}[self.null]
+        if not flags:
+            return self.column, self.values, list(self.ranges)
+        return self.column, self.values, list(self.ranges), flags
+
+
+def _prefix_range(p) -> Tuple[object, bool, object, bool]:
+    """The values that start with p, as a range: [p, succ(p)), succ(p) being p without its trailing 0xff bytes and its
+    last byte incremented; open above when nothing is left."""
+    b = _as_bytes(p).rstrip(b"\xff")
+    return (p, False, b[:-1] + bytes([b[-1] + 1]), True) if b else (p, False, None, False)
 
 
 def _merge_values(a, b):
@@ -168,13 +213,39 @@ class Predicate:
         if other._single_column().lower() != c.lower():
             raise LE.HyperspaceException(f"an OR across columns ({c}, {other._single_column()}) is not handled by the GPU path")
         merged = AnyTerm(c)
+        nulls = []  # what a null row gives in each branch
         for branch in (self, other):
-            if branch.anys:
-                merged.values = _merge_values(merged.values, branch.anys[0].values)
-                merged.ranges += branch.anys[0].ranges
+            a = branch.anys[0] if branch.anys else None
+            if a is not None and a.negated:
+                raise LE.HyperspaceException("a NOT inside an OR is not handled by the GPU path")
+            if a is not None and a.pattern not in (None, "startswith"):
+                raise LE.HyperspaceException(f"a {a.pattern} pattern inside an OR is not handled by the GPU path")
+            if a is None or a.pattern:
+                merged.ranges.append(_prefix_range(a.values[0]) if a is not None else branch._one_range())
+                nulls.append(None)
             else:
-                merged.ranges.append(branch._one_range())
+                merged.values = _merge_values(merged.values, a.values)
+                merged.ranges += a.ranges
+                merged.null_in_list = merged.null_in_list or a.null_in_list
+                nulls.append(a.null)
+        merged.null = True if True in nulls else (False if all(n is False for n in nulls) else None)
         return Predicate({}, [], [merged])
+
+    def __invert__(self) -> "Predicate":
+        """Not of a filter on one column: of one comparison or range, or of one isin, OR, null test or pattern."""
+        cols = {c.lower(): c for c in self.columns}
+        if len(cols) != 1:
+            raise LE.HyperspaceException(f"a NOT over several columns ({', '.join(cols.values())}) is not handled by the GPU "
+                                         "path: it would be an OR across columns")
+        if self.anys:
+            if len(self.anys) > 1 or self._as_terms():
+                raise LE.HyperspaceException("a NOT must cover one comparison, range, isin, OR, null test or pattern")
+            return Predicate({}, [], [dataclasses.replace(self.anys[0], negated=not self.anys[0].negated)])
+        try:
+            rng = self._one_range()
+        except LE.HyperspaceException:
+            raise LE.HyperspaceException("a NOT must cover one range: at most one lower and one upper bound") from None
+        return Predicate({}, [], [AnyTerm(next(iter(cols.values())), [], [rng], negated=True)])
 
     def _single_column(self) -> str:
         cols = {c.lower(): c for c in self.columns}
@@ -284,19 +355,60 @@ class Column:
             return Predicate({self.name: (1, 0)}, [(self.name, "==", v)])  # an integer never equals a fraction: empty range
         return Predicate({self.name: (int(n), int(n))}, [(self.name, "==", v)])
 
+    def __ne__(self, v):  # noqa: A003
+        """Not(EqualTo): a null row, or a None literal, gives unknown."""
+        return ~self.isin([v])
+
     def isin(self, *values) -> Predicate:
         """PySpark's Column.isin: varargs, or one list / tuple / set / numpy array.  None is dropped (it never makes a row
-        qualify); ints, floats, Decimals, datetimes, str and bytes are accepted, and the list is cast as Spark casts it
-        (a float makes every value a double, Decimals share one scale).  Strings mixed with numbers raise."""
+        qualify; under ~ it makes every row unknown); ints, floats, Decimals, datetimes, str and bytes are accepted, and the
+        list is cast as Spark casts it (a float makes every value a double, Decimals share one scale).  Strings mixed with
+        numbers raise."""
+        vals = values[0] if len(values) == 1 and isinstance(values[0], (list, tuple, set, frozenset, np.ndarray)) else values
+        had_none = not isinstance(vals, np.ndarray) and any(v is None for v in vals)
+        vals = vals if isinstance(vals, np.ndarray) else [v for v in vals if v is not None]
+        return Predicate({}, [], [AnyTerm(self.name, self._checked(vals, "isin"), null_in_list=had_none)])
+
+    def _checked(self, vals, what):
         from ._native import any_values
 
-        vals = values[0] if len(values) == 1 and isinstance(values[0], (list, tuple, set, frozenset, np.ndarray)) else values
-        vals = vals if isinstance(vals, np.ndarray) else [v for v in vals if v is not None]
         try:
             any_values(vals)
         except ValueError as e:
-            raise LE.HyperspaceException(f"isin on '{self.name}': {e}") from None
-        return Predicate({}, [], [AnyTerm(self.name, vals)])
+            raise LE.HyperspaceException(f"{what} on '{self.name}': {e}") from None
+        return vals
+
+    def isNull(self) -> Predicate:
+        return Predicate({}, [], [AnyTerm(self.name, [], null=True)])
+
+    def isNotNull(self) -> Predicate:
+        return Predicate({}, [], [AnyTerm(self.name, [], null=True, negated=True)])
+
+    def eqNullSafe(self, v) -> Predicate:
+        """EqualNullSafe (`<=>`): a null row gives false, and `eqNullSafe(None)` is isNull()."""
+        if v is None:
+            return self.isNull()
+        return Predicate({}, [], [AnyTerm(self.name, self._checked([v], "eqNullSafe"), null=False)])
+
+    def _pattern(self, kind, p) -> Predicate:
+        if not isinstance(p, (str, bytes)):
+            raise LE.HyperspaceException(f"{kind} on '{self.name}' takes a string pattern, not {p!r}")
+        return Predicate({}, [], [AnyTerm(self.name, [p], pattern=kind)])
+
+    def startswith(self, p) -> Predicate:
+        """StartsWith, in bytes: the range [p, succ(p))."""
+        return self._pattern("startswith", p)
+
+    def endswith(self, s) -> Predicate:
+        return self._pattern("endswith", s)
+
+    def contains(self, s) -> Predicate:
+        return self._pattern("contains", s)
+
+    def like(self, pattern) -> Predicate:
+        """Like with the escape character '\\': '%' matches any run of characters, '_' one character, and the whole value
+        must match.  Values that are not valid UTF-8 are not covered (Spark matches the decoded string)."""
+        return self._pattern("like", pattern)
 
     def between(self, lo, hi):
         terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
@@ -442,7 +554,7 @@ class DataFrame:
     def filter(self, predicate: Predicate) -> "DataFrame":
         resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
                              [(self._resolve(c), op, v) for c, op, v in predicate.terms],
-                             [AnyTerm(self._resolve(a.column), a.values, list(a.ranges)) for a in predicate.anys])
+                             [dataclasses.replace(a, column=self._resolve(a.column), ranges=list(a.ranges)) for a in predicate.anys])
         return DataFrame(self.session, FilterNode(self.plan, resolved))
 
     where = filter

@@ -90,7 +90,8 @@ void hs_shutdown(hs_ctx* ctx);
 void hs_trim(hs_ctx* ctx);
 /* Per-kernel timing: when enabled, the hot kernels are bracketed with CUDA events on the ctx stream; hs_profile_report
  * writes a JSON object {"kernel": {"launches": n, "ms": total}} covering the calls since the last report and resets
- * it.  Used by bench.py for the roofline of the dominant kernel. */
+ * it.  Used by bench.py for the roofline of the dominant kernel.  k_range_bounds also reports "items": the (sorted file,
+ * key range) work items it searched, one per window of the filter scans' key. */
 void hs_profile_enable(hs_ctx* ctx, int on);
 int hs_profile_report(hs_ctx* ctx, char* out_json, size_t outlen);
 /* Page-locked host memory for file images handed to hs_create_index (a JNI direct ByteBuffer can wrap it); pageable
@@ -308,8 +309,34 @@ typedef struct {
   const uint64_t* values_offsets;
   const hs_predicate* ranges;  /* hs_predicate semantics; column NULL or == column */
   int32_t n_ranges;
-  int32_t reserved;
+  int32_t flags;               /* HS_TERM_* below; 0: the disjunction above, a null row never qualifying */
 } hs_predicate_any;
+
+/* hs_predicate_any.flags.  A term is true, false or unknown on each row, as in Spark's three-valued logic, and a row
+ * qualifies only when every AND-ed term is true.  On a non-null row the term is true when the value lies in the term's set
+ * (or matches its pattern) and false otherwise; on a null row it is unknown unless a NULL flag says otherwise.
+ *   HS_TERM_NOT         Not(term): true <-> false, unknown stays (`c != 5`, `~c.isin(...)`, `NOT c LIKE '...'`).  The NULL
+ *                       flags describe the term before NOT.
+ *   HS_TERM_NULL_TRUE   a null row makes the term true: IsNull is NULL_TRUE with no values and no ranges, IsNotNull the same
+ *                       with NOT.
+ *   HS_TERM_NULL_FALSE  a null row makes the term false: EqualNullSafe(c, v) is the value v with NULL_FALSE, so that
+ *                       NOT (c <=> v) keeps the null rows.
+ *   HS_TERM_STARTS_WITH, HS_TERM_ENDS_WITH, HS_TERM_CONTAINS: StringStartsWith / StringEndsWith / StringContains, in bytes;
+ *                       the empty pattern matches every non-null value.
+ *   HS_TERM_LIKE        Like with the escape character '\': '%' matches any run of characters, '_' one UTF-8 character, and
+ *                       the whole value must match.  A pattern ending in the escape character, or with the escape before
+ *                       anything but '%', '_' and '\', is HS_EINVAL with Spark's message.  Values that are not valid UTF-8 are
+ *                       not covered: Spark matches the decoded String.
+ * A pattern term (one of the last four) has literal_type HS_TYPE_STRING, exactly one value -- the pattern, at most 65535
+ * bytes -- and no ranges; on a non-string column it is HS_EUNSUPPORTED.  Both NULL flags, two pattern kinds, a malformed
+ * pattern term or an unknown bit: HS_EINVAL. */
+#define HS_TERM_NOT 1
+#define HS_TERM_NULL_TRUE 2
+#define HS_TERM_NULL_FALSE 4
+#define HS_TERM_STARTS_WITH 8
+#define HS_TERM_ENDS_WITH 16
+#define HS_TERM_CONTAINS 32
+#define HS_TERM_LIKE 64
 
 /* hs_filter_scan_where with disjunction terms AND-ed to the predicates (n_preds + n_anys <= 16).  On sorted files a term on
  * key_column becomes many windows per file, one per disjoint range of its values; terms on other columns (and every term
@@ -317,8 +344,9 @@ typedef struct {
  * assert that the files are bucketed on key_column alone (Spark's bucket hash, as hs_create_index writes them): when the
  * key's windows are points only (listed values, ranges with lo == hi, equalities in preds) and the key is int32, int64,
  * string, timestamp or decimal, only the files of the points' buckets are opened, each point is searched only in the files
- * of its own bucket, and stats count only those files.  The rows are the same, in the same order (file, then row), as
- * without file_buckets.  Without terms and buckets this is hs_filter_scan_where. */
+ * of its own bucket, and stats count only those files (a term on key_column that a null row makes true -- IS NULL,
+ * NOT (k <=> v) -- turns this off: the null keys lie in their own bucket).  The rows are the same, in the same order (file,
+ * then row), as without file_buckets.  Without terms and buckets this is hs_filter_scan_where. */
 int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
                        const hs_predicate_any* anys, int32_t n_anys, const int32_t* file_buckets, int32_t num_buckets,
                        hs_batch** out, hs_stats* stats, char* err, size_t errlen);
