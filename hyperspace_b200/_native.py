@@ -27,6 +27,9 @@ HS_OUT_FILES, HS_OUT_HOST, HS_OUT_DEVICE = 0, 1, 2
 # hs_predicate_any.flags
 HS_TERM_NOT, HS_TERM_NULL_TRUE, HS_TERM_NULL_FALSE = 1, 2, 4
 HS_TERM_STARTS_WITH, HS_TERM_ENDS_WITH, HS_TERM_CONTAINS, HS_TERM_LIKE = 8, 16, 32, 64
+# hs_column_compare.op
+HS_CMP_LT, HS_CMP_LE, HS_CMP_GT, HS_CMP_GE, HS_CMP_EQ, HS_CMP_EQ_NULL_SAFE = 1, 2, 3, 4, 5, 6
+CMP_OPS = {"<": HS_CMP_LT, "<=": HS_CMP_LE, ">": HS_CMP_GT, ">=": HS_CMP_GE, "=": HS_CMP_EQ, "<=>": HS_CMP_EQ_NULL_SAFE}
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -90,6 +93,10 @@ class PredicateAnySpec(C.Structure):
                 ("ranges", C.POINTER(PredicateSpec)), ("n_ranges", C.c_int32), ("flags", C.c_int32)]
 
 
+class ColumnCompareSpec(C.Structure):
+    _fields_ = [("left", C.c_char_p), ("right", C.c_char_p), ("op", C.c_int32), ("flags", C.c_int32)]
+
+
 class JoinSpec(C.Structure):
     _fields_ = [("left_files", C.POINTER(SourceFile)), ("n_left", C.c_int32),
                 ("right_files", C.POINTER(SourceFile)), ("n_right", C.c_int32),
@@ -125,6 +132,7 @@ EXPORTED_SYMBOLS = [
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
+    "hs_filter_scan_cmp", "hs_bucket_join_cmp",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -183,6 +191,16 @@ def load_library() -> C.CDLL:
                                      C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
                                      C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
                                      C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    L.hs_filter_scan_cmp.restype = C.c_int
+    L.hs_filter_scan_cmp.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32,
+                                     C.POINTER(PredicateAnySpec), C.c_int32, C.POINTER(ColumnCompareSpec), C.c_int32, C.c_void_p,
+                                     C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    L.hs_bucket_join_cmp.restype = C.c_int
+    L.hs_bucket_join_cmp.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
+                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                     C.POINTER(ColumnCompareSpec), C.c_int32,
+                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                     C.POINTER(ColumnCompareSpec), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join.restype = C.c_int
     L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join_where.restype = C.c_int
@@ -457,6 +475,20 @@ def _any_array(terms: Sequence[tuple]):
         keep.append(rp)
         a.ranges, a.n_ranges = rp, nr
     return arr, len(terms), keep
+
+
+def _cmp_array(compares: Sequence[tuple]):
+    """``(left, op, right)`` or ``(left, op, right, flags)`` comparisons -> (hs_column_compare array, count, names to keep
+    alive).  op is one of CMP_OPS's keys ("<", "<=", ">", ">=", "=", "<=>") or an HS_CMP_* code; flags is 0 or HS_TERM_NOT."""
+    keep = []
+    arr = (ColumnCompareSpec * max(1, len(compares)))()
+    for c, (left, op, right, *flags) in zip(arr, compares):
+        names = [n.encode() if n is not None else None for n in (left, right)]
+        keep += names
+        c.left, c.right = names
+        c.op = CMP_OPS[op] if isinstance(op, str) else op
+        c.flags = flags[0] if flags else 0
+    return arr, len(compares), keep
 
 
 def _source_array(files: Sequence[FileImage]):
@@ -917,6 +949,26 @@ class Context:
                                     C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
+    def filter_scan_cmp(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
+                        terms: Sequence[tuple], compares: Sequence[tuple], sorted_on_key: bool = True,
+                        deleted_file_ids: Sequence[int] = (), file_buckets: Optional[Sequence[int]] = None, num_buckets: int = 0,
+                        output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_filter_scan_cmp: filter_scan_any with comparisons between two columns of the row AND-ed to the predicates and
+        terms, each ``(left, op, right)`` with op one of "<", "<=", ">", ">=", "=", "<=>" and an optional fourth element,
+        HS_TERM_NOT.  The engine applies Spark's coercion of the two columns' types."""
+        L = load_library()
+        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
+        preds, n_preds = _predicate_array(predicates)
+        anys, n_anys, keep_any = _any_array(terms)
+        cmps, n_cmps, keep_cmp = _cmp_array(compares)
+        fb = np.ascontiguousarray(file_buckets if file_buckets is not None else [0], dtype=np.int32)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_filter_scan_cmp(self._h, C.byref(spec), preds, n_preds, anys, n_anys, cmps, n_cmps,
+                                    fb.ctypes.data if file_buckets is not None else None, num_buckets if file_buckets is not None else 0,
+                                    C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
     def _join_spec(self, left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns, right_columns,
                    output):
         ls, k1 = _source_array(left)
@@ -990,6 +1042,27 @@ class Context:
         err = C.create_string_buffer(1024)
         _check(L.hs_bucket_join_any(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, rp, nrp, ra, nra, C.byref(res),
                                     C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
+    def bucket_join_cmp(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                        right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                        left_columns: Sequence[str], right_columns: Sequence[str], left_predicates: Sequence[tuple] = (),
+                        right_predicates: Sequence[tuple] = (), left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (),
+                        left_compares: Sequence[tuple] = (), right_compares: Sequence[tuple] = (),
+                        output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_cmp: bucket_join_any with filter_scan_cmp's comparisons on either side."""
+        L = load_library()
+        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
+                                                                          left_keys, right_keys, left_columns, right_columns,
+                                                                          left_predicates, right_predicates, output)
+        la, nla, k1 = _any_array(left_terms)
+        ra, nra, k2 = _any_array(right_terms)
+        lc, nlc, k3 = _cmp_array(left_compares)
+        rc, nrc, k4 = _cmp_array(right_compares)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_bucket_join_cmp(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, lc, nlc, rp, nrp, ra, nra, rc, nrc,
+                                    C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------

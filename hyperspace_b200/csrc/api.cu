@@ -168,7 +168,7 @@ void drop_deleted_rows(hs_ctx* ctx, Table& t, const int64_t* deleted, int ndelet
   if (lc < 0) fail(HS_EINVAL, "deleted_file_ids given but the source has no _data_file_id column (index built without lineage)");
   if (t.nrows == 0) return;
   Buf<uint32_t> idx;
-  const int64_t kept = select_rows(ctx, PredSet{}, PatternSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
+  const int64_t kept = select_rows(ctx, PredSet{}, PatternSet{}, CompareSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
   gather_table(ctx, t, idx.get(), kept);
 }
 
@@ -986,6 +986,18 @@ static void add_predicates(hs_ctx* ctx, const Table& t, const hs_predicate* pred
   }
 }
 
+// Appends to cs the comparisons between two columns of t, cmp_col[i] holding the columns of cmps[i]
+static void add_compares(const Table& t, const hs_column_compare* cmps, const std::vector<std::pair<int, int>>& cmp_col, CompareSet* cs) {
+  for (size_t i = 0; i < cmp_col.size(); i++) {
+    const DevColumn& l = t.cols[cmp_col[i].first];
+    const DevColumn& r = t.cols[cmp_col[i].second];
+    CompareDesc d = resolve_compare(cmps[i], pred_column(l), pred_column(r));
+    d.col[0] = l.data.get(), d.col[1] = r.data.get();
+    d.valid[0] = l.has_nulls ? l.valid.get() : nullptr, d.valid[1] = r.has_nulls ? r.valid.get() : nullptr;
+    cs->p[cs->n++] = d;
+  }
+}
+
 // the index of column nm in cols, appended when it is not there yet
 static int column_index(std::vector<std::string>* cols, const std::string& nm) {
   auto it = std::find(cols->begin(), cols->end(), nm);
@@ -1049,10 +1061,12 @@ static std::vector<int> point_buckets(hs_ctx* ctx, const DevColumn& key, const R
 // legacy (hs_filter_scan): predicates may have no bound (the row's key must then not be null, as that call always did),
 // literal types follow the column, and floating-point keys are refused (the call's bounds are int64).
 // anys: disjunction terms.  On the key column they turn the key's one window per file into one window per range of the
-// key's set; elsewhere they are set-form residual predicates.  file_buckets (optional): see hs_filter_scan_any.
+// key's set; elsewhere they are set-form residual predicates.  cmps: comparisons between two columns, always residual (they
+// make no window, so a key that appears only in them is read whole).  file_buckets (optional): see hs_filter_scan_any.
 static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int n_preds, bool legacy,
-                            const hs_predicate_any* anys, int n_anys, const int32_t* file_buckets, int num_buckets,
-                            hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+                            const hs_predicate_any* anys, int n_anys, const hs_column_compare* cmps, int n_cmps,
+                            const int32_t* file_buckets, int num_buckets, hs_batch** out, hs_stats* stats, char* err,
+                            size_t errlen) {
   *out = nullptr;
   hs_stats st;
   memset(&st, 0, sizeof st);
@@ -1073,6 +1087,8 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     std::vector<int> pred_col(n_preds), any_col(n_anys);
     for (int i = 0; i < n_preds; i++) pred_col[i] = column_index(&cols, preds[i].column);
     for (int i = 0; i < n_anys; i++) any_col[i] = column_index(&cols, anys[i].column);
+    std::vector<std::pair<int, int>> cmp_col(n_cmps);
+    for (int i = 0; i < n_cmps; i++) cmp_col[i] = {column_index(&cols, cmps[i].left), column_index(&cols, cmps[i].right)};
     const int lineage_col = spec->n_deleted_file_ids > 0 ? column_index(&cols, "_data_file_id") : -1;
     PredUploads uploads;
     TermResolutions terms(anys, n_anys);
@@ -1230,22 +1246,27 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       idx.alloc(ctx, std::max<int64_t>(1, n_cand));
       if (nseg) launch_windows_to_indices(ctx, d_win.get(), d_oo.get(), nwin, n_cand, idx.get());
       n_out = n_cand;
-      if (on_key < n_preds + n_anys) {
-        // residual: the predicates on other columns, over the window rows, compacted through the candidate list
+      if (on_key < n_preds + n_anys || n_cmps > 0) {
+        // residual: the predicates on other columns and the comparisons, over the window rows, compacted through the
+        // candidate list
         PredSet residual;
         PatternSet pats;
+        CompareSet cs;
         add_predicates(ctx, t, preds, pred_col, terms, any_col, 0, &residual, &pats, &uploads);
+        add_compares(t, cmps, cmp_col, &cs);
         Buf<uint32_t> kept_rows;
-        n_out = select_rows(ctx, residual, pats, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
+        n_out = select_rows(ctx, residual, pats, cs, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
         idx = std::move(kept_rows);
       }
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
       PredSet ps;
       PatternSet pats;
+      CompareSet cs;
       add_predicates(ctx, t, preds, pred_col, terms, any_col, -1, &ps, &pats, &uploads);
+      add_compares(t, cmps, cmp_col, &cs);
       const int64_t* file_ids = lineage_col >= 0 ? (const int64_t*)t.cols[lineage_col].data.get() : nullptr;
-      n_out = select_rows(ctx, ps, pats, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
+      n_out = select_rows(ctx, ps, pats, cs, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
     }
     sync_stream(ctx);
     t_scan.stop();
@@ -1285,7 +1306,7 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
   p.lo_i = spec->lo, p.hi_i = spec->hi;
   p.lo_bytes = spec->lo_bytes, p.hi_bytes = spec->hi_bytes;
   p.lo_len = spec->lo_len, p.hi_len = spec->hi_len;
-  return filter_scan_core(ctx, spec, &p, 1, true, nullptr, 0, nullptr, 0, out, stats, err, errlen);
+  return filter_scan_core(ctx, spec, &p, 1, true, nullptr, 0, nullptr, 0, nullptr, 0, out, stats, err, errlen);
 }
 
 int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
@@ -1296,19 +1317,27 @@ int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predica
 int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
                        const hs_predicate_any* anys, int32_t n_anys, const int32_t* file_buckets, int32_t num_buckets,
                        hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  return hs_filter_scan_cmp(ctx, spec, preds, n_preds, anys, n_anys, nullptr, 0, file_buckets, num_buckets, out, stats, err, errlen);
+}
+
+int hs_filter_scan_cmp(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                       const hs_predicate_any* anys, int32_t n_anys, const hs_column_compare* cmps, int32_t n_cmps,
+                       const int32_t* file_buckets, int32_t num_buckets, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen) {
   if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds) || num_buckets < 0 || (num_buckets > 0 && !file_buckets))
     return HS_EINVAL;
   *out = nullptr;
   int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
   if (rc == HS_OK) rc = check_anys(anys, n_anys, n_preds, stats, err, errlen);
+  if (rc == HS_OK) rc = check_compares(cmps, n_cmps, n_preds + n_anys, stats, err, errlen);
   if (rc != HS_OK) return rc;
   if (num_buckets > kMaxBuckets) {
     if (stats) memset(stats, 0, sizeof *stats);
     if (err && errlen) snprintf(err, errlen, "numBuckets must be in 1..%d", kMaxBuckets);
     return HS_EUNSUPPORTED;
   }
-  return filter_scan_core(ctx, spec, preds, n_preds, false, anys, n_anys, num_buckets > 0 ? file_buckets : nullptr, num_buckets,
-                          out, stats, err, errlen);
+  return filter_scan_core(ctx, spec, preds, n_preds, false, anys, n_anys, cmps, n_cmps, num_buckets > 0 ? file_buckets : nullptr,
+                          num_buckets, out, stats, err, errlen);
 }
 
 }  // extern "C"
@@ -1377,11 +1406,11 @@ static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file*
 
 // Side selection: keeps the rows whose key columns are all non-null and where every predicate of the side holds.  The
 // predicates run over the sorted positions as their candidate list, so the compacted rows stay in sorted order and a
-// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps and pats are empty.
-static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, const PatternSet& pats, int nb) {
-  if (ps.n == 0 && pats.n == 0) return;
+// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps, pats and cmps are empty.
+static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, const PatternSet& pats, const CompareSet& cmps, int nb) {
+  if (ps.n == 0 && pats.n == 0 && cmps.n == 0) return;
   Buf<uint64_t> offs;
-  side->n = select_rows(ctx, ps, pats, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
+  side->n = select_rows(ctx, ps, pats, cmps, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
   side->perm = side->kept.get();
   std::vector<uint32_t> bounds(nb + 1);
   for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
@@ -1398,8 +1427,9 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, con
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                             int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
                             int n_right_preds, const hs_predicate_any* left_anys, int n_left_anys,
-                            const hs_predicate_any* right_anys, int n_right_anys, bool legacy, hs_batch** out, hs_stats* stats,
-                            char* err, size_t errlen) {
+                            const hs_predicate_any* right_anys, int n_right_anys, const hs_column_compare* left_cmps,
+                            int n_left_cmps, const hs_column_compare* right_cmps, int n_right_cmps, bool legacy, hs_batch** out,
+                            hs_stats* stats, char* err, size_t errlen) {
   hs_stats st;
   memset(&st, 0, sizeof st);
   std::unique_ptr<hs_batch> res(new hs_batch());
@@ -1410,10 +1440,11 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.start();
     const int nb = spec->num_buckets;
     if (nb < 1) fail(HS_EINVAL, "num_buckets must be positive");
-    // columns to decode: the keys first, then the projection, then the predicate and term columns
+    // columns to decode: the keys first, then the projection, then the predicate, term and comparison columns
     auto side_columns = [&](const char* const* keys, const char* const* proj, int n_proj, const hs_predicate* preds, int n_preds,
-                            const hs_predicate_any* anys, int n_anys, std::vector<int>* proj_idx, std::vector<int>* pred_idx,
-                            std::vector<int>* any_idx) {
+                            const hs_predicate_any* anys, int n_anys, const hs_column_compare* cmps, int n_cmps,
+                            std::vector<int>* proj_idx, std::vector<int>* pred_idx, std::vector<int>* any_idx,
+                            std::vector<std::pair<int, int>>* cmp_idx) {
       std::vector<std::string> cols;
       for (int k = 0; k < n_keys; k++) {
         if (!keys[k]) fail(HS_EINVAL, "bucket join: missing key column");
@@ -1423,13 +1454,18 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       for (int i = 0; i < n_proj; i++) proj_idx->push_back(column_index(&cols, proj[i]));
       for (int i = 0; i < n_preds; i++) pred_idx->push_back(column_index(&cols, preds[i].column));
       for (int i = 0; i < n_anys; i++) any_idx->push_back(column_index(&cols, anys[i].column));
+      for (int i = 0; i < n_cmps; i++) {
+        const int a = column_index(&cols, cmps[i].left);
+        cmp_idx->push_back({a, column_index(&cols, cmps[i].right)});
+      }
       return cols;
     };
     std::vector<int> lproj, rproj, lpred, rpred, lany, rany;
+    std::vector<std::pair<int, int>> lcmp, rcmp;
     const std::vector<std::string> lcols = side_columns(left_keys, spec->left_columns, spec->n_left_columns, left_preds, n_left_preds,
-                                                        left_anys, n_left_anys, &lproj, &lpred, &lany);
+                                                        left_anys, n_left_anys, left_cmps, n_left_cmps, &lproj, &lpred, &lany, &lcmp);
     const std::vector<std::string> rcols = side_columns(right_keys, spec->right_columns, spec->n_right_columns, right_preds, n_right_preds,
-                                                        right_anys, n_right_anys, &rproj, &rpred, &rany);
+                                                        right_anys, n_right_anys, right_cmps, n_right_cmps, &rproj, &rpred, &rany, &rcmp);
     JoinSide L, R;
     prepare_join_side(ctx, &L, spec->left_files, spec->n_left, spec->left_buckets, nb, lcols, n_keys, legacy, &st);
     prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, n_keys, legacy, &st);
@@ -1465,10 +1501,13 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     };
     PatternSet lpats, rpats;
     const PredSet lps = side_preds(L, left_preds, lpred, lterms, lany, &lpats), rps = side_preds(R, right_preds, rpred, rterms, rany, &rpats);
+    CompareSet lcs, rcs;
+    add_compares(L.t, left_cmps, lcmp, &lcs);
+    add_compares(R.t, right_cmps, rcmp, &rcs);
     StageTimer t_sel(ctx);
     t_sel.start();
-    select_join_side(ctx, &L, lps, lpats, nb);
-    select_join_side(ctx, &R, rps, rpats, nb);
+    select_join_side(ctx, &L, lps, lpats, lcs, nb);
+    select_join_side(ctx, &R, rps, rpats, rcs, nb);
     t_sel.stop();
     // the key columns in (selected) sorted order
     std::vector<Buf<uint8_t>> key_bufs;
@@ -1510,7 +1549,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
-    if (lps.n || rps.n || lpats.n || rpats.n) st.ms_exchange += t_sel.ms();
+    if (lps.n || rps.n || lpats.n || rpats.n || lcs.n || rcs.n) st.ms_exchange += t_sel.ms();
     st.rows_out = (int64_t)total_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;
@@ -1525,8 +1564,8 @@ extern "C" {
 int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out) return HS_EINVAL;
   *out = nullptr;
-  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, true, out,
-                          stats, err, errlen);
+  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                          nullptr, 0, true, out, stats, err, errlen);
 }
 
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
@@ -1540,6 +1579,16 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
                        int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
                        int32_t n_left_anys, const hs_predicate* right_preds, int32_t n_right_preds,
                        const hs_predicate_any* right_anys, int32_t n_right_anys, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen) {
+  return hs_bucket_join_cmp(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, left_anys, n_left_anys, nullptr, 0,
+                            right_preds, n_right_preds, right_anys, n_right_anys, nullptr, 0, out, stats, err, errlen);
+}
+
+int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
+                       int32_t n_left_anys, const hs_column_compare* left_cmps, int32_t n_left_cmps, const hs_predicate* right_preds,
+                       int32_t n_right_preds, const hs_predicate_any* right_anys, int32_t n_right_anys,
+                       const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
                        size_t errlen) {
   if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
       (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
@@ -1557,9 +1606,12 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
   if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
   if (rc == HS_OK) rc = check_anys(left_anys, n_left_anys, n_left_preds, stats, err, errlen);
   if (rc == HS_OK) rc = check_anys(right_anys, n_right_anys, n_right_preds, stats, err, errlen);
+  if (rc == HS_OK) rc = check_compares(left_cmps, n_left_cmps, n_left_preds + n_left_anys, stats, err, errlen);
+  if (rc == HS_OK) rc = check_compares(right_cmps, n_right_cmps, n_right_preds + n_right_anys, stats, err, errlen);
   if (rc != HS_OK) return rc;
   return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, left_anys,
-                          n_left_anys, right_anys, n_right_anys, false, out, stats, err, errlen);
+                          n_left_anys, right_anys, n_right_anys, left_cmps, n_left_cmps, right_cmps, n_right_cmps, false, out, stats,
+                          err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

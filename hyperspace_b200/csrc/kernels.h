@@ -2,6 +2,7 @@
 #pragma once
 #include <functional>
 
+#include "column_compare.h"
 #include "hs_common.h"
 #include "string_match.h"
 
@@ -441,6 +442,12 @@ struct PatternSet {
   PatternDesc p[kMaxPredicates];
   int n = 0;
 };
+// The comparisons between two columns of a scan or join side (predicates.h: resolve_compare), evaluated by compare_holds
+// (column_compare.h).
+struct CompareSet {
+  CompareDesc p[kMaxPredicates];
+  int n = 0;
+};
 // The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
 // work[w] = {s, r} with r indexing `ranges` (device); bounds[2w] = first row of s inside ranges[r], bounds[2w+1] = first
 // row above it (segment-relative).  All ranges are of type ranges_type.
@@ -455,6 +462,9 @@ void launch_predicate_mask(hs_ctx* ctx, const PredSet& preds, const uint32_t* ca
 // mask[i] = 0 where a pattern of `pats` does not hold for row cand[i] (row i when cand is nullptr); launches nothing when
 // pats is empty
 void launch_pattern_mask(hs_ctx* ctx, const PatternSet& pats, const uint32_t* cand, int64_t n, uint32_t* mask);
+// mask[i] = 0 where a comparison of `cmps` does not hold for row cand[i] (row i when cand is nullptr); launches nothing when
+// cmps is empty
+void launch_compare_mask(hs_ctx* ctx, const CompareSet& cmps, const uint32_t* cand, int64_t n, uint32_t* mask);
 // The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its
 // type's width (type[k]: HS_TYPE_INT32 / HS_TYPE_INT64, or HS_TYPE_STRING for string references).  The tuples compare
 // column by column, integers as signed values, strings in byte order.
@@ -478,11 +488,12 @@ void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* val
 void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                          const uint64_t* offsets, uint8_t* out);
 // Row selection over n candidates (cand[i], or row i when cand is nullptr): keeps those where every predicate of `preds`
-// and every pattern of `pats` holds and, when ndeleted > 0, whose file_ids[i] is not in the host array `deleted`.  The kept
-// candidates go to *kept in their order; returns how many there are (after a stream synchronisation).  offsets, when given,
-// receives the exclusive scan of the keep mask (n+1 entries): offsets[i] is the number of kept candidates before i.
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const uint32_t* cand, int64_t n,
-                    const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
+// and every pattern of `pats` and comparison of `cmps` holds and, when ndeleted > 0, whose file_ids[i] is not in the host
+// array `deleted`.  The kept candidates go to *kept in their order; returns how many there are (after a stream
+// synchronisation).  offsets, when given, receives the exclusive scan of the keep mask (n+1 entries): offsets[i] is the
+// number of kept candidates before i.
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
+                    int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
                     Buf<uint64_t>* offsets = nullptr);
 
 }  // namespace hs

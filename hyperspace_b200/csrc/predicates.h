@@ -9,15 +9,18 @@
 // rounding casts (long -> double beyond 2^53) are followed exactly.  String columns keep the bounds' bytes and strictness.
 // A term's flags (HS_TERM_*) add NOT -- the complement of the set over the column's domain --, a null outcome, and string
 // patterns: a prefix is one range; other patterns are compiled for the matcher of string_match.h, their literal prefix
-// bounding the values they can match.
+// bounding the values they can match.  A comparison between two columns (hs_column_compare) resolves to the one domain both
+// sides are compared in (resolve_compare); column_compare.h evaluates it.
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
 #include "device_utils.cuh"
+#include "column_compare.h"
 #include "spark_types.h"
 #include "string_match.h"
 
@@ -548,6 +551,97 @@ inline int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_
       const int rc = check_predicates(&q, 1, false, stats, err, errlen);
       if (rc != HS_OK) return rc;
     }
+  }
+  return HS_OK;
+}
+
+
+// ---- comparisons between two columns (hs_column_compare) ----------------------------------------------------------------
+
+// A column's Spark type as the comparison coercion sees it
+enum CompareKind { kKindInt, kKindLong, kKindFloat, kKindDouble, kKindDecimal, kKindString, kKindBinary, kKindDate, kKindTimestamp, kKindOther };
+
+inline int compare_kind(const PredColumn& c) {
+  if (is_decimal(c.schema)) return kKindDecimal;
+  switch (c.type) {
+    case HS_TYPE_INT32: return c.schema.converted_type == pq::CT_DATE ? kKindDate : kKindInt;  // byte and short count as int
+    case HS_TYPE_INT64: return is_timestamp(c.schema) ? kKindTimestamp : kKindLong;
+    case HS_TYPE_FLOAT: return kKindFloat;
+    case HS_TYPE_DOUBLE: return kKindDouble;
+    case HS_TYPE_STRING: return pq::spark_type_name(c.schema) == "binary" ? kKindBinary : kKindString;
+    default: return kKindOther;  // boolean
+  }
+}
+
+inline int64_t pow10_i64(int k) {
+  int64_t p = 1;
+  while (k-- > 0) p *= 10;
+  return p;
+}
+
+// The comparison `l OP r` (check_compares has checked cc) in its domain, column pointers left for the caller.  Spark 3.1's
+// coercion of BinaryComparison(attribute, attribute), as include/hs_gpu.h states it; other pairs are HS_EUNSUPPORTED.
+inline CompareDesc resolve_compare(const hs_column_compare& cc, const PredColumn& l, const PredColumn& r) {
+  CompareDesc d{};
+  d.type[0] = l.type, d.type[1] = r.type;
+  d.factor[0] = d.factor[1] = 1;
+  d.op = cc.op;
+  d.negate = (cc.flags & HS_TERM_NOT) != 0;
+  const int k[2] = {compare_kind(l), compare_kind(r)};
+  auto has = [&](int kind) { return k[0] == kind || k[1] == kind; };
+  auto all_of_kinds = [&](std::initializer_list<int> kinds) {
+    for (int s = 0; s < 2; s++)
+      if (std::find(kinds.begin(), kinds.end(), k[s]) == kinds.end()) return false;
+    return true;
+  };
+  const int scale[2] = {k[0] == kKindDecimal ? l.schema.scale : 0, k[1] == kKindDecimal ? r.schema.scale : 0};
+  if (all_of_kinds({kKindInt, kKindLong})) {
+    d.domain = kCmpInt;
+  } else if ((k[0] == k[1] && (k[0] == kKindDate || k[0] == kKindTimestamp)) || all_of_kinds({kKindDate, kKindTimestamp})) {
+    d.domain = kCmpInt;
+    for (int s = 0; s < 2; s++)
+      if (k[s] == kKindDate && k[s ^ 1] == kKindTimestamp) d.factor[s] = 86400000000ll;
+  } else if (k[0] == k[1] && (k[0] == kKindString || k[0] == kKindBinary)) {
+    d.domain = kCmpString;
+  } else if (has(kKindDecimal) && all_of_kinds({kKindDecimal, kKindInt, kKindLong})) {
+    d.domain = kCmpInt;  // exact: the side of the smaller scale is rescaled
+    const int lo = scale[0] < scale[1] ? 0 : 1;
+    d.factor[lo] = pow10_i64(scale[lo ^ 1] - scale[lo]);
+  } else if (all_of_kinds({kKindInt, kKindLong, kKindFloat, kKindDouble, kKindDecimal})) {
+    if (has(kKindDouble) || has(kKindDecimal)) {
+      d.domain = kCmpDouble;
+      for (int s = 0; s < 2; s++)
+        if (k[s] == kKindDecimal) d.factor[s] = pow10_i64(scale[s]);
+    } else {
+      d.domain = kCmpFloat;
+    }
+  } else {
+    fail(HS_EUNSUPPORTED, "filter scan: the columns '%s' (%s) and '%s' (%s) cannot be compared", l.name.c_str(),
+         pq::spark_type_name(l.schema).c_str(), r.name.c_str(), pq::spark_type_name(r.schema).c_str());
+  }
+  return d;
+}
+
+// The refusals of a comparison list that need no data, beside n_others predicates and terms: as check_anys.
+inline int check_compares(const hs_column_compare* cmps, int n_cmps, int n_others, hs_stats* stats, char* err, size_t errlen) {
+  char msg[256];
+  auto refuse = [&](int code) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (err && errlen) snprintf(err, errlen, "%s", msg);
+    return code;
+  };
+  if (n_cmps < 0 || (n_cmps > 0 && !cmps)) return snprintf(msg, sizeof msg, "filter scan: bad comparison array"), refuse(HS_EINVAL);
+  if (n_others + n_cmps > kMaxPredicates)
+    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
+  for (int i = 0; i < n_cmps; i++) {
+    const hs_column_compare& c = cmps[i];
+    if (!c.left || !c.right) return snprintf(msg, sizeof msg, "filter scan: comparison without a column"), refuse(HS_EINVAL);
+    if (c.op < HS_CMP_LT || c.op > HS_CMP_EQ_NULL_SAFE)
+      return snprintf(msg, sizeof msg, "filter scan: comparison of '%s' and '%s' has an unknown operator %d", c.left, c.right, c.op),
+             refuse(HS_EINVAL);
+    if (c.flags & ~HS_TERM_NOT)
+      return snprintf(msg, sizeof msg, "filter scan: comparison of '%s' and '%s' has unknown flags 0x%x", c.left, c.right, c.flags),
+             refuse(HS_EINVAL);
   }
   return HS_OK;
 }

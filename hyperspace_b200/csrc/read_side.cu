@@ -149,6 +149,21 @@ __global__ void k_pattern_mask(const __grid_constant__ PatternSet ps, const uint
   }
 }
 
+// The comparisons between two columns, one thread per candidate row: clears mask[i] where one of them does not hold for
+// row cand[i] (row i without a candidate list); rows already dropped by k_predicate_mask or k_pattern_mask are skipped.
+// Inside a window the candidates are consecutive rows, so both columns of a comparison are read coalesced.
+__global__ void __launch_bounds__(256, 8) k_compare_mask(const __grid_constant__ CompareSet cs, const uint32_t* __restrict__ cand, int64_t n,
+                               uint32_t* __restrict__ mask) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (!mask[i]) continue;
+    const int64_t row = cand ? (int64_t)cand[i] : i;
+    bool ok = true;
+    for (int p = 0; p < cs.n && ok; p++) ok = compare_holds(cs.p[p], row);
+    if (!ok) mask[i] = 0;
+  }
+}
+
 // a key value at position p, read at its type's width: int32 sign-extended, int64 as it is, a string as its reference
 template <int KT>
 __device__ __forceinline__ int64_t key_value(const void* col, int64_t p) {
@@ -418,6 +433,14 @@ void launch_pattern_mask(hs_ctx* ctx, const PatternSet& pats, const uint32_t* ca
   HS_LAUNCH_CHECK(ctx);
 }
 
+void launch_compare_mask(hs_ctx* ctx, const CompareSet& cmps, const uint32_t* cand, int64_t n, uint32_t* mask) {
+  if (cmps.n == 0) return;
+  KernelScope _ks(ctx, "k_compare_mask");
+  if (n == 0) return;
+  k_compare_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(cmps, cand, n, mask);
+  HS_LAUNCH_CHECK(ctx);
+}
+
 void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
                        const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
   KernelScope _ks(ctx, "k_join_count");
@@ -449,14 +472,16 @@ void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t
   }
 }
 
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const uint32_t* cand, int64_t n,
-                    const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets) {
+int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
+                    int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
+                    Buf<uint64_t>* offsets) {
   Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
   Buf<uint64_t> own_offsets;
   if (!offsets) offsets = &own_offsets;
   offsets->alloc(ctx, n + 1);
   launch_predicate_mask(ctx, preds, cand, n, mask.get());
   launch_pattern_mask(ctx, pats, cand, n, mask.get());
+  launch_compare_mask(ctx, cmps, cand, n, mask.get());
   Buf<int64_t> d_deleted;
   if (n > 0 && ndeleted > 0) {
     d_deleted.alloc(ctx, ndeleted);

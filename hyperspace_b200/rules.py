@@ -7,7 +7,7 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan_any (K1 + K7) and hs_bucket_join_any (K1 + K8).
+Physical execution is the C ABI: hs_filter_scan_cmp (K1 + K7) and hs_bucket_join_cmp (K1 + K8).
 """
 from __future__ import annotations
 
@@ -185,14 +185,17 @@ def _host_column(d: np.ndarray) -> np.ndarray:
 
 
 def _terms_text(pred) -> str:
-    """The disjunction terms of a filter for explain(), long lists cut short: `k IN (1, 2, 3, ... 997 more)`."""
+    """The disjunction terms and column comparisons of a filter for explain(), long lists cut short: `k IN (1, 2, 3, ... 997
+    more)`, `(a < b)`."""
     anys = pred.disjunctions() if pred else []
-    return "".join(f", where=({a})" for a in anys)
+    cmps = pred.comparisons() if pred else []
+    return "".join(f", where=({a})" for a in anys) + "".join(f", where=({c})" for c in cmps)
 
 
 class ScanExec:
-    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_any with
-    the filter's comparisons as its predicates and its disjunctions (isin, |) as its terms."""
+    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_cmp with
+    the filter's comparisons with literals as its predicates, its disjunctions (isin, |) as its terms and its comparisons
+    between two columns as its compares."""
 
     def __init__(self, session, lin: Linear, cand: Optional[Candidate]):
         self.session, self.lin, self.cand = session, lin, cand
@@ -210,8 +213,9 @@ class ScanExec:
     def _scan(self, files, key, out_cols, sorted_on_key, deleted_ids=(), buckets=None, num_buckets=0):
         preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
         terms = [a.as_native() for a in self.lin.predicate.disjunctions()] if self.lin.predicate else []
+        cmps = [c.as_native() for c in self.lin.predicate.comparisons()] if self.lin.predicate else []
         # file_buckets only where the files are bucketed on the key alone
-        batch, _ = self.session.gpu.filter_scan_any(files, key, out_cols, preds, terms, sorted_on_key=sorted_on_key,
+        batch, _ = self.session.gpu.filter_scan_cmp(files, key, out_cols, preds, terms, cmps, sorted_on_key=sorted_on_key,
                                                     deleted_file_ids=list(deleted_ids), file_buckets=buckets, num_buckets=num_buckets)
         types = dict(self.lin.relation.schema)
         out = {n: spark_values(_host_column(d), types.get(n)) for n, d, _ in batch.columns}
@@ -297,8 +301,9 @@ class BucketJoinExec:
             lp = self.left.predicate.conjuncts() if self.left.predicate else []
             rp = self.right.predicate.conjuncts() if self.right.predicate else []
             lt_, rt_ = ([a.as_native() for a in lin.predicate.disjunctions()] if lin.predicate else [] for lin in (self.left, self.right))
-            batch, _ = self.session.gpu.bucket_join_any(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                        lp, rp, lt_, rt_)
+            lc_, rc_ = ([c.as_native() for c in lin.predicate.comparisons()] if lin.predicate else [] for lin in (self.left, self.right))
+            batch, _ = self.session.gpu.bucket_join_cmp(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                        lp, rp, lt_, rt_, lc_, rc_)
         finally:
             for t in lt + rt:
                 t.free()

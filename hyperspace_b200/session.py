@@ -173,6 +173,25 @@ class AnyTerm:
         return self.column, self.values, list(self.ranges), flags
 
 
+@dataclass
+class ColumnCompare:
+    """A comparison between two columns of the same row (Spark's BinaryComparison of two attributes): ``left op right`` with
+    op one of <, <=, >, >=, = and <=> (EqualNullSafe), under Not when ``negated``.  The engine coerces the two columns'
+    types as Spark does; a null on either side makes it unknown, except for <=>."""
+    left: str
+    op: str
+    right: str
+    negated: bool = False
+
+    def __str__(self) -> str:
+        inner = f"({self.left} {self.op} {self.right})"
+        return f"NOT {inner}" if self.negated else inner
+
+    def as_native(self) -> tuple:
+        """(left, op, right, HS_TERM_* flags) for Context.filter_scan_cmp / bucket_join_cmp."""
+        return self.left, self.op, self.right, _TERM_NOT if self.negated else 0
+
+
 def _prefix_range(p) -> Tuple[object, bool, object, bool]:
     """The values that start with p, as a range: [p, succ(p)), succ(p) being p without its trailing 0xff bytes and its
     last byte incremented; open above when nothing is left."""
@@ -191,10 +210,11 @@ class Predicate:
     """Conjunction of comparisons with literals.  ``bounds`` is the inclusive integer (or byte-string) range per column, which
     the plan layer uses to pick an index; ``terms`` are the comparisons as written -- (column, operator, literal) with the
     operator one of >=, >, <=, <, == -- which the engine evaluates with Spark's type coercion.  ``anys`` are AND-ed
-    disjunctions on one column each (``isin`` and ``|``)."""
+    disjunctions on one column each (``isin`` and ``|``); ``compares`` are AND-ed comparisons between two columns."""
     bounds: Dict[str, Tuple[Optional[int], Optional[int]]]
     terms: List[Tuple[str, str, object]] = field(default_factory=list)
     anys: List[AnyTerm] = field(default_factory=list, repr=False)  # explain() shows them by their SQL form
+    compares: List[ColumnCompare] = field(default_factory=list, repr=False)
 
     def __and__(self, other: "Predicate") -> "Predicate":
         out = dict(self.bounds)
@@ -204,11 +224,14 @@ class Predicate:
                 lo = l0 if lo is None else (lo if l0 is None else max(lo, l0))
                 hi = h0 if hi is None else (hi if h0 is None else min(hi, h0))
             out[c] = (lo, hi)
-        return Predicate(out, self._as_terms() + other._as_terms(), self.anys + other.anys)
+        return Predicate(out, self._as_terms() + other._as_terms(), self.anys + other.anys, self.compares + other.compares)
 
     def __or__(self, other: "Predicate") -> "Predicate":
         """An Or of branches on one and the same column, each a comparison, a conjunction of comparisons that is one range
         (at most one lower and one upper bound), or an isin / Or on that column; anything else raises."""
+        for branch in (self, other):
+            if branch.compares:
+                raise LE.HyperspaceException(f"an OR across columns ({branch.compares[0]}) is not handled by the GPU path")
         c = self._single_column()
         if other._single_column().lower() != c.lower():
             raise LE.HyperspaceException(f"an OR across columns ({c}, {other._single_column()}) is not handled by the GPU path")
@@ -232,9 +255,12 @@ class Predicate:
         return Predicate({}, [], [merged])
 
     def __invert__(self) -> "Predicate":
-        """Not of a filter on one column: of one comparison or range, or of one isin, OR, null test or pattern."""
+        """Not of a filter on one column: of one comparison or range, or of one isin, OR, null test or pattern; or of one
+        comparison between two columns."""
         cols = {c.lower(): c for c in self.columns}
-        if len(cols) != 1:
+        if self.compares and len(self.compares) == 1 and not self.anys and not self._as_terms():
+            return Predicate({}, [], [], [dataclasses.replace(self.compares[0], negated=not self.compares[0].negated)])
+        if len(cols) != 1 or self.compares:
             raise LE.HyperspaceException(f"a NOT over several columns ({', '.join(cols.values())}) is not handled by the GPU "
                                          "path: it would be an OR across columns")
         if self.anys:
@@ -282,9 +308,17 @@ class Predicate:
                 out.append((c, "<=", hi))
         return out
 
+    def comparisons(self) -> List[ColumnCompare]:
+        """The AND-ed comparisons between two columns, which conjuncts() and disjunctions() do not list."""
+        return list(self.compares)
+
     @property
     def columns(self) -> List[str]:
-        return list(self.bounds) + [a.column for a in self.anys if a.column not in self.bounds]
+        out = list(self.bounds)
+        for c in [a.column for a in self.anys] + [n for cc in self.compares for n in (cc.left, cc.right)]:
+            if c not in out:
+                out.append(c)
+        return out
 
     def conjuncts(self) -> List[Tuple[str, object, bool, object, bool]]:
         """The comparisons as (column, lo, lo_strict, hi, hi_strict) ranges for Context.filter_scan_where (a Predicate
@@ -327,27 +361,40 @@ class Column:
     # integer key columns: a non-integral literal is rounded in the direction that keeps the predicate's meaning
     # (k < 1.5  <=>  k <= 1;  k >= 1.5  <=>  k >= 2).  String / binary literals give byte bounds in UTF8String order --
     # `col("Query") == "facebook"` is the predicate of the reference's own filter-rule tests (T/index/E2EHyperspaceRulesTest.scala).
+    def _compare(self, op: str, other: "Column", negated: bool = False) -> Predicate:
+        return Predicate({}, [], [], [ColumnCompare(self.name, op, other.name, negated)])
+
     def __ge__(self, v):
+        if isinstance(v, Column):
+            return self._compare(">=", v)
         if isinstance(v, (str, bytes)):
             return Predicate({self.name: (_as_bytes(v), None)}, [(self.name, ">=", v)])
         return Predicate({self.name: (_ceil(v), None)}, [(self.name, ">=", v)])
 
     def __gt__(self, v):
+        if isinstance(v, Column):
+            return self._compare(">", v)
         if isinstance(v, (str, bytes)):
             return Predicate({self.name: (_as_bytes(v) + b"\x00", None)}, [(self.name, ">", v)])  # the smallest value above v
         return Predicate({self.name: (_floor(v) + 1, None)}, [(self.name, ">", v)])
 
     def __le__(self, v):
+        if isinstance(v, Column):
+            return self._compare("<=", v)
         if isinstance(v, (str, bytes)):
             return Predicate({self.name: (None, _as_bytes(v))}, [(self.name, "<=", v)])
         return Predicate({self.name: (None, _floor(v))}, [(self.name, "<=", v)])
 
     def __lt__(self, v):
+        if isinstance(v, Column):
+            return self._compare("<", v)
         if isinstance(v, (str, bytes)):
             raise ValueError("a strict upper bound on a string column has no inclusive form: use <= or between")
         return Predicate({self.name: (None, _ceil(v) - 1)}, [(self.name, "<", v)])
 
     def __eq__(self, v):  # noqa: A003
+        if isinstance(v, Column):
+            return self._compare("=", v)
         if isinstance(v, (str, bytes)):
             return Predicate({self.name: (_as_bytes(v), _as_bytes(v))}, [(self.name, "==", v)])
         n = _number(v)
@@ -357,6 +404,8 @@ class Column:
 
     def __ne__(self, v):  # noqa: A003
         """Not(EqualTo): a null row, or a None literal, gives unknown."""
+        if isinstance(v, Column):
+            return self._compare("=", v, negated=True)
         return ~self.isin([v])
 
     def isin(self, *values) -> Predicate:
@@ -365,6 +414,9 @@ class Column:
         list is cast as Spark casts it (a float makes every value a double, Decimals share one scale).  Strings mixed with
         numbers raise."""
         vals = values[0] if len(values) == 1 and isinstance(values[0], (list, tuple, set, frozenset, np.ndarray)) else values
+        if not isinstance(vals, np.ndarray) and any(isinstance(v, Column) for v in vals):
+            raise LE.HyperspaceException(f"isin on '{self.name}' with a column value is an OR across columns, which is not "
+                                         "handled by the GPU path")
         had_none = not isinstance(vals, np.ndarray) and any(v is None for v in vals)
         vals = vals if isinstance(vals, np.ndarray) else [v for v in vals if v is not None]
         return Predicate({}, [], [AnyTerm(self.name, self._checked(vals, "isin"), null_in_list=had_none)])
@@ -388,6 +440,8 @@ class Column:
         """EqualNullSafe (`<=>`): a null row gives false, and `eqNullSafe(None)` is isNull()."""
         if v is None:
             return self.isNull()
+        if isinstance(v, Column):
+            return self._compare("<=>", v)
         return Predicate({}, [], [AnyTerm(self.name, self._checked([v], "eqNullSafe"), null=False)])
 
     def _pattern(self, kind, p) -> Predicate:
@@ -411,6 +465,8 @@ class Column:
         return self._pattern("like", pattern)
 
     def between(self, lo, hi):
+        if isinstance(lo, Column) or isinstance(hi, Column):  # two conjuncts: lo <= self AND self <= hi
+            return (self >= lo) & (self <= hi)
         terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
         if isinstance(lo, (str, bytes)) or isinstance(hi, (str, bytes)):
             return Predicate({self.name: (_as_bytes(lo), _as_bytes(hi))}, terms)
@@ -552,10 +608,24 @@ class DataFrame:
         return name if name in hits else hits[0]
 
     def filter(self, predicate: Predicate) -> "DataFrame":
+        self._refuse_join_compares(predicate)
         resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
                              [(self._resolve(c), op, v) for c, op, v in predicate.terms],
-                             [dataclasses.replace(a, column=self._resolve(a.column), ranges=list(a.ranges)) for a in predicate.anys])
+                             [dataclasses.replace(a, column=self._resolve(a.column), ranges=list(a.ranges)) for a in predicate.anys],
+                             [dataclasses.replace(c, left=self._resolve(c.left), right=self._resolve(c.right)) for c in predicate.compares])
         return DataFrame(self.session, FilterNode(self.plan, resolved))
+
+    def _refuse_join_compares(self, predicate: Predicate) -> None:
+        """A comparison between a column of each side of a join is a non-equi join condition, not a filter of one side."""
+        node = self.plan.child if isinstance(self.plan, ProjectNode) else self.plan
+        if not isinstance(node, JoinNode):
+            return
+        sides = [{c.lower() for c in output_columns(node.left)}, {c.lower() for c in output_columns(node.right)}]
+        for c in predicate.compares:
+            in_sides = [{i for i, side in enumerate(sides) if n.lower() in side} for n in (c.left, c.right)]
+            if in_sides[0] and in_sides[1] and not (in_sides[0] & in_sides[1]):
+                raise LE.HyperspaceException(f"{c} compares columns of the two sides of a join: a non-equi join condition, "
+                                             "which the GPU path does not handle")
 
     where = filter
 
@@ -566,6 +636,10 @@ class DataFrame:
     def join(self, other: "DataFrame", on, how: str = "inner") -> "DataFrame":
         if how != "inner":
             raise LE.HyperspaceException("only inner equi-joins are handled by the GPU path")
+        if isinstance(on, Predicate):
+            shown = ", ".join(str(c) for c in on.compares) or "a filter"
+            raise LE.HyperspaceException(f"join `on` {shown}: a non-equi join condition, which the GPU path does not handle; "
+                                         "join on column names")
         if isinstance(on, str):
             pairs = [(on, on)]
         elif isinstance(on, tuple) and len(on) == 2 and all(isinstance(c, str) for c in on):

@@ -351,6 +351,50 @@ int hs_filter_scan_any(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate
                        const hs_predicate_any* anys, int32_t n_anys, const int32_t* file_buckets, int32_t num_buckets,
                        hs_batch** out, hs_stats* stats, char* err, size_t errlen);
 
+/* A comparison between two columns of the same row: `left OP right`, with NOT when flags has HS_TERM_NOT (`a != b` is NOT
+ * of HS_CMP_EQ).  Spark 3.1 semantics:
+ *   Nulls: a null on either side makes LT, LE, GT, GE and EQ unknown, so the row does not qualify, under NOT too.
+ *          EQ_NULL_SAFE (`<=>`) is true on two nulls and false on one; NOT applies to that, so NOT (a <=> b) keeps the rows
+ *          where exactly one side is null.
+ *   Order: as the literal comparisons -- NaN equals NaN and is above +inf, -0.0 equals 0.0, strings in UTF8String byte
+ *          order.
+ *   Coercion (TypeCoercion and DecimalPrecision for BinaryComparison(attribute, attribute)), resolved once per call:
+ *     the same type (int, long, float, double, string, binary, date, timestamp, decimal(p,s) of equal p and s): that type;
+ *     int against long: long;
+ *     int or long against float: float, the integer rounded to nearest (2^24 + 1 equals 16777216f);
+ *     int, long or float against double: double;
+ *     decimal against a decimal of another precision or scale, or against int / long (as decimal(10,0) / decimal(20,0)):
+ *       exactly, the side of the smaller scale rescaled in 128 bits;
+ *     decimal against float or double: double (the decimal rounded to nearest);
+ *     date against timestamp: timestamp, the date's days times 86 400 000 000 micros (dates are UTC midnights, as the
+ *       naive timestamp literals are UTC).
+ *   Any other pair -- string against a number, date or timestamp; date or timestamp against a number; a boolean column --
+ *   is HS_EUNSUPPORTED naming both columns and their Spark types.  A NULL name, an op outside HS_CMP_*, or a flag other
+ *   than HS_TERM_NOT is HS_EINVAL; an unknown column fails as an unknown predicate column does.  Both names may be the
+ *   same column. */
+typedef struct {
+  const char* left;
+  const char* right;
+  int32_t op;     /* HS_CMP_* */
+  int32_t flags;  /* 0 or HS_TERM_NOT */
+} hs_column_compare;
+
+#define HS_CMP_LT 1
+#define HS_CMP_LE 2
+#define HS_CMP_GT 3
+#define HS_CMP_GE 4
+#define HS_CMP_EQ 5
+#define HS_CMP_EQ_NULL_SAFE 6
+
+/* hs_filter_scan_any with column comparisons AND-ed to the predicates and terms (n_preds + n_anys + n_cmps <= 16).  Both
+ * columns of every comparison are decoded like other predicate columns (on sorted files, only inside the key's windows)
+ * and the comparisons run per row.  A comparison makes no key window and prunes no bucket: when the key appears in the
+ * filter only through comparisons, the scan of sorted files reads every row.  With n_cmps = 0 this is hs_filter_scan_any. */
+int hs_filter_scan_cmp(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                       const hs_predicate_any* anys, int32_t n_anys, const hs_column_compare* cmps, int32_t n_cmps,
+                       const int32_t* file_buckets, int32_t num_buckets, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen);
+
 typedef struct {
   const hs_source_file* left_files;  /* index files of the left side, any order; bucket id parsed from the name */
   int32_t n_left;
@@ -398,6 +442,16 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
                        int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
                        int32_t n_left_anys, const hs_predicate* right_preds, int32_t n_right_preds,
                        const hs_predicate_any* right_anys, int32_t n_right_anys, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen);
+
+/* hs_bucket_join_any with hs_column_compare comparisons AND-ed to each side's filter (n_preds + n_anys + n_cmps <= 16 per
+ * side); both columns of a comparison belong to that side.  They run per row in the side selection.  With no comparisons
+ * this is hs_bucket_join_any. */
+int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
+                       int32_t n_left_anys, const hs_column_compare* left_cmps, int32_t n_left_cmps, const hs_predicate* right_preds,
+                       int32_t n_right_preds, const hs_predicate_any* right_anys, int32_t n_right_anys,
+                       const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
                        size_t errlen);
 
 int64_t hs_batch_num_rows(const hs_batch* b);
