@@ -30,6 +30,8 @@ HS_TERM_STARTS_WITH, HS_TERM_ENDS_WITH, HS_TERM_CONTAINS, HS_TERM_LIKE = 8, 16, 
 # hs_column_compare.op
 HS_CMP_LT, HS_CMP_LE, HS_CMP_GT, HS_CMP_GE, HS_CMP_EQ, HS_CMP_EQ_NULL_SAFE = 1, 2, 3, 4, 5, 6
 CMP_OPS = {"<": HS_CMP_LT, "<=": HS_CMP_LE, ">": HS_CMP_GT, ">=": HS_CMP_GE, "=": HS_CMP_EQ, "<=>": HS_CMP_EQ_NULL_SAFE}
+HS_JOIN_LEFT_SEMI, HS_JOIN_LEFT_ANTI = 1, 2  # join_type of hs_bucket_join_exists
+JOIN_TYPES = {"semi": HS_JOIN_LEFT_SEMI, "anti": HS_JOIN_LEFT_ANTI}
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -132,7 +134,7 @@ EXPORTED_SYMBOLS = [
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
-    "hs_filter_scan_cmp", "hs_bucket_join_cmp",
+    "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -201,6 +203,12 @@ def load_library() -> C.CDLL:
                                      C.POINTER(ColumnCompareSpec), C.c_int32,
                                      C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
                                      C.POINTER(ColumnCompareSpec), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    L.hs_bucket_join_exists.restype = C.c_int
+    L.hs_bucket_join_exists.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
+                                        C.c_int32, C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                        C.POINTER(ColumnCompareSpec), C.c_int32,
+                                        C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
+                                        C.POINTER(ColumnCompareSpec), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join.restype = C.c_int
     L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     L.hs_bucket_join_where.restype = C.c_int
@@ -1063,6 +1071,33 @@ class Context:
         err = C.create_string_buffer(1024)
         _check(L.hs_bucket_join_cmp(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, lc, nlc, rp, nrp, ra, nra, rc, nrc,
                                     C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
+    def bucket_join_exists(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                           right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                           left_columns: Sequence[str], join_type="semi", left_predicates: Sequence[tuple] = (),
+                           right_predicates: Sequence[tuple] = (), left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (),
+                           left_compares: Sequence[tuple] = (), right_compares: Sequence[tuple] = (),
+                           output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_exists: the left semi (``join_type="semi"``) or left anti (``"anti"``) join of bucket_join_cmp's
+        sides.  The batch holds left_columns only, each kept left row once, in (bucket, left sorted position) order.  Semi
+        drops left rows with a null key; anti keeps them.  join_type may also be an HS_JOIN_* code (others are refused
+        by the library)."""
+        L = load_library()
+        if isinstance(join_type, str) and join_type not in JOIN_TYPES:
+            raise ValueError(f"join_type must be one of {sorted(JOIN_TYPES)} or an HS_JOIN_* code, not {join_type!r}")
+        jt = JOIN_TYPES[join_type] if isinstance(join_type, str) else join_type
+        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
+                                                                          left_keys, right_keys, left_columns, [],
+                                                                          left_predicates, right_predicates, output)
+        la, nla, k1 = _any_array(left_terms)
+        ra, nra, k2 = _any_array(right_terms)
+        lc, nlc, k3 = _cmp_array(left_compares)
+        rc, nrc, k4 = _cmp_array(right_compares)
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(L.hs_bucket_join_exists(self._h, C.byref(spec), jt, lk, rk, len(left_keys), lp, nlp, la, nla, lc, nlc, rp, nrp, ra, nra,
+                                       rc, nrc, C.byref(res), C.byref(st), err, len(err)), err)
         return Batch(res.value, self), st.as_dict()
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------

@@ -1422,14 +1422,18 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, con
   sync_stream(ctx);
 }
 
-// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  k_join_count
-// probes on the key columns where they lie: the decoded columns, or their gather through the side's permutation.
+// bucket_join_core's join_type for the inner join (include/hs_gpu.h numbers the semi and anti joins from 1)
+constexpr int kJoinInner = 0;
+
+// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  k_join_count (inner)
+// or k_join_exists (join_type HS_JOIN_LEFT_SEMI / HS_JOIN_LEFT_ANTI) probes on the key columns where they lie: the decoded
+// columns, or their gather through the side's permutation.
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                             int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
                             int n_right_preds, const hs_predicate_any* left_anys, int n_left_anys,
                             const hs_predicate_any* right_anys, int n_right_anys, const hs_column_compare* left_cmps,
-                            int n_left_cmps, const hs_column_compare* right_cmps, int n_right_cmps, bool legacy, hs_batch** out,
-                            hs_stats* stats, char* err, size_t errlen) {
+                            int n_left_cmps, const hs_column_compare* right_cmps, int n_right_cmps, bool legacy, int join_type,
+                            hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   hs_stats st;
   memset(&st, 0, sizeof st);
   std::unique_ptr<hs_batch> res(new hs_batch());
@@ -1482,7 +1486,9 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
         fail(HS_EUNSUPPORTED, "bucket join: key columns '%s' and '%s' have different types", left_keys[k], right_keys[k]);
       }
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
-    // side selection: IS NOT NULL on the nullable key columns, then the side's predicates
+    // side selection: IS NOT NULL on the nullable key columns, then the side's predicates.  An anti join keeps the left
+    // rows with a null key (they match nothing, so they are output): its probe reads their validity instead.
+    const bool anti = join_type == HS_JOIN_LEFT_ANTI;
     PredUploads uploads;
     TermResolutions lterms(left_anys, n_left_anys), rterms(right_anys, n_right_anys);  // outlive the copies of their patterns
     auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, TermResolutions& terms,
@@ -1490,7 +1496,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       PredSet ps;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
-        if (c.has_nulls) {
+        if (c.has_nulls && !(anti && &s == &L)) {
           PredDesc d{};
           d.data = c.data.get(), d.valid = c.valid.get(), d.r.type = c.type;
           ps.p[ps.n++] = d;
@@ -1511,18 +1517,19 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     t_sel.stop();
     // the key columns in (selected) sorted order
     std::vector<Buf<uint8_t>> key_bufs;
+    auto sorted_column = [&](const JoinSide& s, const uint8_t* data, int width) {
+      if (!s.perm) return data;
+      key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n) * width);
+      launch_gather_plain(ctx, data, s.perm, s.n, width, key_bufs.back().get());
+      return (const uint8_t*)key_bufs.back().get();
+    };
     auto key_cols = [&](const JoinSide& s) {
       JoinKeyCols kc{};
       kc.n = n_keys;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
         kc.type[k] = c.type;
-        kc.col[k] = c.data.get();
-        if (s.perm) {
-          key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n) * c.width);
-          launch_gather_plain(ctx, c.data.get(), s.perm, s.n, c.width, key_bufs.back().get());
-          kc.col[k] = key_bufs.back().get();
-        }
+        kc.col[k] = sorted_column(s, c.data.get(), c.width);
       }
       return kc;
     };
@@ -1532,20 +1539,37 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     Buf<uint64_t> d_lseg(ctx, nb + 1), d_rseg(ctx, nb + 1);
     copy_h2d(ctx, d_lseg.get(), L.seg.data(), 8 * (nb + 1));
     copy_h2d(ctx, d_rseg.get(), R.seg.data(), 8 * (nb + 1));
-    Buf<uint32_t> counts(ctx, std::max<int64_t>(1, nl)), first(ctx, std::max<int64_t>(1, nl));
-    Buf<uint64_t> offs(ctx, nl + 1);
     const JoinKeyCols lk = key_cols(L), rk = key_cols(R);
-    launch_join_count(ctx, lk, d_lseg.get(), rk, d_rseg.get(), nb, nl, counts.get(), first.get());
-    exclusive_scan_u32_u64(ctx, counts.get(), nl, offs.get());
     uint64_t total_out = 0;
-    copy_d2h(ctx, &total_out, offs.get() + nl, 8);
-    sync_stream(ctx);
-    if (total_out >= (1ull << 32)) fail(HS_EUNSUPPORTED, "join output larger than 2^32-1 rows per call");
-    Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
-    launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, L.perm, R.perm, lrow.get(), rrow.get());
-    t_join.stop();
-    batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
-    batch_from_gather(ctx, R.t, rproj, rrow.get(), (int64_t)total_out, res.get());
+    if (join_type != kJoinInner) {
+      // semi / anti: one keep mask over the left sorted positions, compacted through L.perm into left rows
+      JoinKeyValid lv{};
+      if (anti) {
+        lv.n = n_keys;
+        for (int k = 0; k < n_keys; k++) {
+          const DevColumn& c = L.t.cols[k];
+          if (c.has_nulls) lv.valid[k] = sorted_column(L, c.valid.get(), 1);
+        }
+      }
+      Buf<uint32_t> keep(ctx, std::max<int64_t>(1, nl)), lrow;
+      launch_join_exists(ctx, lk, lv, d_lseg.get(), rk, d_rseg.get(), nb, nl, !anti, keep.get());
+      total_out = (uint64_t)compact_rows(ctx, keep.get(), nl, L.perm, &lrow);
+      t_join.stop();
+      batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
+    } else {
+      Buf<uint32_t> counts(ctx, std::max<int64_t>(1, nl)), first(ctx, std::max<int64_t>(1, nl));
+      Buf<uint64_t> offs(ctx, nl + 1);
+      launch_join_count(ctx, lk, d_lseg.get(), rk, d_rseg.get(), nb, nl, counts.get(), first.get());
+      exclusive_scan_u32_u64(ctx, counts.get(), nl, offs.get());
+      copy_d2h(ctx, &total_out, offs.get() + nl, 8);
+      sync_stream(ctx);
+      if (total_out >= (1ull << 32)) fail(HS_EUNSUPPORTED, "join output larger than 2^32-1 rows per call");
+      Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
+      launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, L.perm, R.perm, lrow.get(), rrow.get());
+      t_join.stop();
+      batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
+      batch_from_gather(ctx, R.t, rproj, rrow.get(), (int64_t)total_out, res.get());
+    }
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
@@ -1565,7 +1589,7 @@ int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_sta
   if (!ctx || !spec || !out) return HS_EINVAL;
   *out = nullptr;
   return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                          nullptr, 0, true, out, stats, err, errlen);
+                          nullptr, 0, true, kJoinInner, out, stats, err, errlen);
 }
 
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
@@ -1584,12 +1608,15 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
                             right_preds, n_right_preds, right_anys, n_right_anys, nullptr, 0, out, stats, err, errlen);
 }
 
-int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
-                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
-                       int32_t n_left_anys, const hs_column_compare* left_cmps, int32_t n_left_cmps, const hs_predicate* right_preds,
-                       int32_t n_right_preds, const hs_predicate_any* right_anys, int32_t n_right_anys,
-                       const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
-                       size_t errlen) {
+}  // extern "C"
+
+// hs_bucket_join_cmp's and hs_bucket_join_exists's checks that need no data, then the join
+static int bucket_join_checked(hs_ctx* ctx, const hs_join_spec* spec, int join_type, const char* const* left_keys,
+                               const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                               const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                               int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
+                               const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
+                               int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
       (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
     return HS_EINVAL;
@@ -1599,6 +1626,10 @@ int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
     if (err && errlen) snprintf(err, errlen, "%s", msg);
     return code;
   };
+  if (join_type != kJoinInner && join_type != HS_JOIN_LEFT_SEMI && join_type != HS_JOIN_LEFT_ANTI)
+    return refuse(HS_EINVAL, "bucket join: join_type must be HS_JOIN_LEFT_SEMI or HS_JOIN_LEFT_ANTI");
+  if (join_type != kJoinInner && spec->n_right_columns != 0)
+    return refuse(HS_EINVAL, "bucket join: a semi or anti join outputs left columns only (n_right_columns must be 0)");
   if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
   if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
   if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
@@ -1610,8 +1641,33 @@ int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
   if (rc == HS_OK) rc = check_compares(right_cmps, n_right_cmps, n_right_preds + n_right_anys, stats, err, errlen);
   if (rc != HS_OK) return rc;
   return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, left_anys,
-                          n_left_anys, right_anys, n_right_anys, left_cmps, n_left_cmps, right_cmps, n_right_cmps, false, out, stats,
-                          err, errlen);
+                          n_left_anys, right_anys, n_right_anys, left_cmps, n_left_cmps, right_cmps, n_right_cmps, false, join_type,
+                          out, stats, err, errlen);
+}
+
+extern "C" {
+
+int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
+                       int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds, const hs_predicate_any* left_anys,
+                       int32_t n_left_anys, const hs_column_compare* left_cmps, int32_t n_left_cmps, const hs_predicate* right_preds,
+                       int32_t n_right_preds, const hs_predicate_any* right_anys, int32_t n_right_anys,
+                       const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
+                       size_t errlen) {
+  return bucket_join_checked(ctx, spec, kJoinInner, left_keys, right_keys, n_keys, left_preds, n_left_preds, left_anys, n_left_anys,
+                             left_cmps, n_left_cmps, right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps,
+                             out, stats, err, errlen);
+}
+
+int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                          const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                          const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                          int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
+                          const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
+                          int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  // an inner join is hs_bucket_join_cmp's: kJoinInner (0) is refused like any other value outside HS_JOIN_*
+  return bucket_join_checked(ctx, spec, join_type == kJoinInner ? -1 : join_type, left_keys, right_keys, n_keys, left_preds,
+                             n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps, right_preds, n_right_preds, right_anys,
+                             n_right_anys, right_cmps, n_right_cmps, out, stats, err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

@@ -480,6 +480,16 @@ void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* ls
 // (perm nullptr: row p)
 void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
                       int64_t nl, const uint32_t* lperm, const uint32_t* rperm, uint32_t* out_lrow, uint32_t* out_rrow);
+// The validity of the n key columns of the left side in sorted order, one byte per position (valid[k] nullptr: key
+// column k has no nulls): a position with a null in any of them matches nothing.
+struct JoinKeyValid {
+  const uint8_t* valid[kMaxJoinKeys];
+  int32_t n;
+};
+// The semi / anti join's probe (k_join_exists): keep[i] = 1 when left position i has an equal key tuple among the right
+// positions of its bucket and keep_match is set (semi), or has none and keep_match is clear (anti); 0 otherwise
+void launch_join_exists(hs_ctx* ctx, const JoinKeyCols& lkeys, const JoinKeyValid& lvalid, const uint64_t* lseg,
+                        const JoinKeyCols& rkeys, const uint64_t* rseg, int nseg, int64_t nl, bool keep_match, uint32_t* keep);
 // exclusive scan of uint32 counts into uint64 offsets (n+1 entries; last = total)
 void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t* out);
 // lens[i] = length of refs[idx[i]] (0 for a null);  then, with offsets = exclusive scan of lens: out[offsets[i] ..] = bytes
@@ -495,5 +505,10 @@ void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid
 int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
                     int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
                     Buf<uint64_t>* offsets = nullptr);
+// The compaction select_rows ends with, over a keep mask of n candidates (1 / 0): the kept cand[i] (i when cand is
+// nullptr) go to *kept in their order; returns how many there are (after a stream synchronisation); offsets as in
+// select_rows.
+int64_t compact_rows(hs_ctx* ctx, const uint32_t* mask, int64_t n, const uint32_t* cand, Buf<uint32_t>* kept,
+                     Buf<uint64_t>* offsets = nullptr);
 
 }  // namespace hs

@@ -187,38 +187,55 @@ __device__ __forceinline__ int compare_column(const JoinKeyCols& l, int64_t i, c
   }
 }
 
-// One thread per left position; the segment of a position is found by binary search over the (few hundred) segment
-// offsets.  The right positions of a bucket are ascending on the key tuples, so the matches of a left position are the
-// range between two lexicographic binary searches.  The leading key column, KT0 its type, decides almost every step: its
-// left value stays in a register and its comparison is compiled in, so a step is one load and a branch-free compare.  The
-// later columns are compared only where the leading ones tie.
+// the segment of position i: the last s with seg[s] <= i, by binary search over the (few hundred) segment offsets
+__device__ __forceinline__ int segment_of(const uint64_t* __restrict__ seg, int nseg, int64_t i) {
+  int lo = 0, hi = nseg;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (seg[mid] <= (uint64_t)i) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// the left tuple at position i, its leading value l0 held in a register, against right position j
+template <int KT0>
+__device__ __forceinline__ int compare_tuple(int64_t l0, const JoinKeyCols& lk, int64_t i, const JoinKeyCols& rk, int64_t j) {
+  int c = compare_keys<KT0>(l0, key_value<KT0>(rk.col[0], j));
+  for (int k = 1; k < rk.n && c == 0; k++) c = compare_column(lk, i, rk, j, k);
+  return c;
+}
+
+// the first of the right positions [rb, rb + rn) whose tuple is >= the left tuple at i, relative to rb (rn: none is)
+template <int KT0>
+__device__ __forceinline__ int64_t lower_bound_tuple(int64_t l0, const JoinKeyCols& lk, int64_t i, const JoinKeyCols& rk, int64_t rb,
+                                                     int64_t rn) {
+  int64_t x = 0, y = rn;
+  while (x < y) {
+    const int64_t mid = x + ((y - x) >> 1);
+    if (compare_tuple<KT0>(l0, lk, i, rk, rb + mid) > 0) x = mid + 1;
+    else y = mid;
+  }
+  return x;
+}
+
+// One thread per left position; the segment of a position is found by segment_of.  The right positions of a bucket are
+// ascending on the key tuples, so the matches of a left position are the range between two lexicographic binary
+// searches.  The leading key column, KT0 its type, decides almost every step: its left value stays in a register and its
+// comparison is compiled in, so a step is one load and a branch-free compare.  The later columns are compared only where
+// the leading ones tie.
 template <int KT0>
 __device__ __forceinline__ void join_count_rows(const JoinKeyCols& lk, const uint64_t* __restrict__ lseg, const JoinKeyCols& rk,
                                                 const uint64_t* __restrict__ rseg, int nseg, int64_t nl,
                                                 uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
-    int lo = 0, hi = nseg;  // last segment with lseg[s] <= i
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (lseg[mid] <= (uint64_t)i) lo = mid;
-      else hi = mid;
-    }
+    const int lo = segment_of(lseg, nseg, i);
     const int64_t l0 = key_value<KT0>(lk.col[0], i);
-    auto compare = [&](int64_t j) {  // the left tuple against right position j
-      int c = compare_keys<KT0>(l0, key_value<KT0>(rk.col[0], j));
-      for (int k = 1; k < rk.n && c == 0; k++) c = compare_column(lk, i, rk, j, k);
-      return c;
-    };
+    auto compare = [&](int64_t j) { return compare_tuple<KT0>(l0, lk, i, rk, j); };
     const int64_t rb = (int64_t)rseg[lo], rn = (int64_t)rseg[lo + 1] - rb;
-    int64_t x = 0, y = rn;  // first right row >= the left tuple
-    while (x < y) {
-      const int64_t mid = x + ((y - x) >> 1);
-      if (compare(rb + mid) > 0) x = mid + 1;
-      else y = mid;
-    }
-    const int64_t f = x;
-    x = 0, y = rn;  // first right row > the left tuple (from the start again: the same path, so cached)
+    const int64_t f = lower_bound_tuple<KT0>(l0, lk, i, rk, rb, rn);  // first right row >= the left tuple
+    int64_t x = 0, y = rn;  // first right row > the left tuple (from the start again: the same path, so cached)
     while (x < y) {
       const int64_t mid = x + ((y - x) >> 1);
       if (compare(rb + mid) >= 0) x = mid + 1;
@@ -236,6 +253,40 @@ __global__ void k_join_count(const __grid_constant__ JoinKeyCols lk, const uint6
     case HS_TYPE_INT32: join_count_rows<HS_TYPE_INT32>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
     case HS_TYPE_INT64: join_count_rows<HS_TYPE_INT64>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
     default: join_count_rows<HS_TYPE_STRING>(lk, lseg, rk, rseg, nseg, nl, counts, first_match); break;
+  }
+}
+
+// The semi / anti join's probe, one thread per left position: one lower-bound search in the right bucket, then one
+// equality test at the position it finds.  A left position with a null in any key column (lv) matches nothing.
+// keep[i] = 1 where the match is what keep_match asks for (1: a match, semi; 0: none, anti).
+template <int KT0>
+__device__ __forceinline__ void join_exists_rows(const JoinKeyCols& lk, const JoinKeyValid& lv, const uint64_t* __restrict__ lseg,
+                                                 const JoinKeyCols& rk, const uint64_t* __restrict__ rseg, int nseg, int64_t nl,
+                                                 uint32_t keep_match, uint32_t* __restrict__ keep) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += stride) {
+    bool null = false;
+    for (int k = 0; k < lv.n; k++) null |= lv.valid[k] != nullptr && lv.valid[k][i] == 0;
+    uint32_t match = 0;
+    if (!null) {
+      const int s = segment_of(lseg, nseg, i);
+      const int64_t l0 = key_value<KT0>(lk.col[0], i);
+      const int64_t rb = (int64_t)rseg[s], rn = (int64_t)rseg[s + 1] - rb;
+      const int64_t f = lower_bound_tuple<KT0>(l0, lk, i, rk, rb, rn);
+      match = f < rn && compare_tuple<KT0>(l0, lk, i, rk, rb + f) == 0;
+    }
+    keep[i] = match == keep_match;
+  }
+}
+
+__global__ void k_join_exists(const __grid_constant__ JoinKeyCols lk, const __grid_constant__ JoinKeyValid lv,
+                              const uint64_t* __restrict__ lseg, const __grid_constant__ JoinKeyCols rk,
+                              const uint64_t* __restrict__ rseg, int nseg, int64_t nl, uint32_t keep_match,
+                              uint32_t* __restrict__ keep) {
+  switch (lk.type[0]) {
+    case HS_TYPE_INT32: join_exists_rows<HS_TYPE_INT32>(lk, lv, lseg, rk, rseg, nseg, nl, keep_match, keep); break;
+    case HS_TYPE_INT64: join_exists_rows<HS_TYPE_INT64>(lk, lv, lseg, rk, rseg, nseg, nl, keep_match, keep); break;
+    default: join_exists_rows<HS_TYPE_STRING>(lk, lv, lseg, rk, rseg, nseg, nl, keep_match, keep); break;
   }
 }
 
@@ -472,13 +523,36 @@ void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t
   }
 }
 
+void launch_join_exists(hs_ctx* ctx, const JoinKeyCols& lkeys, const JoinKeyValid& lvalid, const uint64_t* lseg,
+                        const JoinKeyCols& rkeys, const uint64_t* rseg, int nseg, int64_t nl, bool keep_match, uint32_t* keep) {
+  KernelScope _ks(ctx, "k_join_exists");
+  if (nl == 0) return;
+  k_join_exists<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lvalid, lseg, rkeys, rseg, nseg, nl,
+                                                                       keep_match ? 1u : 0u, keep);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+int64_t compact_rows(hs_ctx* ctx, const uint32_t* mask, int64_t n, const uint32_t* cand, Buf<uint32_t>* kept,
+                     Buf<uint64_t>* offsets) {
+  Buf<uint64_t> own_offsets;
+  if (!offsets) offsets = &own_offsets;
+  offsets->alloc(ctx, n + 1);
+  exclusive_scan_u32_u64(ctx, mask, n, offsets->get());
+  uint64_t count = 0;
+  copy_d2h(ctx, &count, offsets->get() + n, 8);
+  sync_stream(ctx);
+  kept->alloc(ctx, std::max<uint64_t>(1, count));
+  if (n > 0) {
+    k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask, offsets->get(), n, cand, kept->get());
+    HS_LAUNCH_CHECK(ctx);
+  }
+  return (int64_t)count;
+}
+
 int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
                     int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
                     Buf<uint64_t>* offsets) {
   Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
-  Buf<uint64_t> own_offsets;
-  if (!offsets) offsets = &own_offsets;
-  offsets->alloc(ctx, n + 1);
   launch_predicate_mask(ctx, preds, cand, n, mask.get());
   launch_pattern_mask(ctx, pats, cand, n, mask.get());
   launch_compare_mask(ctx, cmps, cand, n, mask.get());
@@ -489,16 +563,7 @@ int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, c
     k_not_in_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(file_ids, n, d_deleted.get(), ndeleted, mask.get());
     HS_LAUNCH_CHECK(ctx);
   }
-  exclusive_scan_u32_u64(ctx, mask.get(), n, offsets->get());
-  uint64_t count = 0;
-  copy_d2h(ctx, &count, offsets->get() + n, 8);
-  sync_stream(ctx);
-  kept->alloc(ctx, std::max<uint64_t>(1, count));
-  if (n > 0) {
-    k_compact<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(mask.get(), offsets->get(), n, cand, kept->get());
-    HS_LAUNCH_CHECK(ctx);
-  }
-  return (int64_t)count;
+  return compact_rows(ctx, mask.get(), n, cand, kept, offsets);
 }
 
 }  // namespace hs

@@ -7,7 +7,8 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan_cmp (K1 + K7) and hs_bucket_join_cmp (K1 + K8).
+Physical execution is the C ABI: hs_filter_scan_cmp (K1 + K7), hs_bucket_join_cmp (K1 + K8) and, for left semi / left anti
+joins, hs_bucket_join_exists.
 """
 from __future__ import annotations
 
@@ -248,12 +249,14 @@ class BucketJoinExec:
     """Join of two index scans bucket by bucket (no exchange), or of two on-the-fly bucketed sides when no index applies.
     ``keys`` are the (left, right) key pairs in the order both sides are bucketed and sorted on: the left index's indexed
     columns when the indexes serve, the condition's order otherwise; None when the condition is not a one-to-one equi-join
-    between the two sides, which the GPU join cannot run.  A filter below a side becomes that side's predicates."""
+    between the two sides, which the GPU join cannot run.  A filter below a side becomes that side's predicates.  ``how``
+    is "inner", or "leftsemi" / "leftanti" (hs_bucket_join_exists: left rows only, each at most once)."""
 
     def __init__(self, session, left: Linear, right: Linear, keys: Optional[List[Tuple[str, str]]], lcand: Optional[Candidate],
-                 rcand: Optional[Candidate], condition: Optional[List[Tuple[str, str]]] = None):
+                 rcand: Optional[Candidate], condition: Optional[List[Tuple[str, str]]] = None, how: str = "inner"):
         self.session, self.left, self.right, self.keys, self.lcand, self.rcand = session, left, right, keys, lcand, rcand
         self.condition = condition if condition is not None else keys
+        self.how = how
 
     def describe(self) -> str:
         def side(c, lin):
@@ -264,7 +267,9 @@ class BucketJoinExec:
         keys = ", ".join(f"{l} = {r}" for l, r in (self.keys or self.condition or []))
         filters = "".join(f", {n}Filter={lin.predicate.conjuncts()}{_terms_text(lin.predicate)}"
                           for n, lin in (("left", self.left), ("right", self.right)) if lin.predicate)
-        return f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, keys=[{keys}]{filters}, exchange=none)"
+        jt = {"leftsemi": ", joinType=LeftSemi", "leftanti": ", joinType=LeftAnti"}.get(self.how, "")
+        return (f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, keys=[{keys}]{jt}{filters}, "
+                "exchange=none)")
 
     def _side(self, lin: Linear, cand: Optional[Candidate], keys: List[str], nb: int):
         """(file images, bucket ids, temporaries to free)."""
@@ -302,8 +307,13 @@ class BucketJoinExec:
             rp = self.right.predicate.conjuncts() if self.right.predicate else []
             lt_, rt_ = ([a.as_native() for a in lin.predicate.disjunctions()] if lin.predicate else [] for lin in (self.left, self.right))
             lc_, rc_ = ([c.as_native() for c in lin.predicate.comparisons()] if lin.predicate else [] for lin in (self.left, self.right))
-            batch, _ = self.session.gpu.bucket_join_cmp(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                        lp, rp, lt_, rt_, lc_, rc_)
+            if self.how == "inner":
+                batch, _ = self.session.gpu.bucket_join_cmp(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                            lp, rp, lt_, rt_, lc_, rc_)
+            else:
+                batch, _ = self.session.gpu.bucket_join_exists(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output,
+                                                               "semi" if self.how == "leftsemi" else "anti", lp, rp, lt_, rt_,
+                                                               lc_, rc_)
         finally:
             for t in lt + rt:
                 t.free()
@@ -448,10 +458,15 @@ def plan_query(session, plan):
         if l is None or r is None:
             raise LE.HyperspaceException("only joins of linear plans (Project?(Filter?(Relation))) are handled")
         keys = join_key_pairs(l, r, node.pairs)
+        semi_or_anti = node.how != "inner"
+        if semi_or_anti:  # the right side of a semi / anti join is only probed: it outputs its keys, its filter is read
+            r = Linear(r.relation, r.predicate, [b for _, b in keys] if keys else [])
         if post_project is not None:  # column pruning: each side outputs only what the final projection needs + its keys
             lout, rout = l.output, r.output
             lneed = [c for c in post_project if c in lout]
             rneed = [c for c in post_project if c not in lout and c in rout]
+            if semi_or_anti and rneed:
+                raise LE.HyperspaceException(f"a left semi / anti join outputs left columns only: cannot resolve {rneed}")
             missing = [c for c in post_project if c not in lout and c not in rout]
             if missing:
                 raise LE.HyperspaceException(f"cannot resolve columns {missing}")
@@ -464,7 +479,7 @@ def plan_query(session, plan):
         if pair:  # both sides bucketed and sorted in the left index's column order
             order = [x.lower() for x in pair[0].entry.indexedColumns]
             keys = sorted(keys, key=lambda p: order.index(p[0].lower()))
-        op = BucketJoinExec(session, l, r, keys, pair[0] if pair else None, pair[1] if pair else None, list(node.pairs))
+        op = BucketJoinExec(session, l, r, keys, pair[0] if pair else None, pair[1] if pair else None, list(node.pairs), node.how)
         if post_project is not None:
             return _Projected(op, post_project)
         return op

@@ -515,11 +515,28 @@ class ProjectNode:
 
 @dataclass
 class JoinNode:
-    """Inner equi-join on the AND of ``left column == right column`` for every pair (a pair may name its columns in
-    either order; rules.join_key_pairs orients them)."""
+    """Equi-join on the AND of ``left column == right column`` for every pair (a pair may name its columns in either
+    order; rules.join_key_pairs orients them).  ``how`` is "inner", "leftsemi" or "leftanti" (normalise_join_type)."""
     left: object
     right: object
     pairs: List[Tuple[str, str]]
+    how: str = "inner"
+
+
+# The join types the GPU path runs, under the spellings JoinType.apply accepts once lower-cased with "_" removed:
+# EXISTS / IN-subquery (LeftSemi) and NOT EXISTS (LeftAnti) besides the inner join.  Outer joins need null-padded
+# output and are not handled.
+_JOIN_TYPES = {"inner": "inner", "leftsemi": "leftsemi", "semi": "leftsemi", "leftanti": "leftanti", "anti": "leftanti"}
+
+
+def normalise_join_type(how: str) -> str:
+    """Spark's JoinType.apply normalisation (lower case, "_" removed) onto "inner", "leftsemi" or "leftanti"; any other
+    join type raises HyperspaceException."""
+    key = str(how).lower().replace("_", "")
+    if key not in _JOIN_TYPES:
+        raise LE.HyperspaceException(f"join type '{how}' is not handled by the GPU path: only inner, left semi and left anti "
+                                     "equi-joins are")
+    return _JOIN_TYPES[key]
 
 
 _SPARK_TYPE_OF_ARROW = {"int32": "integer", "int64": "long", "float": "float", "double": "double", "bool": "boolean",
@@ -634,8 +651,7 @@ class DataFrame:
         return DataFrame(self.session, ProjectNode(self.plan, [self._resolve(c) for c in cols]))
 
     def join(self, other: "DataFrame", on, how: str = "inner") -> "DataFrame":
-        if how != "inner":
-            raise LE.HyperspaceException("only inner equi-joins are handled by the GPU path")
+        how = normalise_join_type(how)
         if isinstance(on, Predicate):
             shown = ", ".join(str(c) for c in on.compares) or "a filter"
             raise LE.HyperspaceException(f"join `on` {shown}: a non-equi join condition, which the GPU path does not handle; "
@@ -648,7 +664,7 @@ class DataFrame:
             pairs = list(on)
             if not pairs or not all(isinstance(p, (tuple, list)) and len(p) == 2 for p in pairs):
                 raise LE.HyperspaceException("join `on` takes a column name, a (left, right) pair or a list of such pairs")
-        return DataFrame(self.session, JoinNode(self.plan, other.plan, [self._join_pair(other, a, b) for a, b in pairs]))
+        return DataFrame(self.session, JoinNode(self.plan, other.plan, [self._join_pair(other, a, b) for a, b in pairs], how))
 
     def _join_pair(self, other: "DataFrame", a: str, b: str) -> Tuple[str, str]:
         """Resolves one equality of a join condition: (this side, other side) when it reads so, else swapped, else (for a
@@ -693,6 +709,8 @@ def output_columns(plan) -> List[str]:
     if isinstance(plan, ProjectNode):
         return list(plan.columns)
     if isinstance(plan, JoinNode):
+        if plan.how != "inner":  # a semi or anti join outputs the left side's columns only
+            return output_columns(plan.left)
         return output_columns(plan.left) + [c for c in output_columns(plan.right)]
     raise TypeError(plan)
 

@@ -454,6 +454,34 @@ int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
                        const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
                        size_t errlen);
 
+/* join_type of hs_bucket_join_exists: Spark 3.1's LeftSemi (EXISTS, IN-subquery) and LeftAnti (NOT EXISTS) */
+#define HS_JOIN_LEFT_SEMI 1
+#define HS_JOIN_LEFT_ANTI 2
+
+/* The left semi or left anti join of hs_bucket_join_cmp's sides, bucket b of the left index with bucket b of the right
+ * index and no exchange -- SortMergeJoinExec with joinType LeftSemi / LeftAnti, which JoinIndexRule rewrites as it does
+ * an inner join (JoinIndexRule.scala:53-110 checks only for an equi-condition, a SortMergeJoin and linear children).
+ * Keys, predicates, terms, comparisons, key types and their refusals (codes and messages) are hs_bucket_join_cmp's.
+ * The output is left rows only, each at most once however many right rows it matches (duplicate left rows stay
+ * duplicates), in (bucket, left sorted position) order:
+ *   HS_JOIN_LEFT_SEMI  keeps a left row when some right row of its bucket has an equal key tuple; a left row with a null
+ *                      in any key column is dropped.
+ *   HS_JOIN_LEFT_ANTI  keeps a left row when no right row matches; a left row with a null in any key column matches
+ *                      nothing and is KEPT.  This is not the null-aware anti join of NOT IN, which Spark 3.1 never plans
+ *                      as a sort-merge join.
+ * A right row with a null key, or that fails the right side's filter, matches nothing; a left row that fails the left
+ * side's filter is never output.  A bucket whose right side is empty (or emptied by its filter) outputs none of its left
+ * rows under semi and all of them under anti.  spec->n_right_columns must be 0 and spec->left_key / right_key NULL
+ * (HS_EINVAL); the right side decodes only its key and filter columns.  A join_type other than HS_JOIN_* is HS_EINVAL.
+ * stats->ms_sort reports the probe (k_join_exists and the compaction of the kept rows), stats->ms_exchange the side
+ * selection, as for the inner join. */
+int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                          const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                          const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                          int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
+                          const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
+                          int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
 int64_t hs_batch_num_rows(const hs_batch* b);
 int32_t hs_batch_on_device(const hs_batch* b); /* != 0: the column pointers are device pointers (output = HS_OUT_DEVICE) */
 int32_t hs_batch_num_columns(const hs_batch* b);
