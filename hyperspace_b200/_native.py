@@ -179,42 +179,24 @@ def load_library() -> C.CDLL:
                                  C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]
     L.hs_result_free.restype = None
     L.hs_result_free.argtypes = [C.c_void_p]
-    L.hs_filter_scan.restype = C.c_int
-    L.hs_filter_scan.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_filter_scan_where.restype = C.c_int
-    L.hs_filter_scan_where.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32, C.POINTER(C.c_void_p),
-                                       C.POINTER(Stats), *err]
-    L.hs_filter_scan_any.restype = C.c_int
-    L.hs_filter_scan_any.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32,
-                                     C.POINTER(PredicateAnySpec), C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p),
-                                     C.POINTER(Stats), *err]
-    L.hs_bucket_join_any.restype = C.c_int
-    L.hs_bucket_join_any.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
-                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                     C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_filter_scan_cmp.restype = C.c_int
-    L.hs_filter_scan_cmp.argtypes = [C.c_void_p, C.POINTER(ScanSpec), C.POINTER(PredicateSpec), C.c_int32,
-                                     C.POINTER(PredicateAnySpec), C.c_int32, C.POINTER(ColumnCompareSpec), C.c_int32, C.c_void_p,
-                                     C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_bucket_join_cmp.restype = C.c_int
-    L.hs_bucket_join_cmp.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
-                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                     C.POINTER(ColumnCompareSpec), C.c_int32,
-                                     C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                     C.POINTER(ColumnCompareSpec), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_bucket_join_exists.restype = C.c_int
-    L.hs_bucket_join_exists.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
-                                        C.c_int32, C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                        C.POINTER(ColumnCompareSpec), C.c_int32,
-                                        C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32,
-                                        C.POINTER(ColumnCompareSpec), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_bucket_join.restype = C.c_int
-    L.hs_bucket_join.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
-    L.hs_bucket_join_where.restype = C.c_int
-    L.hs_bucket_join_where.argtypes = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32,
-                                       C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateSpec), C.c_int32,
-                                       C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    # the read-side calls, from the parameter groups of include/hs_gpu.h: scan head, join head, one side's filter
+    # (predicates, terms, comparisons: a call takes the first one, two or all three), the files' buckets, outputs
+    scan = [C.c_void_p, C.POINTER(ScanSpec)]
+    join = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32]
+    side = [C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32, C.POINTER(ColumnCompareSpec), C.c_int32]
+    buckets = [C.c_void_p, C.c_int32]
+    out = [C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
+    for name, args in (("hs_filter_scan", [*scan, *out]),
+                       ("hs_filter_scan_where", [*scan, *side[:2], *out]),
+                       ("hs_filter_scan_any", [*scan, *side[:4], *buckets, *out]),
+                       ("hs_filter_scan_cmp", [*scan, *side, *buckets, *out]),
+                       ("hs_bucket_join", [*join[:2], *out]),
+                       ("hs_bucket_join_where", [*join, *side[:2], *side[:2], *out]),
+                       ("hs_bucket_join_any", [*join, *side[:4], *side[:4], *out]),
+                       ("hs_bucket_join_cmp", [*join, *side, *side, *out]),
+                       ("hs_bucket_join_exists", [*join[:2], C.c_int32, *join[2:], *side, *side, *out])):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = args
     L.hs_batch_num_rows.restype = C.c_int64
     L.hs_batch_num_rows.argtypes = [C.c_void_p]
     L.hs_batch_on_device.restype = C.c_int32
@@ -497,6 +479,18 @@ def _cmp_array(compares: Sequence[tuple]):
         c.op = CMP_OPS[op] if isinstance(op, str) else op
         c.flags = flags[0] if flags else 0
     return arr, len(compares), keep
+
+
+def _filter_args(*parts, first=0):
+    """One side's filter as the arguments of its parameter group: ``parts`` are its predicates (see _predicate_array),
+    then, for the calls that take them, its terms (_any_array) and its comparisons (_cmp_array); each becomes an array
+    and its count.  first=1: parts start at the terms.  Returns (arguments, buffers to keep alive)."""
+    args, keep = [], []
+    for build, part in zip((_predicate_array, _any_array, _cmp_array)[first:], parts):
+        arr, n, *k = build(part)
+        args += [arr, n]
+        keep += k
+    return args, keep
 
 
 def _source_array(files: Sequence[FileImage]):
@@ -884,15 +878,16 @@ class Context:
         return out.raw[:n.value]
 
     # ---- read side ----------------------------------------------------------------------------------
+    def _read(self, fn, *args) -> Tuple[Batch, Dict[str, float]]:
+        """Calls the read-side entry point fn with the context, args and the outputs: (result batch, stats)."""
+        res, st = C.c_void_p(), Stats()
+        err = C.create_string_buffer(1024)
+        _check(fn(self._h, *args, C.byref(res), C.byref(st), err, len(err)), err)
+        return Batch(res.value, self), st.as_dict()
+
     def filter_scan(self, files: Sequence[FileImage], key: str, projected: Sequence[str], lo=None, hi=None, sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (),
                     output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
-        L = load_library()
-        src, keep = _source_array(files)
-        pc = _cstr_array(projected)
-        spec = ScanSpec()
-        spec.files, spec.n_files, spec.sorted_on_key = src, len(files), 1 if sorted_on_key else 0
-        spec.key_column = key.encode()
-        spec.projected_columns, spec.n_projected = pc, len(projected)
+        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
         spec.has_lo, spec.has_hi = int(lo is not None), int(hi is not None)
         if isinstance(lo, (str, bytes)) or isinstance(hi, (str, bytes)):  # string / binary key: bounds as bytes
             lob = (lo.encode() if isinstance(lo, str) else lo) if lo is not None else b""
@@ -901,17 +896,11 @@ class Context:
             spec.lo, spec.hi = 0, 0
         else:
             spec.lo, spec.hi = lo or 0, hi or 0
-        dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
-        spec.deleted_file_ids, spec.n_deleted_file_ids = dl, len(deleted_file_ids)
-        spec.output = output
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_filter_scan(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._read(load_library().hs_filter_scan, C.byref(spec))
 
     @staticmethod
     def _scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output):
-        """The hs_scan_spec of filter_scan_where / filter_scan_any, and the arrays it points into."""
+        """The hs_scan_spec of the filter scans, and the arrays it points into."""
         src, src_keep = _source_array(files)
         pc = _cstr_array(projected)
         dl = (C.c_int64 * max(1, len(deleted_file_ids)))(*deleted_file_ids)
@@ -923,19 +912,24 @@ class Context:
         spec.output = output
         return spec, (src, src_keep, pc, dl)
 
+    def _filter_scan(self, fn, files, key, projected, parts, sorted_on_key, deleted_file_ids, output, buckets=None):
+        """Runs the filter scan fn on the scan's spec and one filter (_filter_args' parts), then, for the calls that take
+        them, buckets: (file_buckets or None, num_buckets)."""
+        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
+        args, keep_filter = _filter_args(*parts)
+        if buckets is not None:
+            fb = None if buckets[0] is None else np.ascontiguousarray(buckets[0], dtype=np.int32)
+            args += [None, 0] if fb is None else [fb.ctypes.data, buckets[1]]
+        return self._read(fn, C.byref(spec), *args)
+
     def filter_scan_where(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
                           sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (), output: int = HS_OUT_HOST
                           ) -> Tuple[Batch, Dict[str, float]]:
         """hs_filter_scan_where: rows where every predicate holds.  A predicate is ``(column, lo, lo_strict, hi, hi_strict)``
         with None for a missing bound; the literal type follows the Python value (int -> long, float -> double, str / bytes
         -> string) and the engine applies Spark's comparison coercion."""
-        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
-        preds, n_preds = _predicate_array(predicates)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(load_library().hs_filter_scan_where(self._h, C.byref(spec), preds, n_preds, C.byref(res), C.byref(st), err, len(err)),
-               err)
-        return Batch(res.value, self), st.as_dict()
+        return self._filter_scan(load_library().hs_filter_scan_where, files, key, projected, (predicates,), sorted_on_key,
+                                 deleted_file_ids, output)
 
     def filter_scan_any(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
                         terms: Sequence[tuple], sorted_on_key: bool = True, deleted_file_ids: Sequence[int] = (),
@@ -945,17 +939,8 @@ class Context:
         the row's value equals one of `values` (see any_values) or lies in one of `ranges` (``(lo, lo_strict, hi,
         hi_strict)``).  A fourth element gives the term's HS_TERM_* flags: NOT, a null outcome, or a string pattern.  file_buckets / num_buckets: the bucket of every file of an index bucketed on `key` alone, for
         skipping the files a point lookup cannot hit."""
-        L = load_library()
-        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
-        preds, n_preds = _predicate_array(predicates)
-        anys, n_anys, keep_any = _any_array(terms)
-        fb = np.ascontiguousarray(file_buckets if file_buckets is not None else [0], dtype=np.int32)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_filter_scan_any(self._h, C.byref(spec), preds, n_preds, anys, n_anys,
-                                    fb.ctypes.data if file_buckets is not None else None, num_buckets if file_buckets is not None else 0,
-                                    C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._filter_scan(load_library().hs_filter_scan_any, files, key, projected, (predicates, terms), sorted_on_key,
+                                 deleted_file_ids, output, (file_buckets, num_buckets))
 
     def filter_scan_cmp(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
                         terms: Sequence[tuple], compares: Sequence[tuple], sorted_on_key: bool = True,
@@ -964,18 +949,8 @@ class Context:
         """hs_filter_scan_cmp: filter_scan_any with comparisons between two columns of the row AND-ed to the predicates and
         terms, each ``(left, op, right)`` with op one of "<", "<=", ">", ">=", "=", "<=>" and an optional fourth element,
         HS_TERM_NOT.  The engine applies Spark's coercion of the two columns' types."""
-        L = load_library()
-        spec, keep = self._scan_spec(files, key, projected, sorted_on_key, deleted_file_ids, output)
-        preds, n_preds = _predicate_array(predicates)
-        anys, n_anys, keep_any = _any_array(terms)
-        cmps, n_cmps, keep_cmp = _cmp_array(compares)
-        fb = np.ascontiguousarray(file_buckets if file_buckets is not None else [0], dtype=np.int32)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_filter_scan_cmp(self._h, C.byref(spec), preds, n_preds, anys, n_anys, cmps, n_cmps,
-                                    fb.ctypes.data if file_buckets is not None else None, num_buckets if file_buckets is not None else 0,
-                                    C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._filter_scan(load_library().hs_filter_scan_cmp, files, key, projected, (predicates, terms, compares),
+                                 sorted_on_key, deleted_file_ids, output, (file_buckets, num_buckets))
 
     def _join_spec(self, left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns, right_columns,
                    output):
@@ -998,24 +973,32 @@ class Context:
                     right_buckets: Sequence[int], num_buckets: int, left_key: str, right_key: str,
                     left_columns: Sequence[str], right_columns: Sequence[str], output: int = HS_OUT_HOST
                     ) -> Tuple[Batch, Dict[str, float]]:
-        L = load_library()
         spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns,
                                      right_columns, output)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_bucket_join(self._h, C.byref(spec), C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._read(load_library().hs_bucket_join, C.byref(spec))
 
     def _join_where_args(self, left, left_buckets, right, right_buckets, num_buckets, left_keys, right_keys, left_columns,
                          right_columns, left_predicates, right_predicates, output):
-        """What bucket_join_where and bucket_join_any pass alike: the spec (and the arrays it points into), the key name
-        arrays, and each side's predicate array with its count."""
+        """What every multi-key join passes alike: the spec (and the arrays it points into), the key name arrays, and each
+        side's predicate array with its count."""
         if len(left_keys) != len(right_keys):
             raise ValueError("left_keys and right_keys must pair up")
         spec, keep = self._join_spec(left, left_buckets, right, right_buckets, num_buckets, None, None, left_columns,
                                      right_columns, output)
         return (spec, keep, _cstr_array(left_keys), _cstr_array(right_keys), _predicate_array(left_predicates),
                 _predicate_array(right_predicates))
+
+    def _bucket_join(self, fn, join_type, left, left_buckets, right, right_buckets, num_buckets, left_keys, right_keys,
+                     left_columns, right_columns, left_parts, right_parts, output):
+        """Runs the multi-key join fn on its join head (after the spec, join_type when it is not None) and the two sides'
+        filters (_filter_args' parts)."""
+        spec, keep, lk, rk, lp, rp = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets, left_keys,
+                                                           right_keys, left_columns, right_columns, left_parts[0],
+                                                           right_parts[0], output)
+        largs, k1 = _filter_args(*left_parts[1:], first=1)
+        rargs, k2 = _filter_args(*right_parts[1:], first=1)
+        head = [C.byref(spec)] + ([] if join_type is None else [join_type])
+        return self._read(fn, *head, lk, rk, len(left_keys), *lp, *largs, *rp, *rargs)
 
     def bucket_join_where(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
                           right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
@@ -1025,14 +1008,9 @@ class Context:
         columns), keeping on each side only the rows where every predicate of that side holds.  Predicates are
         filter_scan_where's ``(column, lo, lo_strict, hi, hi_strict)`` tuples.  Rows with a null key join nothing.  The
         side selection's time is in ``ms_exchange``."""
-        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
-                                                                          left_keys, right_keys, left_columns, right_columns,
-                                                                          left_predicates, right_predicates, output)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(load_library().hs_bucket_join_where(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, rp, nrp, C.byref(res),
-                                                   C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._bucket_join(load_library().hs_bucket_join_where, None, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, right_columns, (left_predicates,), (right_predicates,),
+                                 output)
 
     def bucket_join_any(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
                         right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
@@ -1040,17 +1018,9 @@ class Context:
                         right_predicates: Sequence[tuple] = (), left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (),
                         output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
         """hs_bucket_join_any: bucket_join_where with filter_scan_any's disjunction terms on either side."""
-        L = load_library()
-        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
-                                                                          left_keys, right_keys, left_columns, right_columns,
-                                                                          left_predicates, right_predicates, output)
-        la, nla, k1 = _any_array(left_terms)
-        ra, nra, k2 = _any_array(right_terms)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_bucket_join_any(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, rp, nrp, ra, nra, C.byref(res),
-                                    C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._bucket_join(load_library().hs_bucket_join_any, None, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, right_columns, (left_predicates, left_terms),
+                                 (right_predicates, right_terms), output)
 
     def bucket_join_cmp(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
                         right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
@@ -1059,19 +1029,9 @@ class Context:
                         left_compares: Sequence[tuple] = (), right_compares: Sequence[tuple] = (),
                         output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
         """hs_bucket_join_cmp: bucket_join_any with filter_scan_cmp's comparisons on either side."""
-        L = load_library()
-        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
-                                                                          left_keys, right_keys, left_columns, right_columns,
-                                                                          left_predicates, right_predicates, output)
-        la, nla, k1 = _any_array(left_terms)
-        ra, nra, k2 = _any_array(right_terms)
-        lc, nlc, k3 = _cmp_array(left_compares)
-        rc, nrc, k4 = _cmp_array(right_compares)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_bucket_join_cmp(self._h, C.byref(spec), lk, rk, len(left_keys), lp, nlp, la, nla, lc, nlc, rp, nrp, ra, nra, rc, nrc,
-                                    C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._bucket_join(load_library().hs_bucket_join_cmp, None, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, right_columns, (left_predicates, left_terms, left_compares),
+                                 (right_predicates, right_terms, right_compares), output)
 
     def bucket_join_exists(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
                            right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
@@ -1083,22 +1043,12 @@ class Context:
         sides.  The batch holds left_columns only, each kept left row once, in (bucket, left sorted position) order.  Semi
         drops left rows with a null key; anti keeps them.  join_type may also be an HS_JOIN_* code (others are refused
         by the library)."""
-        L = load_library()
         if isinstance(join_type, str) and join_type not in JOIN_TYPES:
             raise ValueError(f"join_type must be one of {sorted(JOIN_TYPES)} or an HS_JOIN_* code, not {join_type!r}")
         jt = JOIN_TYPES[join_type] if isinstance(join_type, str) else join_type
-        spec, keep, lk, rk, (lp, nlp), (rp, nrp) = self._join_where_args(left, left_buckets, right, right_buckets, num_buckets,
-                                                                          left_keys, right_keys, left_columns, [],
-                                                                          left_predicates, right_predicates, output)
-        la, nla, k1 = _any_array(left_terms)
-        ra, nra, k2 = _any_array(right_terms)
-        lc, nlc, k3 = _cmp_array(left_compares)
-        rc, nrc, k4 = _cmp_array(right_compares)
-        res, st = C.c_void_p(), Stats()
-        err = C.create_string_buffer(1024)
-        _check(L.hs_bucket_join_exists(self._h, C.byref(spec), jt, lk, rk, len(left_keys), lp, nlp, la, nla, lc, nlc, rp, nrp, ra, nra,
-                                       rc, nrc, C.byref(res), C.byref(st), err, len(err)), err)
-        return Batch(res.value, self), st.as_dict()
+        return self._bucket_join(load_library().hs_bucket_join_exists, jt, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, [], (left_predicates, left_terms, left_compares),
+                                 (right_predicates, right_terms, right_compares), output)
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------
     @staticmethod

@@ -168,7 +168,7 @@ void drop_deleted_rows(hs_ctx* ctx, Table& t, const int64_t* deleted, int ndelet
   if (lc < 0) fail(HS_EINVAL, "deleted_file_ids given but the source has no _data_file_id column (index built without lineage)");
   if (t.nrows == 0) return;
   Buf<uint32_t> idx;
-  const int64_t kept = select_rows(ctx, PredSet{}, PatternSet{}, CompareSet{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
+  const int64_t kept = select_rows(ctx, RowFilter{}, nullptr, t.nrows, (const int64_t*)t.cols[lc].data.get(), deleted, ndeleted, &idx);
   gather_table(ctx, t, idx.get(), kept);
 }
 
@@ -927,8 +927,9 @@ static PredColumn pred_column(const DevColumn& c) { return PredColumn{c.type, c.
 // Every term's resolution (predicates.h: resolve_any), computed once per side of a call: the key's windows and the
 // residual share it.  A term resolves against its own column, which is the same column before and after decoding.
 struct TermResolutions {
-  const hs_predicate_any* anys;
+  const hs_predicate_any* anys = nullptr;
   std::vector<std::unique_ptr<ResolvedTerm>> r;
+  TermResolutions() = default;
   TermResolutions(const hs_predicate_any* a, int n) : anys(a), r(n) {}
   const ResolvedTerm& operator()(int i, const DevColumn& c) {
     if (!r[i]) r[i].reset(new ResolvedTerm(resolve_any(anys[i], pred_column(c))));
@@ -955,55 +956,70 @@ static PatternDesc upload_pattern(hs_ctx* ctx, const DevColumn& c, const hs_pred
   return d;
 }
 
-// Appends to ps the descriptors of the predicates and terms on the columns of t (pred_col[i], any_col[i]), skipping
-// those on column skip_col that its windows already decide: a predicate in scalar form, a term in set form, and to pats
-// a pattern term that is not a prefix (on skip_col too: the windows only bound its values).
-static void add_predicates(hs_ctx* ctx, const Table& t, const hs_predicate* preds, const std::vector<int>& pred_col,
-                           TermResolutions& terms, const std::vector<int>& any_col, int skip_col, PredSet* ps,
-                           PatternSet* pats, PredUploads* up) {
-  for (size_t i = 0; i < pred_col.size(); i++) {
-    if (pred_col[i] == skip_col) continue;
-    const DevColumn& c = t.cols[pred_col[i]];
-    const RangeSet one{resolve_range(preds[i], pred_column(c))};
-    ps->p[ps->n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, upload_set(ctx, c.type, one, up, false)[0]};
-  }
-  for (size_t i = 0; i < any_col.size(); i++) {
-    const DevColumn& c = t.cols[any_col[i]];
-    const ResolvedTerm& rt = terms((int)i, c);
-    const RangeSet& s = rt.set;
-    if (!rt.exact) {
-      pats->p[pats->n++] = upload_pattern(ctx, c, terms.anys[i], rt.pattern, up);
-      continue;
-    }
-    if (any_col[i] == skip_col) continue;
-    upload_set(ctx, c.type, s, up, true);
-    PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
-    d.r.type = c.type;
-    d.set = up->sets.back().get();
-    d.n_set = (int64_t)s.size();
-    d.null_true = term_null_selects(terms.anys[i].flags);
-    ps->p[ps->n++] = d;
-  }
-}
-
-// Appends to cs the comparisons between two columns of t, cmp_col[i] holding the columns of cmps[i]
-static void add_compares(const Table& t, const hs_column_compare* cmps, const std::vector<std::pair<int, int>>& cmp_col, CompareSet* cs) {
-  for (size_t i = 0; i < cmp_col.size(); i++) {
-    const DevColumn& l = t.cols[cmp_col[i].first];
-    const DevColumn& r = t.cols[cmp_col[i].second];
-    CompareDesc d = resolve_compare(cmps[i], pred_column(l), pred_column(r));
-    d.col[0] = l.data.get(), d.col[1] = r.data.get();
-    d.valid[0] = l.has_nulls ? l.valid.get() : nullptr, d.valid[1] = r.has_nulls ? r.valid.get() : nullptr;
-    cs->p[cs->n++] = d;
-  }
-}
-
 // the index of column nm in cols, appended when it is not there yet
 static int column_index(std::vector<std::string>* cols, const std::string& nm) {
   auto it = std::find(cols->begin(), cols->end(), nm);
   if (it != cols->end()) return (int)(it - cols->begin());
   cols->push_back(nm);
   return (int)cols->size() - 1;
+}
+
+// A filter bound to the columns a call decodes: the column of every predicate and term, the two columns of every
+// comparison, and the terms' resolutions
+struct BoundFilter {
+  Filter f;
+  std::vector<int> pred_col, any_col;
+  std::vector<std::pair<int, int>> cmp_col;
+  TermResolutions terms;
+};
+
+// f bound to the columns cols, which gains those not in it yet: the predicates' columns, the terms', then each
+// comparison's left and right column
+static BoundFilter bind_filter(const Filter& f, std::vector<std::string>* cols) {
+  BoundFilter b{f, {}, {}, {}, TermResolutions(f.anys, f.n_anys)};
+  for (int i = 0; i < f.n_preds; i++) b.pred_col.push_back(column_index(cols, f.preds[i].column));
+  for (int i = 0; i < f.n_anys; i++) b.any_col.push_back(column_index(cols, f.anys[i].column));
+  for (int i = 0; i < f.n_cmps; i++)
+    b.cmp_col.push_back({column_index(cols, f.cmps[i].left), column_index(cols, f.cmps[i].right)});
+  return b;
+}
+
+// Appends to rf the descriptors of filter b on the columns of t, skipping those on column skip_col that its windows
+// already decide: a predicate in scalar form and a term in set form.  A pattern term that is not a prefix goes to
+// rf->pats (on skip_col too: the windows only bound its values), and every comparison to rf->cmps.
+static void add_filter(hs_ctx* ctx, const Table& t, BoundFilter& b, int skip_col, RowFilter* rf, PredUploads* up) {
+  PredSet* ps = &rf->preds;
+  for (size_t i = 0; i < b.pred_col.size(); i++) {
+    if (b.pred_col[i] == skip_col) continue;
+    const DevColumn& c = t.cols[b.pred_col[i]];
+    const RangeSet one{resolve_range(b.f.preds[i], pred_column(c))};
+    ps->p[ps->n++] = PredDesc{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, upload_set(ctx, c.type, one, up, false)[0]};
+  }
+  for (size_t i = 0; i < b.any_col.size(); i++) {
+    const DevColumn& c = t.cols[b.any_col[i]];
+    const ResolvedTerm& rt = b.terms((int)i, c);
+    const RangeSet& s = rt.set;
+    if (!rt.exact) {
+      rf->pats.p[rf->pats.n++] = upload_pattern(ctx, c, b.f.anys[i], rt.pattern, up);
+      continue;
+    }
+    if (b.any_col[i] == skip_col) continue;
+    upload_set(ctx, c.type, s, up, true);
+    PredDesc d{c.data.get(), c.has_nulls ? c.valid.get() : nullptr, PredRange{}};
+    d.r.type = c.type;
+    d.set = up->sets.back().get();
+    d.n_set = (int64_t)s.size();
+    d.null_true = term_null_selects(b.f.anys[i].flags);
+    ps->p[ps->n++] = d;
+  }
+  for (size_t i = 0; i < b.cmp_col.size(); i++) {
+    const DevColumn& l = t.cols[b.cmp_col[i].first];
+    const DevColumn& r = t.cols[b.cmp_col[i].second];
+    CompareDesc d = resolve_compare(b.f.cmps[i], pred_column(l), pred_column(r));
+    d.col[0] = l.data.get(), d.col[1] = r.data.get();
+    d.valid[0] = l.has_nulls ? l.valid.get() : nullptr, d.valid[1] = r.has_nulls ? r.valid.get() : nullptr;
+    rf->cmps.p[rf->cmps.n++] = d;
+  }
 }
 
 // the bucket of every point of a key set, by the hash the build used (hash_rows over a column of the key's storage type
@@ -1060,13 +1076,11 @@ static std::vector<int> point_buckets(hs_ctx* ctx, const DevColumn& key, const R
 // Scan's appended files, the lineage NOT-IN) evaluates every predicate over all rows.
 // legacy (hs_filter_scan): predicates may have no bound (the row's key must then not be null, as that call always did),
 // literal types follow the column, and floating-point keys are refused (the call's bounds are int64).
-// anys: disjunction terms.  On the key column they turn the key's one window per file into one window per range of the
-// key's set; elsewhere they are set-form residual predicates.  cmps: comparisons between two columns, always residual (they
+// The filter's terms: on the key column they turn the key's one window per file into one window per range of the key's
+// set; elsewhere they are set-form residual predicates.  Its comparisons between two columns are always residual (they
 // make no window, so a key that appears only in them is read whole).  file_buckets (optional): see hs_filter_scan_any.
-static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int n_preds, bool legacy,
-                            const hs_predicate_any* anys, int n_anys, const hs_column_compare* cmps, int n_cmps,
-                            const int32_t* file_buckets, int num_buckets, hs_batch** out, hs_stats* stats, char* err,
-                            size_t errlen) {
+static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const Filter& filter, bool legacy, const int32_t* file_buckets,
+                            int num_buckets, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   *out = nullptr;
   hs_stats st;
   memset(&st, 0, sizeof st);
@@ -1084,30 +1098,25 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
     if (try_sorted) column_index(&cols, spec->key_column);
     std::vector<int> proj_idx;
     for (int i = 0; i < spec->n_projected; i++) proj_idx.push_back(column_index(&cols, spec->projected_columns[i]));
-    std::vector<int> pred_col(n_preds), any_col(n_anys);
-    for (int i = 0; i < n_preds; i++) pred_col[i] = column_index(&cols, preds[i].column);
-    for (int i = 0; i < n_anys; i++) any_col[i] = column_index(&cols, anys[i].column);
-    std::vector<std::pair<int, int>> cmp_col(n_cmps);
-    for (int i = 0; i < n_cmps; i++) cmp_col[i] = {column_index(&cols, cmps[i].left), column_index(&cols, cmps[i].right)};
+    BoundFilter bf = bind_filter(filter, &cols);
     const int lineage_col = spec->n_deleted_file_ids > 0 ? column_index(&cols, "_data_file_id") : -1;
     PredUploads uploads;
-    TermResolutions terms(anys, n_anys);
     // The key's set (when a term is on the key, or for pruning): the predicates on the key and every term on it,
     // intersected.
     auto on_key_name = [&](const char* column) { return spec->key_column && strcmp(column, spec->key_column) == 0; };
     // a term that selects null keys (IS NULL, NOT (k <=> v)) finds them in the null key's bucket: no pruning then
     bool key_terms = false, key_nulls = false;
-    for (int i = 0; i < n_anys; i++) {
-      key_terms = key_terms || on_key_name(anys[i].column);
-      key_nulls = key_nulls || (on_key_name(anys[i].column) && term_null_selects(anys[i].flags));
+    for (int i = 0; i < filter.n_anys; i++) {
+      key_terms = key_terms || on_key_name(filter.anys[i].column);
+      key_nulls = key_nulls || (on_key_name(filter.anys[i].column) && term_null_selects(filter.anys[i].flags));
     }
     auto key_set_of = [&](const DevColumn& kc) {
       const bool str = kc.type == HS_TYPE_STRING;
       RangeSet s{SetRange{}};  // every value
-      for (int i = 0; i < n_preds; i++)
-        if (on_key_name(preds[i].column)) s = intersect_sets(str, s, RangeSet{resolve_range(preds[i], pred_column(kc))});
-      for (int i = 0; i < n_anys; i++)
-        if (on_key_name(anys[i].column)) s = intersect_sets(str, s, terms(i, kc).set);
+      for (int i = 0; i < filter.n_preds; i++)
+        if (on_key_name(filter.preds[i].column)) s = intersect_sets(str, s, RangeSet{resolve_range(filter.preds[i], pred_column(kc))});
+      for (int i = 0; i < filter.n_anys; i++)
+        if (on_key_name(filter.anys[i].column)) s = intersect_sets(str, s, bf.terms(i, kc).set);
       return s;
     };
     // Bucket pruning: a key whose windows are points lives in the files of the points' buckets only
@@ -1123,7 +1132,7 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       const DevColumn kc = source_column_type(ctx, files[0], spec->key_column);
       const bool hashable = kc.type == HS_TYPE_INT32 || kc.type == HS_TYPE_INT64 || kc.type == HS_TYPE_STRING;
       bool keyed = key_terms;
-      for (int i = 0; i < n_preds; i++) keyed = keyed || on_key_name(preds[i].column);
+      for (int i = 0; i < filter.n_preds; i++) keyed = keyed || on_key_name(filter.preds[i].column);
       if (hashable && keyed && !key_nulls) {
         key_set = key_set_of(kc);
         have_key_set = true;
@@ -1167,8 +1176,8 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       if (ktype < HS_TYPE_INT32 || ktype > HS_TYPE_STRING || ktype == HS_TYPE_BOOL)
         fail(HS_EUNSUPPORTED, "filter scan: the sorted key column '%s' must be int32 / int64 / float / double / string", cols[0].c_str());
       int on_key = 0;  // the predicates and terms the windows decide (a pattern that is not a prefix stays residual)
-      for (int i = 0; i < n_preds; i++) on_key += pred_col[i] == 0;
-      for (int i = 0; i < n_anys; i++) on_key += any_col[i] == 0 && terms(i, t.cols[0]).exact;
+      for (int i = 0; i < filter.n_preds; i++) on_key += bf.pred_col[i] == 0;
+      for (int i = 0; i < filter.n_anys; i++) on_key += bf.any_col[i] == 0 && bf.terms(i, t.cols[0]).exact;
       const int nseg = n_files;
       std::vector<uint64_t> seg(nseg + 1);
       for (int f = 0; f <= nseg; f++) seg[f] = (uint64_t)t.file_row_begin[f];
@@ -1179,8 +1188,8 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       // empty window falls on (below)
       if (!(key_terms || pruned)) {
         SetRange r;
-        for (int i = 0; i < n_preds; i++)
-          if (pred_col[i] == 0) r = intersect_range(ktype == HS_TYPE_STRING, r, resolve_range(preds[i], pred_column(t.cols[0])));
+        for (int i = 0; i < filter.n_preds; i++)
+          if (bf.pred_col[i] == 0) r = intersect_range(ktype == HS_TYPE_STRING, r, resolve_range(filter.preds[i], pred_column(t.cols[0])));
         key_set = RangeSet{r};
       } else if (!have_key_set) {
         key_set = key_set_of(t.cols[0]);
@@ -1246,27 +1255,21 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const hs_pred
       idx.alloc(ctx, std::max<int64_t>(1, n_cand));
       if (nseg) launch_windows_to_indices(ctx, d_win.get(), d_oo.get(), nwin, n_cand, idx.get());
       n_out = n_cand;
-      if (on_key < n_preds + n_anys || n_cmps > 0) {
+      if (on_key < filter.n_preds + filter.n_anys || filter.n_cmps > 0) {
         // residual: the predicates on other columns and the comparisons, over the window rows, compacted through the
         // candidate list
-        PredSet residual;
-        PatternSet pats;
-        CompareSet cs;
-        add_predicates(ctx, t, preds, pred_col, terms, any_col, 0, &residual, &pats, &uploads);
-        add_compares(t, cmps, cmp_col, &cs);
+        RowFilter residual;
+        add_filter(ctx, t, bf, 0, &residual, &uploads);
         Buf<uint32_t> kept_rows;
-        n_out = select_rows(ctx, residual, pats, cs, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
+        n_out = select_rows(ctx, residual, idx.get(), n_cand, nullptr, nullptr, 0, &kept_rows);
         idx = std::move(kept_rows);
       }
     } else {
       // full predicate scan (source files, appended source files under Hybrid Scan, or lineage NOT-IN filter)
-      PredSet ps;
-      PatternSet pats;
-      CompareSet cs;
-      add_predicates(ctx, t, preds, pred_col, terms, any_col, -1, &ps, &pats, &uploads);
-      add_compares(t, cmps, cmp_col, &cs);
+      RowFilter rf;
+      add_filter(ctx, t, bf, -1, &rf, &uploads);
       const int64_t* file_ids = lineage_col >= 0 ? (const int64_t*)t.cols[lineage_col].data.get() : nullptr;
-      n_out = select_rows(ctx, ps, pats, cs, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
+      n_out = select_rows(ctx, rf, nullptr, n, file_ids, spec->deleted_file_ids, spec->n_deleted_file_ids, &idx);
     }
     sync_stream(ctx);
     t_scan.stop();
@@ -1292,11 +1295,7 @@ extern "C" {
 int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out) return HS_EINVAL;
   *out = nullptr;
-  if (!spec->key_column) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "key_column is required");
-    return HS_EINVAL;
-  }
+  if (!spec->key_column) return refuse(HS_EINVAL, stats, err, errlen, "key_column is required");
   // one predicate on the key, its literal type following the column
   hs_predicate p;
   memset(&p, 0, sizeof p);
@@ -1306,7 +1305,8 @@ int hs_filter_scan(hs_ctx* ctx, const hs_scan_spec* spec, hs_batch** out, hs_sta
   p.lo_i = spec->lo, p.hi_i = spec->hi;
   p.lo_bytes = spec->lo_bytes, p.hi_bytes = spec->hi_bytes;
   p.lo_len = spec->lo_len, p.hi_len = spec->hi_len;
-  return filter_scan_core(ctx, spec, &p, 1, true, nullptr, 0, nullptr, 0, nullptr, 0, out, stats, err, errlen);
+  const Filter f{&p, 1};
+  return filter_scan_core(ctx, spec, f, true, nullptr, 0, out, stats, err, errlen);
 }
 
 int hs_filter_scan_where(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds, hs_batch** out,
@@ -1327,17 +1327,11 @@ int hs_filter_scan_cmp(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate
   if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds) || num_buckets < 0 || (num_buckets > 0 && !file_buckets))
     return HS_EINVAL;
   *out = nullptr;
-  int rc = check_predicates(preds, n_preds, spec->has_lo || spec->has_hi, stats, err, errlen);
-  if (rc == HS_OK) rc = check_anys(anys, n_anys, n_preds, stats, err, errlen);
-  if (rc == HS_OK) rc = check_compares(cmps, n_cmps, n_preds + n_anys, stats, err, errlen);
+  const Filter f{preds, n_preds, anys, n_anys, cmps, n_cmps};
+  const int rc = check_filters(&f, 1, spec->has_lo || spec->has_hi, stats, err, errlen);
   if (rc != HS_OK) return rc;
-  if (num_buckets > kMaxBuckets) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "numBuckets must be in 1..%d", kMaxBuckets);
-    return HS_EUNSUPPORTED;
-  }
-  return filter_scan_core(ctx, spec, preds, n_preds, false, anys, n_anys, cmps, n_cmps, num_buckets > 0 ? file_buckets : nullptr,
-                          num_buckets, out, stats, err, errlen);
+  if (num_buckets > kMaxBuckets) return refuse(HS_EUNSUPPORTED, stats, err, errlen, "numBuckets must be in 1..%d", kMaxBuckets);
+  return filter_scan_core(ctx, spec, f, false, num_buckets > 0 ? file_buckets : nullptr, num_buckets, out, stats, err, errlen);
 }
 
 }  // extern "C"
@@ -1353,6 +1347,9 @@ struct JoinSide {
   const uint32_t* perm = nullptr;
   Buf<uint32_t> kept;
   int64_t n = 0;  // rows in sorted order
+  std::vector<int> proj;  // the projected columns of t
+  BoundFilter filter;
+  RowFilter sel;  // the side selection: IS NOT NULL on the nullable key columns, then the filter
 };
 
 // Orders the decoded rows of one join side bucket-major and key-sorted.  When every bucket holds exactly one file the
@@ -1404,13 +1401,13 @@ static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file*
   side->n = t->nrows;
 }
 
-// Side selection: keeps the rows whose key columns are all non-null and where every predicate of the side holds.  The
-// predicates run over the sorted positions as their candidate list, so the compacted rows stay in sorted order and a
-// bucket's new boundaries are the scan's values at the old ones.  Launches nothing when ps, pats and cmps are empty.
-static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, const PatternSet& pats, const CompareSet& cmps, int nb) {
-  if (ps.n == 0 && pats.n == 0 && cmps.n == 0) return;
+// Side selection: keeps the rows that pass side->sel.  It runs over the sorted positions as its candidate list, so the
+// compacted rows stay in sorted order and a bucket's new boundaries are the scan's values at the old ones.  Launches
+// nothing when side->sel is empty.
+static void select_join_side(hs_ctx* ctx, JoinSide* side, int nb) {
+  if (side->sel.empty()) return;
   Buf<uint64_t> offs;
-  side->n = select_rows(ctx, ps, pats, cmps, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
+  side->n = select_rows(ctx, side->sel, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
   side->perm = side->kept.get();
   std::vector<uint32_t> bounds(nb + 1);
   for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
@@ -1425,15 +1422,12 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, const PredSet& ps, con
 // bucket_join_core's join_type for the inner join (include/hs_gpu.h numbers the semi and anti joins from 1)
 constexpr int kJoinInner = 0;
 
-// The one bucket join.  legacy (hs_bucket_join): one key per side, no predicates, null keys refused.  k_join_count (inner)
-// or k_join_exists (join_type HS_JOIN_LEFT_SEMI / HS_JOIN_LEFT_ANTI) probes on the key columns where they lie: the decoded
-// columns, or their gather through the side's permutation.
+// The one bucket join of the sides' filters (left, right).  legacy (hs_bucket_join): one key per side, no filters, null
+// keys refused.  k_join_count (inner) or k_join_exists (join_type HS_JOIN_LEFT_SEMI / HS_JOIN_LEFT_ANTI) probes on the
+// key columns where they lie: the decoded columns, or their gather through the side's permutation.
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
-                            int n_keys, const hs_predicate* left_preds, int n_left_preds, const hs_predicate* right_preds,
-                            int n_right_preds, const hs_predicate_any* left_anys, int n_left_anys,
-                            const hs_predicate_any* right_anys, int n_right_anys, const hs_column_compare* left_cmps,
-                            int n_left_cmps, const hs_column_compare* right_cmps, int n_right_cmps, bool legacy, int join_type,
-                            hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+                            int n_keys, const Filter filters[2], bool legacy, int join_type, hs_batch** out, hs_stats* stats,
+                            char* err, size_t errlen) {
   hs_stats st;
   memset(&st, 0, sizeof st);
   std::unique_ptr<hs_batch> res(new hs_batch());
@@ -1444,35 +1438,25 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.start();
     const int nb = spec->num_buckets;
     if (nb < 1) fail(HS_EINVAL, "num_buckets must be positive");
-    // columns to decode: the keys first, then the projection, then the predicate, term and comparison columns
-    auto side_columns = [&](const char* const* keys, const char* const* proj, int n_proj, const hs_predicate* preds, int n_preds,
-                            const hs_predicate_any* anys, int n_anys, const hs_column_compare* cmps, int n_cmps,
-                            std::vector<int>* proj_idx, std::vector<int>* pred_idx, std::vector<int>* any_idx,
-                            std::vector<std::pair<int, int>>* cmp_idx) {
-      std::vector<std::string> cols;
+    JoinSide side[2];
+    JoinSide &L = side[0], &R = side[1];
+    // columns to decode: the keys first, then the projection, then the filter's columns
+    std::vector<std::string> cols[2];
+    for (int s = 0; s < 2; s++) {
+      const char* const* keys = s == 0 ? left_keys : right_keys;
       for (int k = 0; k < n_keys; k++) {
         if (!keys[k]) fail(HS_EINVAL, "bucket join: missing key column");
-        if (std::find(cols.begin(), cols.end(), keys[k]) != cols.end()) fail(HS_EINVAL, "bucket join: key column '%s' given twice", keys[k]);
-        cols.push_back(keys[k]);
+        if (std::find(cols[s].begin(), cols[s].end(), keys[k]) != cols[s].end())
+          fail(HS_EINVAL, "bucket join: key column '%s' given twice", keys[k]);
+        cols[s].push_back(keys[k]);
       }
-      for (int i = 0; i < n_proj; i++) proj_idx->push_back(column_index(&cols, proj[i]));
-      for (int i = 0; i < n_preds; i++) pred_idx->push_back(column_index(&cols, preds[i].column));
-      for (int i = 0; i < n_anys; i++) any_idx->push_back(column_index(&cols, anys[i].column));
-      for (int i = 0; i < n_cmps; i++) {
-        const int a = column_index(&cols, cmps[i].left);
-        cmp_idx->push_back({a, column_index(&cols, cmps[i].right)});
-      }
-      return cols;
-    };
-    std::vector<int> lproj, rproj, lpred, rpred, lany, rany;
-    std::vector<std::pair<int, int>> lcmp, rcmp;
-    const std::vector<std::string> lcols = side_columns(left_keys, spec->left_columns, spec->n_left_columns, left_preds, n_left_preds,
-                                                        left_anys, n_left_anys, left_cmps, n_left_cmps, &lproj, &lpred, &lany, &lcmp);
-    const std::vector<std::string> rcols = side_columns(right_keys, spec->right_columns, spec->n_right_columns, right_preds, n_right_preds,
-                                                        right_anys, n_right_anys, right_cmps, n_right_cmps, &rproj, &rpred, &rany, &rcmp);
-    JoinSide L, R;
-    prepare_join_side(ctx, &L, spec->left_files, spec->n_left, spec->left_buckets, nb, lcols, n_keys, legacy, &st);
-    prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, rcols, n_keys, legacy, &st);
+      const char* const* proj = s == 0 ? spec->left_columns : spec->right_columns;
+      const int n_proj = s == 0 ? spec->n_left_columns : spec->n_right_columns;
+      for (int i = 0; i < n_proj; i++) side[s].proj.push_back(column_index(&cols[s], proj[i]));
+      side[s].filter = bind_filter(filters[s], &cols[s]);
+    }
+    prepare_join_side(ctx, &L, spec->left_files, spec->n_left, spec->left_buckets, nb, cols[0], n_keys, legacy, &st);
+    prepare_join_side(ctx, &R, spec->right_files, spec->n_right, spec->right_buckets, nb, cols[1], n_keys, legacy, &st);
     // hashInt and hashLong put equal values into different buckets: both sides must have been bucketed on the same types
     // (JoinIndexRule only pairs indexes whose indexed columns have the same data types)
     // the same holds for the decimals and timestamps riding on them: decimal(p <= 9) hashes as a long, an int32 as an int,
@@ -1486,34 +1470,25 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
         fail(HS_EUNSUPPORTED, "bucket join: key columns '%s' and '%s' have different types", left_keys[k], right_keys[k]);
       }
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
-    // side selection: IS NOT NULL on the nullable key columns, then the side's predicates.  An anti join keeps the left
-    // rows with a null key (they match nothing, so they are output): its probe reads their validity instead.
+    // side selection: IS NOT NULL on the nullable key columns, then the side's filter.  An anti join keeps the left rows
+    // with a null key (they match nothing, so they are output): its probe reads their validity instead.
     const bool anti = join_type == HS_JOIN_LEFT_ANTI;
     PredUploads uploads;
-    TermResolutions lterms(left_anys, n_left_anys), rterms(right_anys, n_right_anys);  // outlive the copies of their patterns
-    auto side_preds = [&](const JoinSide& s, const hs_predicate* preds, const std::vector<int>& pred_idx, TermResolutions& terms,
-                          const std::vector<int>& any_idx, PatternSet* pats) {
-      PredSet ps;
-      for (int k = 0; k < n_keys; k++) {
-        const DevColumn& c = s.t.cols[k];
-        if (c.has_nulls && !(anti && &s == &L)) {
+    for (int s = 0; s < 2; s++) {
+      PredSet& ps = side[s].sel.preds;
+      for (int k = 0; k < n_keys && !(anti && s == 0); k++) {
+        const DevColumn& c = side[s].t.cols[k];
+        if (c.has_nulls) {
           PredDesc d{};
           d.data = c.data.get(), d.valid = c.valid.get(), d.r.type = c.type;
           ps.p[ps.n++] = d;
         }
       }
-      add_predicates(ctx, s.t, preds, pred_idx, terms, any_idx, -1, &ps, pats, &uploads);
-      return ps;
-    };
-    PatternSet lpats, rpats;
-    const PredSet lps = side_preds(L, left_preds, lpred, lterms, lany, &lpats), rps = side_preds(R, right_preds, rpred, rterms, rany, &rpats);
-    CompareSet lcs, rcs;
-    add_compares(L.t, left_cmps, lcmp, &lcs);
-    add_compares(R.t, right_cmps, rcmp, &rcs);
+      add_filter(ctx, side[s].t, side[s].filter, -1, &side[s].sel, &uploads);
+    }
     StageTimer t_sel(ctx);
     t_sel.start();
-    select_join_side(ctx, &L, lps, lpats, lcs, nb);
-    select_join_side(ctx, &R, rps, rpats, rcs, nb);
+    for (JoinSide& s : side) select_join_side(ctx, &s, nb);
     t_sel.stop();
     // the key columns in (selected) sorted order
     std::vector<Buf<uint8_t>> key_bufs;
@@ -1555,7 +1530,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       launch_join_exists(ctx, lk, lv, d_lseg.get(), rk, d_rseg.get(), nb, nl, !anti, keep.get());
       total_out = (uint64_t)compact_rows(ctx, keep.get(), nl, L.perm, &lrow);
       t_join.stop();
-      batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
+      batch_from_gather(ctx, L.t, L.proj, lrow.get(), (int64_t)total_out, res.get());
     } else {
       Buf<uint32_t> counts(ctx, std::max<int64_t>(1, nl)), first(ctx, std::max<int64_t>(1, nl));
       Buf<uint64_t> offs(ctx, nl + 1);
@@ -1567,13 +1542,13 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
       Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
       launch_join_emit(ctx, counts.get(), first.get(), offs.get(), nl, L.perm, R.perm, lrow.get(), rrow.get());
       t_join.stop();
-      batch_from_gather(ctx, L.t, lproj, lrow.get(), (int64_t)total_out, res.get());
-      batch_from_gather(ctx, R.t, rproj, rrow.get(), (int64_t)total_out, res.get());
+      batch_from_gather(ctx, L.t, L.proj, lrow.get(), (int64_t)total_out, res.get());
+      batch_from_gather(ctx, R.t, R.proj, rrow.get(), (int64_t)total_out, res.get());
     }
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
-    if (lps.n || rps.n || lpats.n || rpats.n || lcs.n || rcs.n) st.ms_exchange += t_sel.ms();
+    if (!L.sel.empty() || !R.sel.empty()) st.ms_exchange += t_sel.ms();
     st.rows_out = (int64_t)total_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;
@@ -1588,8 +1563,8 @@ extern "C" {
 int hs_bucket_join(hs_ctx* ctx, const hs_join_spec* spec, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out) return HS_EINVAL;
   *out = nullptr;
-  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                          nullptr, 0, true, kJoinInner, out, stats, err, errlen);
+  const Filter none[2];
+  return bucket_join_core(ctx, spec, &spec->left_key, &spec->right_key, 1, none, true, kJoinInner, out, stats, err, errlen);
 }
 
 int hs_bucket_join_where(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
@@ -1610,39 +1585,24 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
 
 }  // extern "C"
 
-// hs_bucket_join_cmp's and hs_bucket_join_exists's checks that need no data, then the join
+// hs_bucket_join_cmp's and hs_bucket_join_exists's checks that need no data, then the join of the sides' filters
 static int bucket_join_checked(hs_ctx* ctx, const hs_join_spec* spec, int join_type, const char* const* left_keys,
-                               const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
-                               const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
-                               int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
-                               const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
-                               int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
-  if (!ctx || !spec || !out || !left_keys || !right_keys || n_left_preds < 0 || n_right_preds < 0 ||
-      (n_left_preds > 0 && !left_preds) || (n_right_preds > 0 && !right_preds))
-    return HS_EINVAL;
+                               const char* const* right_keys, int n_keys, const Filter filters[2], hs_batch** out, hs_stats* stats,
+                               char* err, size_t errlen) {
+  if (!ctx || !spec || !out || !left_keys || !right_keys) return HS_EINVAL;
+  for (int s = 0; s < 2; s++)
+    if (filters[s].n_preds < 0 || (filters[s].n_preds > 0 && !filters[s].preds)) return HS_EINVAL;
   *out = nullptr;
-  auto refuse = [&](int code, const char* msg) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "%s", msg);
-    return code;
-  };
   if (join_type != kJoinInner && join_type != HS_JOIN_LEFT_SEMI && join_type != HS_JOIN_LEFT_ANTI)
-    return refuse(HS_EINVAL, "bucket join: join_type must be HS_JOIN_LEFT_SEMI or HS_JOIN_LEFT_ANTI");
+    return refuse(HS_EINVAL, stats, err, errlen, "bucket join: join_type must be HS_JOIN_LEFT_SEMI or HS_JOIN_LEFT_ANTI");
   if (join_type != kJoinInner && spec->n_right_columns != 0)
-    return refuse(HS_EINVAL, "bucket join: a semi or anti join outputs left columns only (n_right_columns must be 0)");
-  if (n_keys < 1) return refuse(HS_EINVAL, "bucket join: at least one key column per side");
-  if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, "bucket join: more than 8 key columns");
-  if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, "bucket join: the keys go in left_keys / right_keys");
-  int rc = check_predicates(left_preds, n_left_preds, false, stats, err, errlen);
-  if (rc == HS_OK) rc = check_predicates(right_preds, n_right_preds, false, stats, err, errlen);
-  if (rc == HS_OK) rc = check_anys(left_anys, n_left_anys, n_left_preds, stats, err, errlen);
-  if (rc == HS_OK) rc = check_anys(right_anys, n_right_anys, n_right_preds, stats, err, errlen);
-  if (rc == HS_OK) rc = check_compares(left_cmps, n_left_cmps, n_left_preds + n_left_anys, stats, err, errlen);
-  if (rc == HS_OK) rc = check_compares(right_cmps, n_right_cmps, n_right_preds + n_right_anys, stats, err, errlen);
+    return refuse(HS_EINVAL, stats, err, errlen, "bucket join: a semi or anti join outputs left columns only (n_right_columns must be 0)");
+  if (n_keys < 1) return refuse(HS_EINVAL, stats, err, errlen, "bucket join: at least one key column per side");
+  if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, stats, err, errlen, "bucket join: more than 8 key columns");
+  if (spec->left_key || spec->right_key) return refuse(HS_EINVAL, stats, err, errlen, "bucket join: the keys go in left_keys / right_keys");
+  const int rc = check_filters(filters, 2, false, stats, err, errlen);
   if (rc != HS_OK) return rc;
-  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, left_preds, n_left_preds, right_preds, n_right_preds, left_anys,
-                          n_left_anys, right_anys, n_right_anys, left_cmps, n_left_cmps, right_cmps, n_right_cmps, false, join_type,
-                          out, stats, err, errlen);
+  return bucket_join_core(ctx, spec, left_keys, right_keys, n_keys, filters, false, join_type, out, stats, err, errlen);
 }
 
 extern "C" {
@@ -1653,9 +1613,9 @@ int hs_bucket_join_cmp(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
                        int32_t n_right_preds, const hs_predicate_any* right_anys, int32_t n_right_anys,
                        const hs_column_compare* right_cmps, int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err,
                        size_t errlen) {
-  return bucket_join_checked(ctx, spec, kJoinInner, left_keys, right_keys, n_keys, left_preds, n_left_preds, left_anys, n_left_anys,
-                             left_cmps, n_left_cmps, right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps,
-                             out, stats, err, errlen);
+  const Filter filters[2] = {{left_preds, n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps},
+                             {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps}};
+  return bucket_join_checked(ctx, spec, kJoinInner, left_keys, right_keys, n_keys, filters, out, stats, err, errlen);
 }
 
 int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
@@ -1664,10 +1624,11 @@ int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_ty
                           int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
                           const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
                           int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  const Filter filters[2] = {{left_preds, n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps},
+                             {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps}};
   // an inner join is hs_bucket_join_cmp's: kJoinInner (0) is refused like any other value outside HS_JOIN_*
-  return bucket_join_checked(ctx, spec, join_type == kJoinInner ? -1 : join_type, left_keys, right_keys, n_keys, left_preds,
-                             n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps, right_preds, n_right_preds, right_anys,
-                             n_right_anys, right_cmps, n_right_cmps, out, stats, err, errlen);
+  return bucket_join_checked(ctx, spec, join_type == kJoinInner ? -1 : join_type, left_keys, right_keys, n_keys, filters, out, stats,
+                             err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

@@ -448,6 +448,13 @@ struct CompareSet {
   CompareDesc p[kMaxPredicates];
   int n = 0;
 };
+// The row filter of a scan or join side: a row is kept when every predicate, pattern and comparison holds
+struct RowFilter {
+  PredSet preds;
+  PatternSet pats;
+  CompareSet cmps;
+  bool empty() const { return preds.n == 0 && pats.n == 0 && cmps.n == 0; }
+};
 // The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
 // work[w] = {s, r} with r indexing `ranges` (device); bounds[2w] = first row of s inside ranges[r], bounds[2w+1] = first
 // row above it (segment-relative).  All ranges are of type ranges_type.
@@ -497,14 +504,12 @@ void launch_string_lengths(hs_ctx* ctx, const uint64_t* refs, const uint8_t* val
                            uint32_t* lens);
 void launch_copy_strings(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
                          const uint64_t* offsets, uint8_t* out);
-// Row selection over n candidates (cand[i], or row i when cand is nullptr): keeps those where every predicate of `preds`
-// and every pattern of `pats` and comparison of `cmps` holds and, when ndeleted > 0, whose file_ids[i] is not in the host
-// array `deleted`.  The kept candidates go to *kept in their order; returns how many there are (after a stream
-// synchronisation).  offsets, when given, receives the exclusive scan of the keep mask (n+1 entries): offsets[i] is the
-// number of kept candidates before i.
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
-                    int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
-                    Buf<uint64_t>* offsets = nullptr);
+// Row selection over n candidates (cand[i], or row i when cand is nullptr): keeps those that pass `filter` and, when
+// ndeleted > 0, whose file_ids[i] is not in the host array `deleted`.  The kept candidates go to *kept in their order;
+// returns how many there are (after a stream synchronisation).  offsets, when given, receives the exclusive scan of the
+// keep mask (n+1 entries): offsets[i] is the number of kept candidates before i.
+int64_t select_rows(hs_ctx* ctx, const RowFilter& filter, const uint32_t* cand, int64_t n, const int64_t* file_ids,
+                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets = nullptr);
 // The compaction select_rows ends with, over a keep mask of n candidates (1 / 0): the kept cand[i] (i when cand is
 // nullptr) go to *kept in their order; returns how many there are (after a stream synchronisation); offsets as in
 // select_rows.

@@ -13,7 +13,9 @@
 // sides are compared in (resolve_compare); column_compare.h evaluates it.
 #pragma once
 #include <algorithm>
+#include <cstdarg>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <initializer_list>
 #include <string>
@@ -474,78 +476,79 @@ inline ResolvedTerm resolve_any(const hs_predicate_any& a, const PredColumn& c) 
   return rt;
 }
 
+// A call refused before it runs: stats zeroed, the message in err.  Returns code.
+__attribute__((format(printf, 5, 6))) inline int refuse(int code, hs_stats* stats, char* err, size_t errlen, const char* fmt, ...) {
+  if (stats) memset(stats, 0, sizeof *stats);
+  if (err && errlen) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(err, errlen, fmt, ap);
+    va_end(ap);
+  }
+  return code;
+}
+
 // The refusals of a predicate list that need no data: HS_OK or the code, with stats zeroed and the message in err.
 // bounds_in_spec: hs_filter_scan_where was also given the bounds of hs_filter_scan.
 inline int check_predicates(const hs_predicate* preds, int n_preds, bool bounds_in_spec, hs_stats* stats, char* err, size_t errlen) {
-  auto refuse = [&](int code, const char* msg, const char* what) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, msg, what);
-    return code;
-  };
-  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, "filter scan: more than 16 predicates%s", "");
-  if (bounds_in_spec) return refuse(HS_EINVAL, "filter scan: the bounds go in the predicates%s", "");
+  if (n_preds > kMaxPredicates) return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: more than 16 predicates");
+  if (bounds_in_spec) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the bounds go in the predicates");
   for (int i = 0; i < n_preds; i++) {
     const hs_predicate& p = preds[i];
-    if (!p.column) return refuse(HS_EINVAL, "filter scan: predicate without a column%s", "");
-    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, "filter scan: predicate on '%s' has no bound", p.column);
+    if (!p.column) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: predicate without a column");
+    if (!p.has_lo && !p.has_hi) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: predicate on '%s' has no bound", p.column);
     if (p.literal_type != HS_TYPE_INT64 && p.literal_type != HS_TYPE_DOUBLE && p.literal_type != HS_TYPE_STRING &&
         p.literal_type != HS_TYPE_DECIMAL)
-      return refuse(HS_EINVAL, "filter scan: predicate on '%s' has an unknown literal type", p.column);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: predicate on '%s' has an unknown literal type", p.column);
   }
   return HS_OK;
 }
 
 // The same for the disjunction terms beside n_preds predicates: their counts, arrays, offsets and string lengths.
 inline int check_anys(const hs_predicate_any* anys, int n_anys, int n_preds, hs_stats* stats, char* err, size_t errlen) {
-  char msg[256];
-  auto refuse = [&](int code) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "%s", msg);
-    return code;
-  };
-  if (n_anys < 0 || (n_anys > 0 && !anys)) return snprintf(msg, sizeof msg, "filter scan: bad term array"), refuse(HS_EINVAL);
+  if (n_anys < 0 || (n_anys > 0 && !anys)) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: bad term array");
   if (n_preds + n_anys > kMaxPredicates)
-    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
+    return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: more than 16 predicates and terms");
   for (int i = 0; i < n_anys; i++) {
     const hs_predicate_any& a = anys[i];
-    if (!a.column) return snprintf(msg, sizeof msg, "filter scan: term without a column"), refuse(HS_EINVAL);
+    if (!a.column) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term without a column");
     const char* c = a.column;
     if (a.n_values < 0 || a.n_ranges < 0 || (a.n_ranges > 0 && !a.ranges))
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has a bad value or range array", c), refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has a bad value or range array", c);
     if (a.n_values + a.n_ranges > (1ll << 24))
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than 2^24 values and ranges", c), refuse(HS_EUNSUPPORTED);
+      return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: term on '%s' has more than 2^24 values and ranges", c);
     if (a.literal_type != HS_TYPE_INT64 && a.literal_type != HS_TYPE_DOUBLE && a.literal_type != HS_TYPE_STRING &&
         a.literal_type != HS_TYPE_DECIMAL)
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has an unknown literal type", c), refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has an unknown literal type", c);
     const int kind = a.flags & kTermPatterns;
-    if (a.flags & ~kTermFlags) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has unknown flags 0x%x", c, a.flags), refuse(HS_EINVAL);
+    if (a.flags & ~kTermFlags) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has unknown flags 0x%x", c, a.flags);
     if ((a.flags & HS_TERM_NULL_TRUE) && (a.flags & HS_TERM_NULL_FALSE))
-      return snprintf(msg, sizeof msg, "filter scan: term on '%s' has two null outcomes", c), refuse(HS_EINVAL);
-    if (kind & (kind - 1)) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has more than one pattern kind", c), refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has two null outcomes", c);
+    if (kind & (kind - 1)) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has more than one pattern kind", c);
     if (kind && (a.literal_type != HS_TYPE_STRING || a.n_values != 1 || a.n_ranges != 0))
-      return snprintf(msg, sizeof msg, "filter scan: the pattern term on '%s' needs one string value and no ranges", c), refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the pattern term on '%s' needs one string value and no ranges", c);
     if (a.n_values > 0) {
       const bool missing = a.literal_type == HS_TYPE_STRING ? (!a.values_offsets || (!a.values_bytes && a.values_offsets[a.n_values] != a.values_offsets[0]))
                                                             : (a.literal_type == HS_TYPE_DOUBLE ? !a.values_f : !a.values_i);
-      if (missing) return snprintf(msg, sizeof msg, "filter scan: term on '%s' has no value array", c), refuse(HS_EINVAL);
+      if (missing) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has no value array", c);
       if (a.literal_type == HS_TYPE_STRING)
         for (int64_t k = 0; k < a.n_values; k++) {
           if (a.values_offsets[k + 1] < a.values_offsets[k])
-            return snprintf(msg, sizeof msg, "filter scan: term on '%s' has descending value offsets", c), refuse(HS_EINVAL);
+            return refuse(HS_EINVAL, stats, err, errlen, "filter scan: term on '%s' has descending value offsets", c);
           if (a.values_offsets[k + 1] - a.values_offsets[k] > kMaxStringLen)
-            return snprintf(msg, sizeof msg, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c), refuse(HS_EUNSUPPORTED);
+            return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: a value of the term on '%s' is longer than 65535 bytes", c);
         }
     }
     if (kind == HS_TERM_LIKE) {
       try {
         parse_like(term_pattern(a));
       } catch (const Error& e) {
-        return snprintf(msg, sizeof msg, "%s", e.what()), refuse(e.code);
+        return refuse(e.code, stats, err, errlen, "%s", e.what());
       }
     }
     for (int r = 0; r < a.n_ranges; r++) {
       if (a.ranges[r].column && strcmp(a.ranges[r].column, c) != 0)
-        return snprintf(msg, sizeof msg, "filter scan: a range of the term on '%s' names another column", c), refuse(HS_EINVAL);
+        return refuse(HS_EINVAL, stats, err, errlen, "filter scan: a range of the term on '%s' names another column", c);
       hs_predicate q = a.ranges[r];
       q.column = c;
       const int rc = check_predicates(&q, 1, false, stats, err, errlen);
@@ -624,26 +627,44 @@ inline CompareDesc resolve_compare(const hs_column_compare& cc, const PredColumn
 
 // The refusals of a comparison list that need no data, beside n_others predicates and terms: as check_anys.
 inline int check_compares(const hs_column_compare* cmps, int n_cmps, int n_others, hs_stats* stats, char* err, size_t errlen) {
-  char msg[256];
-  auto refuse = [&](int code) {
-    if (stats) memset(stats, 0, sizeof *stats);
-    if (err && errlen) snprintf(err, errlen, "%s", msg);
-    return code;
-  };
-  if (n_cmps < 0 || (n_cmps > 0 && !cmps)) return snprintf(msg, sizeof msg, "filter scan: bad comparison array"), refuse(HS_EINVAL);
+  if (n_cmps < 0 || (n_cmps > 0 && !cmps)) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: bad comparison array");
   if (n_others + n_cmps > kMaxPredicates)
-    return snprintf(msg, sizeof msg, "filter scan: more than 16 predicates and terms"), refuse(HS_EUNSUPPORTED);
+    return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: more than 16 predicates and terms");
   for (int i = 0; i < n_cmps; i++) {
     const hs_column_compare& c = cmps[i];
-    if (!c.left || !c.right) return snprintf(msg, sizeof msg, "filter scan: comparison without a column"), refuse(HS_EINVAL);
+    if (!c.left || !c.right) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: comparison without a column");
     if (c.op < HS_CMP_LT || c.op > HS_CMP_EQ_NULL_SAFE)
-      return snprintf(msg, sizeof msg, "filter scan: comparison of '%s' and '%s' has an unknown operator %d", c.left, c.right, c.op),
-             refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: comparison of '%s' and '%s' has an unknown operator %d", c.left,
+                    c.right, c.op);
     if (c.flags & ~HS_TERM_NOT)
-      return snprintf(msg, sizeof msg, "filter scan: comparison of '%s' and '%s' has unknown flags 0x%x", c.left, c.right, c.flags),
-             refuse(HS_EINVAL);
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: comparison of '%s' and '%s' has unknown flags 0x%x", c.left,
+                    c.right, c.flags);
   }
   return HS_OK;
+}
+
+// The filter of a filter scan or of one join side, as its entry point was given it: predicates, disjunction terms and
+// comparisons between two columns, all AND-ed.
+struct Filter {
+  const hs_predicate* preds = nullptr;
+  int n_preds = 0;
+  const hs_predicate_any* anys = nullptr;
+  int n_anys = 0;
+  const hs_column_compare* cmps = nullptr;
+  int n_cmps = 0;
+};
+
+// The refusals of the filters of a call's n_sides sides that need no data, in one order whatever side a fault is on:
+// every side's predicates, then every side's terms, then every side's comparisons.  bounds_in_spec: as check_predicates.
+inline int check_filters(const Filter* sides, int n_sides, bool bounds_in_spec, hs_stats* stats, char* err, size_t errlen) {
+  int rc = HS_OK;
+  for (int s = 0; s < n_sides && rc == HS_OK; s++)
+    rc = check_predicates(sides[s].preds, sides[s].n_preds, bounds_in_spec, stats, err, errlen);
+  for (int s = 0; s < n_sides && rc == HS_OK; s++)
+    rc = check_anys(sides[s].anys, sides[s].n_anys, sides[s].n_preds, stats, err, errlen);
+  for (int s = 0; s < n_sides && rc == HS_OK; s++)
+    rc = check_compares(sides[s].cmps, sides[s].n_cmps, sides[s].n_preds + sides[s].n_anys, stats, err, errlen);
+  return rc;
 }
 
 }  // namespace hs

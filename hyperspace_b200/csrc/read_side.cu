@@ -549,13 +549,12 @@ int64_t compact_rows(hs_ctx* ctx, const uint32_t* mask, int64_t n, const uint32_
   return (int64_t)count;
 }
 
-int64_t select_rows(hs_ctx* ctx, const PredSet& preds, const PatternSet& pats, const CompareSet& cmps, const uint32_t* cand,
-                    int64_t n, const int64_t* file_ids, const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept,
-                    Buf<uint64_t>* offsets) {
+int64_t select_rows(hs_ctx* ctx, const RowFilter& filter, const uint32_t* cand, int64_t n, const int64_t* file_ids,
+                    const int64_t* deleted, int ndeleted, Buf<uint32_t>* kept, Buf<uint64_t>* offsets) {
   Buf<uint32_t> mask(ctx, std::max<int64_t>(1, n));
-  launch_predicate_mask(ctx, preds, cand, n, mask.get());
-  launch_pattern_mask(ctx, pats, cand, n, mask.get());
-  launch_compare_mask(ctx, cmps, cand, n, mask.get());
+  launch_predicate_mask(ctx, filter.preds, cand, n, mask.get());
+  launch_pattern_mask(ctx, filter.pats, cand, n, mask.get());
+  launch_compare_mask(ctx, filter.cmps, cand, n, mask.get());
   Buf<int64_t> d_deleted;
   if (n > 0 && ndeleted > 0) {
     d_deleted.alloc(ctx, ndeleted);

@@ -3,6 +3,8 @@
 // One case per line on stdin, one line out per case.
 //   resolve L R <op> <flags>         resolve_compare: "ok <domain> <factor0> <factor1>", or "refused <code> <message>"
 //   check <left|-> <right|-> <op> <flags> <n_others>   check_compares of one comparison: "ok" or "refused <code> <message>"
+//   sides <left op> <left pred ok> <right op> <right pred ok>   check_filters of two sides, each with the comparison a OP b
+//                                    and one predicate on a, without a column when "pred ok" is 0: as check
 //   rows L R <op> <flags> <n> then n times: <lnull> <lvalue> <rnull> <rvalue>    compare_holds per row: "ok" and 0 / 1 each
 //   d2d <unscaled> <scale>           decimal_to_double: "ok" and the double's bits in hex
 // A column L / R is "<kind> <precision> <scale>": kind one of integer long float double string binary date timestamp decimal
@@ -139,6 +141,20 @@ void run(const std::string& line) {
       const int n_others = (int)in.i();
       char err[256] = "";
       const int rc = check_compares(&cc, 1, n_others, nullptr, err, sizeof err);
+      if (rc == HS_OK) printf("ok\n");
+      else printf("refused %d %s\n", rc, err);
+    } else if (op == "sides") {
+      hs_column_compare cc[2];
+      hs_predicate p[2];
+      Filter f[2];
+      for (int s = 0; s < 2; s++) {
+        cc[s] = hs_column_compare{"a", "b", (int32_t)in.i(), 0};
+        p[s] = hs_predicate{};
+        p[s].column = in.i() ? "a" : nullptr, p[s].has_lo = 1, p[s].literal_type = HS_TYPE_INT64;
+        f[s].preds = &p[s], f[s].n_preds = 1, f[s].cmps = &cc[s], f[s].n_cmps = 1;
+      }
+      char err[256] = "";
+      const int rc = check_filters(f, 2, false, nullptr, err, sizeof err);
       if (rc == HS_OK) printf("ok\n");
       else printf("refused %d %s\n", rc, err);
     } else if (op == "d2d") {

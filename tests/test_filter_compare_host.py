@@ -100,6 +100,15 @@ def test_check_compares(native):
     assert got[7] == "refused -6 filter scan: more than 16 predicates and terms"
 
 
+def test_check_filters_order_across_sides(native):
+    # every side's predicates before any side's comparisons, and the left side before the right one
+    got = run(native, ["sides 1 1 5 1", "sides 7 1 1 0", "sides 7 1 9 1", "sides 1 1 9 1", "sides 1 0 7 0"])
+    assert got[0] == "ok"
+    assert got[1] == got[4] == "refused -1 filter scan: predicate without a column"
+    assert got[2] == "refused -1 filter scan: comparison of 'a' and 'b' has an unknown operator 7"
+    assert got[3] == "refused -1 filter scan: comparison of 'a' and 'b' has an unknown operator 9"
+
+
 # ---- the scalar comparison on hard values -------------------------------------------------------------------------------
 
 def _fmt(t, v):
