@@ -32,6 +32,8 @@ HS_CMP_LT, HS_CMP_LE, HS_CMP_GT, HS_CMP_GE, HS_CMP_EQ, HS_CMP_EQ_NULL_SAFE = 1, 
 CMP_OPS = {"<": HS_CMP_LT, "<=": HS_CMP_LE, ">": HS_CMP_GT, ">=": HS_CMP_GE, "=": HS_CMP_EQ, "<=>": HS_CMP_EQ_NULL_SAFE}
 HS_JOIN_LEFT_SEMI, HS_JOIN_LEFT_ANTI = 1, 2  # join_type of hs_bucket_join_exists
 JOIN_TYPES = {"semi": HS_JOIN_LEFT_SEMI, "anti": HS_JOIN_LEFT_ANTI}
+HS_JOIN_LEFT_OUTER, HS_JOIN_RIGHT_OUTER, HS_JOIN_FULL_OUTER = 3, 4, 5  # join_type of hs_bucket_join_outer
+OUTER_JOIN_TYPES = {"left": HS_JOIN_LEFT_OUTER, "right": HS_JOIN_RIGHT_OUTER, "full": HS_JOIN_FULL_OUTER}
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -134,7 +136,7 @@ EXPORTED_SYMBOLS = [
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
-    "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists",
+    "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists", "hs_bucket_join_outer",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -194,7 +196,8 @@ def load_library() -> C.CDLL:
                        ("hs_bucket_join_where", [*join, *side[:2], *side[:2], *out]),
                        ("hs_bucket_join_any", [*join, *side[:4], *side[:4], *out]),
                        ("hs_bucket_join_cmp", [*join, *side, *side, *out]),
-                       ("hs_bucket_join_exists", [*join[:2], C.c_int32, *join[2:], *side, *side, *out])):
+                       ("hs_bucket_join_exists", [*join[:2], C.c_int32, *join[2:], *side, *side, *out]),
+                       ("hs_bucket_join_outer", [*join[:2], C.c_int32, *join[2:], *side, *side, *out])):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     L.hs_batch_num_rows.restype = C.c_int64
@@ -1048,6 +1051,23 @@ class Context:
         jt = JOIN_TYPES[join_type] if isinstance(join_type, str) else join_type
         return self._bucket_join(load_library().hs_bucket_join_exists, jt, left, left_buckets, right, right_buckets, num_buckets,
                                  left_keys, right_keys, left_columns, [], (left_predicates, left_terms, left_compares),
+                                 (right_predicates, right_terms, right_compares), output)
+
+    def bucket_join_outer(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                          right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                          left_columns: Sequence[str], right_columns: Sequence[str], join_type="left",
+                          left_predicates: Sequence[tuple] = (), right_predicates: Sequence[tuple] = (),
+                          left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (), left_compares: Sequence[tuple] = (),
+                          right_compares: Sequence[tuple] = (), output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_outer: the left (``join_type="left"``), right (``"right"``) or full (``"full"``) outer join of
+        bucket_join_cmp's sides.  The batch holds left_columns, then right_columns; a row padded on one side has that
+        side's columns null (their validity is 0), and every column of a side that may be padded has a validity array.
+        join_type may also be an HS_JOIN_* code (others are refused by the library)."""
+        if isinstance(join_type, str) and join_type not in OUTER_JOIN_TYPES:
+            raise ValueError(f"join_type must be one of {sorted(OUTER_JOIN_TYPES)} or an HS_JOIN_* code, not {join_type!r}")
+        jt = OUTER_JOIN_TYPES[join_type] if isinstance(join_type, str) else join_type
+        return self._bucket_join(load_library().hs_bucket_join_outer, jt, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, right_columns, (left_predicates, left_terms, left_compares),
                                  (right_predicates, right_terms, right_compares), output)
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------

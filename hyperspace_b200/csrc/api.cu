@@ -800,8 +800,10 @@ void hs_result_free(hs_index_result* r) {
 // read side
 // ---------------------------------------------------------------------------------------------------------------------
 
+// padded: d_idx may hold kNoRow (an outer join's null-supplying side), which gives a null; every column then has a
+// validity vector
 static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int>& col_idx, const uint32_t* d_idx,
-                              int64_t n_out, hs_batch* b) {
+                              int64_t n_out, hs_batch* b, bool padded = false) {
   // all gathers first, then all copies, one synchronisation at the end
   std::vector<Buf<uint8_t>> d_data, d_valid;
   std::vector<Buf<uint64_t>> d_offsets(col_idx.size());
@@ -809,6 +811,24 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
   for (size_t k = 0; k < col_idx.size(); k++) {
     const int ci = col_idx[k];
     const DevColumn& c = t.cols[ci];
+    if (padded) {
+      const uint8_t* valid = c.has_nulls ? c.valid.get() : nullptr;
+      d_valid.emplace_back(ctx, (size_t)std::max<int64_t>(1, n_out));
+      if (c.type == HS_TYPE_STRING) {
+        Buf<uint32_t> lens(ctx, (size_t)std::max<int64_t>(1, n_out));
+        d_offsets[k].alloc(ctx, (size_t)n_out + 1);
+        launch_string_lengths_padded(ctx, (const uint64_t*)c.data.get(), valid, d_idx, n_out, lens.get(), d_valid.back().get());
+        exclusive_scan_u32_u64(ctx, lens.get(), n_out, d_offsets[k].get());
+        copy_d2h(ctx, &str_bytes[k], d_offsets[k].get() + n_out, 8);
+        sync_stream(ctx);
+        d_data.emplace_back(ctx, std::max<uint64_t>(1, str_bytes[k]));
+        launch_copy_strings_padded(ctx, (const uint64_t*)c.data.get(), valid, d_idx, n_out, d_offsets[k].get(), d_data.back().get());
+      } else {
+        d_data.emplace_back(ctx, (size_t)std::max<int64_t>(1, n_out) * c.width);
+        launch_gather_padded(ctx, c.data.get(), valid, d_idx, n_out, c.width, d_data.back().get(), d_valid.back().get());
+      }
+      continue;
+    }
     if (c.type == HS_TYPE_STRING) {
       // values are references into the source images (still alive here): lengths -> offsets -> one copy of the bytes
       const uint8_t* valid = c.has_nulls ? c.valid.get() : nullptr;
@@ -840,14 +860,14 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
     hs_batch::Col bc;
     bc.name = c.name;
     bc.type = c.type;
-    bc.has_valid = c.has_nulls;
+    bc.has_valid = c.has_nulls || padded;
     const bool is_str = c.type == HS_TYPE_STRING;
     const size_t data_bytes = is_str ? (size_t)str_bytes[i] : (size_t)n_out * c.width;
     bc.total_bytes = is_str ? str_bytes[i] : 0;
     if (b->on_device) {  // the next GPU operator consumes the columns where they are
       bc.data = std::move(d_data[i]);
       if (is_str) bc.offsets = std::move(d_offsets[i]);
-      if (c.has_nulls) bc.valid = std::move(d_valid[i]);
+      if (bc.has_valid) bc.valid = std::move(d_valid[i]);
     } else {
       // result columns go straight to their pinned buffers on the copy engine (the ring of copy_d2h would stage results of
       // up to 16 MB through a host memcpy)
@@ -857,7 +877,7 @@ static void batch_from_gather(hs_ctx* ctx, const Table& t, const std::vector<int
         bc.offsets.alloc(ctx, (size_t)n_out + 1, true);
         copy_d2h_engine(ctx, bc.offsets.get(), d_offsets[i].get(), 8 * ((size_t)n_out + 1));
       }
-      if (c.has_nulls) {
+      if (bc.has_valid) {
         bc.valid.alloc(ctx, (size_t)std::max<int64_t>(1, n_out), true);
         if (n_out) copy_d2h_engine(ctx, bc.valid.get(), d_valid[i].get(), (size_t)n_out);
       }
@@ -1349,7 +1369,14 @@ struct JoinSide {
   int64_t n = 0;  // rows in sorted order
   std::vector<int> proj;  // the projected columns of t
   BoundFilter filter;
-  RowFilter sel;  // the side selection: IS NOT NULL on the nullable key columns, then the filter
+  RowFilter sel;  // the side selection: IS NOT NULL on the nullable key columns (not on a preserved side), then the filter
+  // FullOuter: the selected positions with no null key, the ones the other side's probe searches (a binary search over
+  // positions with a null key would not be over sorted data: a null sorts first only at its own column).  The same as
+  // the above when no key column has nulls.
+  const uint32_t* nn_perm = nullptr;
+  Buf<uint32_t> nn_kept;
+  int64_t nn_n = 0;
+  std::vector<uint64_t> nn_seg;
 };
 
 // Orders the decoded rows of one join side bucket-major and key-sorted.  When every bucket holds exactly one file the
@@ -1404,27 +1431,45 @@ static void prepare_join_side(hs_ctx* ctx, JoinSide* side, const hs_source_file*
 // Side selection: keeps the rows that pass side->sel.  It runs over the sorted positions as its candidate list, so the
 // compacted rows stay in sorted order and a bucket's new boundaries are the scan's values at the old ones.  Launches
 // nothing when side->sel is empty.
-static void select_join_side(hs_ctx* ctx, JoinSide* side, int nb) {
-  if (side->sel.empty()) return;
-  Buf<uint64_t> offs;
-  side->n = select_rows(ctx, side->sel, side->perm, side->n, nullptr, nullptr, 0, &side->kept, &offs);
-  side->perm = side->kept.get();
+// d_out[b] = d_scan[seg[b]] for the nb + 1 bucket boundaries seg (< 2^32: the caller checked the side's size)
+static void at_bucket_bounds(hs_ctx* ctx, const uint64_t* d_scan, const std::vector<uint64_t>& seg, int nb, Buf<uint64_t>* d_out) {
   std::vector<uint32_t> bounds(nb + 1);
-  for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)side->seg[b];  // < 2^32: the caller checked the side's size
+  for (int b = 0; b <= nb; b++) bounds[b] = (uint32_t)seg[b];
   Buf<uint32_t> d_bounds(ctx, nb + 1);
-  Buf<uint64_t> d_seg(ctx, nb + 1);
+  d_out->alloc(ctx, nb + 1);
   copy_h2d(ctx, d_bounds.get(), bounds.data(), 4 * (nb + 1));
-  launch_gather_plain(ctx, offs.get(), d_bounds.get(), nb + 1, 8, d_seg.get());
-  copy_d2h(ctx, side->seg.data(), d_seg.get(), 8 * (nb + 1));
+  launch_gather_plain(ctx, d_scan, d_bounds.get(), nb + 1, 8, d_out->get());
+}
+
+// Keeps the sorted positions (*perm, *n, *seg) that pass sel: compacted into *kept, which *perm then points into
+static void select_positions(hs_ctx* ctx, const RowFilter& sel, int nb, Buf<uint32_t>* kept, const uint32_t** perm, int64_t* n,
+                             std::vector<uint64_t>* seg) {
+  Buf<uint64_t> offs;
+  *n = select_rows(ctx, sel, *perm, *n, nullptr, nullptr, 0, kept, &offs);
+  *perm = kept->get();
+  Buf<uint64_t> d_seg;
+  at_bucket_bounds(ctx, offs.get(), *seg, nb, &d_seg);
+  copy_d2h(ctx, seg->data(), d_seg.get(), 8 * (nb + 1));
   sync_stream(ctx);
 }
 
-// bucket_join_core's join_type for the inner join (include/hs_gpu.h numbers the semi and anti joins from 1)
+static void select_join_side(hs_ctx* ctx, JoinSide* side, int nb) {
+  if (side->sel.empty()) return;
+  select_positions(ctx, side->sel, nb, &side->kept, &side->perm, &side->n, &side->seg);
+}
+
+// bucket_join_core's join_type for the inner join (include/hs_gpu.h numbers the semi and anti joins from 1, the outer
+// joins from 3)
 constexpr int kJoinInner = 0;
 
+static bool is_outer_join(int join_type) {
+  return join_type == HS_JOIN_LEFT_OUTER || join_type == HS_JOIN_RIGHT_OUTER || join_type == HS_JOIN_FULL_OUTER;
+}
+
 // The one bucket join of the sides' filters (left, right).  legacy (hs_bucket_join): one key per side, no filters, null
-// keys refused.  k_join_count (inner) or k_join_exists (join_type HS_JOIN_LEFT_SEMI / HS_JOIN_LEFT_ANTI) probes on the
-// key columns where they lie: the decoded columns, or their gather through the side's permutation.
+// keys refused.  k_join_count (inner), k_join_exists (join_type HS_JOIN_LEFT_SEMI / HS_JOIN_LEFT_ANTI) or
+// k_join_count_outer (HS_JOIN_*_OUTER) probes on the key columns where they lie: the decoded columns, or their gather
+// through the side's permutation.
 static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* const* left_keys, const char* const* right_keys,
                             int n_keys, const Filter filters[2], bool legacy, int join_type, hs_batch** out, hs_stats* stats,
                             char* err, size_t errlen) {
@@ -1470,13 +1515,16 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
         fail(HS_EUNSUPPORTED, "bucket join: key columns '%s' and '%s' have different types", left_keys[k], right_keys[k]);
       }
     if (R.n >= (1ll << 32) || L.n >= (1ll << 32)) fail(HS_EUNSUPPORTED, "join side larger than 2^32-1 rows");
-    // side selection: IS NOT NULL on the nullable key columns, then the side's filter.  An anti join keeps the left rows
-    // with a null key (they match nothing, so they are output): its probe reads their validity instead.
-    const bool anti = join_type == HS_JOIN_LEFT_ANTI;
+    // side selection: IS NOT NULL on the nullable key columns, then the side's filter.  A preserved side -- the left side
+    // of an anti join, the output sides of an outer join -- keeps the rows with a null key (they match nothing, so they
+    // are output): its probe reads their validity instead.
+    const bool anti = join_type == HS_JOIN_LEFT_ANTI, outer = is_outer_join(join_type), full = join_type == HS_JOIN_FULL_OUTER;
+    const bool preserved[2] = {anti || join_type == HS_JOIN_LEFT_OUTER || full, join_type == HS_JOIN_RIGHT_OUTER || full};
     PredUploads uploads;
+    RowFilter not_null[2];  // FullOuter: IS NOT NULL on the side's nullable key columns, for its searched positions
     for (int s = 0; s < 2; s++) {
-      PredSet& ps = side[s].sel.preds;
-      for (int k = 0; k < n_keys && !(anti && s == 0); k++) {
+      PredSet& ps = (preserved[s] ? not_null[s] : side[s].sel).preds;
+      for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = side[s].t.cols[k];
         if (c.has_nulls) {
           PredDesc d{};
@@ -1489,24 +1537,42 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     StageTimer t_sel(ctx);
     t_sel.start();
     for (JoinSide& s : side) select_join_side(ctx, &s, nb);
+    if (full) {  // the searched positions: the selected ones again, through IS NOT NULL alone
+      for (int s = 0; s < 2; s++) {
+        JoinSide& S = side[s];
+        S.nn_perm = S.perm, S.nn_n = S.n, S.nn_seg = S.seg;
+        if (!not_null[s].empty()) select_positions(ctx, not_null[s], nb, &S.nn_kept, &S.nn_perm, &S.nn_n, &S.nn_seg);
+      }
+    }
     t_sel.stop();
     // the key columns in (selected) sorted order
     std::vector<Buf<uint8_t>> key_bufs;
-    auto sorted_column = [&](const JoinSide& s, const uint8_t* data, int width) {
-      if (!s.perm) return data;
-      key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, s.n) * width);
-      launch_gather_plain(ctx, data, s.perm, s.n, width, key_bufs.back().get());
+    auto sorted_column = [&](const uint32_t* perm, int64_t n, const uint8_t* data, int width) {
+      if (!perm) return data;
+      key_bufs.emplace_back(ctx, (size_t)std::max<int64_t>(1, n) * width);
+      launch_gather_plain(ctx, data, perm, n, width, key_bufs.back().get());
       return (const uint8_t*)key_bufs.back().get();
     };
-    auto key_cols = [&](const JoinSide& s) {
+    auto key_cols_at = [&](const JoinSide& s, const uint32_t* perm, int64_t n) {
       JoinKeyCols kc{};
       kc.n = n_keys;
       for (int k = 0; k < n_keys; k++) {
         const DevColumn& c = s.t.cols[k];
         kc.type[k] = c.type;
-        kc.col[k] = sorted_column(s, c.data.get(), c.width);
+        kc.col[k] = sorted_column(perm, n, c.data.get(), c.width);
       }
       return kc;
+    };
+    auto key_cols = [&](const JoinSide& s) { return key_cols_at(s, s.perm, s.n); };
+    // the validity of a preserved side's nullable key columns, in its selected sorted order
+    auto key_valid = [&](const JoinSide& s) {
+      JoinKeyValid kv{};
+      kv.n = n_keys;
+      for (int k = 0; k < n_keys; k++) {
+        const DevColumn& c = s.t.cols[k];
+        if (c.has_nulls) kv.valid[k] = sorted_column(s.perm, s.n, c.valid.get(), 1);
+      }
+      return kv;
     };
     const int64_t nl = L.n;
     StageTimer t_join(ctx);
@@ -1516,16 +1582,65 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     copy_h2d(ctx, d_rseg.get(), R.seg.data(), 8 * (nb + 1));
     const JoinKeyCols lk = key_cols(L), rk = key_cols(R);
     uint64_t total_out = 0;
-    if (join_type != kJoinInner) {
+    if (outer) {
+      // the probing side p is the preserved one (the left side of FullOuter), q the side it searches: RightOuter is
+      // LeftOuter with the roles swapped, the batch still the left columns, then the right ones
+      const int p = join_type == HS_JOIN_RIGHT_OUTER ? 1 : 0, q = 1 - p;
+      const JoinSide& P = side[p];
+      const JoinKeyCols kc[2] = {lk, rk};
+      const uint64_t* d_seg[2] = {d_lseg.get(), d_rseg.get()};
+      // the searched positions: FullOuter's non-null ones where a side has them apart
+      JoinKeyCols sk[2] = {lk, rk};
+      const uint64_t* d_sseg[2] = {d_seg[0], d_seg[1]};
+      const uint32_t* sperm[2] = {L.perm, R.perm};
+      Buf<uint64_t> d_nn_seg[2];
+      for (int s = 0; s < 2 && full; s++) {
+        const JoinSide& S = side[s];
+        sperm[s] = S.nn_perm;
+        if (S.nn_perm == S.perm) continue;
+        sk[s] = key_cols_at(S, S.nn_perm, S.nn_n);
+        d_nn_seg[s].alloc(ctx, nb + 1);
+        copy_h2d(ctx, d_nn_seg[s].get(), S.nn_seg.data(), 8 * (nb + 1));
+        d_sseg[s] = d_nn_seg[s].get();
+      }
+      const int64_t np = P.n;
+      Buf<uint32_t> counts(ctx, std::max<int64_t>(1, np)), first(ctx, std::max<int64_t>(1, np));
+      Buf<uint64_t> offs(ctx, np + 1);
+      launch_join_count_outer(ctx, kc[p], key_valid(P), d_seg[p], sk[q], d_sseg[q], nb, np, counts.get(), first.get());
+      exclusive_scan_u32_u64(ctx, counts.get(), np, offs.get());
+      copy_d2h(ctx, &total_out, offs.get() + np, 8);
+      sync_stream(ctx);
+      // FullOuter: the right positions that match nothing (k_join_exists in anti mode into the left side's searched
+      // positions), compacted into right rows; ranks[i] = how many of them come before right position i
+      Buf<uint32_t> urow;
+      Buf<uint64_t> ranks;
+      int64_t nu = 0;
+      if (full) {
+        Buf<uint32_t> keep(ctx, std::max<int64_t>(1, R.n));
+        launch_join_exists(ctx, rk, key_valid(R), d_rseg.get(), sk[0], d_sseg[0], nb, R.n, false, keep.get());
+        nu = compact_rows(ctx, keep.get(), R.n, R.perm, &urow, &ranks);
+        total_out += (uint64_t)nu;
+      }
+      if (total_out >= (1ull << 32)) fail(HS_EUNSUPPORTED, "join output larger than 2^32-1 rows per call");
+      Buf<uint32_t> lrow(ctx, std::max<uint64_t>(1, total_out)), rrow(ctx, std::max<uint64_t>(1, total_out));
+      uint32_t* out_row[2] = {lrow.get(), rrow.get()};
+      // FullOuter's placement: bucket b's left-outer rows move up by the unmatched right rows of the buckets before it
+      // (ucum[b]); its unmatched right rows follow its left-outer rows (the scan of counts at the next bucket's start)
+      Buf<uint64_t> ucum, lcum;
+      if (full) {
+        at_bucket_bounds(ctx, ranks.get(), R.seg, nb, &ucum);
+        at_bucket_bounds(ctx, offs.get(), L.seg, nb, &lcum);
+        launch_join_place_unmatched(ctx, urow.get(), nu, ucum.get(), lcum.get() + 1, nb, lrow.get(), rrow.get());
+      }
+      launch_join_emit_outer(ctx, counts.get(), first.get(), offs.get(), d_seg[p], full ? ucum.get() : nullptr, nb, np, P.perm,
+                             sperm[q], out_row[p], out_row[q]);
+      t_join.stop();
+      batch_from_gather(ctx, L.t, L.proj, lrow.get(), (int64_t)total_out, res.get(), preserved[1]);
+      batch_from_gather(ctx, R.t, R.proj, rrow.get(), (int64_t)total_out, res.get(), preserved[0]);
+    } else if (join_type != kJoinInner) {
       // semi / anti: one keep mask over the left sorted positions, compacted through L.perm into left rows
       JoinKeyValid lv{};
-      if (anti) {
-        lv.n = n_keys;
-        for (int k = 0; k < n_keys; k++) {
-          const DevColumn& c = L.t.cols[k];
-          if (c.has_nulls) lv.valid[k] = sorted_column(L, c.valid.get(), 1);
-        }
-      }
+      if (anti) lv = key_valid(L);
       Buf<uint32_t> keep(ctx, std::max<int64_t>(1, nl)), lrow;
       launch_join_exists(ctx, lk, lv, d_lseg.get(), rk, d_rseg.get(), nb, nl, !anti, keep.get());
       total_out = (uint64_t)compact_rows(ctx, keep.get(), nl, L.perm, &lrow);
@@ -1548,7 +1663,7 @@ static int bucket_join_core(hs_ctx* ctx, const hs_join_spec* spec, const char* c
     total.stop();
     sync_stream(ctx);
     st.ms_sort += t_join.ms();
-    if (!L.sel.empty() || !R.sel.empty()) st.ms_exchange += t_sel.ms();
+    if (!L.sel.empty() || !R.sel.empty() || (full && (!not_null[0].empty() || !not_null[1].empty()))) st.ms_exchange += t_sel.ms();
     st.rows_out = (int64_t)total_out;
     st.ms_total = total.ms();
     st.gpu_launches = ctx->launches;
@@ -1585,7 +1700,11 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
 
 }  // extern "C"
 
-// hs_bucket_join_cmp's and hs_bucket_join_exists's checks that need no data, then the join of the sides' filters
+// bucket_join_checked's join_type for a join_type hs_bucket_join_exists / hs_bucket_join_outer does not take
+constexpr int kBadExistsJoin = -1, kBadOuterJoin = -2;
+
+// hs_bucket_join_cmp's, hs_bucket_join_exists's and hs_bucket_join_outer's checks that need no data, then the join of the
+// sides' filters
 static int bucket_join_checked(hs_ctx* ctx, const hs_join_spec* spec, int join_type, const char* const* left_keys,
                                const char* const* right_keys, int n_keys, const Filter filters[2], hs_batch** out, hs_stats* stats,
                                char* err, size_t errlen) {
@@ -1593,9 +1712,12 @@ static int bucket_join_checked(hs_ctx* ctx, const hs_join_spec* spec, int join_t
   for (int s = 0; s < 2; s++)
     if (filters[s].n_preds < 0 || (filters[s].n_preds > 0 && !filters[s].preds)) return HS_EINVAL;
   *out = nullptr;
-  if (join_type != kJoinInner && join_type != HS_JOIN_LEFT_SEMI && join_type != HS_JOIN_LEFT_ANTI)
+  if (join_type == kBadExistsJoin)
     return refuse(HS_EINVAL, stats, err, errlen, "bucket join: join_type must be HS_JOIN_LEFT_SEMI or HS_JOIN_LEFT_ANTI");
-  if (join_type != kJoinInner && spec->n_right_columns != 0)
+  if (join_type == kBadOuterJoin)
+    return refuse(HS_EINVAL, stats, err, errlen,
+                  "bucket join: join_type must be HS_JOIN_LEFT_OUTER, HS_JOIN_RIGHT_OUTER or HS_JOIN_FULL_OUTER");
+  if ((join_type == HS_JOIN_LEFT_SEMI || join_type == HS_JOIN_LEFT_ANTI) && spec->n_right_columns != 0)
     return refuse(HS_EINVAL, stats, err, errlen, "bucket join: a semi or anti join outputs left columns only (n_right_columns must be 0)");
   if (n_keys < 1) return refuse(HS_EINVAL, stats, err, errlen, "bucket join: at least one key column per side");
   if (n_keys > kMaxJoinKeys) return refuse(HS_EUNSUPPORTED, stats, err, errlen, "bucket join: more than 8 key columns");
@@ -1626,9 +1748,22 @@ int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_ty
                           int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   const Filter filters[2] = {{left_preds, n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps},
                              {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps}};
-  // an inner join is hs_bucket_join_cmp's: kJoinInner (0) is refused like any other value outside HS_JOIN_*
-  return bucket_join_checked(ctx, spec, join_type == kJoinInner ? -1 : join_type, left_keys, right_keys, n_keys, filters, out, stats,
-                             err, errlen);
+  // an inner join is hs_bucket_join_cmp's: kJoinInner (0) is refused like any other value outside the two
+  const bool ok = join_type == HS_JOIN_LEFT_SEMI || join_type == HS_JOIN_LEFT_ANTI;
+  return bucket_join_checked(ctx, spec, ok ? join_type : kBadExistsJoin, left_keys, right_keys, n_keys, filters, out, stats, err,
+                             errlen);
+}
+
+int hs_bucket_join_outer(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                         const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                         const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                         int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
+                         const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
+                         int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
+  const Filter filters[2] = {{left_preds, n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps},
+                             {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps}};
+  return bucket_join_checked(ctx, spec, is_outer_join(join_type) ? join_type : kBadOuterJoin, left_keys, right_keys, n_keys, filters,
+                             out, stats, err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

@@ -487,7 +487,7 @@ void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* ls
 // (perm nullptr: row p)
 void launch_join_emit(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
                       int64_t nl, const uint32_t* lperm, const uint32_t* rperm, uint32_t* out_lrow, uint32_t* out_rrow);
-// The validity of the n key columns of the left side in sorted order, one byte per position (valid[k] nullptr: key
+// The validity of the n key columns of the probing side in sorted order, one byte per position (valid[k] nullptr: key
 // column k has no nulls): a position with a null in any of them matches nothing.
 struct JoinKeyValid {
   const uint8_t* valid[kMaxJoinKeys];
@@ -497,6 +497,34 @@ struct JoinKeyValid {
 // positions of its bucket and keep_match is set (semi), or has none and keep_match is clear (anti); 0 otherwise
 void launch_join_exists(hs_ctx* ctx, const JoinKeyCols& lkeys, const JoinKeyValid& lvalid, const uint64_t* lseg,
                         const JoinKeyCols& rkeys, const uint64_t* rseg, int nseg, int64_t nl, bool keep_match, uint32_t* keep);
+// The outer joins' "no row": the row an output pair holds for a side padded with nulls.  Never a real row: a join side
+// has fewer than 2^32 - 1 rows.
+constexpr uint32_t kNoRow = 0xFFFFFFFFu;
+// The outer joins' probe (k_join_count_outer), from the np positions of the preserved side p into the searched side t:
+// k_join_count's counts and first matches, except that a position with a null in a key column (pvalid) or with no match
+// gets count 1 and first_match kNoRow
+void launch_join_count_outer(hs_ctx* ctx, const JoinKeyCols& pkeys, const JoinKeyValid& pvalid, const uint64_t* pseg,
+                             const JoinKeyCols& tkeys, const uint64_t* tseg, int nseg, int64_t np, uint32_t* counts,
+                             uint32_t* first_match);
+// The outer joins' (preserved row, searched row) pairs at out_offsets (the scan of counts), the searched row kNoRow where
+// first_match is; shift (nseg + 1 entries, or nullptr) moves every output position of bucket b up by shift[b]
+void launch_join_emit_outer(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
+                            const uint64_t* pseg, const uint64_t* shift, int nseg, int64_t np, const uint32_t* pperm,
+                            const uint32_t* tperm, uint32_t* out_prow, uint32_t* out_trow);
+// FullOuter: the right row urow[r] (rank r; ucum: the ranks at which the nseg buckets start, nseg + 1 entries) goes to
+// output position base[b] + r of the bucket b holding r, its left row kNoRow
+void launch_join_place_unmatched(hs_ctx* ctx, const uint32_t* urow, int64_t nu, const uint64_t* ucum, const uint64_t* base,
+                                 int nseg, uint32_t* out_lrow, uint32_t* out_rrow);
+// launch_gather_plain for a padded side: out[i] = src[idx[i]] and out_valid[i] = valid[idx[i]] (1 when valid is nullptr),
+// 0 and 0 where idx[i] is kNoRow
+void launch_gather_padded(hs_ctx* ctx, const void* src, const uint8_t* valid, const uint32_t* idx, int64_t n, int width, void* out,
+                          uint8_t* out_valid);
+// launch_string_lengths / launch_copy_strings for a padded side: a kNoRow value is a null of length 0; the lengths pass
+// also writes every value's validity
+void launch_string_lengths_padded(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
+                                  uint32_t* lens, uint8_t* out_valid);
+void launch_copy_strings_padded(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
+                                const uint64_t* offsets, uint8_t* out);
 // exclusive scan of uint32 counts into uint64 offsets (n+1 entries; last = total)
 void exclusive_scan_u32_u64(hs_ctx* ctx, const uint32_t* in, int64_t n, uint64_t* out);
 // lens[i] = length of refs[idx[i]] (0 for a null);  then, with offsets = exclusive scan of lens: out[offsets[i] ..] = bytes

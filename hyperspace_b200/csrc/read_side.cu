@@ -308,6 +308,135 @@ __global__ void k_join_emit(const uint32_t* __restrict__ counts, const uint32_t*
   }
 }
 
+// The outer joins' probe, one thread per position of the preserved (probing) side: k_join_exists' key-validity test and
+// equality test at the lower bound, then, where that matches, k_join_count's search for the end of the match range.  A
+// position with a null in any key column (pv), or with no match, is output once with the other side padded: counts[i] =
+// max(matches, 1), and first_match[i] = kNoRow where there is no match.
+template <int KT0>
+__device__ __forceinline__ void join_count_outer_rows(const JoinKeyCols& pk, const JoinKeyValid& pv, const uint64_t* __restrict__ pseg,
+                                                      const JoinKeyCols& tk, const uint64_t* __restrict__ tseg, int nseg, int64_t np,
+                                                      uint32_t* __restrict__ counts, uint32_t* __restrict__ first_match) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += stride) {
+    bool null = false;
+    for (int k = 0; k < pv.n; k++) null |= pv.valid[k] != nullptr && pv.valid[k][i] == 0;
+    uint32_t count = 1, first = kNoRow;
+    if (!null) {
+      const int s = segment_of(pseg, nseg, i);
+      const int64_t p0 = key_value<KT0>(pk.col[0], i);
+      const int64_t tb = (int64_t)tseg[s], tn = (int64_t)tseg[s + 1] - tb;
+      const int64_t f = lower_bound_tuple<KT0>(p0, pk, i, tk, tb, tn);
+      if (f < tn && compare_tuple<KT0>(p0, pk, i, tk, tb + f) == 0) {
+        int64_t x = 0, y = tn;  // first position > the tuple (from the start again: the same path, so cached)
+        while (x < y) {
+          const int64_t mid = x + ((y - x) >> 1);
+          if (compare_tuple<KT0>(p0, pk, i, tk, tb + mid) >= 0) x = mid + 1;
+          else y = mid;
+        }
+        count = (uint32_t)(x - f);
+        first = (uint32_t)(tb + f);
+      }
+    }
+    counts[i] = count;
+    first_match[i] = first;
+  }
+}
+
+__global__ void k_join_count_outer(const __grid_constant__ JoinKeyCols pk, const __grid_constant__ JoinKeyValid pv,
+                                   const uint64_t* __restrict__ pseg, const __grid_constant__ JoinKeyCols tk,
+                                   const uint64_t* __restrict__ tseg, int nseg, int64_t np, uint32_t* __restrict__ counts,
+                                   uint32_t* __restrict__ first_match) {
+  switch (pk.type[0]) {
+    case HS_TYPE_INT32: join_count_outer_rows<HS_TYPE_INT32>(pk, pv, pseg, tk, tseg, nseg, np, counts, first_match); break;
+    case HS_TYPE_INT64: join_count_outer_rows<HS_TYPE_INT64>(pk, pv, pseg, tk, tseg, nseg, np, counts, first_match); break;
+    default: join_count_outer_rows<HS_TYPE_STRING>(pk, pv, pseg, tk, tseg, nseg, np, counts, first_match); break;
+  }
+}
+
+// The outer joins' pairs: preserved position i (row pperm[i]) with each of its matches, the searched positions
+// [first_match[i], + counts[i]) (rows tperm[...]), or once with kNoRow when first_match[i] is kNoRow.  shift (FullOuter,
+// else nullptr): every output position of bucket b moves up by shift[b], the rows placed before the bucket's own
+// (k_join_place_unmatched); the bucket of i is found by segment_of over pseg.
+__global__ void k_join_emit_outer(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ first_match,
+                                  const uint64_t* __restrict__ out_offsets, const uint64_t* __restrict__ pseg,
+                                  const uint64_t* __restrict__ shift, int nseg, int64_t np, const uint32_t* __restrict__ pperm,
+                                  const uint32_t* __restrict__ tperm, uint32_t* __restrict__ out_prow, uint32_t* __restrict__ out_trow) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += stride) {
+    uint64_t o = out_offsets[i];
+    if (shift) o += shift[segment_of(pseg, nseg, i)];
+    const uint32_t prow = pperm ? pperm[i] : (uint32_t)i;
+    const uint32_t f = first_match[i];
+    if (f == kNoRow) {
+      out_prow[o] = prow;
+      out_trow[o] = kNoRow;
+      continue;
+    }
+    const uint32_t c = counts[i];
+    for (uint32_t j = 0; j < c; j++) {
+      out_prow[o + j] = prow;
+      out_trow[o + j] = tperm ? tperm[f + j] : f + j;
+    }
+  }
+}
+
+// FullOuter's right rows that match nothing: urow[r], of global rank r in (bucket, right sorted position) order, goes to
+// output position base[b] + r with its left row kNoRow; b is the bucket holding rank r (ucum: the nseg + 1 ranks at which
+// the buckets start), base[b] the number of left-outer rows in buckets 0..b.
+__global__ void k_join_place_unmatched(const uint32_t* __restrict__ urow, int64_t nu, const uint64_t* __restrict__ ucum,
+                                       const uint64_t* __restrict__ base, int nseg, uint32_t* __restrict__ out_lrow,
+                                       uint32_t* __restrict__ out_rrow) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nu; r += stride) {
+    const uint64_t o = base[segment_of(ucum, nseg, r)] + (uint64_t)r;
+    out_lrow[o] = kNoRow;
+    out_rrow[o] = urow[r];
+  }
+}
+
+// The gathers of a side an outer join pads: row idx[i], or a null (value 0, validity 0) where idx[i] is kNoRow.  The
+// validity is always written; valid nullptr: the column has no nulls.
+template <typename T>
+__global__ void k_gather_padded(const T* __restrict__ src, const uint8_t* __restrict__ valid, const uint32_t* __restrict__ idx,
+                                int64_t n, T* __restrict__ out, uint8_t* __restrict__ out_valid) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const uint32_t r = idx[i];
+    const bool pad = r == kNoRow;
+    out[i] = pad ? T(0) : src[r];
+    out_valid[i] = pad ? 0 : (valid ? valid[r] : 1);
+  }
+}
+
+// k_string_lengths over a padded side: a padded value has length 0 and validity 0
+__global__ void k_string_lengths_padded(const uint64_t* __restrict__ refs, const uint8_t* __restrict__ valid,
+                                        const uint32_t* __restrict__ idx, int64_t n, uint32_t* __restrict__ lens,
+                                        uint8_t* __restrict__ out_valid) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const uint32_t r = idx[i];
+    const uint8_t v = r == kNoRow ? 0 : (valid ? valid[r] : 1);
+    lens[i] = v ? ref_len(refs[r]) : 0u;
+    out_valid[i] = v;
+  }
+}
+
+// k_copy_strings over a padded side: padded values (and nulls) copy nothing
+__global__ void k_copy_strings_padded(const uint64_t* __restrict__ refs, const uint8_t* __restrict__ valid,
+                                      const uint32_t* __restrict__ idx, int64_t n, const uint64_t* __restrict__ offsets,
+                                      uint8_t* __restrict__ out) {
+  const unsigned lane = threadIdx.x & 31;
+  const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+    const uint32_t r = idx[i];
+    if (r == kNoRow || (valid && !valid[r])) continue;
+    const uint64_t ref = refs[r];
+    const uint8_t* src = ref_ptr(ref);
+    uint8_t* dst = out + offsets[i];
+    for (uint32_t j = lane, len = ref_len(ref); j < len; j += 32) dst[j] = src[j];
+  }
+}
+
 // ---- exclusive scan uint32 -> uint64 (three kernels; block of 256 threads x 8 items) --------------------------------
 constexpr int kScanThreads = 256;
 constexpr int kScanItems = 8;
@@ -529,6 +658,62 @@ void launch_join_exists(hs_ctx* ctx, const JoinKeyCols& lkeys, const JoinKeyVali
   if (nl == 0) return;
   k_join_exists<<<grid_for(ctx, nl, 256, 16), 256, 0, ctx->stream>>>(lkeys, lvalid, lseg, rkeys, rseg, nseg, nl,
                                                                        keep_match ? 1u : 0u, keep);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_join_count_outer(hs_ctx* ctx, const JoinKeyCols& pkeys, const JoinKeyValid& pvalid, const uint64_t* pseg,
+                             const JoinKeyCols& tkeys, const uint64_t* tseg, int nseg, int64_t np, uint32_t* counts,
+                             uint32_t* first_match) {
+  KernelScope _ks(ctx, "k_join_count_outer");
+  if (np == 0) return;
+  k_join_count_outer<<<grid_for(ctx, np, 256, 16), 256, 0, ctx->stream>>>(pkeys, pvalid, pseg, tkeys, tseg, nseg, np, counts,
+                                                                            first_match);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_join_emit_outer(hs_ctx* ctx, const uint32_t* counts, const uint32_t* first_match, const uint64_t* out_offsets,
+                            const uint64_t* pseg, const uint64_t* shift, int nseg, int64_t np, const uint32_t* pperm,
+                            const uint32_t* tperm, uint32_t* out_prow, uint32_t* out_trow) {
+  KernelScope _ks(ctx, "k_join_emit_outer");
+  if (np == 0) return;
+  k_join_emit_outer<<<grid_for(ctx, np, 256, 16), 256, 0, ctx->stream>>>(counts, first_match, out_offsets, pseg, shift, nseg, np,
+                                                                           pperm, tperm, out_prow, out_trow);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_join_place_unmatched(hs_ctx* ctx, const uint32_t* urow, int64_t nu, const uint64_t* ucum, const uint64_t* base,
+                                 int nseg, uint32_t* out_lrow, uint32_t* out_rrow) {
+  KernelScope _ks(ctx, "k_join_place_unmatched");
+  if (nu == 0) return;
+  k_join_place_unmatched<<<grid_for(ctx, nu, 256, 16), 256, 0, ctx->stream>>>(urow, nu, ucum, base, nseg, out_lrow, out_rrow);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_gather_padded(hs_ctx* ctx, const void* src, const uint8_t* valid, const uint32_t* idx, int64_t n, int width, void* out,
+                          uint8_t* out_valid) {
+  KernelScope _ks(ctx, "k_gather_padded");
+  if (n == 0) return;
+  const int grid = grid_for(ctx, n, 256, 16);
+  switch (width) {
+    case 8: k_gather_padded<uint64_t><<<grid, 256, 0, ctx->stream>>>((const uint64_t*)src, valid, idx, n, (uint64_t*)out, out_valid); break;
+    case 4: k_gather_padded<uint32_t><<<grid, 256, 0, ctx->stream>>>((const uint32_t*)src, valid, idx, n, (uint32_t*)out, out_valid); break;
+    case 1: k_gather_padded<uint8_t><<<grid, 256, 0, ctx->stream>>>((const uint8_t*)src, valid, idx, n, (uint8_t*)out, out_valid); break;
+    default: fail(HS_EINVAL, "gather: unsupported width %d", width);
+  }
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_string_lengths_padded(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
+                                  uint32_t* lens, uint8_t* out_valid) {
+  if (n == 0) return;
+  k_string_lengths_padded<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(refs, valid, idx, n, lens, out_valid);
+  HS_LAUNCH_CHECK(ctx);
+}
+
+void launch_copy_strings_padded(hs_ctx* ctx, const uint64_t* refs, const uint8_t* valid, const uint32_t* idx, int64_t n,
+                                const uint64_t* offsets, uint8_t* out) {
+  if (n == 0) return;
+  k_copy_strings_padded<<<grid_for(ctx, n * 32, 256, 16), 256, 0, ctx->stream>>>(refs, valid, idx, n, offsets, out);
   HS_LAUNCH_CHECK(ctx);
 }
 

@@ -245,12 +245,17 @@ class ScanExec:
         return _concat(parts, out_cols)
 
 
+# JoinNode.how of the outer joins -> join_type of Context.bucket_join_outer
+_OUTER = {"leftouter": "left", "rightouter": "right", "fullouter": "full"}
+
+
 class BucketJoinExec:
     """Join of two index scans bucket by bucket (no exchange), or of two on-the-fly bucketed sides when no index applies.
     ``keys`` are the (left, right) key pairs in the order both sides are bucketed and sorted on: the left index's indexed
     columns when the indexes serve, the condition's order otherwise; None when the condition is not a one-to-one equi-join
     between the two sides, which the GPU join cannot run.  A filter below a side becomes that side's predicates.  ``how``
-    is "inner", or "leftsemi" / "leftanti" (hs_bucket_join_exists: left rows only, each at most once)."""
+    is "inner", "leftsemi" / "leftanti" (hs_bucket_join_exists: left rows only, each at most once), or "leftouter" /
+    "rightouter" / "fullouter" (hs_bucket_join_outer: rows padded with nulls where the other side has no match)."""
 
     def __init__(self, session, left: Linear, right: Linear, keys: Optional[List[Tuple[str, str]]], lcand: Optional[Candidate],
                  rcand: Optional[Candidate], condition: Optional[List[Tuple[str, str]]] = None, how: str = "inner"):
@@ -267,7 +272,8 @@ class BucketJoinExec:
         keys = ", ".join(f"{l} = {r}" for l, r in (self.keys or self.condition or []))
         filters = "".join(f", {n}Filter={lin.predicate.conjuncts()}{_terms_text(lin.predicate)}"
                           for n, lin in (("left", self.left), ("right", self.right)) if lin.predicate)
-        jt = {"leftsemi": ", joinType=LeftSemi", "leftanti": ", joinType=LeftAnti"}.get(self.how, "")
+        jt = {"leftsemi": ", joinType=LeftSemi", "leftanti": ", joinType=LeftAnti", "leftouter": ", joinType=LeftOuter",
+              "rightouter": ", joinType=RightOuter", "fullouter": ", joinType=FullOuter"}.get(self.how, "")
         return (f"GpuBucketJoin({side(self.lcand, self.left)}, {side(self.rcand, self.right)}, keys=[{keys}]{jt}{filters}, "
                 "exchange=none)")
 
@@ -310,6 +316,9 @@ class BucketJoinExec:
             if self.how == "inner":
                 batch, _ = self.session.gpu.bucket_join_cmp(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
                                                             lp, rp, lt_, rt_, lc_, rc_)
+            elif self.how in _OUTER:
+                batch, _ = self.session.gpu.bucket_join_outer(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
+                                                              _OUTER[self.how], lp, rp, lt_, rt_, lc_, rc_)
             else:
                 batch, _ = self.session.gpu.bucket_join_exists(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output,
                                                                "semi" if self.how == "leftsemi" else "anti", lp, rp, lt_, rt_,
@@ -319,10 +328,12 @@ class BucketJoinExec:
                 t.free()
         out: Dict[str, np.ndarray] = {}
         nleft = len(self.left.output)
-        for i, (n, d, _) in enumerate(batch.columns):
+        for i, (n, d, v) in enumerate(batch.columns):
             name = n if n not in out else f"{n}_right"
             types = dict((self.left if i < nleft else self.right).relation.schema)
             out[name] = spark_values(_host_column(d), types.get(n))
+            if self.how in _OUTER and v is not None:  # an outer join's nulls: masked where the column is not valid
+                out[name] = np.ma.MaskedArray(out[name], mask=np.asarray(v) == 0)
         batch.free()
         return out
 
@@ -458,7 +469,7 @@ def plan_query(session, plan):
         if l is None or r is None:
             raise LE.HyperspaceException("only joins of linear plans (Project?(Filter?(Relation))) are handled")
         keys = join_key_pairs(l, r, node.pairs)
-        semi_or_anti = node.how != "inner"
+        semi_or_anti = node.how in ("leftsemi", "leftanti")
         if semi_or_anti:  # the right side of a semi / anti join is only probed: it outputs its keys, its filter is read
             r = Linear(r.relation, r.predicate, [b for _, b in keys] if keys else [])
         if post_project is not None:  # column pruning: each side outputs only what the final projection needs + its keys

@@ -516,7 +516,8 @@ class ProjectNode:
 @dataclass
 class JoinNode:
     """Equi-join on the AND of ``left column == right column`` for every pair (a pair may name its columns in either
-    order; rules.join_key_pairs orients them).  ``how`` is "inner", "leftsemi" or "leftanti" (normalise_join_type)."""
+    order; rules.join_key_pairs orients them).  ``how`` is "inner", "leftsemi" or "leftanti" (normalise_join_type), or
+    "leftouter", "rightouter" or "fullouter" -- the canonical names of Spark's JoinType.apply -- for an outer join."""
     left: object
     right: object
     pairs: List[Tuple[str, str]]
@@ -524,8 +525,8 @@ class JoinNode:
 
 
 # The join types the GPU path runs, under the spellings JoinType.apply accepts once lower-cased with "_" removed:
-# EXISTS / IN-subquery (LeftSemi) and NOT EXISTS (LeftAnti) besides the inner join.  Outer joins need null-padded
-# output and are not handled.
+# EXISTS / IN-subquery (LeftSemi) and NOT EXISTS (LeftAnti) besides the inner join.  The outer joins run from a JoinNode
+# whose how is "leftouter", "rightouter" or "fullouter"; DataFrame.join does not take their spellings yet.
 _JOIN_TYPES = {"inner": "inner", "leftsemi": "leftsemi", "semi": "leftsemi", "leftanti": "leftanti", "anti": "leftanti"}
 
 
@@ -691,7 +692,8 @@ class DataFrame:
 
     # ---- actions ------------------------------------------------------------------------------------
     def collect(self) -> Dict[str, np.ndarray]:
-        """Executes the plan on the GPU and returns the result columns as numpy arrays (row order unspecified)."""
+        """Executes the plan on the GPU and returns the result columns as numpy arrays (row order unspecified).  Under an
+        outer join a column that can hold nulls comes back as a numpy.ma.MaskedArray, masked where the value is null."""
         from .rules import plan_query
 
         return plan_query(self.session, self.plan).execute()
@@ -709,7 +711,7 @@ def output_columns(plan) -> List[str]:
     if isinstance(plan, ProjectNode):
         return list(plan.columns)
     if isinstance(plan, JoinNode):
-        if plan.how != "inner":  # a semi or anti join outputs the left side's columns only
+        if plan.how in ("leftsemi", "leftanti"):  # a semi or anti join outputs the left side's columns only
             return output_columns(plan.left)
         return output_columns(plan.left) + [c for c in output_columns(plan.right)]
     raise TypeError(plan)

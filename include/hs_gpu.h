@@ -482,11 +482,44 @@ int hs_bucket_join_exists(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_ty
                           const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
                           int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
 
+/* join_type of hs_bucket_join_outer: Spark 3.1's LeftOuter, RightOuter and FullOuter */
+#define HS_JOIN_LEFT_OUTER 3
+#define HS_JOIN_RIGHT_OUTER 4
+#define HS_JOIN_FULL_OUTER 5
+
+/* The left, right or full outer join of hs_bucket_join_cmp's sides, bucket b of the left index with bucket b of the right
+ * index and no exchange -- SortMergeJoinExec with joinType LeftOuter / RightOuter / FullOuter over Filter(left) and
+ * Filter(right), which JoinIndexRule rewrites as it does an inner join (JoinIndexRule.scala:54 matches any join type).
+ * Keys, predicates, terms, comparisons, key types and their refusals (codes and messages) are hs_bucket_join_cmp's.  Both
+ * projections are allowed, and either may be empty; the batch holds the left columns, then the right ones.  A side whose
+ * rows are output whether they match or not is preserved (the left side of LeftOuter, the right side of RightOuter, both
+ * of FullOuter); the other side supplies nulls.
+ *   A row that fails its side's filter is not output when its side is preserved, and matches nothing otherwise.  A row
+ *   with a null in any key column matches nothing; on a preserved side it is output once, padded.
+ *   HS_JOIN_LEFT_OUTER   every selected left row comes out once per matching right row, or once with every right column
+ *                        null; order (bucket, left sorted position, right sorted position).
+ *   HS_JOIN_RIGHT_OUTER  the mirror image, in (bucket, right sorted position, left sorted position) order; the columns are
+ *                        still the left ones, then the right ones.
+ *   HS_JOIN_FULL_OUTER   within each bucket, the bucket's HS_JOIN_LEFT_OUTER rows in the order above, then the bucket's
+ *                        right rows that matched nothing, in right sorted position order, with every left column null.
+ *                        Spark 3.1 gives a full outer join no output ordering; this order is the library's own.
+ * Every column of a null-supplying side has a validity vector, even when no row was padded (both sides under FullOuter);
+ * a padded value is 0, or a string of length 0.  More than 2^32 - 1 output rows is HS_EUNSUPPORTED, as for the inner
+ * join.  A join_type other than the three above is HS_EINVAL.  stats->ms_sort reports the probe, the emit and the
+ * placement of FullOuter's unmatched right rows, stats->ms_exchange the side selections, stats->rows_out the output rows. */
+int hs_bucket_join_outer(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                         const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                         const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                         int32_t n_left_cmps, const hs_predicate* right_preds, int32_t n_right_preds,
+                         const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
+                         int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
 int64_t hs_batch_num_rows(const hs_batch* b);
 int32_t hs_batch_on_device(const hs_batch* b); /* != 0: the column pointers are device pointers (output = HS_OUT_DEVICE) */
 int32_t hs_batch_num_columns(const hs_batch* b);
 /* Column i: name, HS_TYPE_*, pointer to num_rows values, pointer to one validity byte per row (NULL when the column
- * has no nulls); host pointers unless hs_batch_on_device. */
+ * has no nulls; an outer join's null-supplying side always has one, see hs_bucket_join_outer); host pointers unless
+ * hs_batch_on_device. */
 int hs_batch_column(const hs_batch* b, int32_t i, const char** name, int32_t* type, const void** data,
                     const uint8_t** valid);
 /* A HS_TYPE_STRING column: `data` of hs_batch_column points to the values' bytes back to back, and value r occupies
