@@ -48,19 +48,21 @@ __global__ void __launch_bounds__(kThreads) k_dict_build(const void* __restrict_
         continue;
       }
       uint32_t h = dict_hash(v) & mask;
-      // A thread inserts only while the distinct count is still below max_distinct; threads that passed that check
-      // concurrently can overshoot by at most two inserts each, and the launcher caps the grid so that
-      // max_distinct + 2 * #threads stays below the table capacity: the table never fills, probing terminates.
+      // A thread counts an insert only while the distinct count is still below max_distinct; threads that passed that
+      // check concurrently can overshoot by at most two inserts each, and the launcher caps the grid so that
+      // max_distinct + 2 * #threads stays below the table capacity: the table never fills, probing terminates.  At the
+      // limit only a value that wins an empty slot is new: another thread may be inserting the same value right now.
       for (uint32_t probes = 0; probes <= mask; probes++) {
         const unsigned long long cur = keys[h];
         if (cur == v) break;
         if (cur == kEmpty) {
-          if (*(volatile uint32_t*)&state[0] >= max_distinct) {
-            state[1] = 1;
-            return;
-          }
+          const bool full = *(volatile uint32_t*)&state[0] >= max_distinct;
           const unsigned long long old = atomicCAS(&keys[h], kEmpty, (unsigned long long)v);
           if (old == kEmpty) {
+            if (full) {
+              state[1] = 1;
+              return;
+            }
             atomicAdd(&state[0], 1u);
             break;
           }
@@ -73,7 +75,7 @@ __global__ void __launch_bounds__(kThreads) k_dict_build(const void* __restrict_
 }
 
 // Hash set filled from the dictionary pages of the source chunks (one CTA per data page; pages of one chunk insert the same
-// few values again, which costs nothing).  Used when every page of a column was dictionary-encoded.
+// few values again).  Used when every page of a column was dictionary-encoded; entries no row uses stay in the set.
 __global__ void __launch_bounds__(kThreads) k_dict_build_from_pages(const PageDesc* __restrict__ pages, int col, int width,
                                                                      unsigned long long* __restrict__ keys, uint32_t mask,
                                                                      uint32_t max_distinct, uint32_t* __restrict__ state) {
@@ -88,16 +90,17 @@ __global__ void __launch_bounds__(kThreads) k_dict_build_from_pages(const PageDe
       continue;
     }
     uint32_t h = dict_hash(v) & mask;
-    for (uint32_t probes = 0; probes <= mask; probes++) {
+    for (uint32_t probes = 0; probes <= mask; probes++) {  // the insert of k_dict_build
       const unsigned long long cur = keys[h];
       if (cur == v) break;
       if (cur == kEmpty) {
-        if (*(volatile uint32_t*)&state[0] >= max_distinct) {
-          state[1] = 1;
-          return;
-        }
+        const bool full = *(volatile uint32_t*)&state[0] >= max_distinct;
         const unsigned long long old = atomicCAS(&keys[h], kEmpty, (unsigned long long)v);
         if (old == kEmpty) {
+          if (full) {
+            state[1] = 1;
+            return;
+          }
           atomicAdd(&state[0], 1u);
           break;
         }

@@ -811,7 +811,7 @@ void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>&
       for (int c : cand) {
         DevColumn& dc = out->cols[c];
         memcpy(dc.dict_state, &h_states[4 * c], 16);
-        dc.dict_ready = dc.dict_state[1] == 0;
+        dc.dict_ready = dc.dict_state[1] == 0 && dc.dict_state[0] <= kMaxDictEntries;  // (the count can pass it unflagged)
         if (!dc.dict_ready) dc.dict_keys.release();
       }
     }
