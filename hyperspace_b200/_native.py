@@ -34,6 +34,11 @@ HS_JOIN_LEFT_SEMI, HS_JOIN_LEFT_ANTI = 1, 2  # join_type of hs_bucket_join_exist
 JOIN_TYPES = {"semi": HS_JOIN_LEFT_SEMI, "anti": HS_JOIN_LEFT_ANTI}
 HS_JOIN_LEFT_OUTER, HS_JOIN_RIGHT_OUTER, HS_JOIN_FULL_OUTER = 3, 4, 5  # join_type of hs_bucket_join_outer
 OUTER_JOIN_TYPES = {"left": HS_JOIN_LEFT_OUTER, "right": HS_JOIN_RIGHT_OUTER, "full": HS_JOIN_FULL_OUTER}
+HS_JOIN_INNER = 0  # join_type of hs_bucket_join_expr, besides the five above
+ALL_JOIN_TYPES = {"inner": HS_JOIN_INNER, **JOIN_TYPES, **OUTER_JOIN_TYPES}
+# hs_expr_node.kind
+HS_EXPR_COLUMN, HS_EXPR_LITERAL, HS_EXPR_ADD, HS_EXPR_SUB, HS_EXPR_MUL, HS_EXPR_DIV, HS_EXPR_REM, HS_EXPR_NEG = range(1, 9)
+EXPR_OPS = {"+": HS_EXPR_ADD, "-": HS_EXPR_SUB, "*": HS_EXPR_MUL, "/": HS_EXPR_DIV, "%": HS_EXPR_REM, "neg": HS_EXPR_NEG}
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -101,6 +106,16 @@ class ColumnCompareSpec(C.Structure):
     _fields_ = [("left", C.c_char_p), ("right", C.c_char_p), ("op", C.c_int32), ("flags", C.c_int32)]
 
 
+class ExprNodeSpec(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("column", C.c_char_p), ("literal_type", C.c_int32), ("scale", C.c_int32),
+                ("value_i", C.c_int64), ("value_f", C.c_double)]
+
+
+class ExprCompareSpec(C.Structure):
+    _fields_ = [("left", C.POINTER(ExprNodeSpec)), ("n_left", C.c_int32), ("right", C.POINTER(ExprNodeSpec)),
+                ("n_right", C.c_int32), ("op", C.c_int32), ("flags", C.c_int32)]
+
+
 class JoinSpec(C.Structure):
     _fields_ = [("left_files", C.POINTER(SourceFile)), ("n_left", C.c_int32),
                 ("right_files", C.POINTER(SourceFile)), ("n_right", C.c_int32),
@@ -136,7 +151,8 @@ EXPORTED_SYMBOLS = [
     "hs_create_index_async", "hs_pending_wait", "hs_pending_cancel", "hs_verify_index", "hs_synth_checksum",
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
-    "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists", "hs_bucket_join_outer",
+    "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists", "hs_bucket_join_outer", "hs_filter_scan_expr",
+    "hs_bucket_join_expr",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -182,10 +198,13 @@ def load_library() -> C.CDLL:
     L.hs_result_free.restype = None
     L.hs_result_free.argtypes = [C.c_void_p]
     # the read-side calls, from the parameter groups of include/hs_gpu.h: scan head, join head, one side's filter
-    # (predicates, terms, comparisons: a call takes the first one, two or all three), the files' buckets, outputs
+    # (predicates, terms, comparisons, expression comparisons: a call takes the first one, two, three or all four), the
+    # files' buckets, outputs
     scan = [C.c_void_p, C.POINTER(ScanSpec)]
     join = [C.c_void_p, C.POINTER(JoinSpec), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32]
-    side = [C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32, C.POINTER(ColumnCompareSpec), C.c_int32]
+    side_x = [C.POINTER(PredicateSpec), C.c_int32, C.POINTER(PredicateAnySpec), C.c_int32, C.POINTER(ColumnCompareSpec), C.c_int32,
+              C.POINTER(ExprCompareSpec), C.c_int32]
+    side = side_x[:6]
     buckets = [C.c_void_p, C.c_int32]
     out = [C.POINTER(C.c_void_p), C.POINTER(Stats), *err]
     for name, args in (("hs_filter_scan", [*scan, *out]),
@@ -197,7 +216,9 @@ def load_library() -> C.CDLL:
                        ("hs_bucket_join_any", [*join, *side[:4], *side[:4], *out]),
                        ("hs_bucket_join_cmp", [*join, *side, *side, *out]),
                        ("hs_bucket_join_exists", [*join[:2], C.c_int32, *join[2:], *side, *side, *out]),
-                       ("hs_bucket_join_outer", [*join[:2], C.c_int32, *join[2:], *side, *side, *out])):
+                       ("hs_bucket_join_outer", [*join[:2], C.c_int32, *join[2:], *side, *side, *out]),
+                       ("hs_filter_scan_expr", [*scan, *side_x, *buckets, *out]),
+                       ("hs_bucket_join_expr", [*join[:2], C.c_int32, *join[2:], *side_x, *side_x, *out])):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = args
     L.hs_batch_num_rows.restype = C.c_int64
@@ -484,12 +505,77 @@ def _cmp_array(compares: Sequence[tuple]):
     return arr, len(compares), keep
 
 
+def expr_literal(v) -> Tuple[int, int, int, float]:
+    """A Python literal of an expression as (literal_type, scale, value_i, value_f), as py4j hands it to Spark: an int that
+    fits in 32 bits is an int, a larger one a long; a float is a double; a Decimal is a decimal of its own scale (its
+    unscaled value must fit in 64 bits).  bool and anything else raise ValueError."""
+    if isinstance(v, (bool, np.bool_)):
+        raise ValueError(f"a boolean literal ({v!r}) cannot be used in arithmetic")
+    if isinstance(v, (int, np.integer)):
+        v = int(v)
+        if not -2**63 <= v < 2**63:
+            raise ValueError(f"the integer literal {v} does not fit in a long")
+        return (HS_TYPE_INT32 if -2**31 <= v < 2**31 else HS_TYPE_INT64), 0, v, 0.0
+    if isinstance(v, (float, np.floating)):
+        return HS_TYPE_DOUBLE, 0, 0, float(v)
+    if isinstance(v, decimal.Decimal):
+        if not v.is_finite():
+            raise ValueError(f"the decimal literal {v} is not finite")
+        sign, digits, exp = v.as_tuple()
+        scale = max(0, -exp)
+        unscaled = int(v.scaleb(scale))
+        if not -2**63 <= unscaled < 2**63:
+            raise ValueError(f"the decimal literal {v} has more than 18 digits")
+        return HS_TYPE_DECIMAL, scale, unscaled, 0.0
+    raise ValueError(f"the literal {v!r} cannot be used in arithmetic")
+
+
+def _expr_nodes(nodes: Sequence[tuple]):
+    """One side of an expression comparison, postfix: ``("column", name)``, ``("literal", value)`` (typed by expr_literal)
+    or an operator ``(op,)`` with op one of EXPR_OPS's keys ("+", "-", "*", "/", "%", "neg") or an HS_EXPR_* code; a raw
+    ``(kind, column, literal_type, scale, value_i, value_f)`` tuple passes as it is.  Returns (array, count, keep)."""
+    keep = []
+    arr = (ExprNodeSpec * max(1, len(nodes)))()
+    for x, node in zip(arr, nodes):
+        tag = node[0]
+        if tag == "column":
+            name = node[1].encode() if node[1] is not None else None
+            keep.append(name)
+            x.kind, x.column = HS_EXPR_COLUMN, name
+        elif tag == "literal":
+            x.kind = HS_EXPR_LITERAL
+            x.literal_type, x.scale, x.value_i, x.value_f = expr_literal(node[1])
+        elif len(node) == 6:
+            name = node[1].encode() if node[1] is not None else None
+            keep.append(name)
+            x.kind, x.column, x.literal_type, x.scale, x.value_i, x.value_f = node[0], name, *node[2:]
+        else:
+            x.kind = EXPR_OPS[tag] if isinstance(tag, str) else tag
+    return arr, len(nodes), keep
+
+
+def _expr_array(exprs: Sequence[tuple]):
+    """``(left nodes, op, right nodes)`` or ``(left nodes, op, right nodes, flags)`` expression comparisons -> (hs_expr_compare
+    array, count, buffers to keep alive).  Nodes are _expr_nodes'; op and flags are _cmp_array's."""
+    keep = []
+    arr = (ExprCompareSpec * max(1, len(exprs)))()
+    for e, (left, op, right, *flags) in zip(arr, exprs):
+        la, nl, k1 = _expr_nodes(left)
+        ra, nr, k2 = _expr_nodes(right)
+        keep += [la, ra, k1, k2]
+        e.left, e.n_left, e.right, e.n_right = la, nl, ra, nr
+        e.op = CMP_OPS[op] if isinstance(op, str) else op
+        e.flags = flags[0] if flags else 0
+    return arr, len(exprs), keep
+
+
 def _filter_args(*parts, first=0):
     """One side's filter as the arguments of its parameter group: ``parts`` are its predicates (see _predicate_array),
-    then, for the calls that take them, its terms (_any_array) and its comparisons (_cmp_array); each becomes an array
-    and its count.  first=1: parts start at the terms.  Returns (arguments, buffers to keep alive)."""
+    then, for the calls that take them, its terms (_any_array), its comparisons (_cmp_array) and its expression
+    comparisons (_expr_array); each becomes an array and its count.  first=1: parts start at the terms.  Returns
+    (arguments, buffers to keep alive)."""
     args, keep = [], []
-    for build, part in zip((_predicate_array, _any_array, _cmp_array)[first:], parts):
+    for build, part in zip((_predicate_array, _any_array, _cmp_array, _expr_array)[first:], parts):
         arr, n, *k = build(part)
         args += [arr, n]
         keep += k
@@ -955,6 +1041,17 @@ class Context:
         return self._filter_scan(load_library().hs_filter_scan_cmp, files, key, projected, (predicates, terms, compares),
                                  sorted_on_key, deleted_file_ids, output, (file_buckets, num_buckets))
 
+    def filter_scan_expr(self, files: Sequence[FileImage], key: Optional[str], projected: Sequence[str], predicates: Sequence[tuple],
+                         terms: Sequence[tuple], compares: Sequence[tuple], exprs: Sequence[tuple], sorted_on_key: bool = True,
+                         deleted_file_ids: Sequence[int] = (), file_buckets: Optional[Sequence[int]] = None, num_buckets: int = 0,
+                         output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_filter_scan_expr: filter_scan_cmp with expression comparisons AND-ed to the filter, each ``(left nodes, op,
+        right nodes)`` with an optional fourth element, HS_TERM_NOT.  Nodes are postfix: ``("column", name)``,
+        ``("literal", value)`` and operators ``("+",)``, ``("-",)``, ``("*",)``, ``("/",)``, ``("%",)``, ``("neg",)``.
+        The engine types them as Spark 3.1 does."""
+        return self._filter_scan(load_library().hs_filter_scan_expr, files, key, projected, (predicates, terms, compares, exprs),
+                                 sorted_on_key, deleted_file_ids, output, (file_buckets, num_buckets))
+
     def _join_spec(self, left, left_buckets, right, right_buckets, num_buckets, left_key, right_key, left_columns, right_columns,
                    output):
         ls, k1 = _source_array(left)
@@ -1069,6 +1166,25 @@ class Context:
         return self._bucket_join(load_library().hs_bucket_join_outer, jt, left, left_buckets, right, right_buckets, num_buckets,
                                  left_keys, right_keys, left_columns, right_columns, (left_predicates, left_terms, left_compares),
                                  (right_predicates, right_terms, right_compares), output)
+
+    def bucket_join_expr(self, left: Sequence[FileImage], left_buckets: Sequence[int], right: Sequence[FileImage],
+                         right_buckets: Sequence[int], num_buckets: int, left_keys: Sequence[str], right_keys: Sequence[str],
+                         left_columns: Sequence[str], right_columns: Sequence[str], join_type="inner",
+                         left_predicates: Sequence[tuple] = (), right_predicates: Sequence[tuple] = (),
+                         left_terms: Sequence[tuple] = (), right_terms: Sequence[tuple] = (), left_compares: Sequence[tuple] = (),
+                         right_compares: Sequence[tuple] = (), left_exprs: Sequence[tuple] = (), right_exprs: Sequence[tuple] = (),
+                         output: int = HS_OUT_HOST) -> Tuple[Batch, Dict[str, float]]:
+        """hs_bucket_join_expr: the join of any type -- ``join_type`` "inner" (bucket_join_cmp), "semi" / "anti"
+        (bucket_join_exists: right_columns must be empty) or "left" / "right" / "full" (bucket_join_outer) -- with
+        filter_scan_expr's expression comparisons on either side.  join_type may also be an HS_JOIN_* code (others are
+        refused by the library)."""
+        if isinstance(join_type, str) and join_type not in ALL_JOIN_TYPES:
+            raise ValueError(f"join_type must be one of {sorted(ALL_JOIN_TYPES)} or an HS_JOIN_* code, not {join_type!r}")
+        jt = ALL_JOIN_TYPES[join_type] if isinstance(join_type, str) else join_type
+        return self._bucket_join(load_library().hs_bucket_join_expr, jt, left, left_buckets, right, right_buckets, num_buckets,
+                                 left_keys, right_keys, left_columns, right_columns,
+                                 (left_predicates, left_terms, left_compares, left_exprs),
+                                 (right_predicates, right_terms, right_compares, right_exprs), output)
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------
     @staticmethod

@@ -985,28 +985,82 @@ static int column_index(std::vector<std::string>* cols, const std::string& nm) {
 }
 
 // A filter bound to the columns a call decodes: the column of every predicate and term, the two columns of every
-// comparison, and the terms' resolutions
+// comparison, the column of every COLUMN node of each expression comparison, and the terms' resolutions
 struct BoundFilter {
   Filter f;
   std::vector<int> pred_col, any_col;
   std::vector<std::pair<int, int>> cmp_col;
   TermResolutions terms;
+  std::vector<std::vector<int>> expr_col;  // per expression comparison: its COLUMN nodes' columns, the left side's first
 };
 
-// f bound to the columns cols, which gains those not in it yet: the predicates' columns, the terms', then each
-// comparison's left and right column
+// f bound to the columns cols, which gains those not in it yet: the predicates' columns, the terms', each comparison's
+// left and right column, then each expression comparison's columns (after the others, so that a call without
+// expressions decodes what it always has)
 static BoundFilter bind_filter(const Filter& f, std::vector<std::string>* cols) {
   BoundFilter b{f, {}, {}, {}, TermResolutions(f.anys, f.n_anys)};
   for (int i = 0; i < f.n_preds; i++) b.pred_col.push_back(column_index(cols, f.preds[i].column));
   for (int i = 0; i < f.n_anys; i++) b.any_col.push_back(column_index(cols, f.anys[i].column));
   for (int i = 0; i < f.n_cmps; i++)
     b.cmp_col.push_back({column_index(cols, f.cmps[i].left), column_index(cols, f.cmps[i].right)});
+  for (int i = 0; i < f.n_exprs; i++) {
+    const hs_expr_compare& e = f.exprs[i];
+    std::vector<int> ec;
+    for (int s = 0; s < 2; s++)
+      for (int k = 0; k < (s ? e.n_right : e.n_left); k++) {
+        const hs_expr_node& x = (s ? e.right : e.left)[k];
+        if (x.kind == HS_EXPR_COLUMN) ec.push_back(column_index(cols, x.column));
+      }
+    b.expr_col.push_back(std::move(ec));
+  }
   return b;
+}
+
+// A host array copied to a new device buffer of up->bytes; the host copy is kept in up->staged_bytes until the copy has run
+template <typename T>
+static const T* upload_array(hs_ctx* ctx, const std::vector<T>& h, PredUploads* up) {
+  const size_t nb = sizeof(T) * h.size();
+  up->staged_bytes.emplace_back((const uint8_t*)h.data(), (const uint8_t*)h.data() + nb);
+  up->bytes.emplace_back(ctx, std::max<size_t>(16, nb));
+  if (nb) copy_h2d(ctx, up->bytes.back().get(), up->staged_bytes.back().data(), nb);
+  return (const T*)up->bytes.back().get();
+}
+
+// The expression comparisons of filter b on the columns of t, resolved (predicates.h: resolve_expr) into one program per
+// comparison and uploaded in one set: the descriptors, every instruction and every column they read
+static ExprSet upload_exprs(hs_ctx* ctx, const Table& t, const BoundFilter& b, PredUploads* up) {
+  std::vector<ExprDesc> descs;
+  std::vector<ExprInst> insts;
+  std::vector<ExprColumn> ecols;
+  for (size_t i = 0; i < b.expr_col.size(); i++) {
+    std::vector<PredColumn> pcs;
+    for (int c : b.expr_col[i]) pcs.push_back(pred_column(t.cols[c]));
+    const ExprProgram pg = resolve_expr(b.f.exprs[i], pcs);
+    const int32_t base = (int32_t)ecols.size();
+    for (int c : b.expr_col[i]) {
+      const DevColumn& dc = t.cols[c];
+      ecols.push_back(ExprColumn{dc.data.get(), dc.has_nulls ? dc.valid.get() : nullptr, dc.type});
+    }
+    ExprDesc d{(int32_t)insts.size(), 0, pg.domain, pg.op, pg.negate};
+    for (ExprInst in : pg.insts) {
+      if (in.op == kXLoad) in.arg += base;
+      insts.push_back(in);
+    }
+    d.end = (int32_t)insts.size();
+    descs.push_back(d);
+  }
+  ExprSet es;
+  es.descs = upload_array(ctx, descs, up);
+  es.insts = upload_array(ctx, insts, up);
+  es.cols = upload_array(ctx, ecols, up);
+  es.n = (int)descs.size();
+  return es;
 }
 
 // Appends to rf the descriptors of filter b on the columns of t, skipping those on column skip_col that its windows
 // already decide: a predicate in scalar form and a term in set form.  A pattern term that is not a prefix goes to
-// rf->pats (on skip_col too: the windows only bound its values), and every comparison to rf->cmps.
+// rf->pats (on skip_col too: the windows only bound its values), every comparison to rf->cmps, and the expression
+// comparisons to rf->exprs.
 static void add_filter(hs_ctx* ctx, const Table& t, BoundFilter& b, int skip_col, RowFilter* rf, PredUploads* up) {
   PredSet* ps = &rf->preds;
   for (size_t i = 0; i < b.pred_col.size(); i++) {
@@ -1040,6 +1094,7 @@ static void add_filter(hs_ctx* ctx, const Table& t, BoundFilter& b, int skip_col
     d.valid[0] = l.has_nulls ? l.valid.get() : nullptr, d.valid[1] = r.has_nulls ? r.valid.get() : nullptr;
     rf->cmps.p[rf->cmps.n++] = d;
   }
+  if (!b.expr_col.empty()) rf->exprs = upload_exprs(ctx, t, b, up);
 }
 
 // the bucket of every point of a key set, by the hash the build used (hash_rows over a column of the key's storage type
@@ -1275,9 +1330,9 @@ static int filter_scan_core(hs_ctx* ctx, const hs_scan_spec* spec, const Filter&
       idx.alloc(ctx, std::max<int64_t>(1, n_cand));
       if (nseg) launch_windows_to_indices(ctx, d_win.get(), d_oo.get(), nwin, n_cand, idx.get());
       n_out = n_cand;
-      if (on_key < filter.n_preds + filter.n_anys || filter.n_cmps > 0) {
-        // residual: the predicates on other columns and the comparisons, over the window rows, compacted through the
-        // candidate list
+      if (on_key < filter.n_preds + filter.n_anys || filter.n_cmps > 0 || filter.n_exprs > 0) {
+        // residual: the predicates on other columns, the comparisons and the expression comparisons, over the window
+        // rows, compacted through the candidate list
         RowFilter residual;
         add_filter(ctx, t, bf, 0, &residual, &uploads);
         Buf<uint32_t> kept_rows;
@@ -1344,10 +1399,18 @@ int hs_filter_scan_cmp(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate
                        const hs_predicate_any* anys, int32_t n_anys, const hs_column_compare* cmps, int32_t n_cmps,
                        const int32_t* file_buckets, int32_t num_buckets, hs_batch** out, hs_stats* stats, char* err,
                        size_t errlen) {
+  return hs_filter_scan_expr(ctx, spec, preds, n_preds, anys, n_anys, cmps, n_cmps, nullptr, 0, file_buckets, num_buckets, out, stats,
+                             err, errlen);
+}
+
+int hs_filter_scan_expr(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                        const hs_predicate_any* anys, int32_t n_anys, const hs_column_compare* cmps, int32_t n_cmps,
+                        const hs_expr_compare* exprs, int32_t n_exprs, const int32_t* file_buckets, int32_t num_buckets,
+                        hs_batch** out, hs_stats* stats, char* err, size_t errlen) {
   if (!ctx || !spec || !out || n_preds < 0 || (n_preds > 0 && !preds) || num_buckets < 0 || (num_buckets > 0 && !file_buckets))
     return HS_EINVAL;
   *out = nullptr;
-  const Filter f{preds, n_preds, anys, n_anys, cmps, n_cmps};
+  const Filter f{preds, n_preds, anys, n_anys, cmps, n_cmps, exprs, n_exprs};
   const int rc = check_filters(&f, 1, spec->has_lo || spec->has_hi, stats, err, errlen);
   if (rc != HS_OK) return rc;
   if (num_buckets > kMaxBuckets) return refuse(HS_EUNSUPPORTED, stats, err, errlen, "numBuckets must be in 1..%d", kMaxBuckets);
@@ -1460,7 +1523,7 @@ static void select_join_side(hs_ctx* ctx, JoinSide* side, int nb) {
 
 // bucket_join_core's join_type for the inner join (include/hs_gpu.h numbers the semi and anti joins from 1, the outer
 // joins from 3)
-constexpr int kJoinInner = 0;
+constexpr int kJoinInner = HS_JOIN_INNER;
 
 static bool is_outer_join(int join_type) {
   return join_type == HS_JOIN_LEFT_OUTER || join_type == HS_JOIN_RIGHT_OUTER || join_type == HS_JOIN_FULL_OUTER;
@@ -1700,8 +1763,9 @@ int hs_bucket_join_any(hs_ctx* ctx, const hs_join_spec* spec, const char* const*
 
 }  // extern "C"
 
-// bucket_join_checked's join_type for a join_type hs_bucket_join_exists / hs_bucket_join_outer does not take
-constexpr int kBadExistsJoin = -1, kBadOuterJoin = -2;
+// bucket_join_checked's join_type for a join_type hs_bucket_join_exists / hs_bucket_join_outer / hs_bucket_join_expr does
+// not take
+constexpr int kBadExistsJoin = -1, kBadOuterJoin = -2, kBadJoin = -3;
 
 // hs_bucket_join_cmp's, hs_bucket_join_exists's and hs_bucket_join_outer's checks that need no data, then the join of the
 // sides' filters
@@ -1717,6 +1781,9 @@ static int bucket_join_checked(hs_ctx* ctx, const hs_join_spec* spec, int join_t
   if (join_type == kBadOuterJoin)
     return refuse(HS_EINVAL, stats, err, errlen,
                   "bucket join: join_type must be HS_JOIN_LEFT_OUTER, HS_JOIN_RIGHT_OUTER or HS_JOIN_FULL_OUTER");
+  if (join_type == kBadJoin)
+    return refuse(HS_EINVAL, stats, err, errlen,
+                  "bucket join: join_type must be HS_JOIN_INNER, HS_JOIN_LEFT_SEMI, HS_JOIN_LEFT_ANTI or an HS_JOIN_*_OUTER");
   if ((join_type == HS_JOIN_LEFT_SEMI || join_type == HS_JOIN_LEFT_ANTI) && spec->n_right_columns != 0)
     return refuse(HS_EINVAL, stats, err, errlen, "bucket join: a semi or anti join outputs left columns only (n_right_columns must be 0)");
   if (n_keys < 1) return refuse(HS_EINVAL, stats, err, errlen, "bucket join: at least one key column per side");
@@ -1764,6 +1831,20 @@ int hs_bucket_join_outer(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_typ
                              {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps}};
   return bucket_join_checked(ctx, spec, is_outer_join(join_type) ? join_type : kBadOuterJoin, left_keys, right_keys, n_keys, filters,
                              out, stats, err, errlen);
+}
+
+int hs_bucket_join_expr(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                        const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                        const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                        int32_t n_left_cmps, const hs_expr_compare* left_exprs, int32_t n_left_exprs,
+                        const hs_predicate* right_preds, int32_t n_right_preds, const hs_predicate_any* right_anys,
+                        int32_t n_right_anys, const hs_column_compare* right_cmps, int32_t n_right_cmps,
+                        const hs_expr_compare* right_exprs, int32_t n_right_exprs, hs_batch** out, hs_stats* stats, char* err,
+                        size_t errlen) {
+  const Filter filters[2] = {{left_preds, n_left_preds, left_anys, n_left_anys, left_cmps, n_left_cmps, left_exprs, n_left_exprs},
+                             {right_preds, n_right_preds, right_anys, n_right_anys, right_cmps, n_right_cmps, right_exprs, n_right_exprs}};
+  const bool ok = join_type == HS_JOIN_INNER || join_type == HS_JOIN_LEFT_SEMI || join_type == HS_JOIN_LEFT_ANTI || is_outer_join(join_type);
+  return bucket_join_checked(ctx, spec, ok ? join_type : kBadJoin, left_keys, right_keys, n_keys, filters, out, stats, err, errlen);
 }
 
 int64_t hs_batch_num_rows(const hs_batch* b) { return b ? b->nrows : 0; }

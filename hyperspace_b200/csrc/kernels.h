@@ -448,12 +448,26 @@ struct CompareSet {
   CompareDesc p[kMaxPredicates];
   int n = 0;
 };
-// The row filter of a scan or join side: a row is kept when every predicate, pattern and comparison holds
+struct ExprDesc;  // column_expr.h
+struct ExprInst;
+struct ExprColumn;
+// The expression comparisons of a scan or join side (predicates.h: resolve_expr), evaluated by expr_holds
+// (column_expr.h).  Device arrays, uploaded once per call: descs[n], the instructions they index and the columns those
+// read.  Pointers and a count only, so that the kernel's parameter block stays small whatever the programs' length.
+struct ExprSet {
+  const ExprDesc* descs = nullptr;
+  const ExprInst* insts = nullptr;
+  const ExprColumn* cols = nullptr;
+  int n = 0;
+};
+// The row filter of a scan or join side: a row is kept when every predicate, pattern, comparison and expression
+// comparison holds
 struct RowFilter {
   PredSet preds;
   PatternSet pats;
   CompareSet cmps;
-  bool empty() const { return preds.n == 0 && pats.n == 0 && cmps.n == 0; }
+  ExprSet exprs;
+  bool empty() const { return preds.n == 0 && pats.n == 0 && cmps.n == 0 && exprs.n == 0; }
 };
 // The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
 // work[w] = {s, r} with r indexing `ranges` (device); bounds[2w] = first row of s inside ranges[r], bounds[2w+1] = first
@@ -472,6 +486,9 @@ void launch_pattern_mask(hs_ctx* ctx, const PatternSet& pats, const uint32_t* ca
 // mask[i] = 0 where a comparison of `cmps` does not hold for row cand[i] (row i when cand is nullptr); launches nothing when
 // cmps is empty
 void launch_compare_mask(hs_ctx* ctx, const CompareSet& cmps, const uint32_t* cand, int64_t n, uint32_t* mask);
+// mask[i] = 0 where an expression comparison of `exprs` does not hold for row cand[i] (row i when cand is nullptr);
+// launches nothing when exprs is empty
+void launch_expr_mask(hs_ctx* ctx, const ExprSet& exprs, const uint32_t* cand, int64_t n, uint32_t* mask);
 // The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its
 // type's width (type[k]: HS_TYPE_INT32 / HS_TYPE_INT64, or HS_TYPE_STRING for string references).  The tuples compare
 // column by column, integers as signed values, strings in byte order.

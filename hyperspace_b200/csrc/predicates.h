@@ -10,7 +10,8 @@
 // A term's flags (HS_TERM_*) add NOT -- the complement of the set over the column's domain --, a null outcome, and string
 // patterns: a prefix is one range; other patterns are compiled for the matcher of string_match.h, their literal prefix
 // bounding the values they can match.  A comparison between two columns (hs_column_compare) resolves to the one domain both
-// sides are compared in (resolve_compare); column_compare.h evaluates it.
+// sides are compared in (resolve_compare); column_compare.h evaluates it.  An expression comparison (hs_expr_compare)
+// resolves to a typed postfix program with every implicit cast explicit (resolve_expr); column_expr.h evaluates it.
 #pragma once
 #include <algorithm>
 #include <cstdarg>
@@ -23,6 +24,7 @@
 
 #include "device_utils.cuh"
 #include "column_compare.h"
+#include "column_expr.h"
 #include "spark_types.h"
 #include "string_match.h"
 
@@ -643,8 +645,270 @@ inline int check_compares(const hs_column_compare* cmps, int n_cmps, int n_other
   return HS_OK;
 }
 
-// The filter of a filter scan or of one join side, as its entry point was given it: predicates, disjunction terms and
-// comparisons between two columns, all AND-ed.
+// ---- arithmetic expressions compared (hs_expr_compare) ------------------------------------------------------------------
+
+// The refusals of one side's postfix program that need no data: HS_OK or the code (message in err, stats zeroed)
+inline int check_expr_side(const hs_expr_node* nodes, int n, int i, const char* side, hs_stats* stats, char* err, size_t errlen) {
+  if (n < 1 || !nodes) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has an empty %s side", i, side);
+  if (n > kMaxExprNodes)
+    return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: the %s side of expression comparison %d has more than %d nodes", side,
+                  i, kMaxExprNodes);
+  int depth = 0;
+  for (int k = 0; k < n; k++) {
+    const hs_expr_node& x = nodes[k];
+    switch (x.kind) {
+      case HS_EXPR_COLUMN:
+        if (!x.column) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a column node without a name", i);
+        depth++;
+        break;
+      case HS_EXPR_LITERAL:
+        if (x.literal_type != HS_TYPE_INT32 && x.literal_type != HS_TYPE_INT64 && x.literal_type != HS_TYPE_DOUBLE &&
+            x.literal_type != HS_TYPE_DECIMAL)
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a literal of unknown type %d", i,
+                        x.literal_type);
+        if (x.literal_type == HS_TYPE_INT32 && x.value_i != (int32_t)x.value_i)
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has an int literal outside int32", i);
+        if (x.literal_type == HS_TYPE_DECIMAL && (x.scale < 0 || x.scale > 38))
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a decimal literal of scale %d", i, x.scale);
+        depth++;
+        break;
+      case HS_EXPR_NEG:
+        if (depth < 1) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d underflows its stack", side, i);
+        break;
+      case HS_EXPR_ADD:
+      case HS_EXPR_SUB:
+      case HS_EXPR_MUL:
+      case HS_EXPR_DIV:
+      case HS_EXPR_REM:
+        if (depth < 2) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d underflows its stack", side, i);
+        depth--;
+        break;
+      default: return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a node of unknown kind %d", i, x.kind);
+    }
+    if (depth > kMaxExprDepth)
+      return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: the %s side of expression comparison %d is deeper than %d values", side,
+                    i, kMaxExprDepth);
+  }
+  if (depth != 1)
+    return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d leaves %d values", side, i, depth);
+  return HS_OK;
+}
+
+// The refusals of an expression comparison list that need no data, beside n_others predicates, terms and comparisons: as
+// check_compares, then each side's postfix shape, kinds, literals and names
+inline int check_exprs(const hs_expr_compare* exprs, int n_exprs, int n_others, hs_stats* stats, char* err, size_t errlen) {
+  if (n_exprs < 0 || (n_exprs > 0 && !exprs)) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: bad expression array");
+  if (n_others + n_exprs > kMaxPredicates)
+    return refuse(HS_EUNSUPPORTED, stats, err, errlen, "filter scan: more than 16 predicates and terms");
+  for (int i = 0; i < n_exprs; i++) {
+    const hs_expr_compare& e = exprs[i];
+    if (e.op < HS_CMP_LT || e.op > HS_CMP_EQ_NULL_SAFE)
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has an unknown operator %d", i, e.op);
+    if (e.flags & ~HS_TERM_NOT)
+      return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has unknown flags 0x%x", i, e.flags);
+    int rc = check_expr_side(e.left, e.n_left, i, "left", stats, err, errlen);
+    if (rc == HS_OK) rc = check_expr_side(e.right, e.n_right, i, "right", stats, err, errlen);
+    if (rc != HS_OK) return rc;
+  }
+  return HS_OK;
+}
+
+// An operand's Spark type as the arithmetic coercion sees it: kind (kKindInt / Long / Float / Double / Decimal), a
+// decimal's precision and scale, and, for an integer literal, its digits (DecimalType.fromLiteral)
+struct ExprType {
+  int kind;
+  int p = 0, s = 0;
+  int lit_digits = 0;  // > 0: an integer literal
+  bool narrow = false;  // a byte or short column: Spark's arithmetic between two of them wraps at their width
+};
+
+inline int decimal_digits(uint64_t v) {
+  int d = 1;
+  while (v >= 10) v /= 10, d++;
+  return d;
+}
+
+inline __int128 pow10_i128(int k) {
+  __int128 p = 1;
+  while (k-- > 0) p *= 10;
+  return p;
+}
+
+// the decimal type an integral or decimal operand takes beside a decimal: int column decimal(10,0), long column
+// decimal(20,0), integer literal decimal(its digits, 0)
+inline void as_decimal(const ExprType& t, int* p, int* s) {
+  if (t.kind == kKindDecimal) *p = t.p, *s = t.s;
+  else *p = t.lit_digits ? t.lit_digits : (t.kind == kKindInt ? 10 : 20), *s = 0;
+}
+
+// A resolved expression comparison: the program of column_expr.h (kXLoad's arg: the ordinal of the COLUMN node, left side
+// first), the comparison's domain, op and NOT
+struct ExprProgram {
+  std::vector<ExprInst> insts;
+  int32_t domain = kCmpInt, op = 0, negate = 0;
+};
+
+// The expression comparison e (check_exprs has checked it) typed and lowered to column_expr.h's instructions, every
+// implicit cast explicit.  cols: one column per COLUMN node, the left side's first.  Spark 3.1's coercion, as
+// include/hs_gpu.h states it; what it cannot evaluate exactly as Spark would is HS_EUNSUPPORTED.
+inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<PredColumn>& cols) {
+  ExprProgram pg;
+  pg.op = e.op;
+  pg.negate = (e.flags & HS_TERM_NOT) != 0;
+  std::vector<ExprType> ts;    // the type stack
+  std::vector<std::string> txt;  // the nodes' SQL text, for messages
+  auto emit = [&](int op, int arg, __int128 v = 0) {
+    ExprInst in{};
+    in.op = op, in.arg = arg, in.v.i = v;
+    pg.insts.push_back(in);
+  };
+  auto to_double = [&](int at, ExprType& t, const std::string& what) {
+    switch (t.kind) {
+      case kKindInt:
+      case kKindLong: emit(kXIntToDouble, at); break;
+      case kKindFloat: emit(kXFloatToDouble, at); break;
+      case kKindDecimal:
+        if (t.p > 18) fail(HS_EUNSUPPORTED, "filter scan: %s turns a decimal of more than 18 digits into a double", what.c_str());
+        emit(kXDecToDouble, at, pow10_i128(t.s));
+        break;
+      default: break;
+    }
+    t = ExprType{kKindDouble};
+  };
+  auto to_float = [&](int at, ExprType& t) {
+    if (t.kind == kKindInt || t.kind == kKindLong) emit(kXIntToFloat, at);
+    t = ExprType{kKindFloat};
+  };
+  // both operands (a at slot 1, b at slot 0) to one domain for `what`: kXInt / kXLong / kXDec / kXFloat / kXDouble.
+  // Decimals: to the scale `scale_to` when >= 0 (rescaling the smaller), returned in *p / *s as each side's decimal type.
+  auto is_dec = [](const ExprType& t) { return t.kind == kKindDecimal; };
+  auto is_fp = [](const ExprType& t) { return t.kind == kKindFloat || t.kind == kKindDouble; };
+  auto unify = [&](ExprType& a, ExprType& b, const std::string& what, bool rescale) {
+    if ((is_dec(a) || is_dec(b)) && !is_fp(a) && !is_fp(b)) {
+      int pa, sa, pb, sb;
+      as_decimal(a, &pa, &sa);
+      as_decimal(b, &pb, &sb);
+      const int s = std::max(sa, sb), wider = std::max(pa - sa, pb - sb) + s;
+      if (wider > 38) fail(HS_EUNSUPPORTED, "filter scan: %s needs a decimal of more than 38 digits", what.c_str());
+      if (rescale) {
+        if (sa < s) emit(kXRescale, 1, pow10_i128(s - sa));
+        if (sb < s) emit(kXRescale, 0, pow10_i128(s - sb));
+      }
+      a = ExprType{kKindDecimal, pa, sa}, b = ExprType{kKindDecimal, pb, sb};
+      return (int)kXDec;
+    }
+    if (a.kind == kKindDouble || b.kind == kKindDouble || is_dec(a) || is_dec(b)) {
+      to_double(1, a, what), to_double(0, b, what);
+      return (int)kXDouble;
+    }
+    if (a.kind == kKindFloat || b.kind == kKindFloat) {
+      to_float(1, a), to_float(0, b);
+      return (int)kXFloat;
+    }
+    return (a.kind == kKindLong || b.kind == kKindLong) ? (int)kXLong : (int)kXInt;
+  };
+  static const char* const kOpText[] = {"", "", "", "+", "-", "*", "/", "%"};
+  int col_ord = 0;
+  auto side = [&](const hs_expr_node* nodes, int n) {
+    for (int k = 0; k < n; k++) {
+      const hs_expr_node& x = nodes[k];
+      if (x.kind == HS_EXPR_COLUMN) {
+        const PredColumn& c = cols[col_ord];
+        const int kind = compare_kind(c);
+        if (kind != kKindInt && kind != kKindLong && kind != kKindFloat && kind != kKindDouble && kind != kKindDecimal)
+          fail(HS_EUNSUPPORTED, "filter scan: the column '%s' (%s) cannot be used in arithmetic", c.name.c_str(),
+               pq::spark_type_name(c.schema).c_str());
+        ExprType t{kind};
+        if (kind == kKindDecimal) t.p = c.schema.precision, t.s = c.schema.scale;
+        t.narrow = c.schema.converted_type == 15 || c.schema.converted_type == 16;  // INT_8, INT_16
+        emit(kXLoad, col_ord++);
+        ts.push_back(t);
+        txt.push_back(c.name);
+      } else if (x.kind == HS_EXPR_LITERAL) {
+        ExprType t{kKindInt};
+        char buf[64];
+        switch (x.literal_type) {
+          case HS_TYPE_INT32:
+          case HS_TYPE_INT64:
+            t.kind = x.literal_type == HS_TYPE_INT32 ? kKindInt : kKindLong;
+            t.lit_digits = decimal_digits(x.value_i < 0 ? 0ull - (uint64_t)x.value_i : (uint64_t)x.value_i);
+            emit(kXConst, 0, x.value_i);
+            snprintf(buf, sizeof buf, "%lld", (long long)x.value_i);
+            break;
+          case HS_TYPE_DOUBLE: {
+            t.kind = kKindDouble;
+            ExprInst in{};
+            in.op = kXConst, in.v.d = x.value_f;
+            pg.insts.push_back(in);
+            snprintf(buf, sizeof buf, "%.17g", x.value_f);
+            break;
+          }
+          default: {  // HS_TYPE_DECIMAL: DecimalType(max(digits, scale), scale)
+            t.kind = kKindDecimal, t.s = x.scale;
+            t.p = std::max(decimal_digits(x.value_i < 0 ? 0ull - (uint64_t)x.value_i : (uint64_t)x.value_i), x.scale);
+            emit(kXConst, 0, x.value_i);
+            snprintf(buf, sizeof buf, "%lldE-%d", (long long)x.value_i, x.scale);
+            break;
+          }
+        }
+        ts.push_back(t);
+        txt.push_back(buf);
+      } else if (x.kind == HS_EXPR_NEG) {
+        const ExprType& t = ts.back();
+        if (t.narrow) fail(HS_EUNSUPPORTED, "filter scan: (- %s) is byte or short arithmetic, which wraps at its width: not handled", txt.back().c_str());
+        const int dom = t.kind == kKindInt ? kXInt : t.kind == kKindLong ? kXLong : t.kind == kKindDecimal ? kXDec
+                        : t.kind == kKindFloat ? kXFloat : kXDouble;
+        emit(dom + kXNeg, 0);
+        ts.back().lit_digits = 0;
+        txt.back() = "(- " + txt.back() + ")";
+      } else {
+        ExprType b = ts.back();
+        ts.pop_back();
+        ExprType a = ts.back();
+        ts.pop_back();
+        const std::string what = "(" + txt[txt.size() - 2] + " " + kOpText[x.kind] + " " + txt.back() + ")";
+        txt.pop_back();
+        txt.back() = what;
+        if (a.narrow && b.narrow) fail(HS_EUNSUPPORTED, "filter scan: %s is byte or short arithmetic, which wraps at its width: not handled", what.c_str());
+        ExprType r;
+        int dom;
+        if (x.kind == HS_EXPR_DIV) {  // TypeCoercion.Division: double, unless DecimalPrecision made it a decimal division
+          if ((is_dec(a) || is_dec(b)) && !is_fp(a) && !is_fp(b))
+            fail(HS_EUNSUPPORTED, "filter scan: decimal division is not handled: %s", what.c_str());
+          to_double(1, a, what), to_double(0, b, what);
+          dom = kXDouble, r = ExprType{kKindDouble};
+        } else {
+          dom = unify(a, b, what, x.kind != HS_EXPR_MUL);
+          if (dom == kXDec) {  // DecimalPrecision's result types
+            const int s = std::max(a.s, b.s), range = std::max(a.p - a.s, b.p - b.s);
+            switch (x.kind) {
+              case HS_EXPR_ADD:
+              case HS_EXPR_SUB: r = ExprType{kKindDecimal, range + s + 1, s}; break;
+              case HS_EXPR_MUL: r = ExprType{kKindDecimal, a.p + b.p + 1, a.s + b.s}; break;
+              default: r = ExprType{kKindDecimal, std::min(a.p - a.s, b.p - b.s) + s, s}; break;  // HS_EXPR_REM
+            }
+            if (r.p > 38) fail(HS_EUNSUPPORTED, "filter scan: %s needs a decimal of more than 38 digits", what.c_str());
+          } else {
+            r = ExprType{dom == kXInt ? kKindInt : dom == kXLong ? kKindLong : dom == kXFloat ? kKindFloat : kKindDouble};
+          }
+        }
+        emit(dom + (x.kind - HS_EXPR_ADD), 0);
+        ts.push_back(r);
+      }
+    }
+  };
+  side(e.left, e.n_left);
+  side(e.right, e.n_right);
+  ExprType b = ts.back(), a = ts[0];
+  static const char* const kCmpText[] = {"", "<", "<=", ">", ">=", "=", "<=>"};
+  const std::string what = "(" + txt[0] + " " + kCmpText[e.op] + " " + txt[1] + ")";
+  const int dom = unify(a, b, what, true);  // resolve_compare's table, decimals widened to 38 digits
+  pg.domain = dom == kXFloat ? kCmpFloat : (dom == kXDouble ? kCmpDouble : kCmpInt);
+  return pg;
+}
+
+// The filter of a filter scan or of one join side, as its entry point was given it: predicates, disjunction terms,
+// comparisons between two columns and expression comparisons, all AND-ed.
 struct Filter {
   const hs_predicate* preds = nullptr;
   int n_preds = 0;
@@ -652,10 +916,13 @@ struct Filter {
   int n_anys = 0;
   const hs_column_compare* cmps = nullptr;
   int n_cmps = 0;
+  const hs_expr_compare* exprs = nullptr;
+  int n_exprs = 0;
 };
 
 // The refusals of the filters of a call's n_sides sides that need no data, in one order whatever side a fault is on:
-// every side's predicates, then every side's terms, then every side's comparisons.  bounds_in_spec: as check_predicates.
+// every side's predicates, then every side's terms, then every side's comparisons, then every side's expression
+// comparisons.  bounds_in_spec: as check_predicates.
 inline int check_filters(const Filter* sides, int n_sides, bool bounds_in_spec, hs_stats* stats, char* err, size_t errlen) {
   int rc = HS_OK;
   for (int s = 0; s < n_sides && rc == HS_OK; s++)
@@ -664,6 +931,8 @@ inline int check_filters(const Filter* sides, int n_sides, bool bounds_in_spec, 
     rc = check_anys(sides[s].anys, sides[s].n_anys, sides[s].n_preds, stats, err, errlen);
   for (int s = 0; s < n_sides && rc == HS_OK; s++)
     rc = check_compares(sides[s].cmps, sides[s].n_cmps, sides[s].n_preds + sides[s].n_anys, stats, err, errlen);
+  for (int s = 0; s < n_sides && rc == HS_OK; s++)
+    rc = check_exprs(sides[s].exprs, sides[s].n_exprs, sides[s].n_preds + sides[s].n_anys + sides[s].n_cmps, stats, err, errlen);
   return rc;
 }
 

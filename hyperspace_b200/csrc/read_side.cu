@@ -8,6 +8,7 @@
 // the right index; every left row binary-searches its match range in the right bucket, a scan turns match counts into
 // output offsets, and a second kernel emits the (left row, right row) pairs in (left, right) order.  The key tuples of
 // 1-8 columns are compared column by column (k_join_count).
+#include "column_expr.h"
 #include "device_utils.cuh"
 #include "kernels.h"
 
@@ -160,6 +161,22 @@ __global__ void __launch_bounds__(256, 8) k_compare_mask(const __grid_constant__
     const int64_t row = cand ? (int64_t)cand[i] : i;
     bool ok = true;
     for (int p = 0; p < cs.n && ok; p++) ok = compare_holds(cs.p[p], row);
+    if (!ok) mask[i] = 0;
+  }
+}
+
+// The expression comparisons, one thread per candidate row: clears mask[i] where one of them does not hold for row
+// cand[i] (row i without a candidate list); rows already dropped by the earlier masks are skipped.  The evaluator's value
+// stack is indexed at run time, so it lives in local memory (DESIGN.md section 6 gives ptxas' frame); the programs and
+// their columns are read through the set's device arrays, the same addresses in every thread.
+__global__ void __launch_bounds__(256, 8) k_expr_mask(const __grid_constant__ ExprSet es, const uint32_t* __restrict__ cand, int64_t n,
+                                                      uint32_t* __restrict__ mask) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (!mask[i]) continue;
+    const int64_t row = cand ? (int64_t)cand[i] : i;
+    bool ok = true;
+    for (int p = 0; p < es.n && ok; p++) ok = expr_holds(es.descs[p], es.insts, es.cols, row);
     if (!ok) mask[i] = 0;
   }
 }
@@ -621,6 +638,14 @@ void launch_compare_mask(hs_ctx* ctx, const CompareSet& cmps, const uint32_t* ca
   HS_LAUNCH_CHECK(ctx);
 }
 
+void launch_expr_mask(hs_ctx* ctx, const ExprSet& exprs, const uint32_t* cand, int64_t n, uint32_t* mask) {
+  if (exprs.n == 0) return;
+  KernelScope _ks(ctx, "k_expr_mask");
+  if (n == 0) return;
+  k_expr_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(exprs, cand, n, mask);
+  HS_LAUNCH_CHECK(ctx);
+}
+
 void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
                        const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
   KernelScope _ks(ctx, "k_join_count");
@@ -740,6 +765,7 @@ int64_t select_rows(hs_ctx* ctx, const RowFilter& filter, const uint32_t* cand, 
   launch_predicate_mask(ctx, filter.preds, cand, n, mask.get());
   launch_pattern_mask(ctx, filter.pats, cand, n, mask.get());
   launch_compare_mask(ctx, filter.cmps, cand, n, mask.get());
+  launch_expr_mask(ctx, filter.exprs, cand, n, mask.get());
   Buf<int64_t> d_deleted;
   if (n > 0 && ndeleted > 0) {
     d_deleted.alloc(ctx, ndeleted);

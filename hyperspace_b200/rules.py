@@ -7,8 +7,8 @@ are the linear ``Project?(Filter?(Relation))`` and ``Join(linear, linear)`` the 
   * FilterIndexRule / FilterIndexRanker             -- index/covering/FilterIndexRule.scala:33-174, FilterIndexRanker.scala:28-65
   * JoinIndexRule / JoinIndexRanker                 -- index/covering/JoinIndexRule.scala:47-720, JoinIndexRanker.scala:28-95
   * transformPlanToUseIndex / Hybrid Scan           -- index/covering/CoveringIndexRuleUtils.scala:55-288
-Physical execution is the C ABI: hs_filter_scan_cmp (K1 + K7), hs_bucket_join_cmp (K1 + K8) and, for left semi / left anti
-joins, hs_bucket_join_exists.
+Physical execution is the C ABI: hs_filter_scan_expr (K1 + K7) and hs_bucket_join_expr (K1 + K8), which takes the join
+type (inner, left semi / left anti, left / right / full outer).
 """
 from __future__ import annotations
 
@@ -186,17 +186,18 @@ def _host_column(d: np.ndarray) -> np.ndarray:
 
 
 def _terms_text(pred) -> str:
-    """The disjunction terms and column comparisons of a filter for explain(), long lists cut short: `k IN (1, 2, 3, ... 997
-    more)`, `(a < b)`."""
+    """The disjunction terms, column comparisons and expression comparisons of a filter for explain(), long lists cut
+    short: `k IN (1, 2, 3, ... 997 more)`, `(a < b)`, `((a + b) < c)`."""
     anys = pred.disjunctions() if pred else []
     cmps = pred.comparisons() if pred else []
-    return "".join(f", where=({a})" for a in anys) + "".join(f", where=({c})" for c in cmps)
+    exprs = pred.expressions() if pred else []
+    return "".join(f", where=({a})" for a in anys + cmps + exprs)
 
 
 class ScanExec:
-    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_cmp with
-    the filter's comparisons with literals as its predicates, its disjunctions (isin, |) as its terms and its comparisons
-    between two columns as its compares."""
+    """Filter / projection over a relation: index-only scan, Hybrid Scan, or plain source scan -- hs_filter_scan_expr with
+    the filter's comparisons with literals as its predicates, its disjunctions (isin, |) as its terms, its comparisons
+    between two columns as its compares and its comparisons of arithmetic expressions as its exprs."""
 
     def __init__(self, session, lin: Linear, cand: Optional[Candidate]):
         self.session, self.lin, self.cand = session, lin, cand
@@ -215,9 +216,10 @@ class ScanExec:
         preds = self.lin.predicate.conjuncts() if self.lin.predicate else []
         terms = [a.as_native() for a in self.lin.predicate.disjunctions()] if self.lin.predicate else []
         cmps = [c.as_native() for c in self.lin.predicate.comparisons()] if self.lin.predicate else []
+        exprs = [e.as_native() for e in self.lin.predicate.expressions()] if self.lin.predicate else []
         # file_buckets only where the files are bucketed on the key alone
-        batch, _ = self.session.gpu.filter_scan_cmp(files, key, out_cols, preds, terms, cmps, sorted_on_key=sorted_on_key,
-                                                    deleted_file_ids=list(deleted_ids), file_buckets=buckets, num_buckets=num_buckets)
+        batch, _ = self.session.gpu.filter_scan_expr(files, key, out_cols, preds, terms, cmps, exprs, sorted_on_key=sorted_on_key,
+                                                     deleted_file_ids=list(deleted_ids), file_buckets=buckets, num_buckets=num_buckets)
         types = dict(self.lin.relation.schema)
         out = {n: spark_values(_host_column(d), types.get(n)) for n, d, _ in batch.columns}
         batch.free()
@@ -245,8 +247,9 @@ class ScanExec:
         return _concat(parts, out_cols)
 
 
-# JoinNode.how of the outer joins -> join_type of Context.bucket_join_outer
+# JoinNode.how of the outer joins -> join_type of Context.bucket_join_expr
 _OUTER = {"leftouter": "left", "rightouter": "right", "fullouter": "full"}
+_JOIN_TYPE = {"inner": "inner", "leftsemi": "semi", "leftanti": "anti", **_OUTER}
 
 
 class BucketJoinExec:
@@ -254,8 +257,8 @@ class BucketJoinExec:
     ``keys`` are the (left, right) key pairs in the order both sides are bucketed and sorted on: the left index's indexed
     columns when the indexes serve, the condition's order otherwise; None when the condition is not a one-to-one equi-join
     between the two sides, which the GPU join cannot run.  A filter below a side becomes that side's predicates.  ``how``
-    is "inner", "leftsemi" / "leftanti" (hs_bucket_join_exists: left rows only, each at most once), or "leftouter" /
-    "rightouter" / "fullouter" (hs_bucket_join_outer: rows padded with nulls where the other side has no match)."""
+    is "inner", "leftsemi" / "leftanti" (left rows only, each at most once), or "leftouter" / "rightouter" / "fullouter"
+    (rows padded with nulls where the other side has no match); hs_bucket_join_expr runs them all."""
 
     def __init__(self, session, left: Linear, right: Linear, keys: Optional[List[Tuple[str, str]]], lcand: Optional[Candidate],
                  rcand: Optional[Candidate], condition: Optional[List[Tuple[str, str]]] = None, how: str = "inner"):
@@ -313,16 +316,10 @@ class BucketJoinExec:
             rp = self.right.predicate.conjuncts() if self.right.predicate else []
             lt_, rt_ = ([a.as_native() for a in lin.predicate.disjunctions()] if lin.predicate else [] for lin in (self.left, self.right))
             lc_, rc_ = ([c.as_native() for c in lin.predicate.comparisons()] if lin.predicate else [] for lin in (self.left, self.right))
-            if self.how == "inner":
-                batch, _ = self.session.gpu.bucket_join_cmp(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                            lp, rp, lt_, rt_, lc_, rc_)
-            elif self.how in _OUTER:
-                batch, _ = self.session.gpu.bucket_join_outer(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, self.right.output,
-                                                              _OUTER[self.how], lp, rp, lt_, rt_, lc_, rc_)
-            else:
-                batch, _ = self.session.gpu.bucket_join_exists(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output,
-                                                               "semi" if self.how == "leftsemi" else "anti", lp, rp, lt_, rt_,
-                                                               lc_, rc_)
+            lx_, rx_ = ([e.as_native() for e in lin.predicate.expressions()] if lin.predicate else [] for lin in (self.left, self.right))
+            right_out = [] if self.how in ("leftsemi", "leftanti") else self.right.output
+            batch, _ = self.session.gpu.bucket_join_expr(li, lb, ri, rb, nb, lkeys, rkeys, self.left.output, right_out,
+                                                         _JOIN_TYPE[self.how], lp, rp, lt_, rt_, lc_, rc_, lx_, rx_)
         finally:
             for t in lt + rt:
                 t.free()

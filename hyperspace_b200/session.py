@@ -192,6 +192,122 @@ class ColumnCompare:
         return self.left, self.op, self.right, _TERM_NOT if self.negated else 0
 
 
+class Expr:
+    """Arithmetic over columns and literals (Spark's Add, Subtract, Multiply, Divide, Remainder and UnaryMinus over
+    attributes and literals): a column (``op`` "column", ``value`` its name), a literal (``op`` "literal"), a unary minus
+    (``op`` "neg", one argument) or a binary operation (``op`` one of + - * / %, two arguments).  Its comparison
+    operators, ``eqNullSafe`` and ``between`` give a Predicate holding an ExprCompare; the engine types the arithmetic as
+    Spark 3.1 does (include/hs_gpu.h)."""
+    __hash__ = None  # == builds a comparison
+
+    def __init__(self, op: str, args: Tuple["Expr", ...] = (), value=None):
+        self.op, self.args, self.value = op, tuple(args), value
+
+    @staticmethod
+    def of(v) -> "Expr":
+        """A Column, an Expr or a literal as an Expr; a literal must be an int, a float or a Decimal."""
+        if isinstance(v, Expr):
+            return v
+        if isinstance(v, Column):
+            return Expr("column", value=v.name)
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, decimal.Decimal, np.integer, np.floating)):
+            raise LE.HyperspaceException(f"the literal {v!r} cannot be used in arithmetic on the GPU path")
+        return Expr("literal", value=v)
+
+    def __str__(self) -> str:
+        if self.op == "column":
+            return self.value
+        if self.op == "literal":
+            return str(self.value)
+        if self.op == "neg":
+            return f"(- {self.args[0]})"
+        return f"({self.args[0]} {self.op} {self.args[1]})"
+
+    def postfix(self) -> List[tuple]:
+        """The nodes in postfix order, as Context.filter_scan_expr takes them."""
+        if self.op in ("column", "literal"):
+            return [(self.op, self.value)]
+        return [n for a in self.args for n in a.postfix()] + [(self.op,)]
+
+    @property
+    def columns(self) -> List[str]:
+        if self.op == "column":
+            return [self.value]
+        out = []
+        for a in self.args:
+            out += [c for c in a.columns if c not in out]
+        return out
+
+    def renamed(self, fn) -> "Expr":
+        """The expression with every column name passed through fn."""
+        if self.op == "column":
+            return Expr("column", value=fn(self.value))
+        if self.op == "literal":
+            return self
+        return Expr(self.op, tuple(a.renamed(fn) for a in self.args))
+
+    def _bin(self, op, other, reflected=False) -> "Expr":
+        other = Expr.of(other)
+        return Expr(op, (other, self) if reflected else (self, other))
+
+    def __add__(self, o): return self._bin("+", o)
+    def __radd__(self, o): return self._bin("+", o, True)
+    def __sub__(self, o): return self._bin("-", o)
+    def __rsub__(self, o): return self._bin("-", o, True)
+    def __mul__(self, o): return self._bin("*", o)
+    def __rmul__(self, o): return self._bin("*", o, True)
+    def __truediv__(self, o): return self._bin("/", o)
+    def __rtruediv__(self, o): return self._bin("/", o, True)
+    def __mod__(self, o): return self._bin("%", o)
+    def __rmod__(self, o): return self._bin("%", o, True)
+    def __neg__(self): return Expr("neg", (self,))
+
+    def _compare(self, op: str, other, negated: bool = False) -> "Predicate":
+        return Predicate({}, [], [], [], [ExprCompare(self, op, Expr.of(other), negated)])
+
+    def __lt__(self, o): return self._compare("<", o)
+    def __le__(self, o): return self._compare("<=", o)
+    def __gt__(self, o): return self._compare(">", o)
+    def __ge__(self, o): return self._compare(">=", o)
+    def __eq__(self, o): return self._compare("=", o)  # noqa: A003
+    def __ne__(self, o): return self._compare("=", o, negated=True)  # noqa: A003
+
+    def eqNullSafe(self, o) -> "Predicate":
+        return self._compare("<=>", o)
+
+    def between(self, lo, hi) -> "Predicate":
+        return (self >= lo) & (self <= hi)
+
+    def isin(self, *values):
+        raise LE.HyperspaceException(f"isin on the expression {self} is an OR across columns, which is not handled by the GPU path")
+
+    def __bool__(self):
+        raise LE.HyperspaceException(f"the expression {self} is not a filter: compare it")
+
+
+@dataclass
+class ExprCompare:
+    """A comparison of two arithmetic expressions of the same row (Spark's BinaryComparison over Add, Subtract, Multiply,
+    Divide, Remainder, UnaryMinus, attributes and literals): ``left op right``, op as in ColumnCompare, under Not when
+    ``negated``.  A null side makes it unknown, except for <=>."""
+    left: Expr
+    op: str
+    right: Expr
+    negated: bool = False
+
+    def __str__(self) -> str:
+        inner = f"({self.left} {self.op} {self.right})"
+        return f"NOT {inner}" if self.negated else inner
+
+    @property
+    def columns(self) -> List[str]:
+        return self.left.columns + [c for c in self.right.columns if c not in self.left.columns]
+
+    def as_native(self) -> tuple:
+        """(left nodes, op, right nodes, HS_TERM_* flags) for Context.filter_scan_expr / bucket_join_expr."""
+        return self.left.postfix(), self.op, self.right.postfix(), _TERM_NOT if self.negated else 0
+
+
 def _prefix_range(p) -> Tuple[object, bool, object, bool]:
     """The values that start with p, as a range: [p, succ(p)), succ(p) being p without its trailing 0xff bytes and its
     last byte incremented; open above when nothing is left."""
@@ -210,11 +326,13 @@ class Predicate:
     """Conjunction of comparisons with literals.  ``bounds`` is the inclusive integer (or byte-string) range per column, which
     the plan layer uses to pick an index; ``terms`` are the comparisons as written -- (column, operator, literal) with the
     operator one of >=, >, <=, <, == -- which the engine evaluates with Spark's type coercion.  ``anys`` are AND-ed
-    disjunctions on one column each (``isin`` and ``|``); ``compares`` are AND-ed comparisons between two columns."""
+    disjunctions on one column each (``isin`` and ``|``); ``compares`` are AND-ed comparisons between two columns;
+    ``exprs`` are AND-ed comparisons of arithmetic expressions."""
     bounds: Dict[str, Tuple[Optional[int], Optional[int]]]
     terms: List[Tuple[str, str, object]] = field(default_factory=list)
     anys: List[AnyTerm] = field(default_factory=list, repr=False)  # explain() shows them by their SQL form
     compares: List[ColumnCompare] = field(default_factory=list, repr=False)
+    exprs: List[ExprCompare] = field(default_factory=list, repr=False)
 
     def __and__(self, other: "Predicate") -> "Predicate":
         out = dict(self.bounds)
@@ -224,7 +342,8 @@ class Predicate:
                 lo = l0 if lo is None else (lo if l0 is None else max(lo, l0))
                 hi = h0 if hi is None else (hi if h0 is None else min(hi, h0))
             out[c] = (lo, hi)
-        return Predicate(out, self._as_terms() + other._as_terms(), self.anys + other.anys, self.compares + other.compares)
+        return Predicate(out, self._as_terms() + other._as_terms(), self.anys + other.anys, self.compares + other.compares,
+                         self.exprs + other.exprs)
 
     def __or__(self, other: "Predicate") -> "Predicate":
         """An Or of branches on one and the same column, each a comparison, a conjunction of comparisons that is one range
@@ -232,6 +351,8 @@ class Predicate:
         for branch in (self, other):
             if branch.compares:
                 raise LE.HyperspaceException(f"an OR across columns ({branch.compares[0]}) is not handled by the GPU path")
+            if branch.exprs:
+                raise LE.HyperspaceException(f"an OR across columns ({branch.exprs[0]}) is not handled by the GPU path")
         c = self._single_column()
         if other._single_column().lower() != c.lower():
             raise LE.HyperspaceException(f"an OR across columns ({c}, {other._single_column()}) is not handled by the GPU path")
@@ -258,9 +379,11 @@ class Predicate:
         """Not of a filter on one column: of one comparison or range, or of one isin, OR, null test or pattern; or of one
         comparison between two columns."""
         cols = {c.lower(): c for c in self.columns}
-        if self.compares and len(self.compares) == 1 and not self.anys and not self._as_terms():
+        if self.compares and len(self.compares) == 1 and not self.anys and not self._as_terms() and not self.exprs:
             return Predicate({}, [], [], [dataclasses.replace(self.compares[0], negated=not self.compares[0].negated)])
-        if len(cols) != 1 or self.compares:
+        if self.exprs and len(self.exprs) == 1 and not self.anys and not self._as_terms() and not self.compares:
+            return Predicate({}, [], [], [], [dataclasses.replace(self.exprs[0], negated=not self.exprs[0].negated)])
+        if len(cols) != 1 or self.compares or self.exprs:
             raise LE.HyperspaceException(f"a NOT over several columns ({', '.join(cols.values())}) is not handled by the GPU "
                                          "path: it would be an OR across columns")
         if self.anys:
@@ -312,10 +435,15 @@ class Predicate:
         """The AND-ed comparisons between two columns, which conjuncts() and disjunctions() do not list."""
         return list(self.compares)
 
+    def expressions(self) -> List[ExprCompare]:
+        """The AND-ed comparisons of arithmetic expressions, which the other accessors do not list."""
+        return list(self.exprs)
+
     @property
     def columns(self) -> List[str]:
         out = list(self.bounds)
-        for c in [a.column for a in self.anys] + [n for cc in self.compares for n in (cc.left, cc.right)]:
+        for c in ([a.column for a in self.anys] + [n for cc in self.compares for n in (cc.left, cc.right)] +
+                  [n for e in self.exprs for n in e.columns]):
             if c not in out:
                 out.append(c)
         return out
@@ -364,7 +492,22 @@ class Column:
     def _compare(self, op: str, other: "Column", negated: bool = False) -> Predicate:
         return Predicate({}, [], [], [ColumnCompare(self.name, op, other.name, negated)])
 
+    # arithmetic: an Expr, which compares into an expression comparison
+    def __add__(self, o): return Expr.of(self) + o
+    def __radd__(self, o): return Expr.of(o) + Expr.of(self)
+    def __sub__(self, o): return Expr.of(self) - o
+    def __rsub__(self, o): return Expr.of(o) - Expr.of(self)
+    def __mul__(self, o): return Expr.of(self) * o
+    def __rmul__(self, o): return Expr.of(o) * Expr.of(self)
+    def __truediv__(self, o): return Expr.of(self) / o
+    def __rtruediv__(self, o): return Expr.of(o) / Expr.of(self)
+    def __mod__(self, o): return Expr.of(self) % o
+    def __rmod__(self, o): return Expr.of(o) % Expr.of(self)
+    def __neg__(self): return -Expr.of(self)
+
     def __ge__(self, v):
+        if isinstance(v, Expr):
+            return Expr.of(self) >= v
         if isinstance(v, Column):
             return self._compare(">=", v)
         if isinstance(v, (str, bytes)):
@@ -372,6 +515,8 @@ class Column:
         return Predicate({self.name: (_ceil(v), None)}, [(self.name, ">=", v)])
 
     def __gt__(self, v):
+        if isinstance(v, Expr):
+            return Expr.of(self) > v
         if isinstance(v, Column):
             return self._compare(">", v)
         if isinstance(v, (str, bytes)):
@@ -379,6 +524,8 @@ class Column:
         return Predicate({self.name: (_floor(v) + 1, None)}, [(self.name, ">", v)])
 
     def __le__(self, v):
+        if isinstance(v, Expr):
+            return Expr.of(self) <= v
         if isinstance(v, Column):
             return self._compare("<=", v)
         if isinstance(v, (str, bytes)):
@@ -386,6 +533,8 @@ class Column:
         return Predicate({self.name: (None, _floor(v))}, [(self.name, "<=", v)])
 
     def __lt__(self, v):
+        if isinstance(v, Expr):
+            return Expr.of(self) < v
         if isinstance(v, Column):
             return self._compare("<", v)
         if isinstance(v, (str, bytes)):
@@ -393,6 +542,8 @@ class Column:
         return Predicate({self.name: (None, _ceil(v) - 1)}, [(self.name, "<", v)])
 
     def __eq__(self, v):  # noqa: A003
+        if isinstance(v, Expr):
+            return Expr.of(self) == v
         if isinstance(v, Column):
             return self._compare("=", v)
         if isinstance(v, (str, bytes)):
@@ -404,6 +555,8 @@ class Column:
 
     def __ne__(self, v):  # noqa: A003
         """Not(EqualTo): a null row, or a None literal, gives unknown."""
+        if isinstance(v, Expr):
+            return Expr.of(self) != v
         if isinstance(v, Column):
             return self._compare("=", v, negated=True)
         return ~self.isin([v])
@@ -414,7 +567,7 @@ class Column:
         list is cast as Spark casts it (a float makes every value a double, Decimals share one scale).  Strings mixed with
         numbers raise."""
         vals = values[0] if len(values) == 1 and isinstance(values[0], (list, tuple, set, frozenset, np.ndarray)) else values
-        if not isinstance(vals, np.ndarray) and any(isinstance(v, Column) for v in vals):
+        if not isinstance(vals, np.ndarray) and any(isinstance(v, (Column, Expr)) for v in vals):
             raise LE.HyperspaceException(f"isin on '{self.name}' with a column value is an OR across columns, which is not "
                                          "handled by the GPU path")
         had_none = not isinstance(vals, np.ndarray) and any(v is None for v in vals)
@@ -440,6 +593,8 @@ class Column:
         """EqualNullSafe (`<=>`): a null row gives false, and `eqNullSafe(None)` is isNull()."""
         if v is None:
             return self.isNull()
+        if isinstance(v, Expr):
+            return Expr.of(self).eqNullSafe(v)
         if isinstance(v, Column):
             return self._compare("<=>", v)
         return Predicate({}, [], [AnyTerm(self.name, self._checked([v], "eqNullSafe"), null=False)])
@@ -465,7 +620,7 @@ class Column:
         return self._pattern("like", pattern)
 
     def between(self, lo, hi):
-        if isinstance(lo, Column) or isinstance(hi, Column):  # two conjuncts: lo <= self AND self <= hi
+        if isinstance(lo, (Column, Expr)) or isinstance(hi, (Column, Expr)):  # two conjuncts: lo <= self AND self <= hi
             return (self >= lo) & (self <= hi)
         terms = [(self.name, ">=", lo), (self.name, "<=", hi)]
         if isinstance(lo, (str, bytes)) or isinstance(hi, (str, bytes)):
@@ -626,11 +781,16 @@ class DataFrame:
         return name if name in hits else hits[0]
 
     def filter(self, predicate: Predicate) -> "DataFrame":
+        if isinstance(predicate, Expr):
+            raise LE.HyperspaceException(f"the expression {predicate} is not a filter: compare it (a boolean column is not "
+                                         "handled by the GPU path)")
         self._refuse_join_compares(predicate)
         resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
                              [(self._resolve(c), op, v) for c, op, v in predicate.terms],
                              [dataclasses.replace(a, column=self._resolve(a.column), ranges=list(a.ranges)) for a in predicate.anys],
-                             [dataclasses.replace(c, left=self._resolve(c.left), right=self._resolve(c.right)) for c in predicate.compares])
+                             [dataclasses.replace(c, left=self._resolve(c.left), right=self._resolve(c.right)) for c in predicate.compares],
+                             [dataclasses.replace(e, left=e.left.renamed(self._resolve), right=e.right.renamed(self._resolve))
+                              for e in predicate.exprs])
         return DataFrame(self.session, FilterNode(self.plan, resolved))
 
     def _refuse_join_compares(self, predicate: Predicate) -> None:
@@ -644,6 +804,11 @@ class DataFrame:
             if in_sides[0] and in_sides[1] and not (in_sides[0] & in_sides[1]):
                 raise LE.HyperspaceException(f"{c} compares columns of the two sides of a join: a non-equi join condition, "
                                              "which the GPU path does not handle")
+        for e in predicate.exprs:  # an expression over columns of both sides is a join condition too
+            in_sides = [x for x in ({i for i, side in enumerate(sides) if n.lower() in side} for n in e.columns) if x]
+            if in_sides and not set.intersection(*in_sides):
+                raise LE.HyperspaceException(f"{e} compares columns of the two sides of a join: a non-equi join condition, "
+                                             "which the GPU path does not handle")
 
     where = filter
 
@@ -654,7 +819,7 @@ class DataFrame:
     def join(self, other: "DataFrame", on, how: str = "inner") -> "DataFrame":
         how = normalise_join_type(how)
         if isinstance(on, Predicate):
-            shown = ", ".join(str(c) for c in on.compares) or "a filter"
+            shown = ", ".join([str(c) for c in on.compares] + [str(e) for e in on.exprs]) or "a filter"
             raise LE.HyperspaceException(f"join `on` {shown}: a non-equi join condition, which the GPU path does not handle; "
                                          "join on column names")
         if isinstance(on, str):

@@ -514,6 +514,85 @@ int hs_bucket_join_outer(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_typ
                          const hs_predicate_any* right_anys, int32_t n_right_anys, const hs_column_compare* right_cmps,
                          int32_t n_right_cmps, hs_batch** out, hs_stats* stats, char* err, size_t errlen);
 
+/* Arithmetic over the columns of a row, compared: `a + b < c`, `price * (1 - discount) > 100`, `k % 7 = 0`.  One side of
+ * an hs_expr_compare is an array of hs_expr_node in postfix order (`a + b` is COLUMN a, COLUMN b, ADD); a side of one
+ * COLUMN or LITERAL node is a bare column or literal.  Spark 3.1 semantics with spark.sql.ansi.enabled=false:
+ *   Operands: int (byte and short count as int), long, float, double and decimal(p <= 18) columns, and literals.  An
+ *     operation between two byte or short columns, and NEG of one, is HS_EUNSUPPORTED: Spark wraps it at 8 or 16 bits.  A
+ *     HS_TYPE_INT32 literal is an int, HS_TYPE_INT64 a long, HS_TYPE_DOUBLE a double, and HS_TYPE_DECIMAL (unscaled
+ *     value_i, `scale`) is decimal(max(digits, scale), scale).  String, binary, boolean, date and timestamp columns are
+ *     HS_EUNSUPPORTED naming the column and its Spark type.
+ *   Operand types (TypeCoercion.ImplicitTypeCasts, DecimalPrecision): int with long is long; int or long with float is
+ *     float (the integer rounded to nearest); anything with double is double; decimal with int or long is decimal, an
+ *     int column counting as decimal(10,0), a long column as decimal(20,0) and an integer literal as decimal(its digits,
+ *     0); decimal with float or double is double.  DIV casts every operand to double (TypeCoercion.Division), so int / int
+ *     is double.
+ *   Nulls: a null operand makes the node null; so does a zero divisor of DIV and REM (0, 0.0 and -0.0 alike).
+ *   Integers: ADD, SUB, MUL and NEG wrap in two's complement at the operand width (int arithmetic at 2^31); REM is Java's
+ *     truncated remainder, the sign of the dividend, and MIN % -1 is 0.
+ *   Float and double: every operation rounds to nearest on its own, never fused; REM is fmod.
+ *   Decimals: exact.  ADD / SUB give scale max(s1,s2) and precision max(p1-s1, p2-s2) + scale + 1; MUL (p1+p2+1, s1+s2);
+ *     REM (min(p1-s1, p2-s2) + max(s1,s2), max(s1,s2)).  A node whose result, or whose operands' wider type (max(p1-s1,
+ *     p2-s2) + max(s1,s2)), would exceed 38 digits is HS_EUNSUPPORTED: Spark would bound or adjust it.  Decimal DIV is
+ *     HS_EUNSUPPORTED, and so is a decimal of more than 18 digits that would have to become a double.
+ *   The comparison: HS_CMP_* with HS_TERM_NOT, after hs_column_compare's coercion of the two sides' types (decimals up to
+ *     38 digits compare exactly, the side of the smaller scale rescaled; a common decimal type above 38 digits is
+ *     HS_EUNSUPPORTED).  NaN equals NaN and is above +inf; -0.0 equals 0.0.  A null side makes LT, LE, GT, GE and EQ
+ *     unknown, under NOT too; EQ_NULL_SAFE is true on two null sides and false on one.
+ *   Limits: at most 32 nodes per side (HS_EUNSUPPORTED) and a stack depth of 8 per side (HS_EUNSUPPORTED).  Stack underflow,
+ *   values left over, an unknown kind, op or flag, a NULL column name, a HS_TYPE_INT32 literal outside int32 or a decimal
+ *   scale outside 0..38 is HS_EINVAL. */
+#define HS_EXPR_COLUMN 1
+#define HS_EXPR_LITERAL 2
+#define HS_EXPR_ADD 3
+#define HS_EXPR_SUB 4
+#define HS_EXPR_MUL 5
+#define HS_EXPR_DIV 6
+#define HS_EXPR_REM 7
+#define HS_EXPR_NEG 8
+
+typedef struct {
+  int32_t kind;          /* HS_EXPR_* */
+  const char* column;    /* HS_EXPR_COLUMN */
+  int32_t literal_type;  /* HS_EXPR_LITERAL: HS_TYPE_INT32 / HS_TYPE_INT64 / HS_TYPE_DOUBLE / HS_TYPE_DECIMAL */
+  int32_t scale;         /* HS_TYPE_DECIMAL literal */
+  int64_t value_i;       /* INT32, INT64, DECIMAL (unscaled) */
+  double value_f;        /* DOUBLE */
+} hs_expr_node;
+
+typedef struct {
+  const hs_expr_node* left;
+  int32_t n_left;
+  const hs_expr_node* right;
+  int32_t n_right;
+  int32_t op;     /* HS_CMP_* */
+  int32_t flags;  /* 0 or HS_TERM_NOT */
+} hs_expr_compare;
+
+/* hs_filter_scan_cmp with expression comparisons AND-ed to the filter (n_preds + n_anys + n_cmps + n_exprs <= 16).  Their
+ * columns are decoded like other predicate columns (on sorted files, only inside the key's windows) and they run per row.
+ * An expression makes no key window and prunes no bucket.  With n_exprs = 0 this is hs_filter_scan_cmp. */
+int hs_filter_scan_expr(hs_ctx* ctx, const hs_scan_spec* spec, const hs_predicate* preds, int32_t n_preds,
+                        const hs_predicate_any* anys, int32_t n_anys, const hs_column_compare* cmps, int32_t n_cmps,
+                        const hs_expr_compare* exprs, int32_t n_exprs, const int32_t* file_buckets, int32_t num_buckets,
+                        hs_batch** out, hs_stats* stats, char* err, size_t errlen);
+
+/* join_type of hs_bucket_join_expr besides HS_JOIN_LEFT_SEMI .. HS_JOIN_FULL_OUTER: the inner join */
+#define HS_JOIN_INNER 0
+
+/* One bucket join of any type, with expression comparisons AND-ed to each side's filter (their columns belong to that
+ * side; they run per row in the side selection).  join_type HS_JOIN_INNER is hs_bucket_join_cmp, HS_JOIN_LEFT_SEMI /
+ * HS_JOIN_LEFT_ANTI hs_bucket_join_exists, HS_JOIN_*_OUTER hs_bucket_join_outer, with their rules and refusals; any other
+ * join_type is HS_EINVAL.  With no expressions each is exactly that call. */
+int hs_bucket_join_expr(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_type, const char* const* left_keys,
+                        const char* const* right_keys, int32_t n_keys, const hs_predicate* left_preds, int32_t n_left_preds,
+                        const hs_predicate_any* left_anys, int32_t n_left_anys, const hs_column_compare* left_cmps,
+                        int32_t n_left_cmps, const hs_expr_compare* left_exprs, int32_t n_left_exprs,
+                        const hs_predicate* right_preds, int32_t n_right_preds, const hs_predicate_any* right_anys,
+                        int32_t n_right_anys, const hs_column_compare* right_cmps, int32_t n_right_cmps,
+                        const hs_expr_compare* right_exprs, int32_t n_right_exprs, hs_batch** out, hs_stats* stats, char* err,
+                        size_t errlen);
+
 int64_t hs_batch_num_rows(const hs_batch* b);
 int32_t hs_batch_on_device(const hs_batch* b); /* != 0: the column pointers are device pointers (output = HS_OUT_DEVICE) */
 int32_t hs_batch_num_columns(const hs_batch* b);
