@@ -620,6 +620,7 @@ int hs_create_index_async(hs_ctx* ctx, const hs_index_spec* spec, hs_pending** o
       }
       SourceSet src;
       open_sources(ctx, spec->files, spec->n_files, &src, &st);
+      refuse_boolean_keys(src, std::vector<std::string>(cols.begin(), cols.begin() + spec->n_indexed));
       decode_sources(ctx, src, cols, nullptr, &table, &st, &carry);
       const bool has_strings = table.has_strings;
       if (has_strings && ctx->world > 1)

@@ -52,7 +52,7 @@ int find_column(const pq::FileMeta& fm, const std::string& name) {
 const char* decode_error_text(uint32_t code) {
   switch (code) {
     case DERR_BAD_HEADER: return "malformed page header";
-    case DERR_UNSUPPORTED_ENCODING: return "unsupported page encoding (PLAIN and PLAIN_/RLE_DICTIONARY are handled)";
+    case DERR_UNSUPPORTED_ENCODING: return "unsupported page encoding (PLAIN, PLAIN_/RLE_DICTIONARY and RLE for BOOLEAN are handled)";
     case DERR_VALUE_COUNT: return "page value counts do not add up to the column chunk's num_values";
     case DERR_COMPRESSED: return "page sizes disagree in an UNCOMPRESSED chunk";
     case DERR_OVERRUN: return "page data shorter than its header claims";
@@ -1096,8 +1096,8 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
   L.t_plan.start();
   for (int c = 0; c < ncols; c++) {
     const DevColumn& dc = table.cols[c];
-    if (dc.width != 4 && dc.width != 8)
-      fail(HS_EUNSUPPORTED, "column '%s': %d-byte values cannot be written by the GPU encoder yet", dc.name.c_str(), dc.width);
+    if (dc.type == HS_TYPE_BOOL ? P > INT32_MAX : dc.width != 4 && dc.width != 8)  // (a boolean's schema type is the source's)
+      fail(HS_EUNSUPPORTED, dc.type == HS_TYPE_BOOL ? "column '%s': boolean pages hold at most 2^31 - 1 rows" : "column '%s': %d-byte values cannot be written by the GPU encoder yet", dc.name.c_str(), dc.width);
   }
   std::vector<pq::SchemaColumn>& schema = L.schema;
   schema.resize(ncols);
@@ -1193,7 +1193,7 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
     bool any_sampled = false;
     for (int c = 0; c < ncols; c++) {
       const DevColumn& dc = table.cols[c];
-      if (dc.has_nulls || dc.carried || dc.type == HS_TYPE_STRING) continue;
+      if (dc.has_nulls || dc.carried || dc.type == HS_TYPE_STRING || dc.width == 1) continue;  // booleans: PLAIN, as parquet-mr
       ColDict& cd = dicts[c];
       if (dc.dict_ready && dc.dict_keys) {
         cd.keys_ptr = dc.dict_keys.get();
@@ -1215,7 +1215,7 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
     if (any_sampled) sync_stream(ctx);
     for (int c = 0; c < ncols; c++) {
       const DevColumn& dc = table.cols[c];
-      if (dc.has_nulls || dc.carried || dc.type == HS_TYPE_STRING) continue;
+      if (dc.has_nulls || dc.carried || dc.type == HS_TYPE_STRING || dc.width == 1) continue;
       ColDict& cd = dicts[c];
       uint32_t* st = &h_states[4 * (size_t)c];
       const bool ready = dc.dict_ready && dc.dict_keys;
@@ -1373,17 +1373,17 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
             cursor += value_bytes;
             ch.null_count += np - non_null;
           } else if (!table.cols[c].has_nulls) {
-            pq::write_plain_page_prefix(skeleton, cursor, np, W);  // file images start 64-byte aligned in the arena
+            W == 1 ? pq::write_bool_page_prefix(skeleton, np) : pq::write_plain_page_prefix(skeleton, cursor, np, W);  // (arena: 64-byte aligned files)
             emit(cursor, b);
             cursor += skeleton.size() - b;
             page_value_offset[c][page_counter + (p0 / P)] = cursor;
-            cursor += (uint64_t)np * W;
+            cursor += W == 1 ? (uint64_t)(np + 7) / 8 : (uint64_t)np * W;  // booleans bit-packed
           } else {
             // tiles of this page: [t0, t1) in the segment's tile list
             const int64_t t0 = seg_tile_begin[s] + p0 / kSortTile, t1 = seg_tile_begin[s] + ceil_div(p0 + np, (int64_t)kSortTile);
             int64_t non_null = 0;
             for (int64_t t = t0; t < t1; t++) non_null += tile_valid[c][t];
-            pq::write_nullable_page_prefix(skeleton, np, non_null, W);
+            pq::write_nullable_page_prefix_bytes(skeleton, np, W == 1 ? (uint64_t)(non_null + 7) / 8 : (uint64_t)non_null * W);
             emit(cursor, b);
             cursor += skeleton.size() - b;
             const uint64_t def_bits = cursor;
@@ -1395,7 +1395,7 @@ void layout_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout* lay, E
               tile_val_off[c][t] = voff;
               voff += (uint64_t)tile_valid[c][t] * W;
             }
-            cursor += (uint64_t)non_null * W;
+            cursor += W == 1 ? (uint64_t)(non_null + 7) / 8 : (uint64_t)non_null * W;  // (booleans: one CTA per page, see k_gather_encode_bool_nullable)
             ch.null_count += np - non_null;
           }
           if (compress) {
@@ -1667,6 +1667,15 @@ void write_segments(hs_ctx* ctx, const EncodeRequest& req, EncodeLayout& lay, bo
   stats->bytes_out += (int64_t)cursor;
   stats->files_out += (int32_t)out->files.size();
   lay.impl.reset();
+}
+
+void refuse_boolean_keys(const SourceSet& set, const std::vector<std::string>& keys) {
+  for (const FileImage& img : set.impl->imgs)
+    for (const std::string& k : keys) {
+      const int idx = find_column(img.meta, k);
+      if (idx >= 0 && img.meta.columns[idx].type == pq::BOOLEAN)
+        fail(HS_EUNSUPPORTED, "column '%s' is boolean: boolean columns can be included in an index but not indexed", k.c_str());
+    }
 }
 
 }  // namespace hs

@@ -145,6 +145,9 @@ struct FileWindows {
 // file_windows (optional): only the pages that intersect one of their file's windows are decoded
 void decode_sources(hs_ctx* ctx, SourceSet& set, const std::vector<std::string>& columns, const FileWindows* file_windows,
                     Table* out, hs_stats* stats, const CarryOptions* carry = nullptr);
+// HS_EUNSUPPORTED when one of `keys` is a BOOLEAN column of any opened file: a boolean indexed column could never be read
+// back (filters and join keys on booleans are refused), so an index build refuses it before it decodes anything
+void refuse_boolean_keys(const SourceSet& set, const std::vector<std::string>& keys);
 // type, width and schema of column `name` as decode_sources would decode it, read from the footer of `file` alone
 DevColumn source_column_type(hs_ctx* ctx, const hs_source_file& file, const std::string& name);
 

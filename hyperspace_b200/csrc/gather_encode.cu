@@ -147,6 +147,122 @@ __global__ void __launch_bounds__(kThreads) k_gather_encode_nullable(const SortT
   }
 }
 
+// ---- boolean columns ----------------------------------------------------------------------------------------------
+// PLAIN BOOLEAN is bit-packed, LSB first.  A page starts on a multiple of kSortTile rows, so a tile of a null-free page
+// starts on a byte of the page body ((lr0 mod P) / 8) and ends on one unless it is its bucket's last: no two tiles share
+// a byte.  Each warp ballot packs 32 rows into one word of shared memory; the tile's bytes leave as unaligned words, the
+// ragged tail as single bytes (the byte after a page body belongs to the next page header).
+static_assert(kSortTile % 32 == 0, "a tile packs into whole words and starts on a byte boundary");
+__global__ void __launch_bounds__(kThreads) k_gather_encode_bool(const SortTile* __restrict__ tiles,
+                                                                  const uint64_t* __restrict__ seg_start,
+                                                                  const uint32_t* __restrict__ perm,
+                                                                  const uint8_t* __restrict__ src,
+                                                                  const uint64_t* __restrict__ page_value_offset,
+                                                                  const uint32_t* __restrict__ bucket_page_begin,
+                                                                  int64_t rows_per_page, uint8_t* __restrict__ arena) {
+  constexpr int kPer = kSortTile / kThreads;
+  __shared__ uint32_t s_words[kSortTile / 32];
+  const SortTile t = tiles[blockIdx.x];
+  const uint64_t lr0 = t.start - seg_start[t.seg];
+  const uint64_t page = lr0 / (uint64_t)rows_per_page;
+  uint8_t* const base = arena + page_value_offset[bucket_page_begin[t.seg] + page] + (lr0 - page * (uint64_t)rows_per_page) / 8;
+  // all of a thread's row indices first, then all its value loads in flight together (as k_gather_encode does)
+  uint32_t r[kPer];
+#pragma unroll
+  for (int it = 0; it < kPer; it++) {
+    const uint32_t i = it * kThreads + threadIdx.x;
+    r[it] = i < t.count ? perm[t.start + i] : 0u;
+  }
+  uint8_t v[kPer];
+#pragma unroll
+  for (int it = 0; it < kPer; it++) v[it] = it * kThreads + threadIdx.x < t.count ? src[r[it]] : (uint8_t)0;
+#pragma unroll
+  for (int it = 0; it < kPer; it++) {
+    const unsigned bits = __ballot_sync(0xffffffffu, v[it] != 0);
+    if ((threadIdx.x & 31) == 0) s_words[(it * kThreads + threadIdx.x) / 32] = bits;
+  }
+  __syncthreads();
+  const uint32_t nbytes = (t.count + 7) / 8, nwords = nbytes / 4;
+  for (uint32_t w0 = 0; w0 < kSortTile / 32; w0 += kThreads) {
+    const uint32_t w = w0 + threadIdx.x;
+    warp_store_unaligned<4>(base + 4 * (size_t)w, w < nwords ? s_words[w] : 0u, w < nwords);
+  }
+  if (threadIdx.x < nbytes - 4 * nwords) base[4 * nwords + threadIdx.x] = (uint8_t)(s_words[nwords] >> (8 * threadIdx.x));
+}
+
+// Nullable boolean columns, one CTA per page.  The non-null values of a page are one bit stream that crosses its tiles at
+// any bit, and the page's definition bits end in the middle of a word: a CTA that owns the whole page writes every byte of
+// it, so no two CTAs touch the same byte.  The grid is the tile list; the CTA of a page's first tile walks the page's
+// tiles (those of its segment whose definition bits follow on, kSortTile / 8 bytes apart), the others return at once.  Per
+// step of kBoolStep rows: definition bits by warp ballot (as k_gather_encode_nullable writes them), positions of the
+// non-null rows by block scan, their value bits OR-ed into a shared bit buffer that carries its partial last word from one
+// step to the next; whole words are stored as they fill.  The value bits follow the definition bits of the page.
+constexpr int kBoolStep = 1024;  // rows per step: four gathers in flight per thread
+__global__ void __launch_bounds__(kThreads) k_gather_encode_bool_nullable(const SortTile* __restrict__ tiles, int64_t ntiles,
+                                                                           const uint32_t* __restrict__ perm,
+                                                                           const uint8_t* __restrict__ src,
+                                                                           const uint8_t* __restrict__ valid,
+                                                                           const uint64_t* __restrict__ tile_def_offset,
+                                                                           uint8_t* __restrict__ arena) {
+  constexpr int kPer = kBoolStep / kThreads;
+  constexpr uint32_t kWords = kBoolStep / 32 + 2;
+  __shared__ uint32_t s_bits[kWords];
+  __shared__ uint32_t warp_sums[40];
+  const int64_t t0 = blockIdx.x;
+  const uint32_t seg = tiles[t0].seg;
+  auto follows = [&](int64_t t) {  // tile t continues the page of tile t - 1
+    return tiles[t].seg == seg && tile_def_offset[t] == tile_def_offset[t - 1] + kSortTile / 8;
+  };
+  if (t0 > 0 && follows(t0)) return;
+  int64_t t1 = t0 + 1;
+  uint32_t count = tiles[t0].count;
+  while (t1 < ntiles && follows(t1)) count += tiles[t1++].count;
+  const uint64_t start = tiles[t0].start;
+  uint8_t* const def_out = arena + tile_def_offset[t0];
+  uint8_t* const val_out = def_out + (count + 7) / 8;
+  for (uint32_t j = threadIdx.x; j < kWords; j += kThreads) s_bits[j] = 0;
+  uint32_t carry_bits = 0;  // value bits in s_bits[0] not yet stored
+  uint64_t stored_words = 0;
+  for (uint32_t step = 0; step < count; step += kBoolStep) {
+    uint32_t flag[kPer];
+    uint8_t v[kPer];
+#pragma unroll
+    for (int k = 0; k < kPer; k++) {
+      const uint32_t i = step + k * kThreads + threadIdx.x;
+      const uint32_t row = i < count ? perm[start + i] : 0u;
+      flag[k] = i < count && valid[row] ? 1u : 0u;
+      v[k] = flag[k] ? src[row] : (uint8_t)0;
+    }
+#pragma unroll
+    for (int k = 0; k < kPer; k++) {
+      const uint32_t first = step + k * kThreads + (threadIdx.x & ~31u);
+      const unsigned bits = __ballot_sync(0xffffffffu, flag[k] != 0);
+      if ((threadIdx.x & 31) == 0 && first < count) {  // 32 levels = 4 bytes, LSB first
+        const uint32_t nb = min(4u, (count - first + 7) / 8);
+        for (uint32_t b = 0; b < nb; b++) def_out[first / 8 + b] = (uint8_t)(bits >> (8 * b));
+      }
+      uint32_t total = 0;
+      const uint32_t pos = carry_bits + block_exclusive_scan(flag[k], warp_sums, &total);
+      if (flag[k] && v[k]) atomicOr(&s_bits[pos / 32], 1u << (pos % 32));
+      carry_bits += total;
+    }
+    __syncthreads();
+    const uint32_t full = carry_bits / 32;
+    for (uint32_t w0 = 0; w0 < kWords; w0 += kThreads) {
+      const uint32_t w = w0 + threadIdx.x;
+      warp_store_unaligned<4>(val_out + 4 * (stored_words + w), w < full ? s_bits[w] : 0u, w < full);
+    }
+    __syncthreads();
+    const uint32_t tail = s_bits[full];
+    __syncthreads();
+    for (uint32_t j = threadIdx.x; j < kWords; j += kThreads) s_bits[j] = j == 0 ? tail : 0u;
+    __syncthreads();
+    stored_words += full;
+    carry_bits %= 32;
+  }
+  if (threadIdx.x < (carry_bits + 7) / 8) val_out[4 * stored_words + threadIdx.x] = (uint8_t)(s_bits[0] >> (8 * threadIdx.x));
+}
+
 // ---- string columns -----------------------------------------------------------------------------------------------
 // PLAIN BYTE_ARRAY: every non-null value is [u32 length][bytes].  First the tiles are measured (the host needs every
 // page's byte size to lay the files out), then each tile writes its definition bits and its values: a block scan of the
@@ -229,7 +345,7 @@ __global__ void __launch_bounds__(kThreads) k_gather_encode_strings(const SortTi
   }
 }
 
-// width-1 columns (BOOLEAN is bit-packed in PLAIN; handled by a byte-per-row staging column + k_pack_bits)
+// fixed-width values through a permutation (width 1: the read side's boolean columns, one byte per row)
 template <typename T>
 __global__ void k_gather_plain(const T* __restrict__ src, const uint32_t* __restrict__ perm, int64_t n,
                                T* __restrict__ out) {
@@ -314,9 +430,12 @@ inline int grid_for(hs_ctx* ctx, int64_t n, int threads, int per_sm) {
 void launch_gather_encode(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles, const uint64_t* seg_start,
                           const uint32_t* perm, const GatherColumn& col, const uint32_t* bucket_page_begin,
                           int64_t rows_per_page, uint8_t* arena) {
-  KernelScope _ks(ctx, "k_gather_encode");
+  KernelScope _ks(ctx, col.width == 1 ? "k_gather_encode_bool" : "k_gather_encode");
   if (ntiles == 0) return;
-  if (col.width == 8)
+  if (col.width == 1)
+    k_gather_encode_bool<<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(tiles, seg_start, perm, (const uint8_t*)col.src,
+                                                                         col.page_value_offset, bucket_page_begin, rows_per_page, arena);
+  else if (col.width == 8)
     k_gather_encode<8><<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(tiles, seg_start, perm, col, bucket_page_begin,
                                                                         rows_per_page, arena);
   else if (col.width == 4)
@@ -338,9 +457,12 @@ void launch_tile_valid_counts(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles
 void launch_gather_encode_nullable(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles, const uint32_t* perm,
                                    const void* src, const uint8_t* valid, int width, const uint64_t* tile_value_offset,
                                    const uint64_t* tile_def_offset, uint8_t* arena) {
-  KernelScope _ks(ctx, "k_gather_encode_nullable");
+  KernelScope _ks(ctx, width == 1 ? "k_gather_encode_bool_nullable" : "k_gather_encode_nullable");
   if (ntiles == 0) return;
-  if (width == 8)
+  if (width == 1)
+    k_gather_encode_bool_nullable<<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(tiles, ntiles, perm, (const uint8_t*)src, valid,
+                                                                                   tile_def_offset, arena);
+  else if (width == 8)
     k_gather_encode_nullable<8><<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(tiles, perm, src, valid, tile_value_offset,
                                                                                  tile_def_offset, arena);
   else if (width == 4)

@@ -301,12 +301,12 @@ struct GatherColumn {
   int32_t width;
   const uint64_t* page_value_offset;  // device: arena offset of the first value byte of each (bucket, page)
 };
-// For every sorted position p (tile by tile): value = src[perm[p]] written PLAIN into its page body in the arena.
+// For every sorted position p (tile by tile): value = src[perm[p]] written PLAIN into its page body (width 1: bit-packed).
 // page index of local row lr in bucket b = bucket_page_begin[b] + lr / rows_per_page.
 void launch_gather_encode(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles, const uint64_t* seg_start,
                           const uint32_t* perm, const GatherColumn& col, const uint32_t* bucket_page_begin,
                           int64_t rows_per_page, uint8_t* arena);
-// nullable columns: per-tile non-null counts, then bit-packed definition levels + dense values per tile
+// nullable columns: per-tile non-null counts, then bit-packed definition levels + dense values per tile (width 1: per page)
 void launch_tile_valid_counts(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles, const uint32_t* perm,
                               const uint8_t* valid, uint32_t* counts);
 void launch_gather_encode_nullable(hs_ctx* ctx, const SortTile* tiles, int64_t ntiles, const uint32_t* perm,

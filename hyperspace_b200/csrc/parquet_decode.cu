@@ -11,6 +11,7 @@
 //   definition levels (optional) same hybrid decoder at bit width 1, block scan -> dense value positions
 //   converted values (ValueConv) INT96 / MILLIS timestamps -> int64 micros, FIXED_LEN_BYTE_ARRAY / INT64 decimals -> their
 //                                unscaled int32 / int64, value by value (dictionary entries once, into the smem cache)
+//   RLE BOOLEAN                  [4-byte length] + hybrid stream at bit width 1, through the dictionary-index reader
 // Supported: data page v1 and v2, UNCOMPRESSED codec, BOOLEAN/INT32/INT64/FLOAT/DOUBLE, flat schemas.
 #include "device_utils.cuh"
 #include "kernels.h"
@@ -319,6 +320,29 @@ __device__ bool def_levels_all_valid(const uint8_t* def_p, const uint8_t* def_en
   return all_ones && covered >= n;
 }
 
+// An RLE BOOLEAN stream [q, end) whose runs, up to the first that reaches value n, all lie inside it: every run header,
+// every RLE run's value byte and every bit-packed run's bytes (the hybrid reader would decode a run cut short by the end
+// of the stream as far as it goes; a stream that holds too few values is caught while decoding)
+__device__ bool rle_bool_stream_ok(const uint8_t* q, const uint8_t* end, uint32_t n) {
+  uint64_t covered = 0;
+  while (covered < n && q < end) {
+    uint32_t h = 0;
+    int shift = 0;
+    uint8_t b;
+    do {
+      if (q >= end || shift > 28) return false;
+      b = *q++;
+      h |= (uint32_t)(b & 0x7f) << shift;
+      shift += 7;
+    } while (b & 0x80);
+    const uint64_t len = h & 1 ? (uint64_t)(h >> 1) : 1;  // bytes behind the header: groups of 8 bits, or the value
+    if (len > (uint64_t)(end - q)) return false;
+    q += len;
+    covered += h & 1 ? 8ull * (h >> 1) : (uint64_t)(h >> 1);
+  }
+  return true;
+}
+
 // where the definition levels of a page sit; returns false when the page is malformed
 __device__ __forceinline__ bool locate_def_levels(const PageDesc& pg, const uint8_t*& p, const uint8_t*& def_p,
                                                   const uint8_t*& def_end) {
@@ -513,9 +537,12 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
   };
   const int n = pg.num_values;
   const uint8_t* p = pg.data;
-  const uint8_t* pend = pg.data + pg.size;
+  const uint8_t* pend = pg.data + pg.size;  // from the values on: the end of their bytes
   const bool is_dict = pg.encoding == pq::ENC_PLAIN_DICTIONARY || pg.encoding == pq::ENC_RLE_DICTIONARY;
-  if (!is_dict && pg.encoding != pq::ENC_PLAIN) {
+  // RLE BOOLEAN: the values are a hybrid stream of bit width 1, read like dictionary indices that are their own values
+  const bool rle_bool = W == 1 && pg.encoding == pq::ENC_RLE;
+  const bool hybrid_values = is_dict || rle_bool;
+  if (!hybrid_values && pg.encoding != pq::ENC_PLAIN) {
     if (threadIdx.x == 0) set_error(d_error, DERR_UNSUPPORTED_ENCODING, (uint32_t)pg.encoding);
     return;
   }
@@ -573,11 +600,29 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
     }
     if (threadIdx.x == 0) hybrid_init(sm.idx.st, p, pend, idx_bw);
   }
+  if (rle_bool) {  // [4-byte length][stream], in v1 and v2 pages alike
+    const uint32_t len = pend - p >= 4 ? load_le32_unaligned(p) : 0xffffffffu;
+    if ((int64_t)len > (int64_t)(pend - p) - 4) {
+      if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
+      return;
+    }
+    p += 4;
+    pend = p + len;
+    if (threadIdx.x == 0) sm.flag = rle_bool_stream_ok(p, pend, (uint32_t)n) ? 1u : 0u;
+    __syncthreads();
+    if (!sm.flag) {
+      if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
+      return;
+    }
+    idx_bw = 1;
+    if (threadIdx.x == 0) hybrid_init(sm.idx.st, p, pend, 1);
+  }
   if (has_def && threadIdx.x == 0) hybrid_init(sm.def.st, def_p, def_end, 1);
   __syncthreads();
   const int64_t row0 = pg.first_row;
   const uint32_t dict_count = (uint32_t)pg.dict_count;
   auto dict_lookup = [&](uint32_t ix) -> uint64_t {
+    if (rle_bool) return ix & 1u;
     if (ix >= dict_count) {
       set_error(d_error, DERR_DICT_INDEX, ix);
       return 0;
@@ -598,7 +643,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
 
   // ---- fast paths: no nulls in this page -----------------------------------------------------------------------
   if (!has_def) {
-    if (!is_dict) {
+    if (!hybrid_values) {
       if (W == 1) {
         if ((int64_t)(pend - p) < ((int64_t)n + 7) / 8) {
           if (threadIdx.x == 0) set_error(d_error, DERR_OVERRUN, (uint32_t)pg.col);
@@ -760,7 +805,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
       }
     }
     __syncthreads();
-    if (is_dict) {
+    if (hybrid_values) {
       ok = hybrid_decode_next(sm.idx, total, [&](uint32_t j, uint32_t v) { sm.tile_idx[j] = v; });
       __syncthreads();
       if (!ok) {
@@ -779,7 +824,7 @@ __device__ void decode_page(const PageDesc& pg, const ColumnOut& co, uint32_t* c
       uint64_t v = 0;
       if (valid) {
         const uint32_t pos = sm.tile_pos[i];
-        if (is_dict) v = dict_lookup(sm.tile_idx[pos]);
+        if (hybrid_values) v = dict_lookup(sm.tile_idx[pos]);
         else if (W == 1) {
           const int64_t bit = val_cursor + pos;
           v = (p[bit >> 3] >> (bit & 7)) & 1;

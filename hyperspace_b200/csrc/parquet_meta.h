@@ -387,6 +387,15 @@ inline void write_plain_page_prefix(std::vector<uint8_t>& out, uint64_t page_off
   out.insert(out.end(), bt->second.begin(), bt->second.end());
 }
 
+// [page header][definition levels] for a PLAIN v1 BOOLEAN data page of `n` non-null values, as parquet-mr writes it: one
+// RLE run of ones, then ceil(n / 8) bytes of values bit-packed LSB first (written by the GPU)
+inline void write_bool_page_prefix(std::vector<uint8_t>& out, int64_t n) {
+  std::vector<uint8_t> defs;
+  write_all_valid_def_levels(defs, n);
+  write_data_page_header(out, (int32_t)(defs.size() + (size_t)(n + 7) / 8), (int32_t)n, ENC_PLAIN);
+  out.insert(out.end(), defs.begin(), defs.end());
+}
+
 // [page header][4-byte length][bit-packed run header] for a v1 data page of `n` rows whose definition levels are written as
 // ONE bit-packed run of ceil(n/8) groups (the bits themselves are written by the GPU right after this prefix) followed by
 // `non_null` dense PLAIN values.

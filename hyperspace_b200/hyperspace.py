@@ -144,6 +144,11 @@ class CreateAction(_DataAction):
         if missing:  # same first sentence as CreateAction.scala:63-65; the rest tells which columns
             raise HyperspaceException(f"Index config is not applicable to dataframe schema. Columns '{','.join(missing)}' could "
                                       f"not be resolved from available source columns '{','.join(self.df.plan.column_names)}'")
+        type_of = {n.lower(): t for n, t in self.df.plan.schema}
+        for c in self.config.indexedColumns:
+            if type_of.get(c.lower()) == "boolean":  # filters and join keys on booleans are not handled: never readable
+                raise HyperspaceException(f"Index config is not applicable: column '{c}' is boolean; boolean columns can be "
+                                          "included in an index but not indexed")
         latest = self.log_manager.get_latest_log()
         if latest is not None and latest.state != States.DOESNOTEXIST:
             raise HyperspaceException(f"Another Index with name {self.config.indexName} already exists")

@@ -50,7 +50,9 @@ extern "C" {
 #define HS_TYPE_INT64 1  /* Spark long / timestamp(us)  */
 #define HS_TYPE_FLOAT 2
 #define HS_TYPE_DOUBLE 3
-#define HS_TYPE_BOOL 4
+#define HS_TYPE_BOOL 4   /* Spark boolean, one byte (0 / 1) per row: included columns of an index (written as PLAIN BOOLEAN
+                            pages, bit-packed), projected columns of scans and joins; sources PLAIN or RLE.  Never an
+                            indexed column (HS_EUNSUPPORTED before any source is decoded), a filter or a join key */
 #define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): indexed and included columns (one GPU), filter scan keys and
                             predicates, join keys (alone or with other key columns); compared in UTF8String byte order */
 #define HS_TYPE_DECIMAL 6 /* hs_predicate literal only: a decimal, unscaled value in lo_i / hi_i, scale in `scale` */
