@@ -39,6 +39,12 @@ ALL_JOIN_TYPES = {"inner": HS_JOIN_INNER, **JOIN_TYPES, **OUTER_JOIN_TYPES}
 # hs_expr_node.kind
 HS_EXPR_COLUMN, HS_EXPR_LITERAL, HS_EXPR_ADD, HS_EXPR_SUB, HS_EXPR_MUL, HS_EXPR_DIV, HS_EXPR_REM, HS_EXPR_NEG = range(1, 9)
 EXPR_OPS = {"+": HS_EXPR_ADD, "-": HS_EXPR_SUB, "*": HS_EXPR_MUL, "/": HS_EXPR_DIV, "%": HS_EXPR_REM, "neg": HS_EXPR_NEG}
+# the function kinds, HS_EXPR_YEAR (9) .. HS_EXPR_COALESCE (25), by their Spark names
+EXPR_FUNCS = {name: 9 + k for k, name in enumerate(
+    ("year", "quarter", "month", "dayofmonth", "dayofweek", "dayofyear", "weekofyear", "hour", "minute", "second", "date_add",
+     "date_sub", "datediff", "length", "substring", "abs", "coalesce"))}
+HS_EXPR_COALESCE = EXPR_FUNCS["coalesce"]
+HS_TYPE_DATE, HS_TYPE_TIMESTAMP = 7, 8  # expression literals only
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
@@ -531,9 +537,11 @@ def expr_literal(v) -> Tuple[int, int, int, float]:
 
 
 def _expr_nodes(nodes: Sequence[tuple]):
-    """One side of an expression comparison, postfix: ``("column", name)``, ``("literal", value)`` (typed by expr_literal)
-    or an operator ``(op,)`` with op one of EXPR_OPS's keys ("+", "-", "*", "/", "%", "neg") or an HS_EXPR_* code; a raw
-    ``(kind, column, literal_type, scale, value_i, value_f)`` tuple passes as it is.  Returns (array, count, keep)."""
+    """One side of an expression comparison, postfix: ``("column", name)``, ``("literal", value)`` (typed by expr_literal;
+    str and bytes are HS_TYPE_STRING literals, datetime.date HS_TYPE_DATE days and datetime.datetime HS_TYPE_TIMESTAMP
+    micros), an operator ``(op,)`` with op one of EXPR_OPS's keys ("+", "-", "*", "/", "%", "neg") or EXPR_FUNCS's
+    ("year" .. "abs"), ``("coalesce", n)``, or an HS_EXPR_* code; a raw ``(kind, column, literal_type, scale, value_i,
+    value_f)`` tuple passes as it is.  Returns (array, count, keep)."""
     keep = []
     arr = (ExprNodeSpec * max(1, len(nodes)))()
     for x, node in zip(arr, nodes):
@@ -542,9 +550,23 @@ def _expr_nodes(nodes: Sequence[tuple]):
             name = node[1].encode() if node[1] is not None else None
             keep.append(name)
             x.kind, x.column = HS_EXPR_COLUMN, name
+        elif tag == "literal" and isinstance(node[1], (str, bytes)):
+            b = node[1].encode("utf-8") if isinstance(node[1], str) else bytes(node[1])
+            buf = C.create_string_buffer(b, max(1, len(b)))
+            keep.append(buf)
+            x.kind, x.literal_type, x.value_i = HS_EXPR_LITERAL, HS_TYPE_STRING, len(b)
+            x.column = C.addressof(buf)
+        elif tag == "literal" and isinstance(node[1], datetime.datetime):
+            x.kind, x.literal_type, x.value_i = HS_EXPR_LITERAL, HS_TYPE_TIMESTAMP, timestamp_micros(node[1])
+        elif tag == "literal" and isinstance(node[1], datetime.date):
+            x.kind, x.literal_type, x.value_i = HS_EXPR_LITERAL, HS_TYPE_DATE, (node[1] - datetime.date(1970, 1, 1)).days
         elif tag == "literal":
             x.kind = HS_EXPR_LITERAL
             x.literal_type, x.scale, x.value_i, x.value_f = expr_literal(node[1])
+        elif tag == "coalesce":
+            x.kind, x.value_i = HS_EXPR_COALESCE, node[1]
+        elif tag in EXPR_FUNCS:
+            x.kind = EXPR_FUNCS[tag]
         elif len(node) == 6:
             name = node[1].encode() if node[1] is not None else None
             keep.append(name)

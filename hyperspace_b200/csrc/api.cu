@@ -1028,16 +1028,22 @@ static const T* upload_array(hs_ctx* ctx, const std::vector<T>& h, PredUploads* 
 }
 
 // The expression comparisons of filter b on the columns of t, resolved (predicates.h: resolve_expr) into one program per
-// comparison and uploaded in one set: the descriptors, every instruction and every column they read
-static ExprSet upload_exprs(hs_ctx* ctx, const Table& t, const BoundFilter& b, PredUploads* up) {
+// comparison and uploaded in one set: the descriptors, every instruction, every column they read and the bytes of their
+// string literals.  *funcs: some program uses a function or a string, date or timestamp value, so the set runs in
+// k_func_mask.
+static ExprSet upload_exprs(hs_ctx* ctx, const Table& t, const BoundFilter& b, PredUploads* up, bool* funcs) {
   std::vector<ExprDesc> descs;
   std::vector<ExprInst> insts;
   std::vector<ExprColumn> ecols;
+  std::vector<uint8_t> pool;
+  *funcs = false;
   for (size_t i = 0; i < b.expr_col.size(); i++) {
     std::vector<PredColumn> pcs;
     for (int c : b.expr_col[i]) pcs.push_back(pred_column(t.cols[c]));
     const ExprProgram pg = resolve_expr(b.f.exprs[i], pcs);
-    const int32_t base = (int32_t)ecols.size();
+    *funcs = *funcs || pg.funcs;
+    const int32_t base = (int32_t)ecols.size(), pool_base = (int32_t)pool.size();
+    pool.insert(pool.end(), pg.pool.begin(), pg.pool.end());
     for (int c : b.expr_col[i]) {
       const DevColumn& dc = t.cols[c];
       ecols.push_back(ExprColumn{dc.data.get(), dc.has_nulls ? dc.valid.get() : nullptr, dc.type});
@@ -1045,11 +1051,15 @@ static ExprSet upload_exprs(hs_ctx* ctx, const Table& t, const BoundFilter& b, P
     ExprDesc d{(int32_t)insts.size(), 0, pg.domain, pg.op, pg.negate};
     for (ExprInst in : pg.insts) {
       if (in.op == kXLoad) in.arg += base;
+      if (in.op == kXStringConst) in.arg += pool_base;
       insts.push_back(in);
     }
     d.end = (int32_t)insts.size();
     descs.push_back(d);
   }
+  // every kXStringConst becomes a kXConst, also when every string literal is empty: upload_array allocates at least
+  // 16 bytes, so the pool has an address
+  relocate_strings(&insts, upload_array(ctx, pool, up));
   ExprSet es;
   es.descs = upload_array(ctx, descs, up);
   es.insts = upload_array(ctx, insts, up);
@@ -1061,7 +1071,7 @@ static ExprSet upload_exprs(hs_ctx* ctx, const Table& t, const BoundFilter& b, P
 // Appends to rf the descriptors of filter b on the columns of t, skipping those on column skip_col that its windows
 // already decide: a predicate in scalar form and a term in set form.  A pattern term that is not a prefix goes to
 // rf->pats (on skip_col too: the windows only bound its values), every comparison to rf->cmps, and the expression
-// comparisons to rf->exprs.
+// comparisons to rf->exprs, or to rf->funcs when they use functions.
 static void add_filter(hs_ctx* ctx, const Table& t, BoundFilter& b, int skip_col, RowFilter* rf, PredUploads* up) {
   PredSet* ps = &rf->preds;
   for (size_t i = 0; i < b.pred_col.size(); i++) {
@@ -1095,7 +1105,11 @@ static void add_filter(hs_ctx* ctx, const Table& t, BoundFilter& b, int skip_col
     d.valid[0] = l.has_nulls ? l.valid.get() : nullptr, d.valid[1] = r.has_nulls ? r.valid.get() : nullptr;
     rf->cmps.p[rf->cmps.n++] = d;
   }
-  if (!b.expr_col.empty()) rf->exprs = upload_exprs(ctx, t, b, up);
+  if (!b.expr_col.empty()) {
+    bool funcs;
+    const ExprSet es = upload_exprs(ctx, t, b, up, &funcs);
+    (funcs ? rf->funcs : rf->exprs) = es;
+  }
 }
 
 // the bucket of every point of a key set, by the hash the build used (hash_rows over a column of the key's storage type

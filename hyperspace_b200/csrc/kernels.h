@@ -461,13 +461,15 @@ struct ExprSet {
   int n = 0;
 };
 // The row filter of a scan or join side: a row is kept when every predicate, pattern, comparison and expression
-// comparison holds
+// comparison holds.  A side's expression comparisons are in exprs when they are arithmetic only, in funcs (k_func_mask)
+// when one of them uses a function, a string, date or timestamp value.
 struct RowFilter {
   PredSet preds;
   PatternSet pats;
   CompareSet cmps;
   ExprSet exprs;
-  bool empty() const { return preds.n == 0 && pats.n == 0 && cmps.n == 0 && exprs.n == 0; }
+  ExprSet funcs;
+  bool empty() const { return preds.n == 0 && pats.n == 0 && cmps.n == 0 && exprs.n == 0 && funcs.n == 0; }
 };
 // The window search over sorted segments (each ascending on `keys`), one pair (segment, range) per work item:
 // work[w] = {s, r} with r indexing `ranges` (device); bounds[2w] = first row of s inside ranges[r], bounds[2w+1] = first
@@ -489,6 +491,8 @@ void launch_compare_mask(hs_ctx* ctx, const CompareSet& cmps, const uint32_t* ca
 // mask[i] = 0 where an expression comparison of `exprs` does not hold for row cand[i] (row i when cand is nullptr);
 // launches nothing when exprs is empty
 void launch_expr_mask(hs_ctx* ctx, const ExprSet& exprs, const uint32_t* cand, int64_t n, uint32_t* mask);
+// the same for expression comparisons with functions (k_func_mask)
+void launch_func_mask(hs_ctx* ctx, const ExprSet& funcs, const uint32_t* cand, int64_t n, uint32_t* mask);
 // The n key columns of one join side in sorted order: col[k] holds key column k at sorted position p, read at its
 // type's width (type[k]: HS_TYPE_INT32 / HS_TYPE_INT64, or HS_TYPE_STRING for string references).  The tuples compare
 // column by column, integers as signed values, strings in byte order.

@@ -663,16 +663,33 @@ inline int check_expr_side(const hs_expr_node* nodes, int n, int i, const char* 
         break;
       case HS_EXPR_LITERAL:
         if (x.literal_type != HS_TYPE_INT32 && x.literal_type != HS_TYPE_INT64 && x.literal_type != HS_TYPE_DOUBLE &&
-            x.literal_type != HS_TYPE_DECIMAL)
+            x.literal_type != HS_TYPE_DECIMAL && x.literal_type != HS_TYPE_STRING && x.literal_type != HS_TYPE_DATE &&
+            x.literal_type != HS_TYPE_TIMESTAMP)
           return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a literal of unknown type %d", i,
                         x.literal_type);
-        if (x.literal_type == HS_TYPE_INT32 && x.value_i != (int32_t)x.value_i)
-          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has an int literal outside int32", i);
+        if ((x.literal_type == HS_TYPE_INT32 || x.literal_type == HS_TYPE_DATE) && x.value_i != (int32_t)x.value_i)
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has %s literal outside int32", i,
+                        x.literal_type == HS_TYPE_DATE ? "a date" : "an int");
         if (x.literal_type == HS_TYPE_DECIMAL && (x.scale < 0 || x.scale > 38))
           return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a decimal literal of scale %d", i, x.scale);
+        if (x.literal_type == HS_TYPE_STRING && (x.value_i < 0 || x.value_i > (int64_t)kMaxStringLen || (x.value_i > 0 && !x.column)))
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a string literal of %lld bytes%s", i,
+                        (long long)x.value_i, x.value_i < 0 || x.value_i > (int64_t)kMaxStringLen ? ", not 0..65535" : " and no bytes");
         depth++;
         break;
       case HS_EXPR_NEG:
+      case HS_EXPR_YEAR:
+      case HS_EXPR_QUARTER:
+      case HS_EXPR_MONTH:
+      case HS_EXPR_DAYOFMONTH:
+      case HS_EXPR_DAYOFWEEK:
+      case HS_EXPR_DAYOFYEAR:
+      case HS_EXPR_WEEKOFYEAR:
+      case HS_EXPR_HOUR:
+      case HS_EXPR_MINUTE:
+      case HS_EXPR_SECOND:
+      case HS_EXPR_LENGTH:
+      case HS_EXPR_ABS:
         if (depth < 1) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d underflows its stack", side, i);
         break;
       case HS_EXPR_ADD:
@@ -680,8 +697,25 @@ inline int check_expr_side(const hs_expr_node* nodes, int n, int i, const char* 
       case HS_EXPR_MUL:
       case HS_EXPR_DIV:
       case HS_EXPR_REM:
+      case HS_EXPR_DATE_ADD:
+      case HS_EXPR_DATE_SUB:
+      case HS_EXPR_DATEDIFF:
         if (depth < 2) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d underflows its stack", side, i);
         depth--;
+        break;
+      case HS_EXPR_SUBSTRING: {
+        auto int_literal = [&](int at) { return at >= 0 && nodes[at].kind == HS_EXPR_LITERAL && nodes[at].literal_type == HS_TYPE_INT32; };
+        if (depth < 3) return refuse(HS_EINVAL, stats, err, errlen, "filter scan: the %s side of expression comparison %d underflows its stack", side, i);
+        if (!int_literal(k - 1) || !int_literal(k - 2))
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a SUBSTRING whose pos and len are not int literals", i);
+        depth -= 2;
+        break;
+      }
+      case HS_EXPR_COALESCE:
+        if (x.value_i < 2 || x.value_i > 8 || x.value_i > depth)
+          return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a COALESCE of %lld arguments over %d values", i,
+                        (long long)x.value_i, depth);
+        depth -= (int)x.value_i - 1;
         break;
       default: return refuse(HS_EINVAL, stats, err, errlen, "filter scan: expression comparison %d has a node of unknown kind %d", i, x.kind);
     }
@@ -713,8 +747,9 @@ inline int check_exprs(const hs_expr_compare* exprs, int n_exprs, int n_others, 
   return HS_OK;
 }
 
-// An operand's Spark type as the arithmetic coercion sees it: kind (kKindInt / Long / Float / Double / Decimal), a
-// decimal's precision and scale, and, for an integer literal, its digits (DecimalType.fromLiteral)
+// An operand's Spark type as the coercion sees it: kind (kKindInt / Long / Float / Double / Decimal, and for the
+// functions kKindString / Binary / Date / Timestamp; kKindOther is a boolean), a decimal's precision and scale, and, for
+// an integer literal, its digits (DecimalType.fromLiteral)
 struct ExprType {
   int kind;
   int p = 0, s = 0;
@@ -741,12 +776,97 @@ inline void as_decimal(const ExprType& t, int* p, int* s) {
   else *p = t.lit_digits ? t.lit_digits : (t.kind == kKindInt ? 10 : 20), *s = 0;
 }
 
+inline bool numeric_kind(int k) { return k == kKindInt || k == kKindLong || k == kKindFloat || k == kKindDouble || k == kKindDecimal; }
+inline bool datetime_kind(int k) { return k == kKindDate || k == kKindTimestamp; }
+
+// Spark's simpleString of an operand's type, for messages
+inline std::string expr_type_text(const ExprType& t) {
+  switch (t.kind) {
+    case kKindInt: return "int";
+    case kKindLong: return "bigint";
+    case kKindFloat: return "float";
+    case kKindDouble: return "double";
+    case kKindDecimal: return "decimal(" + std::to_string(t.p) + "," + std::to_string(t.s) + ")";
+    case kKindString: return "string";
+    case kKindBinary: return "binary";
+    case kKindDate: return "date";
+    case kKindTimestamp: return "timestamp";
+    default: return "boolean";
+  }
+}
+
+// Whether two operand kinds compare without arithmetic coercion: string with string, binary with binary, dates and
+// timestamps with each other
+inline bool comparable_kinds(int a, int b) {
+  return (datetime_kind(a) && datetime_kind(b)) || (a == b && (a == kKindString || a == kKindBinary));
+}
+
 // A resolved expression comparison: the program of column_expr.h (kXLoad's arg: the ordinal of the COLUMN node, left side
-// first), the comparison's domain, op and NOT
+// first), the comparison's domain, op and NOT.  funcs: the program holds a function, or a string, binary, date or
+// timestamp value, and runs in k_func_mask.  String literals are kXStringConst instructions into `pool`, which the caller
+// places (relocate_strings) before the program runs.
 struct ExprProgram {
   std::vector<ExprInst> insts;
   int32_t domain = kCmpInt, op = 0, negate = 0;
+  bool funcs = false;
+  std::string pool;
 };
+
+// kXStringConst instructions (arg: offset into the pool, v.i: length) to kXConst of a reference into the pool at base
+inline void relocate_strings(std::vector<ExprInst>* insts, const uint8_t* base) {
+  for (ExprInst& in : *insts)
+    if (in.op == kXStringConst) {
+      const uint32_t len = (uint32_t)in.v.i;
+      in.v.i = (__int128)string_ref(base + in.arg, len);
+      in.op = kXConst, in.arg = 0;
+    }
+}
+
+// the node kinds that existed before the functions, and their literal types: a comparison of such sides is refused
+// exactly as it was when a column of another type is used
+inline bool arithmetic_only(const hs_expr_node* nodes, int n) {
+  for (int k = 0; k < n; k++) {
+    if (nodes[k].kind > HS_EXPR_NEG) return false;
+    if (nodes[k].kind == HS_EXPR_LITERAL && nodes[k].literal_type > HS_TYPE_DOUBLE && nodes[k].literal_type != HS_TYPE_DECIMAL) return false;
+  }
+  return true;
+}
+
+// the values node x takes from the stack: its operator's or function's arguments, none for a column or a literal
+inline int expr_arity(const hs_expr_node& x) {
+  switch (x.kind) {
+    case HS_EXPR_COLUMN:
+    case HS_EXPR_LITERAL: return 0;
+    case HS_EXPR_COALESCE: return (int)x.value_i;
+    case HS_EXPR_SUBSTRING: return 3;
+    case HS_EXPR_ADD:
+    case HS_EXPR_SUB:
+    case HS_EXPR_MUL:
+    case HS_EXPR_DIV:
+    case HS_EXPR_REM:
+    case HS_EXPR_DATE_ADD:
+    case HS_EXPR_DATE_SUB:
+    case HS_EXPR_DATEDIFF: return 2;
+    default: return 1;
+  }
+}
+
+// whether the value node k of a checked side pushes is an argument of a function, rather than of arithmetic or the
+// comparison
+inline bool consumed_by_function(const hs_expr_node* nodes, int n, int k) {
+  for (int above = 0, j = k + 1; j < n; j++) {  // above: the values pushed after node k's that are still on the stack
+    const int pops = expr_arity(nodes[j]);
+    if (pops > above) return nodes[j].kind > HS_EXPR_NEG;
+    above += 1 - pops;
+  }
+  return false;
+}
+
+inline std::string date_text(int64_t days) {
+  char buf[48];
+  snprintf(buf, sizeof buf, "DATE '%04d-%02d-%02d'", date_part(days, kPartYear), date_part(days, kPartMonth), date_part(days, kPartDayOfMonth));
+  return buf;
+}
 
 // The expression comparison e (check_exprs has checked it) typed and lowered to column_expr.h's instructions, every
 // implicit cast explicit.  cols: one column per COLUMN node, the left side's first.  Spark 3.1's coercion, as
@@ -757,10 +877,21 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
   pg.negate = (e.flags & HS_TERM_NOT) != 0;
   std::vector<ExprType> ts;    // the type stack
   std::vector<std::string> txt;  // the nodes' SQL text, for messages
+  std::vector<int> bare;       // per stack value: the COLUMN node's ordinal when the value is a bare column, else -1
   auto emit = [&](int op, int arg, __int128 v = 0) {
     ExprInst in{};
     in.op = op, in.arg = arg, in.v.i = v;
     pg.insts.push_back(in);
+  };
+  auto column_refused = [&](int ord) {
+    const PredColumn& c = cols[ord];
+    fail(HS_EUNSUPPORTED, "filter scan: the column '%s' (%s) cannot be used in arithmetic", c.name.c_str(), pq::spark_type_name(c.schema).c_str());
+  };
+  // an arithmetic operand at stack index at: numeric, or refused -- a bare column with arithmetic's own message
+  auto arith_operand = [&](size_t at) {
+    if (numeric_kind(ts[at].kind)) return;
+    if (bare[at] >= 0) column_refused(bare[at]);
+    fail(HS_EUNSUPPORTED, "filter scan: %s (%s) cannot be used in arithmetic", txt[at].c_str(), expr_type_text(ts[at]).c_str());
   };
   auto to_double = [&](int at, ExprType& t, const std::string& what) {
     switch (t.kind) {
@@ -807,20 +938,79 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
     }
     return (a.kind == kKindLong || b.kind == kKindLong) ? (int)kXLong : (int)kXInt;
   };
+  auto domain_of = [](const ExprType& t) {
+    return t.kind == kKindInt ? kXInt : t.kind == kKindLong ? kXLong : t.kind == kKindDecimal ? kXDec : t.kind == kKindFloat ? kXFloat : kXDouble;
+  };
+  // COALESCE's findWiderCommonType over the n values at the top, each cast to it in its slot
+  auto coalesce = [&](int n, const std::string& what) {
+    const size_t base = ts.size() - n;
+    ExprType w = ts[base];
+    w.lit_digits = 0;
+    for (int j = 0; j < n; j++) {
+      ExprType t = ts[base + j];
+      t.lit_digits = 0;
+      t.narrow = false;
+      const bool ok = j == 0 ? (numeric_kind(t.kind) || comparable_kinds(t.kind, t.kind))
+                             : (numeric_kind(t.kind) && numeric_kind(w.kind)) || comparable_kinds(t.kind, w.kind);
+      if (!ok) fail(HS_EUNSUPPORTED, "filter scan: %s mixes %s (%s) with %s", what.c_str(), txt[base + j].c_str(), expr_type_text(t).c_str(),
+                    j ? expr_type_text(w).c_str() : "nothing it widens with");
+      if (j == 0) { w = t; continue; }
+      if (datetime_kind(w.kind)) {
+        w.kind = w.kind == kKindTimestamp || t.kind == kKindTimestamp ? kKindTimestamp : kKindDate;
+      } else if (numeric_kind(w.kind)) {
+        if ((is_dec(w) || is_dec(t)) && !is_fp(w) && !is_fp(t)) {
+          int pa, sa, pb, sb;
+          as_decimal(w, &pa, &sa);
+          as_decimal(t, &pb, &sb);
+          const int s = std::max(sa, sb), p = std::max(pa - sa, pb - sb) + s;
+          if (p > 38) fail(HS_EUNSUPPORTED, "filter scan: %s needs a decimal of more than 38 digits", what.c_str());
+          w = ExprType{kKindDecimal, p, s};
+        } else if (w.kind == kKindDouble || t.kind == kKindDouble || is_dec(w) || is_dec(t)) {
+          w = ExprType{kKindDouble};
+        } else if (w.kind == kKindFloat || t.kind == kKindFloat) {
+          w = ExprType{kKindFloat};
+        } else {
+          w = ExprType{w.kind == kKindLong || t.kind == kKindLong ? kKindLong : kKindInt};
+        }
+      }
+    }
+    for (int j = 0; j < n; j++) {
+      ExprType t = ts[base + j];
+      const int slot = n - 1 - j;
+      if (w.kind == kKindTimestamp && t.kind == kKindDate) emit(kXRescale, slot, (__int128)86400000000ll);
+      else if (w.kind == kKindDouble && t.kind != kKindDouble) to_double(slot, t, what);
+      else if (w.kind == kKindFloat && t.kind != kKindFloat) to_float(slot, t);
+      else if (w.kind == kKindDecimal) {
+        int p, s;
+        as_decimal(ExprType{t.kind, t.p, t.s}, &p, &s);
+        if (s < w.s) emit(kXRescale, slot, pow10_i128(w.s - s));
+      }
+    }
+    emit(kXCoalesce, n);
+    return w;
+  };
   static const char* const kOpText[] = {"", "", "", "+", "-", "*", "/", "%"};
+  static const char* const kFuncText[] = {"year", "quarter", "month", "dayofmonth", "dayofweek", "dayofyear", "weekofyear", "hour", "minute",
+                                          "second", "date_add", "date_sub", "datediff", "length", "substring", "abs", "coalesce"};
   int col_ord = 0;
-  auto side = [&](const hs_expr_node* nodes, int n) {
+  auto side = [&](const hs_expr_node* nodes, int n, const hs_expr_node* other, int n_other, int other_bare_kind) {
     for (int k = 0; k < n; k++) {
       const hs_expr_node& x = nodes[k];
       if (x.kind == HS_EXPR_COLUMN) {
         const PredColumn& c = cols[col_ord];
         const int kind = compare_kind(c);
-        if (kind != kKindInt && kind != kKindLong && kind != kKindFloat && kind != kKindDouble && kind != kKindDecimal)
-          fail(HS_EUNSUPPORTED, "filter scan: the column '%s' (%s) cannot be used in arithmetic", c.name.c_str(),
-               pq::spark_type_name(c.schema).c_str());
+        if (!numeric_kind(kind)) {
+          // A boolean never serves.  A column of another type serves as a function's argument, or as a bare side beside a
+          // side it compares with -- decided after that side, unless the comparison is arithmetic only: then it is
+          // refused here, as it always was, unless the other side is a bare column it compares with.
+          const bool deferred = n == 1 && (!arithmetic_only(other, n_other) || comparable_kinds(kind, other_bare_kind));
+          if (kind == kKindOther || (!deferred && !consumed_by_function(nodes, n, k))) column_refused(col_ord);
+          pg.funcs = true;
+        }
         ExprType t{kind};
         if (kind == kKindDecimal) t.p = c.schema.precision, t.s = c.schema.scale;
         t.narrow = c.schema.converted_type == 15 || c.schema.converted_type == 16;  // INT_8, INT_16
+        bare.push_back(col_ord);
         emit(kXLoad, col_ord++);
         ts.push_back(t);
         txt.push_back(c.name);
@@ -843,6 +1033,25 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
             snprintf(buf, sizeof buf, "%.17g", x.value_f);
             break;
           }
+          case HS_TYPE_STRING:
+            t.kind = kKindString;
+            emit(kXStringConst, (int32_t)pg.pool.size(), x.value_i);
+            pg.pool.append(x.value_i ? x.column : "", (size_t)x.value_i);
+            snprintf(buf, sizeof buf, "%.*s", (int)std::min<int64_t>(x.value_i, 40), x.value_i ? x.column : "");
+            pg.funcs = true;
+            break;
+          case HS_TYPE_DATE:
+            t.kind = kKindDate;
+            emit(kXConst, 0, x.value_i);
+            snprintf(buf, sizeof buf, "%s", date_text(x.value_i).c_str());
+            pg.funcs = true;
+            break;
+          case HS_TYPE_TIMESTAMP:
+            t.kind = kKindTimestamp;
+            emit(kXConst, 0, x.value_i);
+            snprintf(buf, sizeof buf, "TIMESTAMP_MICROS(%lld)", (long long)x.value_i);
+            pg.funcs = true;
+            break;
           default: {  // HS_TYPE_DECIMAL: DecimalType(max(digits, scale), scale)
             t.kind = kKindDecimal, t.s = x.scale;
             t.p = std::max(decimal_digits(x.value_i < 0 ? 0ull - (uint64_t)x.value_i : (uint64_t)x.value_i), x.scale);
@@ -853,15 +1062,18 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
         }
         ts.push_back(t);
         txt.push_back(buf);
+        bare.push_back(-1);
       } else if (x.kind == HS_EXPR_NEG) {
+        arith_operand(ts.size() - 1);
         const ExprType& t = ts.back();
         if (t.narrow) fail(HS_EUNSUPPORTED, "filter scan: (- %s) is byte or short arithmetic, which wraps at its width: not handled", txt.back().c_str());
-        const int dom = t.kind == kKindInt ? kXInt : t.kind == kKindLong ? kXLong : t.kind == kKindDecimal ? kXDec
-                        : t.kind == kKindFloat ? kXFloat : kXDouble;
-        emit(dom + kXNeg, 0);
+        emit(domain_of(t) + kXNeg, 0);
         ts.back().lit_digits = 0;
         txt.back() = "(- " + txt.back() + ")";
-      } else {
+        bare.back() = -1;
+      } else if (x.kind <= HS_EXPR_REM) {
+        arith_operand(ts.size() - 2);
+        arith_operand(ts.size() - 1);
         ExprType b = ts.back();
         ts.pop_back();
         ExprType a = ts.back();
@@ -869,6 +1081,8 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
         const std::string what = "(" + txt[txt.size() - 2] + " " + kOpText[x.kind] + " " + txt.back() + ")";
         txt.pop_back();
         txt.back() = what;
+        bare.pop_back();
+        bare.back() = -1;
         if (a.narrow && b.narrow) fail(HS_EUNSUPPORTED, "filter scan: %s is byte or short arithmetic, which wraps at its width: not handled", what.c_str());
         ExprType r;
         int dom;
@@ -894,16 +1108,91 @@ inline ExprProgram resolve_expr(const hs_expr_compare& e, const std::vector<Pred
         }
         emit(dom + (x.kind - HS_EXPR_ADD), 0);
         ts.push_back(r);
+      } else {  // a function (check_exprs: HS_EXPR_YEAR .. HS_EXPR_COALESCE)
+        pg.funcs = true;
+        const int nargs = expr_arity(x);
+        const size_t base = ts.size() - nargs;
+        std::string what = std::string(kFuncText[x.kind - HS_EXPR_YEAR]) + "(";
+        for (int j = 0; j < nargs; j++) what += (j ? ", " : "") + txt[base + j];
+        what += ")";
+        auto need = [&](int j, bool ok, const char* kinds) {
+          if (!ok) fail(HS_EUNSUPPORTED, "filter scan: %s: %s (%s) is not %s", what.c_str(), txt[base + j].c_str(),
+                        expr_type_text(ts[base + j]).c_str(), kinds);
+        };
+        ExprType r{kKindInt};
+        switch (x.kind) {
+          case HS_EXPR_HOUR:
+          case HS_EXPR_MINUTE:
+          case HS_EXPR_SECOND:
+            need(0, ts[base].kind == kKindTimestamp, "a timestamp");
+            emit(kXTimePart, kPartHour + (x.kind - HS_EXPR_HOUR));
+            break;
+          case HS_EXPR_DATE_ADD:
+          case HS_EXPR_DATE_SUB:
+          case HS_EXPR_DATEDIFF: {
+            need(0, datetime_kind(ts[base].kind), "a date or timestamp");
+            if (x.kind == HS_EXPR_DATEDIFF) need(1, datetime_kind(ts[base + 1].kind), "a date or timestamp");
+            else need(1, ts[base + 1].kind == kKindInt, "an int, short or byte");  // days: Spark would cast anything else
+            if (ts[base].kind == kKindTimestamp) emit(kXTsToDate, 1);
+            if (ts[base + 1].kind == kKindTimestamp) emit(kXTsToDate, 0);
+            emit(kXInt + (x.kind == HS_EXPR_DATE_ADD ? kXAdd : kXSub), 0);
+            if (x.kind != HS_EXPR_DATEDIFF) r = ExprType{kKindDate};
+            break;
+          }
+          case HS_EXPR_LENGTH:
+            need(0, ts[base].kind == kKindString || ts[base].kind == kKindBinary, "a string or binary");
+            emit(kXLength, ts[base].kind == kKindBinary);
+            break;
+          case HS_EXPR_SUBSTRING: {
+            need(0, ts[base].kind == kKindString || ts[base].kind == kKindBinary, "a string or binary");
+            pg.insts.pop_back(), pg.insts.pop_back();  // the pos and len literals' kXConst: check_exprs made them literals
+            const uint64_t pos = (uint32_t)(int32_t)nodes[k - 2].value_i, len = (uint32_t)(int32_t)nodes[k - 1].value_i;
+            emit(kXSubstr, ts[base].kind == kKindBinary, (__int128)(pos | len << 32));
+            r = ExprType{ts[base].kind};
+            break;
+          }
+          case HS_EXPR_ABS:
+            need(0, numeric_kind(ts[base].kind), "a number");
+            if (ts[base].narrow) fail(HS_EUNSUPPORTED, "filter scan: %s is byte or short arithmetic, which wraps at its width: not handled", what.c_str());
+            emit(kXAbs, domain_of(ts[base]));
+            r = ts[base];
+            r.lit_digits = 0;
+            break;
+          case HS_EXPR_COALESCE: r = coalesce(nargs, what); break;
+          default:  // HS_EXPR_YEAR .. HS_EXPR_WEEKOFYEAR
+            need(0, datetime_kind(ts[base].kind), "a date or timestamp");
+            if (ts[base].kind == kKindTimestamp) emit(kXTsToDate, 0);
+            emit(kXDatePart, kPartYear + (x.kind - HS_EXPR_YEAR));
+            break;
+        }
+        ts.resize(base), txt.resize(base), bare.resize(base);
+        ts.push_back(r), txt.push_back(what), bare.push_back(-1);
       }
     }
   };
-  side(e.left, e.n_left);
-  side(e.right, e.n_right);
+  // the kind of each side that is one COLUMN node (-1 otherwise); the right side's column follows the left side's columns
+  int n_left_cols = 0;
+  for (int k = 0; k < e.n_left; k++) n_left_cols += e.left[k].kind == HS_EXPR_COLUMN;
+  const int left_bare = e.n_left == 1 && e.left[0].kind == HS_EXPR_COLUMN ? compare_kind(cols[0]) : -1;
+  const int right_bare = e.n_right == 1 && e.right[0].kind == HS_EXPR_COLUMN ? compare_kind(cols[n_left_cols]) : -1;
+  side(e.left, e.n_left, e.right, e.n_right, right_bare);
+  side(e.right, e.n_right, e.left, e.n_left, left_bare);
   ExprType b = ts.back(), a = ts[0];
   static const char* const kCmpText[] = {"", "<", "<=", ">", ">=", "=", "<=>"};
   const std::string what = "(" + txt[0] + " " + kCmpText[e.op] + " " + txt[1] + ")";
-  const int dom = unify(a, b, what, true);  // resolve_compare's table, decimals widened to 38 digits
-  pg.domain = dom == kXFloat ? kCmpFloat : (dom == kXDouble ? kCmpDouble : kCmpInt);
+  if (numeric_kind(a.kind) && numeric_kind(b.kind)) {
+    const int dom = unify(a, b, what, true);  // resolve_compare's table, decimals widened to 38 digits
+    pg.domain = dom == kXFloat ? kCmpFloat : (dom == kXDouble ? kCmpDouble : kCmpInt);
+  } else if (comparable_kinds(a.kind, b.kind)) {
+    pg.domain = datetime_kind(a.kind) ? kCmpInt : kCmpString;
+    if (a.kind == kKindDate && b.kind == kKindTimestamp) emit(kXRescale, 1, (__int128)86400000000ll);
+    if (b.kind == kKindDate && a.kind == kKindTimestamp) emit(kXRescale, 0, (__int128)86400000000ll);
+  } else {
+    for (int s = 0; s < 2; s++)
+      if (bare[s] >= 0 && !numeric_kind((s ? b : a).kind)) column_refused(bare[s]);
+    fail(HS_EUNSUPPORTED, "filter scan: %s (%s) and %s (%s) cannot be compared", txt[0].c_str(), expr_type_text(a).c_str(), txt[1].c_str(),
+         expr_type_text(b).c_str());
+  }
   return pg;
 }
 

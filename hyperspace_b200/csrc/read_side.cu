@@ -181,6 +181,20 @@ __global__ void __launch_bounds__(256, 8) k_expr_mask(const __grid_constant__ Ex
   }
 }
 
+// k_expr_mask for programs with function instructions (column_expr.h: expr_holds<true>): calendar fields, string
+// references and the string domain.  A kernel of its own, so that arithmetic-only programs keep k_expr_mask's code.
+__global__ void __launch_bounds__(256, 8) k_func_mask(const __grid_constant__ ExprSet es, const uint32_t* __restrict__ cand, int64_t n,
+                                                      uint32_t* __restrict__ mask) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (!mask[i]) continue;
+    const int64_t row = cand ? (int64_t)cand[i] : i;
+    bool ok = true;
+    for (int p = 0; p < es.n && ok; p++) ok = expr_holds<true>(es.descs[p], es.insts, es.cols, row);
+    if (!ok) mask[i] = 0;
+  }
+}
+
 // a key value at position p, read at its type's width: int32 sign-extended, int64 as it is, a string as its reference
 template <int KT>
 __device__ __forceinline__ int64_t key_value(const void* col, int64_t p) {
@@ -646,6 +660,14 @@ void launch_expr_mask(hs_ctx* ctx, const ExprSet& exprs, const uint32_t* cand, i
   HS_LAUNCH_CHECK(ctx);
 }
 
+void launch_func_mask(hs_ctx* ctx, const ExprSet& funcs, const uint32_t* cand, int64_t n, uint32_t* mask) {
+  if (funcs.n == 0) return;
+  KernelScope _ks(ctx, "k_func_mask");
+  if (n == 0) return;
+  k_func_mask<<<grid_for(ctx, n, 256, 16), 256, 0, ctx->stream>>>(funcs, cand, n, mask);
+  HS_LAUNCH_CHECK(ctx);
+}
+
 void launch_join_count(hs_ctx* ctx, const JoinKeyCols& lkeys, const uint64_t* lseg, const JoinKeyCols& rkeys,
                        const uint64_t* rseg, int nseg, int64_t nl, uint32_t* counts, uint32_t* first_match) {
   KernelScope _ks(ctx, "k_join_count");
@@ -766,6 +788,7 @@ int64_t select_rows(hs_ctx* ctx, const RowFilter& filter, const uint32_t* cand, 
   launch_pattern_mask(ctx, filter.pats, cand, n, mask.get());
   launch_compare_mask(ctx, filter.cmps, cand, n, mask.get());
   launch_expr_mask(ctx, filter.exprs, cand, n, mask.get());
+  launch_func_mask(ctx, filter.funcs, cand, n, mask.get());
   Buf<int64_t> d_deleted;
   if (n > 0 && ndeleted > 0) {
     d_deleted.alloc(ctx, ndeleted);

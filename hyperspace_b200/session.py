@@ -195,9 +195,10 @@ class ColumnCompare:
 class Expr:
     """Arithmetic over columns and literals (Spark's Add, Subtract, Multiply, Divide, Remainder and UnaryMinus over
     attributes and literals): a column (``op`` "column", ``value`` its name), a literal (``op`` "literal"), a unary minus
-    (``op`` "neg", one argument) or a binary operation (``op`` one of + - * / %, two arguments).  Its comparison
-    operators, ``eqNullSafe`` and ``between`` give a Predicate holding an ExprCompare; the engine types the arithmetic as
-    Spark 3.1 does (include/hs_gpu.h)."""
+    (``op`` "neg", one argument), a binary operation (``op`` one of + - * / %, two arguments) or a Spark function
+    (``op`` one of FUNCTIONS, its arguments; hyperspace_b200.functions builds them).  Its comparison operators,
+    ``eqNullSafe`` and ``between`` give a Predicate holding an ExprCompare; the engine types the arithmetic and the
+    functions as Spark 3.1 does (include/hs_gpu.h)."""
     __hash__ = None  # == builds a comparison
 
     def __init__(self, op: str, args: Tuple["Expr", ...] = (), value=None):
@@ -214,20 +215,31 @@ class Expr:
             raise LE.HyperspaceException(f"the literal {v!r} cannot be used in arithmetic on the GPU path")
         return Expr("literal", value=v)
 
+    @staticmethod
+    def operand(v) -> "Expr":
+        """Expr.of, which also takes the literals a comparison or a function argument may hold: str and bytes (a string),
+        datetime.date (a date) and datetime.datetime (a timestamp; naive is UTC)."""
+        if isinstance(v, (str, bytes, datetime.date)):
+            return Expr("literal", value=v)
+        return Expr.of(v)
+
     def __str__(self) -> str:
         if self.op == "column":
             return self.value
         if self.op == "literal":
-            return str(self.value)
+            return self.value.decode("utf-8", "replace") if isinstance(self.value, bytes) else str(self.value)
         if self.op == "neg":
             return f"(- {self.args[0]})"
+        if self.op in FUNCTIONS:
+            return f"{self.op}({', '.join(str(a) for a in self.args)})"
         return f"({self.args[0]} {self.op} {self.args[1]})"
 
     def postfix(self) -> List[tuple]:
         """The nodes in postfix order, as Context.filter_scan_expr takes them."""
         if self.op in ("column", "literal"):
             return [(self.op, self.value)]
-        return [n for a in self.args for n in a.postfix()] + [(self.op,)]
+        tail = ("coalesce", len(self.args)) if self.op == "coalesce" else (self.op,)
+        return [n for a in self.args for n in a.postfix()] + [tail]
 
     @property
     def columns(self) -> List[str]:
@@ -263,7 +275,7 @@ class Expr:
     def __neg__(self): return Expr("neg", (self,))
 
     def _compare(self, op: str, other, negated: bool = False) -> "Predicate":
-        return Predicate({}, [], [], [], [ExprCompare(self, op, Expr.of(other), negated)])
+        return Predicate({}, [], [], [], [ExprCompare(self, op, Expr.operand(other), negated)])
 
     def __lt__(self, o): return self._compare("<", o)
     def __le__(self, o): return self._compare("<=", o)
@@ -283,6 +295,39 @@ class Expr:
 
     def __bool__(self):
         raise LE.HyperspaceException(f"the expression {self} is not a filter: compare it")
+
+
+# The Spark functions an Expr may apply (hyperspace_b200.functions), by their SQL names
+FUNCTIONS = ("year", "quarter", "month", "dayofmonth", "dayofweek", "dayofyear", "weekofyear", "hour", "minute", "second",
+             "date_add", "date_sub", "datediff", "length", "substring", "abs", "coalesce")
+# the functions whose argument may be a timestamp, which they read in the session time zone
+_TIME_ZONE_FUNCTIONS = ("year", "quarter", "month", "dayofmonth", "dayofweek", "dayofyear", "weekofyear", "hour", "minute",
+                        "second", "date_add", "date_sub", "datediff")
+_UTC_ZONES = ("UTC", "GMT", "Z", "+00:00", "-00:00")
+
+
+def _static_type(e: Expr, types: Dict[str, str]) -> Optional[str]:
+    """The Spark type name of an expression as far as the time-zone rule needs it: a column's, a date / timestamp
+    literal's, and the date or timestamp a function gives; None otherwise."""
+    if e.op == "column":
+        return types.get(e.value.lower())
+    if e.op == "literal":
+        return "timestamp" if isinstance(e.value, datetime.datetime) else ("date" if isinstance(e.value, datetime.date) else None)
+    if e.op in ("date_add", "date_sub"):
+        return "date"
+    if e.op == "coalesce":
+        kinds = [_static_type(a, types) for a in e.args]
+        return "timestamp" if "timestamp" in kinds else ("date" if "date" in kinds else None)
+    return None
+
+
+def _refuse_time_zone(e: Expr, types: Dict[str, str], zone: str) -> None:
+    """A function of a timestamp in a session time zone other than UTC: the engine reads timestamps in UTC."""
+    if e.op in _TIME_ZONE_FUNCTIONS and any(_static_type(a, types) == "timestamp" for a in e.args):
+        raise LE.HyperspaceException(f"{e} reads a timestamp in the session time zone {zone}, and the GPU path reads timestamps in "
+                                     "UTC only: keep it in a Spark Filter")
+    for a in e.args:
+        _refuse_time_zone(a, types, zone)
 
 
 @dataclass
@@ -460,12 +505,40 @@ class Predicate:
 
 
 def _number(v):
-    """A literal as a number for the bounds: a datetime is a timestamp's micros since the epoch (naive = UTC)."""
+    """A literal as a number for the bounds: a datetime is a timestamp's micros since the epoch (naive = UTC), a date its
+    days since the epoch (DataFrame.filter restates a date's bounds in the column's own unit)."""
     if isinstance(v, datetime.datetime):
         from ._native import timestamp_micros
 
         return timestamp_micros(v)
+    if _is_date(v):
+        return (v - datetime.date(1970, 1, 1)).days
     return v
+
+
+def _is_date(v) -> bool:
+    return isinstance(v, datetime.date) and not isinstance(v, datetime.datetime)
+
+
+_DAY_MICROS = 86_400_000_000
+
+
+def _date_literal(column: str, spark_type: Optional[str], v):
+    """A datetime.date literal compared with a column, as Spark casts it: the days on a date column, the day's UTC
+    midnight in micros on a timestamp column; any other column raises.  Other literals pass as they are."""
+    if not _is_date(v):
+        return v
+    days = (v - datetime.date(1970, 1, 1)).days
+    if spark_type == "date":
+        return days
+    if spark_type == "timestamp":
+        return days * _DAY_MICROS
+    raise LE.HyperspaceException(f"the date literal {v} cannot be compared with the {spark_type} column '{column}' on the GPU path")
+
+
+def _term_bounds(op: str, v) -> Tuple[object, object]:
+    """The inclusive integer bounds of one comparison with a number, as Column's comparison operators give them."""
+    return {">=": (_ceil(v), None), ">": (_floor(v) + 1, None), "<=": (None, _floor(v)), "<": (None, _ceil(v) - 1), "==": (v, v)}[op]
 
 
 def _ceil(v):  # NaN and infinities (floating-point columns) stay as they are in the bounds
@@ -491,6 +564,12 @@ class Column:
     # `col("Query") == "facebook"` is the predicate of the reference's own filter-rule tests (T/index/E2EHyperspaceRulesTest.scala).
     def _compare(self, op: str, other: "Column", negated: bool = False) -> Predicate:
         return Predicate({}, [], [], [ColumnCompare(self.name, op, other.name, negated)])
+
+    def substr(self, startPos: int, length: int) -> Expr:
+        """Column.substr with int arguments: substring(self, startPos, length)."""
+        from .functions import substring
+
+        return substring(self, startPos, length)
 
     # arithmetic: an Expr, which compares into an expression comparison
     def __add__(self, o): return Expr.of(self) + o
@@ -785,8 +864,23 @@ class DataFrame:
             raise LE.HyperspaceException(f"the expression {predicate} is not a filter: compare it (a boolean column is not "
                                          "handled by the GPU path)")
         self._refuse_join_compares(predicate)
-        resolved = Predicate({self._resolve(c): b for c, b in predicate.bounds.items()},
-                             [(self._resolve(c), op, v) for c, op, v in predicate.terms],
+        zone = self.session.conf.get("spark.sql.session.timeZone")
+        if zone is not None and str(zone).upper() not in _UTC_ZONES and predicate.exprs:
+            types = {n.lower(): t for n, t in _schema_types(self.plan)}
+            for e in predicate.exprs:
+                _refuse_time_zone(e.left, types, zone)
+                _refuse_time_zone(e.right, types, zone)
+        bounds = {self._resolve(c): b for c, b in predicate.bounds.items()}
+        terms = [(self._resolve(c), op, v) for c, op, v in predicate.terms]
+        dated = {c for c, _, v in terms if _is_date(v)}
+        if dated:  # a date literal in the unit of its column; that column's bounds restated from its terms
+            types = {n.lower(): t for n, t in _schema_types(self.plan)}
+            terms = [(c, op, _date_literal(c, types.get(c.lower()), v)) for c, op, v in terms]
+            for c in dated:
+                los, his = zip(*[_term_bounds(op, v) for t, op, v in terms if t == c])
+                lo, hi = [x for x in los if x is not None], [x for x in his if x is not None]
+                bounds[c] = (max(lo) if lo else None, min(hi) if hi else None)
+        resolved = Predicate(bounds, terms,
                              [dataclasses.replace(a, column=self._resolve(a.column), ranges=list(a.ranges)) for a in predicate.anys],
                              [dataclasses.replace(c, left=self._resolve(c.left), right=self._resolve(c.right)) for c in predicate.compares],
                              [dataclasses.replace(e, left=e.left.renamed(self._resolve), right=e.right.renamed(self._resolve))
@@ -866,6 +960,17 @@ class DataFrame:
     def count(self) -> int:
         res = self.collect()
         return len(next(iter(res.values()))) if res else 0
+
+
+def _schema_types(plan) -> List[Tuple[str, str]]:
+    """(name, Spark type name) of every column of the relations under a plan."""
+    if isinstance(plan, RelationNode):
+        return list(plan.schema)
+    if isinstance(plan, (FilterNode, ProjectNode)):
+        return _schema_types(plan.child)
+    if isinstance(plan, JoinNode):
+        return _schema_types(plan.left) + _schema_types(plan.right)
+    return []
 
 
 def output_columns(plan) -> List[str]:

@@ -56,6 +56,8 @@ extern "C" {
 #define HS_TYPE_STRING 5 /* BYTE_ARRAY (Spark string / binary): indexed and included columns (one GPU), filter scan keys and
                             predicates, join keys (alone or with other key columns); compared in UTF8String byte order */
 #define HS_TYPE_DECIMAL 6 /* hs_predicate literal only: a decimal, unscaled value in lo_i / hi_i, scale in `scale` */
+#define HS_TYPE_DATE 7      /* hs_expr_node literal only: a date, days since the epoch in value_i */
+#define HS_TYPE_TIMESTAMP 8 /* hs_expr_node literal only: a timestamp, microseconds since the epoch in value_i */
 
 /* Spark timestamps and decimals.  Columns keep an int32 / int64 storage type; their Spark type comes from the Parquet
  * converted / logical type:
@@ -553,12 +555,68 @@ int hs_bucket_join_outer(hs_ctx* ctx, const hs_join_spec* spec, int32_t join_typ
 #define HS_EXPR_REM 7
 #define HS_EXPR_NEG 8
 
+/* Spark functions of columns inside an hs_expr_compare side: `year(d) = 1995`, `substring(s, 1, 2) = '13'`,
+ * `datediff(a, b) > 30`, `abs(a - b) < 5`, `coalesce(x, 0) > 0.05`.  Each kind takes its arguments in postfix order below
+ * it, like the arithmetic nodes; arithmetic, functions and comparisons nest freely within the limits above.  Spark 3.1
+ * semantics with spark.sql.ansi.enabled=false:
+ *   Literals besides the numeric ones: HS_TYPE_STRING (the bytes at `column`, value_i of them, at most 65535; a string),
+ *     HS_TYPE_DATE (value_i days since the epoch, within int32) and HS_TYPE_TIMESTAMP (value_i microseconds since the epoch).
+ *   YEAR QUARTER MONTH DAYOFMONTH DAYOFWEEK DAYOFYEAR WEEKOFYEAR (one date or timestamp) -> int.  Proleptic Gregorian, as
+ *     LocalDate.ofEpochDay; DAYOFWEEK is 1 = Sunday .. 7 = Saturday; WEEKOFYEAR is the ISO-8601 week (weeks start on
+ *     Monday, week 1 holds the year's first Thursday).  A timestamp is first cast to a date in UTC, the library's time
+ *     zone (naive literals are UTC, hs_column_compare takes dates as UTC midnights): floorDiv(micros, 86 400 000 000).
+ *   HOUR MINUTE SECOND (one timestamp) -> int: the UTC wall clock.  A date argument is HS_EUNSUPPORTED.
+ *   DATE_ADD DATE_SUB (start: date or timestamp, then days) -> date: start +/- days in int arithmetic, wrapping at 2^31
+ *     (Spark's DateAdd / DateSub).  days is an int literal or a byte, short or int column; a long, decimal or floating
+ *     days is HS_EUNSUPPORTED (Spark would cast it).
+ *   DATEDIFF (end, then start: each a date or timestamp) -> int: end - start in days, wrapping.
+ *   LENGTH (string or binary) -> int: characters of a string, counted as UTF8String.numChars counts them (by the length
+ *     each first byte announces), bytes of a binary.  Values that are not valid UTF-8 are not covered.
+ *   SUBSTRING (string or binary, then pos, then len; pos and len HS_TYPE_INT32 literals, else HS_EINVAL) -> the argument's
+ *     type: UTF8String.substringSQL / ByteArray.subStringSQL.  pos > 0 is 1-based, pos 0 is 1, a negative pos counts from
+ *     the end; the end is start + len clamped to the int range, and start >= end gives the empty value.  The result
+ *     refers to the argument's bytes: nothing is copied.
+ *   ABS (a number) -> its type.  int and long wrap (abs(MIN) = MIN); float and double clear the sign (abs(-0.0) = 0.0,
+ *     NaN stays NaN); decimals are exact.  A byte or short argument is HS_EUNSUPPORTED (Spark wraps at its width).
+ *   COALESCE (value_i arguments, 2..8 and at most the values below it, else HS_EINVAL) -> findWiderCommonType of the
+ *     arguments: the arithmetic's numeric widening (an integer literal counts as int or long here, decimal(10,0) or
+ *     decimal(20,0) beside a decimal; a result above 38 digits is HS_EUNSUPPORTED), string with string, binary with
+ *     binary, date with date, date with timestamp to timestamp.  The value is the first non-null argument; null only
+ *     when every argument is.  Any other mix (a string with a number, for one) is HS_EUNSUPPORTED.  A date promoted to
+ *     a timestamp is its UTC midnight in exact 128-bit micros, also for a date more than 106 751 991 days from the epoch
+ *     (beyond the long micros range, where Spark's cast fails): the functions over it give that midnight's fields.
+ *   Nulls: every function but COALESCE is null when any argument is null.
+ *   The comparison, besides the numeric pairs above: string with string and binary with binary in UTF8String byte order;
+ *     date with date in days; date or timestamp with timestamp in microseconds (a date is its UTC midnight), as
+ *     hs_column_compare.  Any other pair with a string, binary, date or timestamp side is HS_EUNSUPPORTED, naming both
+ *     sides' text and types -- except that a bare column of a type arithmetic refuses keeps the message "the column 'c'
+ *     (type) cannot be used in arithmetic".  The argument of a function of the wrong type is HS_EUNSUPPORTED naming the
+ *     function and the type. */
+#define HS_EXPR_YEAR 9
+#define HS_EXPR_QUARTER 10
+#define HS_EXPR_MONTH 11
+#define HS_EXPR_DAYOFMONTH 12
+#define HS_EXPR_DAYOFWEEK 13
+#define HS_EXPR_DAYOFYEAR 14
+#define HS_EXPR_WEEKOFYEAR 15
+#define HS_EXPR_HOUR 16
+#define HS_EXPR_MINUTE 17
+#define HS_EXPR_SECOND 18
+#define HS_EXPR_DATE_ADD 19
+#define HS_EXPR_DATE_SUB 20
+#define HS_EXPR_DATEDIFF 21
+#define HS_EXPR_LENGTH 22
+#define HS_EXPR_SUBSTRING 23
+#define HS_EXPR_ABS 24
+#define HS_EXPR_COALESCE 25
+
 typedef struct {
   int32_t kind;          /* HS_EXPR_* */
-  const char* column;    /* HS_EXPR_COLUMN */
-  int32_t literal_type;  /* HS_EXPR_LITERAL: HS_TYPE_INT32 / HS_TYPE_INT64 / HS_TYPE_DOUBLE / HS_TYPE_DECIMAL */
+  const char* column;    /* HS_EXPR_COLUMN: the name; HS_TYPE_STRING literal: its bytes (value_i of them) */
+  int32_t literal_type;  /* HS_EXPR_LITERAL: HS_TYPE_INT32 / INT64 / DOUBLE / DECIMAL / STRING / DATE / TIMESTAMP */
   int32_t scale;         /* HS_TYPE_DECIMAL literal */
-  int64_t value_i;       /* INT32, INT64, DECIMAL (unscaled) */
+  int64_t value_i;       /* INT32, INT64, DECIMAL (unscaled), DATE (days), TIMESTAMP (micros), STRING (length);
+                            HS_EXPR_COALESCE: the argument count */
   double value_f;        /* DOUBLE */
 } hs_expr_node;
 
