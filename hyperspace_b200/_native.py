@@ -46,6 +46,8 @@ EXPR_FUNCS = {name: 9 + k for k, name in enumerate(
 HS_EXPR_COALESCE = EXPR_FUNCS["coalesce"]
 HS_TYPE_DATE, HS_TYPE_TIMESTAMP = 7, 8  # expression literals only
 HS_CODEC_UNCOMPRESSED, HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 = 0, 1, 2, 5
+HS_KEY_DECIMAL = 1  # hs_host_column.reserved of a decimal key column
+PARTITION_MODES = {"local": 0, "owner": 1, "peer": 2}  # hs_k_partition's HS_PART_*
 
 _NP_OF_TYPE = {HS_TYPE_INT32: np.int32, HS_TYPE_INT64: np.int64, HS_TYPE_FLOAT: np.float32, HS_TYPE_DOUBLE: np.float64,
                HS_TYPE_BOOL: np.uint8}
@@ -158,7 +160,7 @@ EXPORTED_SYMBOLS = [
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
     "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists", "hs_bucket_join_outer", "hs_filter_scan_expr",
-    "hs_bucket_join_expr",
+    "hs_bucket_join_expr", "hs_k_partition",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -242,6 +244,10 @@ def load_library() -> C.CDLL:
     L.hs_k_bucket_ids.argtypes = [C.c_void_p, C.POINTER(HostColumn), C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, *err]
     L.hs_k_sort_perm.restype = C.c_int
     L.hs_k_sort_perm.argtypes = [C.c_void_p, C.POINTER(HostColumn), C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, *err]
+    L.hs_k_partition.restype = C.c_int
+    L.hs_k_partition.argtypes = [C.c_void_p, C.POINTER(HostColumn), C.c_int32, C.c_int64, C.c_int32, C.POINTER(HostColumn), C.c_int32,
+                                 C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, *err]
     L.hs_synth_table.restype = C.c_int
     L.hs_synth_table.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_void_p), *err]
@@ -1210,13 +1216,14 @@ class Context:
 
     # ---- kernel-level entry points ----------------------------------------------------------------------------------
     @staticmethod
-    def _host_columns(cols: Sequence[np.ndarray], valids):
+    def _host_columns(cols: Sequence[np.ndarray], valids, decimal=None):
         keep = []
-        arr = (HostColumn * len(cols))()
+        arr = (HostColumn * max(1, len(cols)))()
         for i, c in enumerate(cols):
             c = np.ascontiguousarray(c)
             keep.append(c)
             arr[i].type = _TYPE_OF_NP[c.dtype]
+            arr[i].reserved = HS_KEY_DECIMAL if decimal is not None and decimal[i] else 0
             arr[i].data = c.ctypes.data
             v = None if valids is None else valids[i]
             if v is not None:
@@ -1246,3 +1253,44 @@ class Context:
         _check(load_library().hs_k_sort_perm(self._h, arr, len(keys), n, num_buckets, perm.ctypes.data, offs.ctypes.data,
                                              err, len(err)), err)
         return perm, offs
+
+    def k_partition(self, keys: Sequence[np.ndarray], num_buckets: int, valids=None, decimal=None,
+                    payload: Sequence[np.ndarray] = (), codes: Sequence[np.ndarray] = (), mode="local", world: int = 1,
+                    peer_base=None, owner_rows=None, owner_shift=None, fill: int = 0xA5) -> Dict[str, object]:
+        """hs_k_partition: the hash partition alone.  decimal[i]: key i holds a decimal's unscaled values.  payload: columns
+        of 8, 4 or 1 byte values; codes: 0..4 uint16 columns.  mode "local", "owner" or "peer" (or an HS_PART_* code); a
+        peer layout is peer_base (num_buckets rows) with owner_rows (world buffer sizes, rows) and owner_shift (bytes).
+        Returns the output buffers as bytes, slack included: "payload" (per column: one uint8 array, or with a peer layout
+        one per owner), "records" (likewise, None without codes), "offsets" (the bins' nbins + 1 offsets, None with a peer
+        layout) and "key_or_and"."""
+        n = len(keys[0])
+        karr, keep = self._host_columns(keys, valids, decimal)
+        parr, pkeep = self._host_columns(payload, None)
+        code_cols = [np.ascontiguousarray(c, dtype=np.uint16) for c in codes]
+        code_ptrs = (C.c_void_p * max(1, len(code_cols)))(*[c.ctypes.data for c in code_cols])
+        owners = world if peer_base is not None else 1
+        rows = [int(r) for r in owner_rows] if peer_base is not None else [n]
+        shift = [int(s) for s in owner_shift] if owner_shift is not None and peer_base is not None else [0] * owners
+        base = np.ascontiguousarray(peer_base, dtype=np.uint64) if peer_base is not None else None
+        rows_arr = np.ascontiguousarray(rows, dtype=np.uint64)
+        shift_arr = np.ascontiguousarray(shift, dtype=np.int32)
+
+        def buffers(width):
+            return [np.empty(shift[o] + rows[o] * width + 16, dtype=np.uint8) for o in range(owners)]
+        outs = [buffers(np.ascontiguousarray(p).dtype.itemsize) for p in payload]
+        recs = buffers(8) if code_cols else []
+        out_ptrs = (C.c_void_p * max(1, len(outs) * owners))(*[b.ctypes.data for col in outs for b in col])
+        rec_ptrs = (C.c_void_p * max(1, owners))(*[b.ctypes.data for b in recs])
+        nbins = world if mode in ("owner", PARTITION_MODES["owner"]) else num_buckets
+        offs = np.zeros(nbins + 1, dtype=np.uint64)
+        or_and = np.zeros(2, dtype=np.uint64)
+        err = C.create_string_buffer(1024)
+        _check(load_library().hs_k_partition(
+            self._h, karr, len(keys), n, num_buckets, parr, len(payload), code_ptrs if code_cols else None, len(code_cols),
+            PARTITION_MODES.get(mode, mode), world, None if base is None else base.ctypes.data,
+            rows_arr.ctypes.data if base is not None else None, shift_arr.ctypes.data if base is not None else None, fill,
+            out_ptrs, rec_ptrs if code_cols else None, offs.ctypes.data, or_and.ctypes.data, err, len(err)), err)
+        single = base is None
+        return {"payload": [col[0] if single else col for col in outs],
+                "records": (recs[0] if single else recs) if code_cols else None,
+                "offsets": offs if single else None, "key_or_and": (int(or_and[0]), int(or_and[1]))}

@@ -1911,6 +1911,14 @@ static void upload_table(hs_ctx* ctx, const hs_host_column* keys, int nkeys, int
       if (nrows) copy_h2d(ctx, c.valid.get(), keys[k].valid, (size_t)nrows);
       c.has_nulls = true;
     }
+    if (keys[k].reserved == HS_KEY_DECIMAL) {  // hashed as the build hashes a decimal source column (key_column_of)
+      if (c.type != HS_TYPE_INT32 && c.type != HS_TYPE_INT64) fail(HS_EINVAL, "a decimal key is an int32 or int64 column");
+      c.schema.converted_type = pq::CT_DECIMAL;
+      c.schema.precision = c.type == HS_TYPE_INT32 ? 9 : 18;
+      c.schema.scale = 0;
+    } else if (keys[k].reserved != 0) {
+      fail(HS_EINVAL, "key column %d: unknown flags %d", k, keys[k].reserved);
+    }
   }
   sync_stream(ctx);
 }
@@ -1962,6 +1970,98 @@ int hs_k_sort_perm(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64
     sync_stream(ctx);
     for (int64_t i = 0; i < nrows; i++) out_perm[i] = h[i];
     for (int b = 0; b <= num_buckets; b++) out_bucket_offsets[b] = (int64_t)rows.bucket_offsets[b];
+  });
+}
+
+int hs_k_partition(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64_t nrows, int32_t num_buckets,
+                   const hs_host_column* payload, int32_t npayload, const uint16_t* const* codes, int32_t ncodes,
+                   int32_t mode, int32_t world, const uint64_t* peer_base, const uint64_t* owner_rows,
+                   const int32_t* owner_shift, int32_t fill, void* const* out_payload, void* const* out_records,
+                   uint64_t* out_offsets, uint64_t* out_key_or_and, char* err, size_t errlen) {
+  if (!ctx) return HS_EINVAL;
+  return guarded(ctx, err, errlen, [&] {
+    if (num_buckets < 1 || num_buckets > kMaxBuckets) fail(HS_EUNSUPPORTED, "numBuckets must be in 1..%d", kMaxBuckets);
+    if (nkeys < 1 || !keys || nrows < 0 || nrows >= (1ll << 32)) fail(HS_EINVAL, "bad keys or row count");
+    if (mode != HS_PART_LOCAL && mode != HS_PART_OWNER && mode != HS_PART_PEER) fail(HS_EINVAL, "unknown mode %d", mode);
+    if (world < 1 || world > 64) fail(HS_EINVAL, "world = %d: 1..64 owners", world);
+    if (npayload < 0 || (npayload && (!payload || !out_payload))) fail(HS_EINVAL, "bad payload columns");
+    if (ncodes < 0 || ncodes > 4 || (ncodes && (!codes || !out_records))) fail(HS_EINVAL, "bad code columns");
+    if (peer_base && !owner_rows) fail(HS_EINVAL, "a peer layout needs every owner's buffer size");
+    Table t;
+    upload_table(ctx, keys, nkeys, nrows, &t);
+    std::vector<KeyColumn> h_keys(nkeys);
+    for (int k = 0; k < nkeys; k++) h_keys[k] = key_column_of(t.cols[k]);
+    const int owner_mod = mode == HS_PART_OWNER ? world : 0;
+    const int nbins = owner_mod > 0 ? owner_mod : num_buckets;
+    // output buffers: one per column, or one per (column, owner) with a peer layout; `shift` bytes before the first row
+    const int owners = peer_base ? world : 1;
+    auto rows_of = [&](int o) { return peer_base ? (size_t)owner_rows[o] : (size_t)nrows; };
+    auto shift_of = [&](int o) -> size_t {
+      const int s = peer_base && owner_shift ? owner_shift[o] : 0;
+      if (s != 0 && s != 8) fail(HS_EINVAL, "owner %d: shift %d bytes, 0 or 8 expected", o, s);
+      return (size_t)s;
+    };
+    std::vector<Buf<uint8_t>> in(npayload), out((size_t)(npayload + 1) * owners);
+    std::vector<size_t> out_bytes((size_t)(npayload + 1) * owners, 0);
+    std::vector<void*> table((size_t)(npayload + 1) * owners, nullptr);  // the peer table: a row of owners per round
+    std::vector<PartColumn> h_pc(npayload);
+    auto alloc_out = [&](size_t i, int o, int width) {
+      out_bytes[i] = shift_of(o) + rows_of(o) * width + 16;
+      out[i].alloc(ctx, out_bytes[i]);
+      fill_bytes(ctx, out[i].get(), fill & 0xff, out_bytes[i]);
+      table[i] = out[i].get() + shift_of(o);
+    };
+    for (int c = 0; c < npayload; c++) {
+      const int width = payload[c].type == HS_TYPE_STRING ? 0 : type_width(payload[c].type);
+      if (width != 1 && width != 4 && width != 8) fail(HS_EINVAL, "payload column %d: type %d", c, payload[c].type);
+      in[c].alloc(ctx, (size_t)nrows * width + 16);
+      if (nrows) copy_h2d(ctx, in[c].get(), payload[c].data, (size_t)nrows * width);
+      for (int o = 0; o < owners; o++) alloc_out((size_t)c * owners + o, o, width);
+      h_pc[c] = PartColumn{in[c].get(), peer_base ? nullptr : table[(size_t)c * owners], width, 0};
+    }
+    std::vector<Buf<uint16_t>> code_in(ncodes);
+    CodePackRound pack;
+    memset(&pack, 0, sizeof pack);
+    for (int j = 0; j < ncodes; j++) {
+      code_in[j].alloc(ctx, (size_t)nrows + 16);
+      if (nrows) copy_h2d(ctx, code_in[j].get(), codes[j], (size_t)nrows * 2);
+      pack.src[j] = code_in[j].get();
+    }
+    pack.n = ncodes;
+    if (ncodes) {
+      for (int o = 0; o < owners; o++) alloc_out((size_t)npayload * owners + o, o, 8);
+      if (!peer_base) pack.out = table[(size_t)npayload * owners];
+    }
+    Buf<unsigned long long> ghist(ctx, nbins), offsets(ctx, nbins + 1), key_bits(ctx, 2), base;
+    fill_bytes(ctx, ghist.get(), 0, 8 * (size_t)nbins);
+    const unsigned long long init[2] = {0ull, ~0ull};
+    copy_h2d(ctx, key_bits.get(), init, sizeof init);
+    if (peer_base) {
+      base.alloc(ctx, std::max(nbins, num_buckets));
+      fill_bytes(ctx, base.get(), 0, 8 * (size_t)std::max(nbins, num_buckets));
+      copy_h2d(ctx, base.get(), peer_base, 8 * (size_t)num_buckets);
+    }
+    Buf<void*> d_table(ctx, table.size());
+    copy_h2d(ctx, d_table.get(), table.data(), sizeof(void*) * table.size());
+    // the three steps of index_rows (one GPU) and exchange_partition_p2p (the owners' buffers over NVLink)
+    HashedRows hashed;
+    hash_rows(ctx, h_keys.data(), nkeys, nrows, num_buckets, owner_mod, mode == HS_PART_PEER, ghist.get(), key_bits.get(),
+              &hashed);
+    launch_tile_offsets(ctx, hashed.tile_hist.get(), hashed.ntiles, nbins, ghist.get(), peer_base ? nullptr : offsets.get(),
+                        peer_base ? base.get() : nullptr);
+    move_rows(ctx, hashed, h_pc.data(), npayload, &pack, peer_base ? d_table.get() : nullptr, world);
+    for (int c = 0; c < npayload; c++)
+      for (int o = 0; o < owners; o++) {
+        const size_t i = (size_t)c * owners + o;
+        copy_d2h(ctx, out_payload[i], out[i].get(), out_bytes[i]);
+      }
+    for (int o = 0; ncodes && o < owners; o++) {
+      const size_t i = (size_t)npayload * owners + o;
+      copy_d2h(ctx, out_records[o], out[i].get(), out_bytes[i]);
+    }
+    if (out_offsets && !peer_base) copy_d2h(ctx, out_offsets, offsets.get(), 8 * (size_t)(nbins + 1));
+    if (out_key_or_and) copy_d2h(ctx, out_key_or_and, key_bits.get(), sizeof init);
+    sync_stream(ctx);
   });
 }
 

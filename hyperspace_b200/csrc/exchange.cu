@@ -485,7 +485,7 @@ void exchange_partition_p2p(hs_ctx* ctx, Table& table, int nkeys, int num_bucket
   copy_h2d(ctx, d_peer.get(), h_peer.data(), sizeof(void*) * nmoved * world);
   launch_tile_offsets(ctx, hashed.tile_hist.get(), hashed.ntiles, nb, d_mine.get(), nullptr, d_base.get());
   // the peer table holds one row of `world` pointers per column round, then one row for the code records
-  move_rows(ctx, hashed, h_pc.data(), ncolmoved, &pack, (void* const*)d_peer.get());
+  move_rows(ctx, hashed, h_pc.data(), ncolmoved, &pack, (void* const*)d_peer.get(), world);
   // closing barrier: nobody reads its receive buffers before every peer's kernel has completed.  Stream-ordered -- the
   // sort that follows is enqueued behind it, the host does not wait here.
   HS_NCCL(nccl().AllGather(d_mine.get(), d_all.get(), 1, kNcclUint64, ctx->comm->comm, ctx->stream));

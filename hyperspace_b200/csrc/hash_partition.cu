@@ -823,7 +823,7 @@ void hash_rows(hs_ctx* ctx, const KeyColumn* keys, int nkeys, int64_t nrows, int
 }
 
 void move_rows(hs_ctx* ctx, const HashedRows& h, const PartColumn* cols, int ncols, const CodePackRound* pack,
-               void* const* peer_out) {
+               void* const* peer_out, int peers) {
   if ((peer_out != nullptr) != h.to_peers) fail(HS_EINVAL, "move_rows: a peer table is needed exactly when rows go to peers");
   if (h.nbins > kFusedMaxBins) {  // bin ids -> destinations -> one scatter per column
     if (pack && pack->n > 0) fail(HS_EINVAL, "%d bins: code records need at most %d bins", h.nbins, kFusedMaxBins);
@@ -839,7 +839,7 @@ void move_rows(hs_ctx* ctx, const HashedRows& h, const PartColumn* cols, int nco
   KernelScope _ks(ctx, "k_partition_rows");
   if (h.nrows == 0) return;
   PartitionLaunch a{h.keys.get(), h.nkeys, h.nrows, h.num_buckets, h.owner_mod, h.tile_hist.get(), d_cols.get(), ncols,
-                    peer_out, h.to_peers ? ctx->world : 1, {}, h.bin_ids.get()};
+                    peer_out, h.to_peers ? peers : 1, {}, h.bin_ids.get()};
   memset(&a.pack, 0, sizeof a.pack);
   if (pack) a.pack = *pack;
   if (h.to_peers) launch_partition_rows<true>(ctx, a, h.single_key_type);

@@ -208,10 +208,10 @@ struct CodePackRound {
 };
 // K3, after launch_tile_offsets(h.tile_hist): moves the columns (host descriptors, read until the caller's next
 // synchronisation) into bin-major order, stable.  pack (optional): the code records, fused partition only.
-// peer_out (to_peers only): device table of peer-mapped output pointers, one row of ctx->world per column round and then
-// one for the code records; bucket b is written to GPU b % world.
+// peer_out (to_peers only): device table of peer-mapped output pointers, one row of `peers` per column round and then
+// one for the code records; bucket b is written to owner b % peers (exchange.cu: the GPU of that rank, peers = world).
 void move_rows(hs_ctx* ctx, const HashedRows& h, const PartColumn* cols, int ncols, const CodePackRound* pack = nullptr,
-               void* const* peer_out = nullptr);
+               void* const* peer_out = nullptr, int peers = 1);
 // out[i] = sort_encode(in[src ? src[i] : i])  (+ global OR / AND reduction into or_and[0], or_and[1])
 void launch_encode_keys(hs_ctx* ctx, const void* in, int type, const uint32_t* src, int64_t nrows, uint64_t* out,
                         unsigned long long* or_and);

@@ -699,10 +699,13 @@ int hs_synth_checksum(hs_ctx* ctx, int64_t first_row, int64_t nrows, int32_t nco
 
 typedef struct {
   int32_t type;         /* HS_TYPE_* */
-  int32_t reserved;
+  int32_t reserved;     /* key columns: HS_KEY_DECIMAL or 0 */
   const void* data;     /* n values */
   const uint8_t* valid; /* one byte per row or NULL */
 } hs_host_column;
+/* hs_host_column.reserved of an int32 / int64 key column: its values are the unscaled values of a DecimalType(p <= 18),
+ * bucketed as Spark does (hashLong of the unscaled value; for an int32 column that differs from an int's hash) */
+#define HS_KEY_DECIMAL 1
 
 /* K2: bucket id per row (int32) and the num_buckets-bin histogram (int64) of Spark's HashPartitioning. */
 int hs_k_bucket_ids(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64_t nrows, int32_t num_buckets,
@@ -710,6 +713,31 @@ int hs_k_bucket_ids(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int6
 /* K3+K4: permutation ordering rows by (bucket, keys ascending nulls-first); bucket_offsets has num_buckets+1 entries. */
 int hs_k_sort_perm(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64_t nrows, int32_t num_buckets,
                    int64_t* out_perm, int64_t* out_bucket_offsets, char* err, size_t errlen);
+
+/* K2+K3: the hash partition as createIndex runs it, alone.  Every row's bin is its bucket (HS_PART_LOCAL, what one GPU
+ * does; HS_PART_PEER) or its owner bucket % world (HS_PART_OWNER, how several GPUs split their rows above 1024 buckets),
+ * and the rows move stably into bin-major order:
+ *   payload   npayload columns of 8-, 4- or 1-byte values (type gives the width; valid is not read -- validity travels as
+ *             a 1-byte column) moved with the rows;
+ *   codes     ncodes (0..4) uint16 columns moved as ONE 8-byte record per row, code j in bits [16 j, 16 j + 16) (the
+ *             late-materialised dictionary columns of a build; up to 1024 bins only).
+ * HS_PART_PEER: the runs leave as they do for the owners' memory on several GPUs, here to `world` buffers on this one:
+ * bucket b's rows go to owner (b % world)'s buffer from row peer_base[b] on (num_buckets entries).  Owner o's buffer holds
+ * owner_rows[o] rows and starts owner_shift[o] bytes (0 or 8; NULL: all 0) past a 16-byte boundary.  A peer layout
+ * (peer_base) in another mode, or none in HS_PART_PEER, is refused with HS_EINVAL.
+ * Every output buffer is filled with the byte `fill` on the device first and copied back whole, its 16 bytes of slack
+ * included: out_payload[c] (nrows * width + 16 bytes) and out_records[0] (nrows * 8 + 16); with a peer layout
+ * out_payload[c * world + o] (owner_shift[o] + owner_rows[o] * width + 16 bytes) and out_records[o] likewise.
+ * out_offsets (optional, no peer layout): the nbins + 1 row offsets of the bins.  out_key_or_and (optional): the OR and
+ * the AND of the sort encoding of the last key column over all rows, a null counted as 0 (they pick the sort's passes). */
+#define HS_PART_LOCAL 0
+#define HS_PART_OWNER 1
+#define HS_PART_PEER 2
+int hs_k_partition(hs_ctx* ctx, const hs_host_column* keys, int32_t nkeys, int64_t nrows, int32_t num_buckets,
+                   const hs_host_column* payload, int32_t npayload, const uint16_t* const* codes, int32_t ncodes,
+                   int32_t mode, int32_t world, const uint64_t* peer_base, const uint64_t* owner_rows,
+                   const int32_t* owner_shift, int32_t fill, void* const* out_payload, void* const* out_records,
+                   uint64_t* out_offsets, uint64_t* out_key_or_and, char* err, size_t errlen);
 
 /* Synthetic table T of the benchmark (SURVEY.md section 8d): rows [first_row, first_row+nrows) of
  * (k:int64, v1:int64, v2:float64, v3:int32, v4:float32)[:ncols], generated and Parquet-encoded on the GPU into
