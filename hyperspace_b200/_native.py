@@ -160,7 +160,7 @@ EXPORTED_SYMBOLS = [
     "hs_synth_table_ex", "hs_k_snappy_compress", "hs_k_snappy_decompress", "hs_batch_string_offsets", "hs_filter_scan_where",
     "hs_bucket_join_where", "hs_k_inflate", "hs_filter_scan_any", "hs_bucket_join_any", "hs_k_lz4", "hs_k_compress",
     "hs_filter_scan_cmp", "hs_bucket_join_cmp", "hs_bucket_join_exists", "hs_bucket_join_outer", "hs_filter_scan_expr",
-    "hs_bucket_join_expr", "hs_k_partition",
+    "hs_bucket_join_expr", "hs_k_partition", "hs_k_decompress_blobs",
 ]
 
 _lib: Optional[C.CDLL] = None
@@ -285,6 +285,10 @@ def load_library() -> C.CDLL:
     L.hs_k_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
     L.hs_k_lz4.restype = C.c_int
     L.hs_k_lz4.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, *err]
+    L.hs_k_decompress_blobs.restype = C.c_int
+    L.hs_k_decompress_blobs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64,
+                                        C.POINTER(C.c_int32), *err]
     L.hs_k_compress.restype = C.c_int
     L.hs_k_compress.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), *err]
     if L.hs_abi_version() != 1:
@@ -983,6 +987,20 @@ class Context:
         err = C.create_string_buffer(1024)
         _check(load_library().hs_k_lz4(self._h, codec, stream, len(stream), out, uncompressed_len, err, len(err)), err)
         return out.raw[:uncompressed_len]
+
+    def k_decompress_blobs(self, data: bytes, blobs, out_len: int, fill: int = 0) -> Tuple[bytes, List[bool]]:
+        """The page decompressors over several blobs of `data` in one launch.  blobs: (src_off, src_len, dst_off, dst_len,
+        prefix, compressed, codec) per blob.  Returns the whole output buffer of out_len bytes, pre-filled with `fill`, and
+        per blob whether a snappy stream was decoded front to back by one lane."""
+        cols = list(zip(*blobs)) if blobs else [()] * 7
+        arrs = [np.ascontiguousarray(c, dtype=t) for c, t in zip(cols, (np.uint64, np.uint32, np.uint64, np.uint32, np.uint32,
+                                                                          np.int32, np.int32))]
+        out = C.create_string_buffer(max(1, out_len))
+        seq = (C.c_int32 * max(1, len(blobs)))()
+        err = C.create_string_buffer(1024)
+        _check(load_library().hs_k_decompress_blobs(self._h, data, len(data), len(blobs), *(a.ctypes.data for a in arrs), fill,
+                                                    out, out_len, seq, err, len(err)), err)
+        return out.raw[:out_len], [bool(seq[i]) for i in range(len(blobs))]
 
     def k_compress(self, data: bytes, codec: int) -> bytes:
         """The index page compressor on one page body: HS_CODEC_GZIP (one gzip member) or HS_CODEC_LZ4 (Hadoop-framed

@@ -2109,60 +2109,94 @@ int hs_k_compress(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* 
   return compress_one_body(ctx, codec, in, n, out_buf, cap, out_len, err, errlen);
 }
 
+namespace {
+// Blobs of one host buffer through decompress_blobs, in one launch as decompress_pages makes it: each blob's `src` holds
+// its offset in `in` on entry.  The whole scratch is pre-filled with `fill` and copied back to `out`, gaps included, so a
+// caller sees any byte a decoder wrote outside its blob.  sequential (optional): per blob in the caller's order, 1 where
+// a snappy stream was decoded front to back.
+void decompress_host_blobs(hs_ctx* ctx, const void* in, uint64_t n_in, std::vector<PageBlob> blobs, int fill, void* out,
+                           uint64_t out_len, int32_t* sequential) {
+  // decoders read up to 8 bytes past a stream and one aligned word past a page
+  Buf<uint8_t> d_in(ctx, n_in + 16), d_out(ctx, out_len + 32);
+  if (n_in) copy_h2d(ctx, d_in.get(), in, n_in);
+  fill_bytes(ctx, d_out.get(), fill, out_len + 32);
+  Buf<uint32_t> d_error(ctx, 1);
+  fill_bytes(ctx, d_error.get(), 0, 4);
+  std::vector<uint32_t> codecs(blobs.size());
+  for (size_t i = 0; i < blobs.size(); i++) {
+    blobs[i].src = d_in.get() + (uintptr_t)blobs[i].src;
+    codecs[i] = blobs[i].codec;
+  }
+  std::vector<uint32_t> seq;
+  decompress_blobs(ctx, blobs, d_out.get(), d_error.get(), &seq);
+  uint32_t error = 0;
+  copy_d2h(ctx, &error, d_error.get(), 4);
+  sync_stream(ctx);
+  const uint32_t check = error & 0xffffffu;
+  if ((error >> 24) == DERR_SNAPPY) fail(HS_EFORMAT, "corrupt snappy stream (check %u)", check);
+  if ((error >> 24) == DERR_GZIP) fail(HS_EFORMAT, "corrupt gzip stream: %s (check %u)", gz::inflate_error_text(check), check);
+  if ((error >> 24) == DERR_LZ4) fail(HS_EFORMAT, "corrupt lz4 block: %s (check %u)", lz4::lz4_error_text(check), check);
+  if (error) fail(HS_EFORMAT, "page decompression failed (code %u, check %u)", error >> 24, check);
+  if (out_len) HS_CUDA(cudaMemcpy(out, d_out.get(), out_len, cudaMemcpyDeviceToHost));
+  if (sequential) {  // decompress_blobs puts the snappy blobs first, in the caller's order
+    size_t k = 0;
+    for (size_t i = 0; i < codecs.size(); i++) sequential[i] = codecs[i] == (uint32_t)pq::SNAPPY ? (int32_t)seq[k++] : 0;
+  }
+}
+
+PageBlob one_blob(uint64_t n, uint64_t out_len, int codec) {
+  return PageBlob{nullptr, 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)codec};
+}
+}  // namespace
+
+int hs_k_decompress_blobs(hs_ctx* ctx, const void* in, uint64_t n_in, int32_t n_blobs, const uint64_t* src_off,
+                          const uint32_t* src_len, const uint64_t* dst_off, const uint32_t* dst_len, const uint32_t* prefix,
+                          const int32_t* compressed, const int32_t* codec, int32_t fill, void* out, uint64_t out_len,
+                          int32_t* sequential, char* err, size_t errlen) {
+  if (!ctx || n_blobs < 0 || (n_in && !in) || (out_len && !out) ||
+      (n_blobs && (!src_off || !src_len || !dst_off || !dst_len || !prefix || !compressed || !codec)))
+    return HS_EINVAL;
+  return guarded(ctx, err, errlen, [&] {
+    if (n_in > 0xffffffffull || out_len > 0xfffffff0ull) fail(HS_EINVAL, "buffers above 4 GB");
+    std::vector<PageBlob> blobs;
+    std::vector<std::pair<uint64_t, uint64_t>> dst;  // (offset, length) of every blob's decoded bytes
+    for (int32_t i = 0; i < n_blobs; i++) {
+      const int c = codec[i];
+      if (c != pq::SNAPPY && c != pq::GZIP && c != pq::LZ4 && c != pq::LZ4_RAW) fail(HS_EINVAL, "blob %d: codec %d", i, c);
+      if (compressed[i] != 0 && compressed[i] != 1) fail(HS_EINVAL, "blob %d: compressed must be 0 or 1", i);
+      if (src_off[i] > n_in || src_len[i] > n_in - src_off[i]) fail(HS_EINVAL, "blob %d: source range beyond the input", i);
+      if (dst_off[i] > out_len || dst_len[i] > out_len - dst_off[i]) fail(HS_EINVAL, "blob %d: destination range beyond the output", i);
+      if (prefix[i] > src_len[i] || prefix[i] > dst_len[i]) fail(HS_EINVAL, "blob %d: prefix beyond the blob", i);
+      blobs.push_back(PageBlob{(const uint8_t*)(uintptr_t)src_off[i], dst_off[i], src_len[i], dst_len[i], prefix[i],
+                               (uint32_t)compressed[i], 0u, (uint32_t)c});
+      dst.emplace_back(dst_off[i], dst_len[i]);
+    }
+    std::sort(dst.begin(), dst.end());
+    for (size_t i = 1; i < dst.size(); i++)
+      if (dst[i - 1].first + dst[i - 1].second > dst[i].first) fail(HS_EINVAL, "destination ranges overlap");
+    decompress_host_blobs(ctx, in, n_in, std::move(blobs), fill, out, out_len, sequential);
+  });
+}
+
 int hs_k_snappy_decompress(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t out_len, int32_t* sequential,
                            char* err, size_t errlen) {
   if (!ctx || !in || n == 0 || n > 0xffffffffull || out_len > 0xfffffff0ull || (out_len && !out_buf)) return HS_EINVAL;
-  return guarded(ctx, err, errlen, [&] {
-    Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
-    copy_h2d(ctx, d_in.get(), in, n);
-    Buf<uint32_t> d_error(ctx, 1);
-    fill_bytes(ctx, d_error.get(), 0, 4);
-    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::SNAPPY}};
-    std::vector<uint32_t> seq;
-    decompress_blobs(ctx, blob, d_out.get(), d_error.get(), &seq);
-    uint32_t error = 0;
-    copy_d2h(ctx, &error, d_error.get(), 4);
-    sync_stream(ctx);
-    if (error) fail(HS_EFORMAT, "corrupt snappy stream (check %u)", error & 0xffffffu);
-    if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
-    if (sequential) *sequential = (int32_t)seq[0];
-  });
+  return guarded(ctx, err, errlen,
+                 [&] { decompress_host_blobs(ctx, in, n, {one_blob(n, out_len, pq::SNAPPY)}, 0, out_buf, out_len, sequential); });
 }
 
 int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out_buf, uint64_t out_len, char* err, size_t errlen) {
   if (!ctx || (n && !in) || n > 0xffffffffull || out_len > 0xfffffff0ull || (out_len && !out_buf)) return HS_EINVAL;
-  return guarded(ctx, err, errlen, [&] {
-    Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
-    if (n) copy_h2d(ctx, d_in.get(), in, n);
-    Buf<uint32_t> d_error(ctx, 1);
-    fill_bytes(ctx, d_error.get(), 0, 4);
-    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)pq::GZIP}};
-    decompress_blobs(ctx, blob, d_out.get(), d_error.get());
-    uint32_t error = 0;
-    copy_d2h(ctx, &error, d_error.get(), 4);
-    sync_stream(ctx);
-    if (error) fail(HS_EFORMAT, "corrupt gzip stream: %s (check %u)", gz::inflate_error_text(error & 0xffffffu), error & 0xffffffu);
-    if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
-  });
+  return guarded(ctx, err, errlen,
+                 [&] { decompress_host_blobs(ctx, in, n, {one_blob(n, out_len, pq::GZIP)}, 0, out_buf, out_len, nullptr); });
 }
 
 int hs_k_lz4(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out_buf, uint64_t out_len, char* err, size_t errlen) {
   if (!ctx || (codec != pq::LZ4 && codec != pq::LZ4_RAW) || (n && !in) || n > 0xffffffffull || out_len > 0xfffffff0ull ||
       (out_len && !out_buf))
     return HS_EINVAL;
-  return guarded(ctx, err, errlen, [&] {
-    Buf<uint8_t> d_in(ctx, n + 16), d_out(ctx, out_len + 32);
-    if (n) copy_h2d(ctx, d_in.get(), in, n);
-    Buf<uint32_t> d_error(ctx, 1);
-    fill_bytes(ctx, d_error.get(), 0, 4);
-    std::vector<PageBlob> blob{{d_in.get(), 0, (uint32_t)n, (uint32_t)out_len, 0u, 1u, 0u, (uint32_t)codec}};
-    decompress_blobs(ctx, blob, d_out.get(), d_error.get());
-    uint32_t error = 0;
-    copy_d2h(ctx, &error, d_error.get(), 4);
-    sync_stream(ctx);
-    if (error) fail(HS_EFORMAT, "corrupt lz4 block: %s (check %u)", lz4::lz4_error_text(error & 0xffffffu), error & 0xffffffu);
-    if (out_len) HS_CUDA(cudaMemcpy(out_buf, d_out.get(), out_len, cudaMemcpyDeviceToHost));
-  });
+  return guarded(ctx, err, errlen,
+                 [&] { decompress_host_blobs(ctx, in, n, {one_blob(n, out_len, codec)}, 0, out_buf, out_len, nullptr); });
 }
 
 int hs_synth_table_ex(hs_ctx* ctx, int64_t first_row, int64_t nrows, int32_t ncols, int32_t n_files,

@@ -43,8 +43,8 @@ constexpr uint32_t kSeg = 256;           // least compressed bytes per lane and 
 constexpr uint32_t kBroken = 0xffffffffu;
 
 struct Element {
-  uint32_t len, offset, hdr;  // offset == 0: literal of len bytes following hdr tag bytes (len 0: length field overflow)
-};
+  uint32_t len, offset, hdr;  // offset == 0: literal of len bytes following hdr tag bytes
+};                            // len 0: a literal's length field overflows, or a copy has offset 0 -- the callers reject it
 
 // the element whose tag is at p: two aligned words cover the tag and its (up to) four trailing bytes.  Written with
 // selects, not branches: the lanes of a warp parse elements of different kinds in the same instructions.
@@ -61,8 +61,9 @@ __device__ __forceinline__ Element parse_element(const uint8_t* __restrict__ p) 
   const uint32_t t = trailer & (tail >= 4 ? 0xffffffffu : ((1u << (8 * tail)) - 1u));
   Element e;
   e.hdr = 1 + tail;
-  e.len = lit ? (nb ? t : upper) + 1 : (kind == 1 ? (upper & 7) + 4 : upper + 1);  // 0: a 0xffffffff length field, rejected by the callers
   e.offset = lit ? 0u : (kind == 1 ? ((tag >> 5) << 8) | t : t);
+  const uint32_t copy_len = e.offset == 0 ? 0u : (kind == 1 ? (upper & 7) + 4 : upper + 1);  // a copy of offset 0 is invalid
+  e.len = lit ? (nb ? t : upper) + 1 : copy_len;  // 0 for a 0xffffffff length field too
   return e;
 }
 
@@ -260,16 +261,18 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const PageB
       pos = my_in[bi];
       in_hi = (seq || bi + 1 >= n_blocks) ? n_src : min(my_in[bi + 1], n_src);
       out = out_lo;
-      if (bi == 0) {  // preamble: the uncompressed length must be the page header's
+      if (bi == 0) {  // preamble: the uncompressed length must be the page header's, a varint of 32 bits at most
         uint32_t p = 0, ulen = 0;
         int shift = 0;
+        bool ended = false;
         while (p < n_src && p < 5) {
           const uint8_t c = src[p++];
           ulen |= (uint32_t)(c & 0x7f) << shift;
-          if (!(c & 0x80)) break;
+          ended = !(c & 0x80);
+          if (ended) break;
           shift += 7;
         }
-        if (ulen != dst_len || p != pos) error = 1;
+        if (!ended || (p == 5 && src[4] >= 16) || ulen != dst_len || p != pos) error = 1;
       }
     }
   }
@@ -310,7 +313,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) k_snappy_blocks(const PageB
       pos += e.hdr + (e.offset == 0 ? e.len : 0u);
     }
   }
-  if (live && !error && out != out_hi) error = 5;
+  // the block's bytes are all there, and so is nothing else: as the reference decoder, refuse elements after a full output
+  if (live && !error) error = out != out_hi ? 5u : (pos != in_hi ? 6u : 0u);
   if (error) atomicCAS(d_error, 0u, ((uint32_t)DERR_SNAPPY << 24) | error);
 }
 

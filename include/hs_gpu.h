@@ -767,6 +767,18 @@ int hs_k_inflate(hs_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t ou
  * one block) or 5 (LZ4: Hadoop-framed blocks, or one raw block); any other codec is HS_EINVAL.  HS_EFORMAT for a damaged
  * body; the message names the failed check.  Kernel-level entry point for the parity tests. */
 int hs_k_lz4(hs_ctx* ctx, int32_t codec, const void* in, uint64_t n, void* out, uint64_t out_len, char* err, size_t errlen);
+/* The page decompressors over several blobs of one host buffer `in` (n_in bytes) in one launch, as the page reader makes
+ * it.  Blob i is src_len[i] bytes at src_off[i] of `in`, decoded into dst_len[i] bytes at dst_off[i] of `out` (out_len
+ * bytes); codec[i] is HS_CODEC_SNAPPY, HS_CODEC_GZIP, HS_CODEC_LZ4 or 7 (LZ4_RAW).  Its first prefix[i] bytes are stored
+ * verbatim (a v2 page's level bytes); compressed[i] = 0 stores the blob whole.  Source and destination ranges must lie
+ * in their buffers and destination ranges must not overlap (else HS_EINVAL).  The whole of `out` is first filled with the
+ * byte `fill`, so bytes outside the destination ranges come back as `fill` unless a decoder strayed.  sequential
+ * (optional, n_blobs entries): 1 where a snappy stream was decoded front to back by one lane.  HS_EFORMAT for a damaged
+ * blob; the message names the codec and the failed check.  Kernel-level entry point for the decoder tests. */
+int hs_k_decompress_blobs(hs_ctx* ctx, const void* in, uint64_t n_in, int32_t n_blobs, const uint64_t* src_off,
+                          const uint32_t* src_len, const uint64_t* dst_off, const uint32_t* dst_len, const uint32_t* prefix,
+                          const int32_t* compressed, const int32_t* codec, int32_t fill, void* out, uint64_t out_len,
+                          int32_t* sequential, char* err, size_t errlen);
 /* The page compressor of index builds on one page body of n bytes, through the same path as the encoder: codec HS_CODEC_GZIP
  * (one gzip member) or HS_CODEC_LZ4 (Hadoop-framed blocks, one per 64 KB); any other codec is HS_EINVAL.  *out_len is the
  * compressed size; HS_ENOMEM when it exceeds cap.  Kernel-level entry point for the parity tests. */

@@ -26,7 +26,7 @@ pyarrow refuses (empty runs, a run claiming more groups than its stream holds) a
 import functools
 import struct
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import Callable, List, Optional
 
 import numpy as np
 
@@ -298,6 +298,7 @@ class Chunk:
     dict_enc: int = PLAIN            # encoding written in the dictionary page header (parquet-mr v1: PLAIN_DICTIONARY)
     codec: int = UNCOMPRESSED
     gap: int = 0                     # bytes left unused before the chunk
+    snappy: Optional[Callable[[bytes], bytes]] = None  # SNAPPY chunks: the page compressor (default: pyarrow's)
 
 
 @dataclass
@@ -400,12 +401,13 @@ def _data_page(col: Col, ch: Chunk, pg: Page, pos: int, dict_len: int):
     else:
         levels = (struct.pack("<I", len(level_bytes)) + level_bytes) if col.optional else b""
     compress_values = ch.codec == SNAPPY and (pg.compressed or not pg.v2)
+    snappy = ch.snappy or _snappy
     if ch.codec == SNAPPY and not pg.v2:
         body_u = levels + values_part
-        body = _snappy(body_u)
+        body = snappy(body_u)
     else:
         body_u = levels + values_part
-        body = levels + (_snappy(values_part) if compress_values else values_part)
+        body = levels + (snappy(values_part) if compress_values else values_part)
     nulls = n - nvalid
     # the statistics' padding binary moves the values one byte per byte of padding
     pads = list(range(64)) if pg.stats else ([None] + list(range(64)) if pg.align else [None])
@@ -434,7 +436,7 @@ def write_file(spec: FileSpec) -> bytes:
             if ch.dict is not None:
                 dict_len = len(ch.dict)
                 dbody_u = _plain_bytes(col.ptype, ch.dict)
-                dbody = _snappy(dbody_u) if ch.codec == SNAPPY else dbody_u
+                dbody = (ch.snappy or _snappy)(dbody_u) if ch.codec == SNAPPY else dbody_u
                 dict_off = len(out)
                 out += _page_header(col.ptype, len(dbody_u), len(dbody), None, 0, None, dict_count=dict_len,
                                     dict_enc=ch.dict_enc) + dbody
